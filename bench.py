@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Benchmark of the whisper-burn hot path on B200 (contract: see the task statement / DESIGN.md section 6).
+"""Benchmark of the whisper-burn hot path on H100 (see DESIGN.md section 6).
 
-    python bench.py --gpus 1 --steps 5 --warmup 3                 # our arm  (C ABI -> sm_100a kernels)
+    python bench.py --gpus 1 --steps 5 --warmup 3                 # our arm  (C ABI -> sm_90a kernels)
+    python bench.py --gpus 1 --steps 5 --warmup 3 --dump-outputs DIR  # + the token ids of the last timed step as DIR/*.npy
     python bench.py --impl reference --gpus 1 --steps 1 --warmup 0  # reference arm: CPU oracle, reference-cost mode
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
 
@@ -51,7 +52,11 @@ def parse_args():
     ap.add_argument("--max-depth", type=int, default=100)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-baseline-windows", type=int, default=0, help="windows of chunk 0 timed on the CPU (0 = all)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what each workload's timed paths returned in their last step as DIR/<name>.npy")
     a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be at least 1")
     if a.configs is None:
         a.configs = f"{a.model}:{a.chunks_per_gpu}:{a.kv}" if a.model else DEFAULT_CONFIGS
     a.config_list = []
@@ -79,7 +84,7 @@ def peaks():
     if p.exists():
         j = json.loads(p.read_text())
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 def workload_name(model: str, chunks: int, beam: int, depth: int) -> str:
@@ -269,8 +274,8 @@ def run_config(args, cfg, ctx):
     for _ in range(args.warmup):
         step_device()
         step_e2e()
-    # the cyclic collector stays off inside the timed regions: a collection over the weight dictionaries costs milliseconds on a
-    # 10 ms step (the 8-GPU run of round 2 had one 14 ms step among 10.7 ms ones; host-side noise of this kind, cause not isolated)
+    # the cyclic collector stays off inside the timed regions: a collection over the weight dictionaries costs milliseconds, which
+    # is host-side noise on a step of about ten milliseconds
     import gc
     gc.collect()
     gc.disable()
@@ -294,11 +299,12 @@ def run_config(args, cfg, ctx):
     barrier()
     # ---- timed region: end to end through the user-facing call, host buffers
     e2e_ms = []
+    out_e2e = None
     for _ in range(args.steps):
         flush_buf.fill_(1)
         torch.cuda.synchronize()
         t0 = time.perf_counter()
-        step_e2e()
+        out_e2e = step_e2e()
         torch.cuda.synchronize()
         e2e_ms.append(1000.0 * (time.perf_counter() - t0))
     barrier()
@@ -379,7 +385,26 @@ def run_config(args, cfg, ctx):
         if per_rank is not None:
             res["per_rank_ms_wall_dev"] = per_rank
     sess.close()
-    return res, (dims, w_keep, sp, chunks[0], chunk_ids[0])
+    # what the two timed paths returned in their last step: token ids per window (device path) and per chunk (end to end)
+    outputs = {"windows_tokens": padded_ids(toks), "chunks_tokens": padded_ids(out_e2e)} if rank == 0 else None
+    return res, (dims, w_keep, sp, chunks[0], chunk_ids[0]), outputs
+
+
+def padded_ids(seqs) -> np.ndarray:
+    """Token id lists as one float64 array [len(seqs)][longest], padded with -1."""
+    a = np.full((len(seqs), max(1, max(len(x) for x in seqs))), -1.0, dtype=np.float64)
+    for i, x in enumerate(seqs):
+        a[i, :len(x)] = x
+    return a
+
+
+def dump_outputs(dir_: str, index: int, cfg, outputs: dict) -> None:
+    """DIR/<config index>_<model>_<chunks>x<kv>_<what>.npy; inputs are seeded, so two builds can be compared file by file."""
+    d = Path(dir_)
+    d.mkdir(parents=True, exist_ok=True)
+    model_name, chunks, kv = cfg
+    for what, arr in outputs.items():
+        np.save(d / f"{index}_{model_name}_{chunks}x{kv}_{what}.npy", arr)
 
 
 def run_ours(args):
@@ -398,15 +423,17 @@ def run_ours(args):
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     dev = torch.device("cuda", local_rank)
     ctx = {"world": world, "rank": rank, "local_rank": local_rank, "dev": dev, "models": {},
-           "flush": torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)}   # > 126 MB L2
+           "flush": torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)}   # > 50 MB L2
 
     sampler = ClockSampler(local_rank) if rank == 0 else None
     if sampler:
         sampler.start()
     results, head_inputs = [], None
     for i, cfg in enumerate(args.config_list):
-        res, inputs = run_config(args, cfg, ctx)
+        res, inputs, outputs = run_config(args, cfg, ctx)
         results.append(res)
+        if args.dump_outputs and outputs is not None:
+            dump_outputs(args.dump_outputs, i, cfg, outputs)
         if i == 0:
             head_inputs = inputs
     clocks = sampler.stop() if sampler else None

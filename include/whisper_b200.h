@@ -1,9 +1,9 @@
-/* whisper_b200.h -- C ABI of the B200-native Whisper hot path (libwhisper_b200.so).
+/* whisper_b200.h -- C ABI of the H100-native Whisper hot path (libwhisper_b200.so).
  *
  * The reference (Gadersd/whisper-burn) has no FFI: its hot path is Rust generic over
  * burn::tensor::backend::Backend.  This header is the boundary a thin Rust shim (rust/ in
  * this repo, INTEGRATION.md) binds with `extern "C"` so that whisper-burn's own public
- * functions keep their signatures while every tensor op runs in hand-written sm_100a CUDA:
+ * functions keep their signatures while every tensor op runs in hand-written sm_90a CUDA:
  *
  *   audio::max_waveform_samples        src/audio.rs:12-17          -> wb_max_waveform_samples
  *   audio::prep_audio                  src/audio.rs:34-56          -> wb_prep_audio

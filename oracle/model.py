@@ -111,7 +111,7 @@ def attn_decoder_mask(n: int) -> torch.Tensor:
 
 def qkv_attention(q, k, v, mask, n_head: int, kv_f16: bool = False) -> torch.Tensor:
     """mod.rs:493-533.  kv_f16 (not in the reference): the scaled keys and the values are rounded to fp16
-    at the point where the B200 path stores them in its fp16 K/V cache."""
+    at the point where the CUDA path stores them in its fp16 K/V cache."""
     n_batch, n_qctx, n_state = q.shape
     n_ctx = k.shape[1]
     scale = _f32((n_state / n_head) ** -0.25)

@@ -1,7 +1,7 @@
 """A/B of the decoder5.cu options on one GPU (model built once): python scripts/ab_decode5.py [model] [n_chunks] [depth]
 For each (kv, WB200_D5_SPLIT) combination: decode ms of a warm run, us per position, and whether the token ids equal those of the
 unsplit configuration of the same K/V dtype.  (The first version of this script also toggled an L2 prefetch of the cross K/V block
-and bulk-copy staging of the activation planes: both measured slower, profiles/r02_dec5_ab.txt, and were removed from the kernel.)"""
+and bulk-copy staging of the activation planes: both measured slower and were removed from the kernel.)"""
 import itertools, json, os, sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))

@@ -1,5 +1,5 @@
 """Opcode histogram of every compiled translation unit (cuobjdump -sass of whisper-burn_b200/build/*.o): which kernels
-really contain tcgen05 / TMA / TMEM instructions.  python scripts/sass_opcodes.py > profiles/r02_sass_opcodes.txt"""
+really contain wgmma / TMA / bulk-copy instructions.  python scripts/sass_opcodes.py"""
 import collections
 import re
 import subprocess
@@ -7,10 +7,10 @@ import sys
 from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
-KEY = ["UTCHMMA", "UTCQMMA", "UTCIMMA", "UTCBAR", "UTCATOMSWS", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "HMMA", "LDSM", "LDGSTS",
+KEY = ["HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "HMMA", "LDSM", "LDGSTS",
        "FFMA", "HFMA2", "MUFU", "UCGABAR_ARV", "BAR", "ATOMS", "RED", "LDG", "LDS", "STS", "SHFL"]
-print("# SASS opcode counts per translation unit (sm_100a), from cuobjdump -sass; tcgen05.mma = UTCHMMA, tcgen05.ld = LDTM,")
-print("# tcgen05.commit = UTCBAR, TMA tensor load = UTMALDG, 1-D bulk copy = UBLKCP, mbarrier = SYNCS, mma.sync = HMMA, ldmatrix = LDSM")
+print("# SASS opcode counts per translation unit (sm_90a), from cuobjdump -sass; wgmma.mma_async = HGMMA, wgmma fence / wait = WARPGROUP,")
+print("# TMA tensor load = UTMALDG, 1-D bulk copy = UBLKCP, mbarrier = SYNCS, mma.sync = HMMA, ldmatrix = LDSM")
 print(f"{'unit':16s} " + " ".join(f"{k:>8s}" for k in KEY))
 for obj in sorted((ROOT / "whisper-burn_b200" / "build").glob("*.o")):
     out = subprocess.run(["cuobjdump", "-sass", str(obj)], capture_output=True, text=True).stdout

@@ -25,10 +25,7 @@ if trace_file:
 sess.transcribe_windows(waves, sp, isp, 1, depth)
 print("decoder", sess.last_decoder())
 if trace_file:
-    raw = np.array([int(x) for x in open(trace_file).read().split()], dtype=np.uint64)
-    big = raw > np.uint64(1) << np.uint64(62)          # MMA-warp stamps are (time << 2 | kind): larger than any plain globaltimer value
-    np.save(trace_file + ".mma.npy", raw[big])
-    t = raw[~big].astype(np.int64)
+    t = np.array([int(x) for x in open(trace_file).read().split()], dtype=np.int64)
     d = np.diff(t)
     n_pos = 3 + depth
     # prefill positions have fewer stamps than logits positions: report the tail (logits positions)

@@ -46,7 +46,7 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 // V2: ticket (atom.acq_rel) + flag on another line written by the last arriver; the others poll the flag
 // V3: V0 with the counter polled by lane 0 of warp 0 while all OTHER warps skip the leading __syncthreads via a named barrier
 //     arrive (bar.arrive) -- only thread 0 waits for them (bar.sync count NT), nobody else blocks twice
-// V4: two-level: 148 CTAs arrive on one of 8 group counters (stride 128 B); the last of a group (ticket) arrives on the top
+// V4: two-level: one CTA per SM arrives on one of 8 group counters (stride 128 B); the last of a group (ticket) arrives on the top
 //     counter; everybody polls the top counter
 template <int V>
 __device__ __forceinline__ void gsync(unsigned int* bar, unsigned int& gen) {

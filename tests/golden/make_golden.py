@@ -2,8 +2,8 @@
 
 The reference (Rust + un-vendored burn/libtorch) cannot be built or run here and ships no test
 vectors ("parity unpinned", oracle/__init__.py), so these fixtures are outputs of the oracle
-restatement -- they pin the oracle against regressions and travel to the GPU box (which has no
-/root/reference and should not spend minutes re-deriving tiny.en sequences).
+restatement -- they pin the oracle against regressions and spare the GPU tests minutes of re-deriving
+tiny.en sequences on the CPU.
 Run from the repo root:  python tests/golden/make_golden.py
 """
 import json

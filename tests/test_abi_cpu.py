@@ -33,7 +33,7 @@ def test_header_symbols_exported():
     lib = ffi.lib()
     for name in declared:
         assert getattr(lib, name) is not None
-    assert b"sm_100a" in lib.wb_version()
+    assert b"sm_90a" in lib.wb_version()
 
 
 def test_max_waveform_samples_and_windows_match_oracle():

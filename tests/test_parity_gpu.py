@@ -327,7 +327,7 @@ def test_batched_tensor_core_decoder_unsplit_cross_attention():
 
 
 def test_batched_tensor_core_decoder_small_en_width():
-    """d = 768: decoder5.cu splits MLP2 (K = 4d) into 3 slabs of 1024 columns (one round of tiles on 148 CTAs)."""
+    """d = 768: decoder5.cu splits MLP2 (K = 4d) into 3 slabs of 1024 columns (fewer rounds of tiles than 4 slabs)."""
     dims, w_np, w_t = synth.make_weights("test-e", seed=0)
     sp = synth.special_tokens(dims)
     wh = model.Whisper(dims, w_np)

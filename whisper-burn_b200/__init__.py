@@ -1,4 +1,4 @@
-"""whisper-burn_b200: B200-native Whisper hot path behind whisper-burn's API surface.
+"""whisper-burn_b200: H100-native Whisper hot path behind whisper-burn's API surface.
 
 The product is ``libwhisper_b200.so`` (CUDA kernels + C++ host pipeline + C ABI, see
 ``include/whisper_b200.h``).  This Python package is only the test / bench harness side of the

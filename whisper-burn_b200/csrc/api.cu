@@ -139,7 +139,7 @@ FrontendOnly& frontend_for(int device) {
 
 extern "C" {
 
-const char* wb_version(void) { return "whisper_b200 0.1.0 (sm_100a)"; }
+const char* wb_version(void) { return "whisper_b200 0.1.0 (sm_90a)"; }
 const char* wb_last_error(void) { return wb::last_error_string().c_str(); }
 
 int wb_device_count(int* n_out) {

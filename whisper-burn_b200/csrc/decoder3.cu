@@ -1,4 +1,4 @@
-// Persistent cooperative decoder ("megakernel") for sm_100a.
+// Persistent cooperative decoder ("megakernel") for sm_90a.
 //
 // Reference math: TextDecoder::forward src/model/mod.rs:131-157, ResidualDecoderAttentionBlock::forward
 // :345-350, MultiHead{Self,Cross}Attention::forward :428-436 / :482-490, qkv_attention :493-533,

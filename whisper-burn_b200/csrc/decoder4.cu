@@ -1,4 +1,4 @@
-// Cluster / DSMEM persistent decoder for small batches (R <= 8 rows, d <= 512: tiny / base) on sm_100a.
+// Cluster / DSMEM persistent decoder for small batches (R <= 8 rows, d <= 512: tiny / base) on sm_90a.
 //
 // Same math and same single-launch structure as decoder3.cu (prefill + every greedy step in one kernel), but
 // the per-layer stage chain no longer crosses the chip: ONE 16-CTA thread-block cluster owns one batch row.
@@ -996,7 +996,7 @@ bool launch4_t(const Dec3Args& a, cudaStream_t st) {
             return false;
         }
         S.cooperative = getenv("WB200_NO_COOP") == nullptr;   // profilers cannot replay cooperative cluster launches
-        S.clusters = std::min(n_clusters, 8);   // every launched cluster must be co-resident (grid barriers); B200: 7 of size 16
+        S.clusters = std::min(n_clusters, 8);   // every launched cluster must be co-resident (grid barriers)
     }
     if (S.clusters < 0 || a.R > S.clusters) return false;
     cfg.gridDim = dim3(S.clusters * CS);

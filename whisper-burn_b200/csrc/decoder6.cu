@@ -3,7 +3,7 @@
 // Same math and single-launch structure as decoder3.cu (TextDecoder::forward src/model/mod.rs:131-157, blocks :345-350,
 // attention :428-533, MLP :376-382, search closure src/transcribe.rs:253-307; prefill + every greedy step in one kernel), but
 // the per-layer chain is cut from 8 cluster-wide stages (decoder4.cu) to THREE exchanges, and every linear layer runs on the
-// 5th-generation tensor cores:
+// tensor cores (Hopper warpgroup MMA):
 //
 //   one thread-block cluster of CS = H * HS CTAs owns one batch row; CTA (h, hs) owns attention head h.
 //   phase 1  x -> LN1 -> q_h | k_h | v_h (192 weight rows) -> causal self attention of head h -> the head's K-slice of the
@@ -17,16 +17,17 @@
 //   in a fixed order, identically in every CTA) and owns a full copy of the residual stream again.  No hardware cluster barrier
 //   inside the step, no cross-thread release/acquire chains: data and its "ready" signal travel together.
 //
-//   Linear layers = swap-AB tcgen05.mma (kind::f16, M = 128 weight rows, N = 16, K = 16): the weight slices of this CTA are
-//   pre-packed per (layer, CTA) as 128-row x 64-column slabs in the canonical K-major 128B-swizzled shared-memory image
-//   (dec6_pack_kernel), so a slab is ONE 16 KB bulk copy (TMA engine) into a ring slot and IS the A operand; the activation is
-//   the B operand: 16 rows of which row 0 = fp16(x) and row 1 = fp16((x - hi) * 2048) (the decoder5.cu split: exact products,
-//   fp32 accumulation), the rest zero.  The accumulator [128 lanes][16 columns] lives in TMEM (two of them, ping-pong); thread
-//   `row` of an epilogue warp group reads its lane with tcgen05.ld, combines hi + lo / 2048 and applies bias / scale / GELU.
-//   Weights do not depend on activations, so they never wait for the chain: a PRODUCER warp streams weight slabs and the cross
-//   K/V block through the ring (full / empty mbarriers), an MMA warp (one elected thread) issues the tensor-core instructions
-//   as slabs land and releases the slots with tcgen05.commit; the 8 consumer warps run the dependent chain: LayerNorm,
-//   attention (8 lanes per key), epilogues, the exchange.
+//   Linear layers = swap-AB wgmma.mma_async (m64n8k16, fp16 operands, fp32 accumulate; M = weight rows): the weight slices of
+//   this CTA are pre-packed per (layer, CTA) as 128-row x 64-column slabs in the canonical K-major 128B-swizzled shared-memory
+//   image (dec6_pack_kernel), so a slab is ONE 16 KB bulk copy (TMA engine) into a ring slot and IS the A operand of two
+//   m64 MMAs; the activation is the B operand: 8 rows of which row 0 = fp16(x) and row 1 = fp16((x - hi) * 2048) (the
+//   decoder5.cu split: exact products, fp32 accumulation), the rest zero.  The two consumer warpgroups take the 128-row output
+//   tiles in turn (ping-pong: one group's epilogue overlaps the other's MMAs); the accumulator lives in the registers of the
+//   group, columns 0 and 1 of a row in one thread, which combines hi + lo / 2048 after a shuffle that gives every lane one row
+//   and applies bias / scale / GELU.  Weights do not depend on activations, so they never wait for the chain: a PRODUCER warp
+//   streams weight slabs and the cross K/V block through the ring (full / empty mbarriers); the 8 consumer warps run the
+//   dependent chain: LayerNorm, the MMAs (releasing a slot when the MMAs that read it have completed), attention (8 lanes per
+//   key), epilogues, the exchange.
 //
 //   Only the vocabulary projection is chip-wide (as in decoder4.cu: bulk-copy ring of contiguous half-tiles of the tied
 //   embedding, mma.sync swap-AB with fp16 hi/lo activation planes, fused mask / online softmax / arg-max), behind ONE grid
@@ -41,6 +42,7 @@
 #include <mutex>
 
 #include "dec_common.cuh"
+#include "wgmma.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -49,15 +51,13 @@ namespace wb {
 namespace {
 
 constexpr int NCW = 8;                    // consumer warps (threads 0..255)
-constexpr int NPROD = 1;                  // producer warps (more than one issuing warp does not raise the stream rate: the tensor cores' shared-memory
-                                          // A-operand read, ~0.3 us per 16 KB slab, is what paces the ring; measured, profiles/r02_dec6_mma_trace.txt)
-constexpr int W_PROD = NCW, W_MMA = NCW + NPROD;
-constexpr int NTH6 = (NCW + NPROD + 1) * 32;      // + producer warps + MMA warp
+constexpr int NPROD = 1;                  // producer warps (each walks the whole schedule and issues every NPROD-th chunk)
+constexpr int W_PROD = NCW;
+constexpr int NTH6 = (NCW + NPROD) * 32;          // + producer warps
 constexpr int SLOT = 16384;               // bytes per ring slot = one 128-row x 64-column fp16 slab
 constexpr int NSLOT = 8;
 constexpr int LG_NBUF = 2;                // logits stage: ring slots per warp (aliases the weight ring)
-constexpr int BX_SLAB = 2048;             // B operand: 16 rows x 128 bytes per 64-column slab
-constexpr uint32_t TMEM_COLS = 32;        // two 16-column accumulators
+constexpr int BX_SLAB = 1024;             // B operand: 8 rows x 128 bytes (one swizzle atom) per 64-column slab
 
 template <int D, int HS>
 struct Geo {
@@ -110,62 +110,6 @@ __device__ __forceinline__ float group8_sum(float v) {   // sum over the 8 lanes
     v += __shfl_xor_sync(0xffffffffu, v, 2);
     v += __shfl_xor_sync(0xffffffffu, v, 4);
     return v;
-}
-// ---- tcgen05 (see gemm_f16.cu for the same descriptors in a GEMM) ------------------------------------------------------------
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(s32(bar)) : "memory");
-}
-// the MMA thread polls without reading the clock on every probe (a probe of a pending barrier suspends the thread for a while
-// in hardware, so 2^26 failed probes are many seconds): fail loudly instead of hanging the GPU
-__device__ __forceinline__ void mbar_wait_lean(uint64_t* bar, uint32_t parity) {
-    const uint32_t b = s32(bar);
-#pragma unroll 1
-    for (int i = 0; i < (1 << 26); ++i) {
-        uint32_t done;
-        asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}" : "=r"(done) : "r"(b), "r"(parity) : "memory");
-        if (done) return;
-    }
-    __trap();
-}
-__device__ __forceinline__ void umma_f16_first(uint32_t tmem_c, uint64_t desc_a, uint64_t desc_b, uint32_t idesc) {   // D = A * B
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, 0, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_c),
-        "l"(desc_a), "l"(desc_b), "r"(idesc)
-        : "memory");
-}
-__device__ __forceinline__ void umma_f16_acc(uint32_t tmem_c, uint64_t desc_a, uint64_t desc_b, uint32_t idesc) {     // D += A * B
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.eq.b32 p, 0, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_c),
-        "l"(desc_a), "l"(desc_b), "r"(idesc)
-        : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_c, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_c),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// K-major, SWIZZLE_128B operand tile (rows of 128 bytes, 8-row groups of 1024 bytes)
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);         // start address >> 4        bits [0,14)
-    d |= (uint64_t)1 << 16;                          // leading byte offset (unused for swizzled K-major) = 1
-    d |= (uint64_t)(1024 >> 4) << 32;                // stride byte offset: 8 rows * 128 B    bits [32,46)
-    d |= (uint64_t)1 << 46;                          // descriptor version 1 (sm_100)
-    d |= (uint64_t)2 << 61;                          // layout type SWIZZLE_128B
-    return d;
 }
 // byte offset of element (row, k) inside a K-major 128B-swizzled operand whose 64-column slabs are `slab_bytes` apart
 __device__ __host__ __forceinline__ uint32_t sw128_off(int row, int k, int slab_bytes) {
@@ -226,7 +170,7 @@ struct Softmax8 {   // online softmax state of one (warp, rg) key slot; o = the 
 // Segment [N][K] (fp16, source rows n0 + (r / piece) * piece_stride + r % piece, columns k0 .. k0 + K of a [.][ldk] matrix) as
 // tiles of 128 rows (a last tile of 64 rows when N % 128 == 64), each tile as K / 64 slabs of rows x 128 B in the K-major
 // 128B-swizzled shared-memory image: 16-byte unit (row r, chunk c) of a slab at r * 128 + ((c ^ (r & 7)) << 4).  A slab is what
-// one bulk copy moves and what one group of four tcgen05.mma (M = 128 or 64, K = 16 each) reads.
+// one bulk copy moves and what one group of four K steps of wgmma (two m64 row halves, or one for a 64-row tile) reads.
 struct PackSeg {
     const __half* src;
     int ldk, n0, k0, N, K;
@@ -277,14 +221,11 @@ __device__ __forceinline__ void bx_store(uint8_t* bx, int k, float v) {
 struct Pipe {        // shared-memory handles of the ring / tensor-core pipeline
     uint8_t* ring;   // [NSLOT][SLOT]
     uint64_t *full, *empty;      // per slot
-    uint64_t* b_ready;           // B operand written (consumers -> MMA warp)
-    uint64_t *acc_full, *acc_free;   // [2] accumulator ping-pong (MMA warp <-> epilogue warp groups)
-    uint32_t tmem;               // base of the 32 allocated TMEM columns
+    uint8_t* bx;     // [KMAX / 64][BX_SLAB] B operand
 };
 struct Counters {    // progress counters every role keeps in registers (identical sequences by construction)
     uint32_t n;      // ring chunks consumed / issued
     uint32_t tile;   // output tiles
-    uint32_t gemv;   // linear layers
 };
 
 enum { EM_PLAIN = 0, EM_QKV = 1, EM_CQ = 2, EM_HID = 3 };
@@ -297,34 +238,60 @@ struct GemvOut {
     KVT *kdst, *vdst;  // EM_QKV: this position's 64-element head slice of the self K / V cache
 };
 
-// Consumer side of one linear layer y[n] = sum_k W[n][k] x[k] (n < N, N padded to tiles of 128 rows): the B operand has been
-// written; hand it to the MMA warp, then the warp group (tile & 1) reads accumulator (tile & 1) -- TMEM lane = weight row --
-// and applies the epilogue.  Ends with a barrier of the consumer warps.
+// One linear layer y[n] = sum_k W[n][k] x[k] (n < N, N padded to tiles of 128 rows) by the consumer warps, the B operand
+// written: warpgroup (tile & 1) takes the tile -- its K slabs from the ring, one or two m64n8k16 MMAs per K step, the slot
+// released once the MMAs that read it have completed -- and applies the epilogue.  Ends with a barrier of the consumer warps.
 template <typename KVT>
 __device__ __noinline__ Counters gemv_epi6(const Pipe P, Counters c, int N, int n_slabs, const GemvOut<KVT> o) {
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes of the B operand -> tensor-core (async proxy) reads
     bar_consumers();
-    if (tid == 0) mbar_arrive(P.b_ready);
     const int n_tiles = (N + 127) >> 7;
+    const uint32_t ring0 = s32(P.ring), bx0 = s32(P.bx);
 #pragma unroll 1
     for (int t = 0; t < n_tiles; ++t) {
         const uint32_t T = c.tile + (uint32_t)t, g = T & 1;
         if ((uint32_t)(warp >> 2) != g) continue;
-        mbar_wait(P.acc_full + g, (T >> 1) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        uint32_t r0, r1;
-        const uint32_t taddr = P.tmem + ((uint32_t)((warp & 3) * 32) << 16) + g * 16;
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0, %1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(taddr) : "memory");
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(P.acc_free + g);                 // 4 warps: the accumulator may be overwritten
-        // M = 128: TMEM lane = tile row; M = 64 (last tile of a 192- / 64-row segment): the 64 rows sit in lanes 0..15 of each quadrant
-        const bool half_tile = N - t * 128 < 128;
-        const int row = t * 128 + (half_tile ? (warp & 3) * 16 + lane : (warp & 3) * 32 + lane);
+        const bool half_tile = N - t * 128 < 128;   // the last tile of a 192- / 64-row segment has 64 rows
+        float acc0[4] = {0.0f, 0.0f, 0.0f, 0.0f}, acc1[4] = {0.0f, 0.0f, 0.0f, 0.0f};   // rows 0..63 / 64..127 of the tile
+        wgmma_fence_regs(acc0);
+        wgmma_fence_regs(acc1);
+        uint32_t n = c.n + (uint32_t)(t * n_slabs);
+#pragma unroll 1
+        for (int s = 0; s < n_slabs; ++s, ++n) {
+            const uint32_t slot = n % NSLOT;
+            mbar_wait(P.full + slot, (n / NSLOT) & 1);
+            // rows 64..127 of a slab start 8 swizzle atoms (8192 bytes) in; K step = 32 bytes -> +2 in the (>> 4) address field.
+            // A 64-row slab leaves the second half of its slot stale: that MMA runs anyway (no branch between the MMAs, which
+            // would serialise them) and its rows are discarded.
+            const uint64_t da = wgmma_desc(ring0 + slot * SLOT), db = wgmma_desc(bx0 + s * BX_SLAB);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                wgmma_m64n8k16(acc0, da + 2 * k, db + 2 * k);
+                wgmma_m64n8k16(acc1, da + (8192 >> 4) + 2 * k, db + 2 * k);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();   // the previous slab's MMAs have completed: its slot may be overwritten
+            if (s > 0 && (tid & 127) == 0) mbar_arrive(P.empty + (n - 1) % NSLOT);
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc0);
+        wgmma_fence_regs(acc1);
+        if ((tid & 127) == 0) mbar_arrive(P.empty + (n - 1) % NSLOT);
+        // m64n8 fragment: lane 4i of warp w holds columns 0 (hi), 1 (lo) of rows 16 w + i (registers 0, 1) and 16 w + i + 8
+        // (registers 2, 3).  Lane L takes row 64 (L >> 4) + 16 w + 8 ((L >> 3) & 1) + (L & 7) of the tile from lane 4 (L & 7).
+        const int src = (lane & 7) * 4, sel = lane >> 3;
+        float hv[4], lv[4];
+        hv[0] = __shfl_sync(0xffffffffu, acc0[0], src); lv[0] = __shfl_sync(0xffffffffu, acc0[1], src);
+        hv[1] = __shfl_sync(0xffffffffu, acc0[2], src); lv[1] = __shfl_sync(0xffffffffu, acc0[3], src);
+        hv[2] = __shfl_sync(0xffffffffu, acc1[0], src); lv[2] = __shfl_sync(0xffffffffu, acc1[1], src);
+        hv[3] = __shfl_sync(0xffffffffu, acc1[2], src); lv[3] = __shfl_sync(0xffffffffu, acc1[3], src);
+        const float hi = sel == 0 ? hv[0] : sel == 1 ? hv[1] : sel == 2 ? hv[2] : hv[3];
+        const float lo = sel == 0 ? lv[0] : sel == 1 ? lv[1] : sel == 2 ? lv[2] : lv[3];
+        const int row = t * 128 + 64 * (lane >> 4) + 16 * (warp & 3) + 8 * ((lane >> 3) & 1) + (lane & 7);
         if (row < N && (!half_tile || lane < 16)) {
-            const float s = fmaf(__uint_as_float(r1), 1.0f / 2048.0f, __uint_as_float(r0));
+            const float s = fmaf(lo, 1.0f / 2048.0f, hi);
             if (o.mode == EM_PLAIN) {
                 o.out[row] = s;
             } else if (o.mode == EM_QKV) {       // mod.rs:429-431; q and k carry (d/H)^-0.25 each (:500-503)
@@ -345,45 +312,7 @@ __device__ __noinline__ Counters gemv_epi6(const Pipe P, Counters c, int N, int 
     }
     c.tile += (uint32_t)n_tiles;
     c.n += (uint32_t)(n_tiles * n_slabs);
-    c.gemv += 1;
     bar_consumers();
-    return c;
-}
-
-// MMA warp (one thread): the tensor-core side of the same linear layer
-__device__ __forceinline__ Counters gemv_mma6(const Pipe P, Counters c, int N, int n_slabs, uint32_t bx_addr, unsigned long long* tr, int& tn, int tcap) {
-    // instruction descriptor: D = F32 (1 << 4), A = B = F16 (format 0), K-major both, N >> 3 = 2 at bit 17, M >> 4 at bit 24
-    const int n_tiles = (N + 127) >> 7;
-    const uint64_t desc_ring0 = make_smem_desc(s32(P.ring)), desc_bx0 = make_smem_desc(bx_addr);
-    mbar_wait_lean(P.b_ready, c.gemv & 1);
-    if (tr && tn < tcap) tr[tn++] = (gtime() << 2) | 1ull;   // debug trace: B operand ready
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-    for (int t = 0; t < n_tiles; ++t) {
-        const uint32_t T = c.tile, g = T & 1, u = T >> 1;
-        const uint32_t idesc = (1u << 4) | (2u << 17) | ((uint32_t)(min(128, N - t * 128) >> 4) << 24);
-        if (u >= 1) mbar_wait_lean(P.acc_free + g, (u - 1) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-        for (int s = 0; s < n_slabs; ++s) {
-            const uint32_t slot = c.n % NSLOT;
-            mbar_wait_lean(P.full + slot, (c.n / NSLOT) & 1);
-            if (tr && tn < tcap) tr[tn++] = (gtime() << 2) | 2ull;   // debug trace: slab landed
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            // descriptors: ring slots are SLOT apart, B slabs BX_SLAB apart (address field = bytes >> 4)
-            const uint64_t da = desc_ring0 + (uint64_t)(slot * (SLOT >> 4)), db = desc_bx0 + (uint64_t)(s * (BX_SLAB >> 4));
-            const uint32_t acc = P.tmem + g * 16;
-            if (s == 0) umma_f16_first(acc, da, db, idesc); else umma_f16_acc(acc, da, db, idesc);
-            umma_f16_acc(acc, da + 2, db + 2, idesc);   // UMMA_K = 16 halves = 32 bytes -> +2 in the (>> 4) address field
-            umma_f16_acc(acc, da + 4, db + 4, idesc);
-            umma_f16_acc(acc, da + 6, db + 6, idesc);
-            umma_commit(P.empty + slot);   // the slab may be overwritten when these MMAs have read it
-            ++c.n;
-        }
-        umma_commit(P.acc_full + g);       // accumulator complete
-        ++c.tile;
-    }
-    ++c.gemv;
     return c;
 }
 
@@ -515,7 +444,7 @@ __device__ __noinline__ void self_attn6(const float* qkv_s, const KVT* kbase, co
 
 // cross attention of one head over keys [k_begin, k_end) of the window (mod.rs:482-490), the head-major K/V block arriving through
 // the ring in chunks of KPC keys; 8 lanes per key.  A slot is released by the LAST of the 8 warps to finish with it (the slots'
-// empty barriers take one arrival, as tcgen05.commit gives them for weight slabs).  (Waiting for several chunks at once to batch
+// empty barriers take one arrival, as the MMA warpgroup gives them for weight slabs).  (Waiting for several chunks at once to batch
 // the per-key latency chains was measured SLOWER, 6 -> 12 us per layer: the chunks arrive one per ~0.3 us and the batch waits for
 // the last one.)  Returns the ring counter.
 template <typename KVT>
@@ -585,7 +514,7 @@ dec6_kernel(const Dec3Args a) {
 
     // ---- shared memory carve-up (ring and B operand 1024-byte aligned: swizzle atoms)
     uint8_t* ring_mem = smraw;                                              // [NSLOT][SLOT]
-    uint8_t* bx = ring_mem + NSLOT * SLOT;                                  // [KMAX / 64][16 rows][128 B]  B operand (rows 0, 1 live)
+    uint8_t* bx = ring_mem + NSLOT * SLOT;                                  // [KMAX / 64][8 rows][128 B]  B operand (rows 0, 1 live)
     float* params = reinterpret_cast<float*>(bx + (G::KMAX / 64) * BX_SLAB);   // [2][PARAMS]
     float* part = params + 2 * PARAMS;                                      // [2][CS][SEND] partial records of the cluster
     float* y_s = part + 2 * CS * SEND;                                      // [2][SEND]     this CTA's outgoing record
@@ -597,7 +526,7 @@ dec6_kernel(const Dec3Args a) {
     float* wm = wsrc_s + 16;                                                // [8]
     float* wl = wm + 8;                                                     // [8]
     float* wo = wl + 8;                                                     // [8][64]
-    int* ctl = reinterpret_cast<int*>(wo + 512);                            // [4] stop flag, is_last, tmem base
+    int* ctl = reinterpret_cast<int*>(wo + 512);                            // [4] stop flag, is_last
     int* slot_cnt = ctl + 4;                                                // [NSLOT] warps done with a K/V chunk
     uint64_t* bars = reinterpret_cast<uint64_t*>(slot_cnt + NSLOT);
     uint64_t* full = bars;                    // [NSLOT]
@@ -605,10 +534,7 @@ dec6_kernel(const Dec3Args a) {
     uint64_t* pfull = empty + NSLOT;          // [2] parameter block landed
     uint64_t* pfree = pfull + 2;              // [2] consumers are done with the parameter block
     uint64_t* pbar = pfree + 2;               // [2] partial records of a phase landed
-    uint64_t* b_ready = pbar + 2;             // [1]
-    uint64_t* acc_full = b_ready + 1;         // [2]
-    uint64_t* acc_free = acc_full + 2;        // [2]
-    uint64_t* lg_bar = acc_free + 2;          // [NCW][LG_NBUF] logits stage
+    uint64_t* lg_bar = pbar + 2;              // [NCW][LG_NBUF] logits stage
     // logits-stage scratch aliases the (then dead) parameter / partial buffers
     uint4* pl_hi = reinterpret_cast<uint4*>(params);                        // [NT8][D/32][32] fp16 hi plane of the LayerNorm rows, fragment order
     uint4* pl_lo = pl_hi + NT8 * (D / 32) * 32;
@@ -616,29 +542,21 @@ dec6_kernel(const Dec3Args a) {
 
     if (tid == 0) {
         for (int i = 0; i < NSLOT; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, 1); slot_cnt[i] = 0; }
-        for (int i = 0; i < 2; ++i) { mbar_init(pfull + i, 1); mbar_init(pfree + i, NCW); mbar_init(pbar + i, 1); mbar_init(acc_full + i, 1); mbar_init(acc_free + i, 4); }
-        mbar_init(b_ready, 1);
+        for (int i = 0; i < 2; ++i) { mbar_init(pfull + i, 1); mbar_init(pfree + i, NCW); mbar_init(pbar + i, 1); }
         for (int i = 0; i < NCW * LG_NBUF; ++i) mbar_init(lg_bar + i, 1);
         ctl[0] = 0; ctl[1] = 0;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    for (int i = tid; i < (G::KMAX / 64) * BX_SLAB / 16; i += NTH6) reinterpret_cast<uint4*>(bx)[i] = make_uint4(0, 0, 0, 0);   // rows 2..15 stay zero
-    if (warp == W_MMA) {   // TMEM: two 16-column fp32 accumulators
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s32(ctl + 2)), "n"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    cl.sync();   // every CTA's mbarriers exist before any peer signals them; TMEM address published
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    for (int i = tid; i < (G::KMAX / 64) * BX_SLAB / 16; i += NTH6) reinterpret_cast<uint4*>(bx)[i] = make_uint4(0, 0, 0, 0);   // rows 2..7 stay zero
+    cl.sync();   // every CTA's mbarriers exist before any peer signals them
     Pipe P;
-    P.ring = ring_mem; P.full = full; P.empty = empty; P.b_ready = b_ready; P.acc_full = acc_full; P.acc_free = acc_free;
-    P.tmem = *reinterpret_cast<volatile uint32_t*>(ctl + 2);
+    P.ring = ring_mem; P.full = full; P.empty = empty; P.bx = bx;
 
     const uint8_t* pack = reinterpret_cast<const uint8_t*>(a.d6_pack);
     const float* gparams = a.d6_params;
     constexpr int S_D = D / 64, S_NS = NS / 64;   // K slabs of a linear layer
 
-    if (warp >= W_PROD && warp < W_MMA) {
+    if (warp >= W_PROD) {
         // ===================================================== PRODUCERS: weight slabs, parameters and cross K/V, in consumer order;
         // producer warp pw issues chunks n with n % NPROD == pw (every producer walks the whole schedule)
         const uint32_t pw = (uint32_t)(warp - W_PROD);
@@ -691,37 +609,9 @@ dec6_kernel(const Dec3Args a) {
             bar_all();   // the ring is lent to the logits stage until the consumers finish the step
             if (*reinterpret_cast<volatile int*>(ctl) != 0) break;
         }
-    } else if (warp == W_MMA) {
-        // ===================================================== MMA warp: one thread issues every tcgen05.mma of the step
-        Counters c{0, 0, 0};
-        const uint32_t bxa = s32(bx);
-        unsigned long long* mtr = (a.trace && blockIdx.x == 0) ? a.trace + a.trace_cap / 2 : nullptr;   // second half of the trace buffer
-        int mtn = 0;
-        const int mcap = a.trace_cap / 2;
-        for (int step = 0; step < a.n_steps; ++step) {
-            if (lane == 0) {
-                for (int row = cluster_id; row < R; row += n_clusters) {
-                    const int w = __ldg(a.row_window + row);
-                    const int T = __ldg(a.win_T + w);
-                    const int per = (T + HS - 1) / HS, k_begin = min(T, hs * per), k_end = min(T, k_begin + per);
-                    const uint32_t n_kv = (uint32_t)((k_end - k_begin + KPC - 1) / KPC);
-                    for (int l = 0; l < L; ++l) {
-                        if (hs == 0) { c = gemv_mma6(P, c, 192, S_D, bxa, mtr, mtn, mcap); c = gemv_mma6(P, c, D, 1, bxa, mtr, mtn, mcap); }
-                        c = gemv_mma6(P, c, 64, S_D, bxa, mtr, mtn, mcap);
-                        c.n += n_kv;                       // K/V chunks are consumed by the attention warps
-                        c = gemv_mma6(P, c, D, 1, bxa, mtr, mtn, mcap);
-                        c = gemv_mma6(P, c, NS, S_D, bxa, mtr, mtn, mcap);
-                        c = gemv_mma6(P, c, D, S_NS, bxa, mtr, mtn, mcap);
-                    }
-                }
-            }
-            __syncwarp();
-            bar_all();
-            if (*reinterpret_cast<volatile int*>(ctl) != 0) break;
-        }
     } else {
         // ===================================================== CONSUMERS
-        Counters c{0, 0, 0};
+        Counters c{0, 0};
         uint32_t pl = 0;     // parameter blocks consumed
         uint32_t ph = 0;     // exchange phases completed (buffer = ph & 1)
         unsigned int gen = 0;
@@ -1122,12 +1012,7 @@ dec6_kernel(const Dec3Args a) {
             }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     cl.sync();   // no CTA leaves while a peer may still address its shared memory
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(P.tmem), "n"(TMEM_COLS) : "memory");
-    }
 }
 
 template <int D, int HS, int NT8>
@@ -1135,7 +1020,7 @@ constexpr size_t dec6_smem() {
     using G = Geo<D, HS>;
     return 1024 + (size_t)NSLOT * SLOT + (size_t)(G::KMAX / 64) * BX_SLAB +
            sizeof(float) * ((size_t)2 * G::PARAMS + 2 * G::CS * G::SEND + 2 * G::SEND + D + 192 + 64 + G::NS + 16 + 8 + 8 + 512 + 4 + NSLOT) +
-           8 * (size_t)(2 * NSLOT + 6 + 5 + NCW * LG_NBUF) + 64;
+           8 * (size_t)(2 * NSLOT + 6 + NCW * LG_NBUF) + 64;
 }
 
 struct LaunchState {

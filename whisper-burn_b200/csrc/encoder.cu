@@ -302,7 +302,7 @@ __global__ void ckv_relayout_kernel(const float* __restrict__ src, OT* __restric
 void launch_ckv_relayout(const float* src, void* dst, bool dst_half, const int64_t* win_row_off, const int* win_T, int n_windows,
                          int64_t M, int d, cudaStream_t st) {
     const int64_t n4 = M * (2 * d / 4);
-    const int blocks = (int)std::min<int64_t>((n4 + 255) / 256, 148 * 16);
+    const int blocks = (int)std::min<int64_t>((n4 + 255) / 256, 132 * 16);
     if (dst_half) ckv_relayout_kernel<__half><<<blocks, 256, 0, st>>>(src, reinterpret_cast<__half*>(dst), win_row_off, win_T, n_windows, M, d);
     else ckv_relayout_kernel<float><<<blocks, 256, 0, st>>>(src, reinterpret_cast<float*>(dst), win_row_off, win_T, n_windows, M, d);
     WB_LAUNCH_CHECK();

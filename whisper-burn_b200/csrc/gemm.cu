@@ -8,7 +8,7 @@
 // v1 data path: 128x64x16 tiles, 256 threads, 8x4 register tile per thread, operands staged
 // transposed in shared memory (k-major) so the inner loop reads two float4 of A and one of B per
 // 32 FMAs.  fp32 CUDA-core FMA keeps the reference's f32 numerics exactly (up to summation order);
-// the tensor-core (tcgen05, split-TF32) path replaces this kernel for the large GEMMs.
+// the tensor-core path (gemm_f16.cu, wgmma over fp16 hi/lo planes) replaces this kernel for the large GEMMs.
 #include "wb_internal.h"
 
 namespace wb {

@@ -1,4 +1,4 @@
-// Tensor-core GEMM of the encoder: tcgen05.mma kind::f16 fed by TMA, two fp32 accumulators in TMEM.
+// Tensor-core GEMM of the encoder: Hopper wgmma (fp16 operands, fp32 accumulate) fed by TMA through an mbarrier ring.
 // (reference ops: burn nn::Linear / Conv1d at src/model/mod.rs:243-244, :376-382, :429-435, :484-485)
 //
 //   C[g][m][n] = epi( sum_k A[g][m][k] * B[n][k] )      same contract and epilogues as gemm.cu
@@ -8,17 +8,18 @@
 // are stored in fp16), so B is EXACT in fp16; the fp32 activations travel between the encoder kernels as a PAIR of fp16 planes
 //     A = A_hi + A_lo / 2048,   A_hi = fp16(A),  A_lo = fp16((A - A_hi) * 2048)        (22 mantissa bits, decoder5.cu's split)
 // written by the producing kernel (LayerNorm, attention, the GELU epilogue below).  Every product A_hi*B, A_lo*B is exact in the
-// fp32 accumulator; the two planes accumulate into TWO TMEM accumulators (hi at column 0, lo at column BN) that the epilogue
-// combines as hi + lo / 2048.  Against the TF32 hi/lo formulation this kernel replaces: half the bytes per k-block through
-// shared memory, the weight tile loaded once instead of twice, and twice the MMA rate.
+// fp32 accumulator; the two planes accumulate into TWO register accumulators that the epilogue combines as hi + lo / 2048.
+// Against a TF32 hi/lo formulation: half the bytes per k-block through shared memory, the weight tile loaded once instead of
+// twice, and twice the MMA rate.
 //
-// Kernel shape (one 128 x BN output tile per CTA, 192 threads):
-//   warp 0      TMA producer: cp.async.bulk.tensor (3-D maps: k, row, window) of A_hi, A_lo (128 x 64 halves each) and B
-//               (BN x 64) into a 2-stage 128B-swizzled ring, mbarrier expect_tx / complete_tx (two CTAs per SM: four stages in flight)
-//   warp 1      TMEM allocation (2 * BN columns) + single-thread tcgen05.mma issue (UMMA 128 x BN x 16, 4 + 4 per k-block),
-//               tcgen05.commit releases ring slots and finally signals the epilogue
-//   warps 2-5   epilogue: tcgen05.ld (32 lanes x 16 columns, both accumulators) -> bias / GELU / q,k scale / pos-emb /
-//               residual -> fp32 rows and / or fp16 hi/lo planes for the next kernel
+// Kernel shape (one 128 x BN output tile per CTA, 288 threads, one CTA per SM):
+//   warps 0-7   two consumer warpgroups; warpgroup w owns rows [64 w, 64 w + 64) of the tile: per k-block 4 + 4
+//               wgmma.m64nBNk16 (hi and lo planes against the same B tile), one k-block kept in flight, then the epilogue
+//               straight from the accumulator registers -> bias / GELU / q,k scale / pos-emb / residual -> fp32 rows and / or
+//               fp16 hi/lo planes for the next kernel
+//   warp 8      TMA producer: cp.async.bulk.tensor (3-D maps: k, row, window) of A_hi, A_lo (128 x 64 halves each) and B
+//               (BN x 64) into a 4-stage 128B-swizzled ring, mbarrier expect_tx / complete_tx; a slot is released when both
+//               warpgroups' MMAs that read it have completed
 // The conv stems use the same kernel: their A rows are overlapping windows of a token-major buffer, expressed as a tensor map
 // whose row stride is smaller than the row length.
 #include <cuda.h>
@@ -28,20 +29,23 @@
 #include <mutex>
 
 #include "wb_internal.h"
+#include "wgmma.cuh"
 
 namespace wb {
 
 namespace {
 
-constexpr int F_BM = 128, F_BK = 64, F_STAGES = 2;   // 2 stages x 48 KB: TWO CTAs per SM (2 x 256 TMEM columns), so one tile's epilogue
-                                                     // (TMEM -> registers -> GELU -> global) overlaps the other's TMA / MMA main loop
-constexpr int F_THREADS = 192;
+constexpr int F_BM = 128, F_BK = 64, F_STAGES = 4;   // 4 stages x 48 KB (BN = 128): the accumulators of a 128 x 128 tile take
+                                                     // 128 registers per consumer thread, so one CTA per SM and a deeper ring
+constexpr int F_CONSUMERS = 256;                     // two warpgroups
+constexpr int F_THREADS = F_CONSUMERS + 32;          // + the TMA producer warp
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count)); }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory"); }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     uint32_t done = 0;
     while (!done)
@@ -57,29 +61,10 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, u
                  "r"(smem_u32(bar)), "r"(c0), "r"(c1)
                  : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], kind::f16 (fp16 operands, fp32 accumulate), single CTA
-__device__ __forceinline__ void umma_f16(uint32_t tmem_c, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_c),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// K-major, SWIZZLE_128B operand tile (rows of 128 bytes, 8-row groups of 1024 bytes)
-__device__ __forceinline__ uint64_t make_smem_desc(const void* p) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_u32(p) & 0x3FFFF) >> 4);   // start address >> 4        bits [0,14)
-    d |= (uint64_t)1 << 16;                          // leading byte offset (unused for swizzled K-major) = 1
-    d |= (uint64_t)(1024 >> 4) << 32;                // stride byte offset: 8 rows * 128 B    bits [32,46)
-    d |= (uint64_t)1 << 46;                          // descriptor version 1 (sm_100)
-    d |= (uint64_t)2 << 61;                          // layout type SWIZZLE_128B
-    return d;
+template <int BN>
+__device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t desc_a, uint64_t desc_b) {
+    if constexpr (BN == 128) wgmma_m64n128k16(d, desc_a, desc_b);
+    else wgmma_m64n64k16(d, desc_a, desc_b);
 }
 __device__ __forceinline__ float gelu_erf(float x) {
     const float t = __fadd_rn(erff(__fdiv_rn(x, 1.41421356237309504880f)), 1.0f);
@@ -107,7 +92,7 @@ struct F16Args {
 };
 
 template <int BN>
-__global__ void __launch_bounds__(F_THREADS, 2)
+__global__ void __launch_bounds__(F_THREADS, 1)
 gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                    const __grid_constant__ CUtensorMap map_b, const F16Args g) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -117,8 +102,6 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_co
     uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint64_t* full = reinterpret_cast<uint64_t*>(base + F_STAGES * STAGE);
     uint64_t* empty = full + F_STAGES;
-    uint64_t* tmem_full = empty + F_STAGES;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const GemmGroup grp = g.groups ? g.groups[blockIdx.z] : g.single;
@@ -127,27 +110,19 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_co
     const int n0 = blockIdx.x * BN;
     const int nkb = (g.K + F_BK - 1) / F_BK;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == F_CONSUMERS) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a_lo) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
         for (int s = 0; s < F_STAGES; ++s) {
             mbar_init(full + s, 1);
-            mbar_init(empty + s, 1);
+            mbar_init(empty + s, 2);   // one arrival per consumer warpgroup
         }
-        mbar_init(tmem_full, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {   // TMEM: 2 * BN fp32 accumulator columns (power of two >= 32)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "n"(2 * BN) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_c = *tmem_ptr;
 
-    if (warp == 0) {
+    if (threadIdx.x >= F_CONSUMERS) {
         if (lane == 0) {
             // ===== TMA producer
             for (int i = 0; i < nkb; ++i) {
@@ -161,95 +136,71 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_co
                 tma_load_2d(st + 2 * A_BYTES, &map_b, full + s, i * F_BK, n0);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ===== MMA issuer (one thread)
-            // instruction descriptor: D = F32 (1 << 4), A = B = F16 (format 0), K-major both, N >> 3 at bit 17, M >> 4 at bit 24
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(F_BM >> 4) << 24);
-            for (int i = 0; i < nkb; ++i) {
-                const int s = i % F_STAGES;
-                const uint32_t ph = (i / F_STAGES) & 1;
-                mbar_wait(full + s, ph);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                uint8_t* st = base + s * STAGE;
-                const uint64_t dah = make_smem_desc(st), dal = make_smem_desc(st + A_BYTES), db = make_smem_desc(st + 2 * A_BYTES);
-#pragma unroll
-                for (int k = 0; k < F_BK / 16; ++k) {   // UMMA_K = 16 halves = 32 bytes -> +2 in the (>>4) address field
-                    umma_f16(tmem_c, dah + 2 * k, db + 2 * k, idesc, (i | k) != 0 ? 1u : 0u);
-                    umma_f16(tmem_c + BN, dal + 2 * k, db + 2 * k, idesc, (i | k) != 0 ? 1u : 0u);
-                }
-                umma_commit(empty + s);   // frees the ring slot when these MMAs have read it
-            }
-            umma_commit(tmem_full);       // accumulators complete
-        }
-    } else {
-        // ===== epilogue warps 2..5: TMEM lane quarter = warp % 4
-        const int q = warp & 3;
-        const int m = m0 + q * 32 + lane;
-        mbar_wait(tmem_full, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const bool row_ok = m < grp.rows;
-        const int64_t crow = grp.c_off + (int64_t)m * g.ldc;
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 16) {
-            uint32_t rh[16], rl[16];
-            const uint32_t taddr = tmem_c + ((uint32_t)(q * 32) << 16) + (uint32_t)c0;
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                : "=r"(rh[0]), "=r"(rh[1]), "=r"(rh[2]), "=r"(rh[3]), "=r"(rh[4]), "=r"(rh[5]), "=r"(rh[6]), "=r"(rh[7]), "=r"(rh[8]),
-                  "=r"(rh[9]), "=r"(rh[10]), "=r"(rh[11]), "=r"(rh[12]), "=r"(rh[13]), "=r"(rh[14]), "=r"(rh[15])
-                : "r"(taddr)
-                : "memory");
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                : "=r"(rl[0]), "=r"(rl[1]), "=r"(rl[2]), "=r"(rl[3]), "=r"(rl[4]), "=r"(rl[5]), "=r"(rl[6]), "=r"(rl[7]), "=r"(rl[8]),
-                  "=r"(rl[9]), "=r"(rl[10]), "=r"(rl[11]), "=r"(rl[12]), "=r"(rl[13]), "=r"(rl[14]), "=r"(rl[15])
-                : "r"(taddr + (uint32_t)BN)
-                : "memory");
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            if (row_ok) {
-#pragma unroll
-                for (int j4 = 0; j4 < 16; j4 += 4) {
-                    const int n = n0 + c0 + j4;
-                    float v[4];
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        float t = fmaf(__uint_as_float(rl[j4 + j]), 1.0f / 2048.0f, __uint_as_float(rh[j4 + j]));
-                        if (g.bias) t = __fadd_rn(t, __ldg(g.bias + n + j));
-                        if (g.act == ACT_GELU) t = gelu_erf(t);
-                        if (n + j < g.scale_cols) t = __fmul_rn(t, g.scale);
-                        v[j] = t;
-                    }
-                    if (g.pos) {
-                        const float4 p4 = __ldg(reinterpret_cast<const float4*>(g.pos + (int64_t)m * g.N + n));
-                        v[0] = __fadd_rn(v[0], p4.x); v[1] = __fadd_rn(v[1], p4.y);
-                        v[2] = __fadd_rn(v[2], p4.z); v[3] = __fadd_rn(v[3], p4.w);
-                    }
-                    if (g.residual) {
-                        const float4 r4 = *reinterpret_cast<const float4*>(g.residual + crow + n);
-                        v[0] = __fadd_rn(r4.x, v[0]); v[1] = __fadd_rn(r4.y, v[1]);
-                        v[2] = __fadd_rn(r4.z, v[2]); v[3] = __fadd_rn(r4.w, v[3]);
-                    }
-                    if (g.C) *reinterpret_cast<float4*>(g.C + crow + n) = make_float4(v[0], v[1], v[2], v[3]);
-                    if (g.P_hi) {
-                        __half2 h0, l0, h1, l1;
-                        split_pair(v[0], v[1], h0, l0);
-                        split_pair(v[2], v[3], h1, l1);
-                        uint2 uh, ul;
-                        uh.x = *reinterpret_cast<uint32_t*>(&h0); uh.y = *reinterpret_cast<uint32_t*>(&h1);
-                        ul.x = *reinterpret_cast<uint32_t*>(&l0); ul.y = *reinterpret_cast<uint32_t*>(&l1);
-                        *reinterpret_cast<uint2*>(g.P_hi + crow + n) = uh;
-                        *reinterpret_cast<uint2*>(g.P_lo + crow + n) = ul;
-                    }
-                }
-            }
-        }
+        return;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_c), "n"(2 * BN) : "memory");
+    // ===== consumer warpgroup wg: rows [64 wg, 64 wg + 64) of the tile
+    const int wg = warp >> 2;
+    float acc_h[BN / 2], acc_l[BN / 2];
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) { acc_h[j] = 0.0f; acc_l[j] = 0.0f; }
+    wgmma_fence_regs(acc_h);
+    wgmma_fence_regs(acc_l);
+#pragma unroll 1
+    for (int i = 0; i < nkb; ++i) {
+        const int s = i % F_STAGES;
+        mbar_wait(full + s, (i / F_STAGES) & 1);
+        const uint32_t st = smem_u32(base + s * STAGE);
+        // a warpgroup's 64 rows are 8 swizzle atoms of 1024 bytes into the 128-row A tiles
+        const uint64_t dah = wgmma_desc(st + wg * 8192), dal = wgmma_desc(st + A_BYTES + wg * 8192), db = wgmma_desc(st + 2 * A_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < F_BK / 16; ++k) {   // K step = 16 halves = 32 bytes -> +2 in the (>> 4) address field
+            wgmma_tile<BN>(acc_h, dah + 2 * k, db + 2 * k);
+            wgmma_tile<BN>(acc_l, dal + 2 * k, db + 2 * k);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous k-block's MMAs have read their stage
+        if (i > 0 && (threadIdx.x & 127) == 0) mbar_arrive(empty + (i - 1) % F_STAGES);
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc_h);
+    wgmma_fence_regs(acc_l);
+
+    // ===== epilogue.  Accumulator fragment of a m64nBN wgmma: register 4j + e of thread (warp w, lane) holds row
+    // 16 w + lane / 4 (+ 8 for e >= 2), column 8 j + 2 (lane % 4) + (e & 1).
+#pragma unroll
+    for (int hrow = 0; hrow < 2; ++hrow) {
+        const int m = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * hrow;
+        if (m >= grp.rows) continue;
+        const int64_t crow = grp.c_off + (int64_t)m * g.ldc;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+            const int n = n0 + 8 * j + 2 * (lane & 3);
+            float v[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                float t = fmaf(acc_l[4 * j + 2 * hrow + e], 1.0f / 2048.0f, acc_h[4 * j + 2 * hrow + e]);
+                if (g.bias) t = __fadd_rn(t, __ldg(g.bias + n + e));
+                if (g.act == ACT_GELU) t = gelu_erf(t);
+                if (n + e < g.scale_cols) t = __fmul_rn(t, g.scale);
+                v[e] = t;
+            }
+            if (g.pos) {
+                const float2 p2 = __ldg(reinterpret_cast<const float2*>(g.pos + (int64_t)m * g.N + n));
+                v[0] = __fadd_rn(v[0], p2.x); v[1] = __fadd_rn(v[1], p2.y);
+            }
+            if (g.residual) {
+                const float2 r2 = *reinterpret_cast<const float2*>(g.residual + crow + n);
+                v[0] = __fadd_rn(r2.x, v[0]); v[1] = __fadd_rn(r2.y, v[1]);
+            }
+            if (g.C) *reinterpret_cast<float2*>(g.C + crow + n) = make_float2(v[0], v[1]);
+            if (g.P_hi) {
+                __half2 h, l;
+                split_pair(v[0], v[1], h, l);
+                *reinterpret_cast<__half2*>(g.P_hi + crow + n) = h;
+                *reinterpret_cast<__half2*>(g.P_lo + crow + n) = l;
+            }
+        }
     }
 }
 
@@ -301,7 +252,7 @@ CUtensorMap make_map(const __half* base, uint64_t dim0, uint64_t dim1, uint64_t 
 
 template <int BN>
 void launch_f16_t(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b, const F16Args& a, dim3 grid, cudaStream_t st) {
-    constexpr size_t smem = 1024 + (size_t)F_STAGES * (2 * F_BM * F_BK * 2 + BN * F_BK * 2) + 256;
+    constexpr size_t smem = 1024 + (size_t)F_STAGES * (2 * F_BM * F_BK * 2 + BN * F_BK * 2) + 2 * F_STAGES * sizeof(uint64_t);
     static std::mutex mu;
     static bool configured[16] = {};   // per device ordinal
     int dev = 0;
@@ -323,7 +274,7 @@ void launch_split_f16(const float* src, __half* hi, __half* lo, int64_t n, cudaS
     WB_REQUIRE(n % 4 == 0, "split: length must be a multiple of 4");
     const int64_t n4 = n / 4;
     if (n4 == 0) return;
-    const int blocks = (int)std::min<int64_t>((n4 + 255) / 256, 148 * 8);
+    const int blocks = (int)std::min<int64_t>((n4 + 255) / 256, 132 * 8);
     split_f16_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const float4*>(src), reinterpret_cast<uint2*>(hi), reinterpret_cast<uint2*>(lo), n4);
     WB_LAUNCH_CHECK();
 }

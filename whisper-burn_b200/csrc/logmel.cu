@@ -1,4 +1,4 @@
-// Fused log-mel frontend for sm_100a  (reference: src/audio.rs:34-56 prep_audio, :284-367 stfft).
+// Fused log-mel frontend for sm_90a  (reference: src/audio.rs:34-56 prep_audio, :284-367 stfft).
 //
 // One CTA turns 32 STFT frames of one window into 32 token-major rows of 80 log-mel values:
 //   reflect-pad + framing (audio.rs:296-346)  -> staged once in shared memory (hop-row layout,

@@ -103,7 +103,7 @@ Session::Session(Model* model, int64_t max_w, int64_t max_b, int64_t max_text_le
                 auto ln = [&](Dec5Desc& q, const LayerNormW& w, int stage) {
                     q.kind = D5_KIND_LN; q.g = w.g; q.b = w.b; q.eps = w.eps; q.stage = stage; q.ks = d;
                 };
-                // The d x d projections (out, cross query, cross out) have only d/16 feature tiles -- 48 of 148 CTAs busy for small.en, each
+                // The d x d projections (out, cross query, cross out) have only d/16 feature tiles -- 48 of 132 CTAs busy for small.en, each
                 // staging all K columns of every row.  When d/256 slabs x d/16 tiles still fit ONE round of the grid, they run as K slabs of
                 // 256 columns (one 32-column chunk per warp): three times the CTAs, a third of the staging each; the partial sums go to
                 // ypart and are folded, in a fixed order, by the consumer (the next LayerNorm stage / the cross-attention query load).
@@ -130,7 +130,7 @@ Session::Session(Model* model, int64_t max_w, int64_t max_b, int64_t max_text_le
                         gemm(q[9], B.mlp1.w16, B.mlp1.b, 4 * d, 1, D5_ST_PLANES, D5_EM_HID, 3);
                         gemm(q[10], B.mlp2.w16, B.mlp2.b, d, 4, D5_ST_PLANES, D5_EM_PART, 2);
                         // MLP2 K = 4d: 3 slabs of 4d/3 when that keeps the 8-warp K split (multiple of 256, <= 1280): d/16 tiles x 3 slabs
-                        // = 144 items for small.en -> ONE round on 148 CTAs instead of 192 items in two
+                        // = 144 items for small.en -> fewer rounds than 192 items
                         if ((4 * d) % 3 == 0 && (4 * d / 3) % 256 == 0 && 4 * d / 3 <= 1280) { q[10].n_slabs = 3; q[10].ks = 4 * d / 3; }
                         if (split_dd) {
                             for (int sl : {3, 5, 7}) { q[sl].n_slabs = psl; q[sl].ks = 256; q[sl].emit = D5_EM_PART; }
@@ -283,7 +283,7 @@ void Session::run_encoder() {
     encoded = true;
 }
 
-// Tensor-core encoder (fp16-exact weights): conv stems, attention and MLP GEMMs are tcgen05 GEMMs over fp16 hi/lo planes
+// Tensor-core encoder (fp16-exact weights): conv stems, attention and MLP GEMMs are wgmma GEMMs over fp16 hi/lo planes
 // (gemm_f16.cu), attention is enc_attn_tc.cu; only the residual stream x and the encoder output stay fp32 rows.
 void Session::run_encoder_f16() {
     const wb_dims& D = m->dims;
@@ -493,7 +493,7 @@ void Session::launch_v3(int R_, int pos0, int n_steps, int logits_from, bool use
     last_groups = 1;
     if (dec_version == 4) {
         // <= 7 rows: the cluster/DSMEM decoder (decoder4.cu, 131 us per position at 3 rows); 8..24 rows (batched chunks of the small
-        // models): the head-fused tcgen05 cluster decoder (decoder6.cu), whose packed weight slices are built on first use.
+        // models): the head-fused tensor-core cluster decoder (decoder6.cu), whose packed weight slices are built on first use.
         // WB200_DEC6=force sends the small batches through decoder6.cu too (tests, A/B runs).
         if (!force_dec6 && launch_dec4(a, m->fp16_exact, st)) last_decoder = 4;
         if (last_decoder == 3 && use_dec6 && m->fp16_exact && greedy && k == 1 && !use_cur_tok && a.anc == nullptr && a.logits_out == nullptr && R_ <= 24 && ckv_hm &&
@@ -553,7 +553,7 @@ void Session::launch_v3(int R_, int pos0, int n_steps, int logits_from, bool use
         FILE* f = fopen(getenv("WB200_TRACE"), "w");   // debugging aid: WB200_TRACE=<file> receives the stage time stamps of CTA 0
         if (f) {
             for (size_t i = 0; i < h.size(); ++i)
-                if (h[i]) fprintf(f, "%llu\n", h[i]);   // decoder6.cu: first half = consumer stage stamps, second half = MMA-warp stamps (time << 2 | kind)
+                if (h[i]) fprintf(f, "%llu\n", h[i]);   // stage stamps of CTA 0
             fclose(f);
         }
     }

@@ -37,7 +37,7 @@ MODEL_DIMS = {
     "test-b": WhisperDims(80, 1500, 192, 3, 3, 2051, 448, 192, 3, 3),
     "test-c": WhisperDims(80, 1500, 256, 4, 2, 2051, 448, 256, 4, 3),
     "test-e": WhisperDims(80, 1500, 768, 12, 1, 2051, 448, 768, 12, 2),   # d = 768 (small.en width): MLP2 runs as 3 K-slabs of 1024 in decoder5.cu
-    "test-d": WhisperDims(80, 1500, 512, 8, 1, 2051, 448, 512, 8, 2),    # 8 heads: 19+ rows give >= 148 (row, head) units -> unsplit cross attention in decoder5.cu    # d % 256 == 0: the batched tensor-core decoder (decoder5.cu)
+    "test-d": WhisperDims(80, 1500, 512, 8, 1, 2051, 448, 512, 8, 2),    # 8 heads: 17+ rows give >= 132 (row, head) units -> unsplit cross attention in decoder5.cu    # d % 256 == 0: the batched tensor-core decoder (decoder5.cu)
 }
 
 
