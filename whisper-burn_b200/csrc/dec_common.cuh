@@ -41,6 +41,54 @@ __device__ __forceinline__ unsigned int ld_acquire(const unsigned int* p) {
     return v;
 }
 
+// ---- L2 eviction priorities -------------------------------------------------------------------------
+// A persistent decoder reads the same streams at every position.  When their sum exceeds the L2 (H100: 50 MB), near-LRU
+// replacement evicts every line of a cyclic stream before its reuse.  Per-instruction hints split the streams into
+// lines to keep (evict_last) and lines read once per position (evict_first); no device-wide L2 carve-out is involved.
+// A kernel that marks lines evict_last demotes them again before it exits (l2_demote), so no priority outlives the launch.
+__device__ __forceinline__ uint64_t l2_policy_evict_last() {
+    uint64_t p;
+    asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+    uint64_t p;
+    asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+// read-only 16-byte / 1-byte loads with an L2 policy
+__device__ __forceinline__ uint4 ldg_l2(const uint4* p, uint64_t pol) {
+    uint4 v;
+    asm("ld.global.nc.L2::cache_hint.v4.u32 {%0, %1, %2, %3}, [%4], %5;" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(pol));
+    return v;
+}
+__device__ __forceinline__ unsigned int ldg_l2(const uint8_t* p, uint64_t pol) {
+    unsigned int v;
+    asm("ld.global.nc.L2::cache_hint.u8 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
+    return v;
+}
+// 16-byte cp.async (L2 only) with an L2 policy; completion with cp.async.wait_all / wait_group like the plain form
+__device__ __forceinline__ void cp_async16_l2(void* dst, const void* src, uint64_t pol) {
+    asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src),
+                 "l"(pol)
+                 : "memory");
+}
+// 1-D bulk copy global -> shared (TMA engine) with an L2 policy, completion counted on an mbarrier of this CTA
+__device__ __forceinline__ void bulk_g2s_l2(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t pol) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+                     (uint32_t)__cvta_generic_to_shared(dst)),
+                 "l"(src), "r"(bytes), "r"((uint32_t)__cvta_generic_to_shared(bar)), "l"(pol)
+                 : "memory");
+}
+// Back to normal priority: the 128-byte lines of [p, p + bytes) that are resident, line i handled by thread (i - first) % nthreads
+// == tid of the calling grid (p need not be aligned: applypriority addresses the line that contains the address)
+__device__ __forceinline__ void l2_demote(const void* p, size_t bytes, size_t tid, size_t nthreads) {
+    if (p == nullptr) return;
+    const uintptr_t b0 = reinterpret_cast<uintptr_t>(p) & ~uintptr_t(127), e = reinterpret_cast<uintptr_t>(p) + bytes;
+    for (uintptr_t q = b0 + tid * 128; q < e; q += nthreads * 128)
+        asm volatile("applypriority.global.L2::evict_normal [%0], 128;" ::"l"(q) : "memory");
+}
+
 __device__ __forceinline__ unsigned long long gtime() {
     unsigned long long t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -555,9 +603,10 @@ struct AttnBulkGeom {
 };
 // The first NSTG-1 batches of attn_warp_bulk, issued ahead of time (the K/V rows are static: nothing to wait for); the
 // matching attn_warp_bulk call passes prefilled = true and the SAME base / n_keys / wslot / nwarps / ring_count.
-template <int NSTG, typename KT>
+// L2H: the bulk copies carry the L2 policy l2pol (l2_policy_*).
+template <int NSTG, typename KT, bool L2H = false>
 __device__ __forceinline__ void attn_bulk_prefill(const KT* base, int n_keys, int wslot, int nwarps, unsigned char* ring, uint64_t* mbar,
-                                                  unsigned int ring_count) {
+                                                  unsigned int ring_count, uint64_t l2pol = 0) {
     constexpr int ROWB = AttnBulkGeom<KT>::ROWB, STGB = AttnBulkGeom<KT>::STGB, KPB = AttnBulkGeom<KT>::KPB;
     if ((threadIdx.x & 31) != 0) return;
     const int n_batches = (n_keys + KPB - 1) / KPB;
@@ -570,17 +619,21 @@ __device__ __forceinline__ void attn_bulk_prefill(const KT* base, int n_keys, in
             const uint32_t bytes = (uint32_t)min(KPB, n_keys - bb * KPB) * ROWB;
             const uint32_t mb = (uint32_t)__cvta_generic_to_shared(mbar + slot);
             asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mb), "r"(bytes) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                             (uint32_t)__cvta_generic_to_shared(ring + slot * STGB)),
-                         "l"(base + (int64_t)bb * KPB * 128), "r"(bytes), "r"(mb)
-                         : "memory");
+            if constexpr (L2H) {
+                bulk_g2s_l2(ring + slot * STGB, base + (int64_t)bb * KPB * 128, bytes, mbar + slot, l2pol);
+            } else {
+                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+                                 (uint32_t)__cvta_generic_to_shared(ring + slot * STGB)),
+                             "l"(base + (int64_t)bb * KPB * 128), "r"(bytes), "r"(mb)
+                             : "memory");
+            }
         }
     }
 }
-template <int NSTG, typename KT>
+template <int NSTG, typename KT, bool L2H = false>
 __device__ __forceinline__ void attn_warp_bulk(const float* q_smem, const KT* base, int n_keys, int wslot, int nwarps, int swz,
                                                unsigned char* ring, uint64_t* mbar, unsigned int& ring_count, AttnAcc& A,
-                                               bool prefilled = false) {
+                                               bool prefilled = false, uint64_t l2pol = 0) {
     constexpr int CE = 16 / (int)sizeof(KT), NC = 16 / CE;      // chunk elements; chunks per lane and tensor
     constexpr int ROWB = AttnBulkGeom<KT>::ROWB, STGB = AttnBulkGeom<KT>::STGB, KPB = AttnBulkGeom<KT>::KPB;
     const int lane = threadIdx.x & 31, sub = lane >> 2, l4 = lane & 3;
@@ -601,10 +654,14 @@ __device__ __forceinline__ void attn_warp_bulk(const float* q_smem, const KT* ba
             const uint32_t bytes = (uint32_t)min(KPB, n_keys - bb * KPB) * ROWB;
             const uint32_t mb = (uint32_t)__cvta_generic_to_shared(mbar + slot);
             asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mb), "r"(bytes) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                             (uint32_t)__cvta_generic_to_shared(ring + slot * STGB)),
-                         "l"(base + (int64_t)bb * KPB * 128), "r"(bytes), "r"(mb)
-                         : "memory");
+            if constexpr (L2H) {
+                bulk_g2s_l2(ring + slot * STGB, base + (int64_t)bb * KPB * 128, bytes, mbar + slot, l2pol);
+            } else {
+                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+                                 (uint32_t)__cvta_generic_to_shared(ring + slot * STGB)),
+                             "l"(base + (int64_t)bb * KPB * 128), "r"(bytes), "r"(mb)
+                             : "memory");
+            }
         }
     };
     auto load16 = [&](const unsigned char* p16, int par, float (&f)[16]) {   // this lane's 16 dims of one K or V row

@@ -71,6 +71,12 @@ constexpr int CS = 16;   // CTAs per cluster
 constexpr int LG_NBUF = 3;                 // logits stage: ring slots per warp
 constexpr int LG_RB = 8;                   // vocabulary rows per slot
 constexpr int KV_STG = 4;                  // cross attention: stages (8 keys each) of the per-warp K/V ring
+// cross K/V in L2: 1 kept with the weights (evict_last), 0 streamed (evict_first, the faster one on the H100 for fp32 and
+// fp16 K/V: the kept set then outgrows what the L2 holds for reads from all SMs; DESIGN.md section 5)
+#ifndef D4_L2_CKV_KEEP
+#define D4_L2_CKV_KEEP 0
+#endif
+__device__ __forceinline__ uint64_t ckv_policy() { return D4_L2_CKV_KEEP ? l2_policy_evict_last() : l2_policy_evict_first(); }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -92,13 +98,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         "r"(parity)
         : "memory");
 }
-// 1-D bulk copy global -> shared (TMA engine, no tensor map), completion counted on an mbarrier
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
-                 "l"(src), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
-
 // 16-byte asynchronous copy global -> shared (L2 only), lane-private destination: completion with cp_async_wait_all()
 __device__ __forceinline__ void cp_async16(void* dst, const void* src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
@@ -118,7 +117,7 @@ struct RowRegs {
 // rows row0, row0 + step, ... of W[.][K] (fp16) -> registers; lane-strided 16-byte vectors
 template <int NR, int VPL>
 __device__ __forceinline__ void load_rows(const __half* __restrict__ W, const float* __restrict__ bias, int K, int row0, int step,
-                                          RowRegs<NR, VPL>& r) {
+                                          RowRegs<NR, VPL>& r, uint64_t pol) {
     const int lane = threadIdx.x & 31, nv = K / 8;
 #pragma unroll
     for (int i = 0; i < NR; ++i) r.bias[i] = __ldg(bias + row0 + i * step);
@@ -129,7 +128,7 @@ __device__ __forceinline__ void load_rows(const __half* __restrict__ W, const fl
 #pragma unroll
         for (int j = 0; j < VPL; ++j) {
             const int v = j * 32 + lane;
-            r.v[i][j] = v < nv ? __ldg(p + v) : make_uint4(0, 0, 0, 0);
+            r.v[i][j] = v < nv ? ldg_l2(p + v, pol) : make_uint4(0, 0, 0, 0);
         }
     }
 }
@@ -269,12 +268,12 @@ __device__ __forceinline__ void x_update(XRegs<PF>& x, const float* src_s, const
 // gamma | beta of a LayerNorm a few stages ahead -> this WARP's private copy (2D floats), lane-private 16-byte cp.async
 // (each lane copies exactly the vectors it reads in ln_warp): no register stall, no barrier; cp_async_wait_all() before use.
 template <int D, int PF>
-__device__ __forceinline__ void ln_fetch(float* lnp, const float* __restrict__ g, const float* __restrict__ b) {
+__device__ __forceinline__ void ln_fetch(float* lnp, const float* __restrict__ g, const float* __restrict__ b, uint64_t pol) {
     const int lane = threadIdx.x & 31;
 #pragma unroll
     for (int k = 0; k < PF; ++k) {
-        cp_async16(lnp + 4 * (lane + 32 * k), g + 4 * (lane + 32 * k));
-        cp_async16(lnp + D + 4 * (lane + 32 * k), b + 4 * (lane + 32 * k));
+        cp_async16_l2(lnp + 4 * (lane + 32 * k), g + 4 * (lane + 32 * k), pol);
+        cp_async16_l2(lnp + D + 4 * (lane + 32 * k), b + 4 * (lane + 32 * k), pol);
     }
 }
 // LayerNorm (burn 0.9 form, layernorm in oracle/model.py) of the warp's register copy of x -> out_s (shared memory).  Every
@@ -368,6 +367,30 @@ dec4_kernel(const Dec3Args a) {
     unsigned int lstep = 0;      // vocabulary steps this launch has finished (ticket / flag bookkeeping)
     int tr_n = 0;
     const float scale = a.qk_scale;
+    // L2 plan (DESIGN.md section 5): the layer weights, LayerNorm parameters and self K/V are re-read at every position and
+    // kept (evict_last); the vocabulary half-tiles and is_special are read once per position and go first (evict_first);
+    // cross K/V follows D4_L2_CKV_KEEP; biases keep normal priority.
+    // Every line marked evict_last goes back to normal priority before the kernel exits (all CTAs, the ranges split over the grid).
+    auto demote = [&]() {
+        const size_t gt = (size_t)blockIdx.x * NT + tid, gn = (size_t)gridDim.x * NT;
+        for (int l = 0; l < L; ++l) {
+            const Dec3Layer& W = a.layers[l];
+            l2_demote(W.Wqkv, (size_t)3 * D * D * 2, gt, gn);
+            l2_demote(W.Wo, (size_t)D * D * 2, gt, gn);
+            l2_demote(W.Wcq, (size_t)D * D * 2, gt, gn);
+            l2_demote(W.Wco, (size_t)D * D * 2, gt, gn);
+            l2_demote(W.W1, (size_t)4 * D * D * 2, gt, gn);
+            l2_demote(W.W2, (size_t)4 * D * D * 2, gt, gn);
+            l2_demote(W.ln1_g, D * 4, gt, gn); l2_demote(W.ln1_b, D * 4, gt, gn); l2_demote(W.ln2_g, D * 4, gt, gn);
+            l2_demote(W.ln2_b, D * 4, gt, gn); l2_demote(W.ln3_g, D * 4, gt, gn); l2_demote(W.ln3_b, D * 4, gt, gn);
+        }
+        l2_demote(a.lnf_g, D * 4, gt, gn);
+        l2_demote(a.lnf_b, D * 4, gt, gn);
+        const size_t kv_bytes = (size_t)L * a.Rmax * t_max * D * sizeof(KVT);
+        l2_demote(a.kc, kv_bytes, gt, gn);
+        l2_demote(a.vc, kv_bytes, gt, gn);
+        if (D4_L2_CKV_KEEP) l2_demote(a.ckv, (size_t)L * a.Mcap * 2 * D * sizeof(KVT), gt, gn);
+    };
     WB_TRACE();
 
     const __half* nullw = nullptr;
@@ -396,7 +419,7 @@ dec4_kernel(const Dec3Args a) {
                 const int vt = tile_of(it >> 1);
                 const int slot = (int)((lg_count + (unsigned int)it) % LG_NBUF);
                 mbar_expect_tx(wbar + slot, BLKB);
-                bulk_g2s(wring + (size_t)slot * BLKB, Et + ((int64_t)vt * 2 + (it & 1)) * 16 * KH, BLKB, wbar + slot);
+                bulk_g2s_l2(wring + (size_t)slot * BLKB, Et + ((int64_t)vt * 2 + (it & 1)) * 16 * KH, BLKB, wbar + slot, l2_policy_evict_first());
             }
         };
         uint4* gpl_hi = reinterpret_cast<uint4*>(a.att_pl);   // published final-LayerNorm rows: fragment-order fp16 hi / lo planes [D/32][32]
@@ -429,8 +452,8 @@ dec4_kernel(const Dec3Args a) {
                 for (int k = 0; k < PF; ++k) reinterpret_cast<float4*>(xb)[lane + 32 * k] = x.v[k];
             }
             RowRegs<NR_QKV, VPL> w_qkv;
-            load_rows<NR_QKV, VPL>(reinterpret_cast<const __half*>(a.layers[0].Wqkv), a.layers[0].bqkv, D, rank * (3 * D / CS) + warp, NW, w_qkv);
-            if (step == 0) ln_fetch<D, PF>(lnp, a.layers[0].ln1_g, a.layers[0].ln1_b);   // later steps: fetched by the previous step's last layer
+            load_rows<NR_QKV, VPL>(reinterpret_cast<const __half*>(a.layers[0].Wqkv), a.layers[0].bqkv, D, rank * (3 * D / CS) + warp, NW, w_qkv, l2_policy_evict_last());
+            if (step == 0) ln_fetch<D, PF>(lnp, a.layers[0].ln1_g, a.layers[0].ln1_b, l2_policy_evict_last());   // later steps: fetched by the previous step's last layer
             __syncthreads();
             for (int l = 0; l < L; ++l) {
                 const Dec3Layer& W = a.layers[l];
@@ -442,7 +465,7 @@ dec4_kernel(const Dec3Args a) {
                     xsel ^= 1;
                 }
                 ln_warp<D, PF>(x, lnp, W.ln1_eps, a.eps_outside, xn_s);
-                ln_fetch<D, PF>(lnp, W.ln2_g, W.ln2_b);
+                ln_fetch<D, PF>(lnp, W.ln2_g, W.ln2_b, l2_policy_evict_last());
                 {
                     float acc[NR_QKV];
                     dot_rows1<NR_QKV, VPL, false>(w_qkv, xn_s, D, acc);
@@ -459,7 +482,7 @@ dec4_kernel(const Dec3Args a) {
                 constexpr int SNV = sizeof(KVT) == 4 ? 4 : 2;   // 16-byte vectors per lane and tensor (16 dims)
                 uint8_t* sring = ring + (size_t)warp * RINGW;
                 auto pre_s2 = [&]() {
-                    load_rows<NR_D, VPL>(reinterpret_cast<const __half*>(W.Wo), W.bo, D, rank * (D / CS) + warp, NW, w_o);
+                    load_rows<NR_D, VPL>(reinterpret_cast<const __half*>(W.Wo), W.bo, D, rank * (D / CS) + warp, NW, w_o, l2_policy_evict_last());
                     if (rank < H && self_fast) {
 #pragma unroll
                         for (int u = 0; u < 2; ++u) {
@@ -468,8 +491,8 @@ dec4_kernel(const Dec3Args a) {
                                 const int64_t o = ((int64_t)row * t_max + j) * D + rank * 64 + l4 * 16;
 #pragma unroll
                                 for (int c = 0; c < SNV; ++c) {
-                                    cp_async16(sring + ((u * 2 + 0) * 4 + c) * 512 + lane * 16, reinterpret_cast<const uint4*>(kcl + o) + c);
-                                    cp_async16(sring + ((u * 2 + 1) * 4 + c) * 512 + lane * 16, reinterpret_cast<const uint4*>(vcl + o) + c);
+                                    cp_async16_l2(sring + ((u * 2 + 0) * 4 + c) * 512 + lane * 16, reinterpret_cast<const uint4*>(kcl + o) + c, l2_policy_evict_last());
+                                    cp_async16_l2(sring + ((u * 2 + 1) * 4 + c) * 512 + lane * 16, reinterpret_cast<const uint4*>(vcl + o) + c, l2_policy_evict_last());
                                 }
                             }
                         }
@@ -577,10 +600,10 @@ dec4_kernel(const Dec3Args a) {
                 }
                 RowRegs<NR_D, VPL> w_cq;
                 auto pre_s4 = [&]() {
-                    load_rows<NR_D, VPL>(reinterpret_cast<const __half*>(W.Wcq), W.bcq, D, rank * (D / CS) + warp, NW, w_cq);
+                    load_rows<NR_D, VPL>(reinterpret_cast<const __half*>(W.Wcq), W.bcq, D, rank * (D / CS) + warp, NW, w_cq, l2_policy_evict_last());
                     if (a.ckv_hm)   // first batches of this layer's cross K/V: static data, two barriers ahead of its use
-                        attn_bulk_prefill<KV_STG, KVT>(reinterpret_cast<const KVT*>(a.ckv) + (size_t)l * a.Mcap * 2 * D + xoff, xT, xci * NW + warp,
-                                                       xnch * NW, ring + (size_t)warp * RINGW, kv_bar + warp * KV_STG, kv_count);
+                        attn_bulk_prefill<KV_STG, KVT, true>(reinterpret_cast<const KVT*>(a.ckv) + (size_t)l * a.Mcap * 2 * D + xoff, xT, xci * NW + warp,
+                                                             xnch * NW, ring + (size_t)warp * RINGW, kv_bar + warp * KV_STG, kv_count, ckv_policy());
                 };
                 auto send_s3 = [&]() { put_slice<D / CS>(cl, stg_s, dl_s + rank * (D / CS), xbar + 2); };
                 D4_EXCHANGE(2, D * 4, send_s3, pre_s4);
@@ -589,7 +612,7 @@ dec4_kernel(const Dec3Args a) {
                 x_update<PF>(x, xb + xsel * D, dl_s, xb + (xsel ^ 1) * D);
                 xsel ^= 1;
                 ln_warp<D, PF>(x, lnp, W.ln2_eps, a.eps_outside, xn_s);
-                ln_fetch<D, PF>(lnp, W.ln3_g, W.ln3_b);
+                ln_fetch<D, PF>(lnp, W.ln3_g, W.ln3_b, l2_policy_evict_last());
                 WB_FINE();
                 {
                     float acc[NR_D];
@@ -601,7 +624,7 @@ dec4_kernel(const Dec3Args a) {
                     }
                 }
                 RowRegs<NR_D, VPL> w_co;
-                auto pre_s6 = [&]() { load_rows<NR_D, VPL>(reinterpret_cast<const __half*>(W.Wco), W.bco, D, rank * (D / CS) + warp, NW, w_co); };
+                auto pre_s6 = [&]() { load_rows<NR_D, VPL>(reinterpret_cast<const __half*>(W.Wco), W.bco, D, rank * (D / CS) + warp, NW, w_co, l2_policy_evict_last()); };
                 auto send_s4 = [&]() { put_slice<D / CS>(cl, stg_s, q2_s + rank * (D / CS), xbar + 3); };
                 D4_EXCHANGE(3, D * 4, send_s4, pre_s6);
                 WB_TRACE();
@@ -616,8 +639,8 @@ dec4_kernel(const Dec3Args a) {
                     // keys j == ci*NW + warp (mod nch*NW)
                     AttnAcc A;
                     if (a.ckv_hm) {   // contiguous head-major block: 8-key batches by bulk copy into this warp's ring (shared with the logits stage)
-                        attn_warp_bulk<KV_STG, KVT>(q2_s + h * 64, kbase, T, ci * NW + warp, nch * NW, 0, ring + (size_t)warp * RINGW,
-                                                    kv_bar + warp * KV_STG, kv_count, A, true);
+                        attn_warp_bulk<KV_STG, KVT, true>(q2_s + h * 64, kbase, T, ci * NW + warp, nch * NW, 0, ring + (size_t)warp * RINGW,
+                                                          kv_bar + warp * KV_STG, kv_count, A, true, ckv_policy());
                     } else {
                         attn_warp(q2_s + h * 64, T, ci * NW + warp, nch * NW, kp, vp, A, -1);
                     }
@@ -676,7 +699,7 @@ dec4_kernel(const Dec3Args a) {
                     }
                 }
                 RowRegs<NR_H, VPL> w_1;
-                auto pre_s7 = [&]() { load_rows<NR_H, VPL>(reinterpret_cast<const __half*>(W.W1), W.b1, D, rank * (4 * D / CS) + warp, NW, w_1); };
+                auto pre_s7 = [&]() { load_rows<NR_H, VPL>(reinterpret_cast<const __half*>(W.W1), W.b1, D, rank * (4 * D / CS) + warp, NW, w_1, l2_policy_evict_last()); };
                 auto send_s6 = [&]() { put_slice<D / CS>(cl, stg_s, dl_s + rank * (D / CS), xbar + 5); };
                 D4_EXCHANGE(5, D * 4, send_s6, pre_s7);
                 WB_TRACE();
@@ -685,10 +708,10 @@ dec4_kernel(const Dec3Args a) {
                 xsel ^= 1;
                 ln_warp<D, PF>(x, lnp, W.ln3_eps, a.eps_outside, xn_s);
                 if (l == L - 1 && want_logits && rank == 0 && warp == 0) {   // this warp publishes the row: final LayerNorm next
-                    ln_fetch<D, PF>(lnp, a.lnf_g, a.lnf_b);
+                    ln_fetch<D, PF>(lnp, a.lnf_g, a.lnf_b, l2_policy_evict_last());
                 } else {   // LN1 of the next layer, or of layer 0 for the next position
                     const Dec3Layer& Wn = a.layers[l + 1 < L ? l + 1 : 0];
-                    ln_fetch<D, PF>(lnp, Wn.ln1_g, Wn.ln1_b);
+                    ln_fetch<D, PF>(lnp, Wn.ln1_g, Wn.ln1_b, l2_policy_evict_last());
                 }
                 WB_FINE();
                 {
@@ -701,7 +724,7 @@ dec4_kernel(const Dec3Args a) {
                     if (!(lane & 1) && (lane >> 1) < NR_H) stg_s[warp + (lane >> 1) * NW] = mine;
                 }
                 RowRegs<NR_D, VPL4> w_2;
-                auto pre_s8 = [&]() { load_rows<NR_D, VPL4>(reinterpret_cast<const __half*>(W.W2), W.b2, 4 * D, rank * (D / CS) + warp, NW, w_2); };
+                auto pre_s8 = [&]() { load_rows<NR_D, VPL4>(reinterpret_cast<const __half*>(W.W2), W.b2, 4 * D, rank * (D / CS) + warp, NW, w_2, l2_policy_evict_last()); };
                 auto send_s7 = [&]() { put_slice<4 * D / CS>(cl, stg_s, hid_s + rank * (4 * D / CS), xbar + 6); };
                 D4_EXCHANGE(6, 4 * D * 4, send_s7, pre_s8);
                 WB_TRACE();
@@ -716,7 +739,7 @@ dec4_kernel(const Dec3Args a) {
                 }
                 auto pre_s1 = [&]() {
                     if (l + 1 < L)
-                        load_rows<NR_QKV, VPL>(reinterpret_cast<const __half*>(a.layers[l + 1].Wqkv), a.layers[l + 1].bqkv, D, rank * (3 * D / CS) + warp, NW, w_qkv);
+                        load_rows<NR_QKV, VPL>(reinterpret_cast<const __half*>(a.layers[l + 1].Wqkv), a.layers[l + 1].bqkv, D, rank * (3 * D / CS) + warp, NW, w_qkv, l2_policy_evict_last());
                 };
                 auto send_s8 = [&]() { put_slice<D / CS>(cl, stg_s, dl_s + rank * (D / CS), xbar + 7); };
                 D4_EXCHANGE(7, D * 4, send_s8, pre_s1);
@@ -733,7 +756,7 @@ dec4_kernel(const Dec3Args a) {
 #pragma unroll
                 for (int k = 0; k < PF; ++k)
                     store_frag(gpl_hi, RC == 4 ? gpl_hi + 16 : gpl_lo, D / 32, row, 4 * (lane + 32 * k), reinterpret_cast<const float4*>(xn_s)[lane + 32 * k]);
-                ln_fetch<D, PF>(lnp, a.layers[0].ln1_g, a.layers[0].ln1_b);   // LN1 of layer 0 for the next position
+                ln_fetch<D, PF>(lnp, a.layers[0].ln1_g, a.layers[0].ln1_b, l2_policy_evict_last());   // LN1 of layer 0 for the next position
             }
         }
         if (!want_logits) {   // prefill positions: clusters stay independent, no chip-wide step
@@ -771,7 +794,7 @@ dec4_kernel(const Dec3Args a) {
                     for (int c = 0; c < 4; ++c) { ah[c] = 0.0f; al[c] = 0.0f; }
                     if (use_mask) {
                         const int n = tile_of(it >> 1) * 16 + g;
-                        sp01 = (n < V ? (unsigned int)a.is_special[n] : 0u) | (n + 8 < V ? (unsigned int)a.is_special[n + 8] << 8 : 0u);
+                        sp01 = (n < V ? ldg_l2(a.is_special + n, l2_policy_evict_first()) : 0u) | (n + 8 < V ? ldg_l2(a.is_special + n + 8, l2_policy_evict_first()) << 8 : 0u);
                     }
                 }
 #pragma unroll
@@ -931,10 +954,14 @@ dec4_kernel(const Dec3Args a) {
             for (int r = 0; r < R; ++r) live += __ldcg(a.finished + r) ? 0 : 1;
             if (live == 0) {
                 if (blockIdx.x == 0 && tid == 0) { *a.pos = p + 1; *a.n_unfinished = 0; *a.steps_done = step + 1; }
+                demote();   // every CTA is past the flag: no evict_last load is left
                 return;
             }
         }
     }
+    // after a prefill position clusters run independently: all of them finish their loads before any line is demoted
+    if (a.n_steps > 0 && a.pos0 + a.n_steps - 1 < a.logits_from) grid_sync(a.bar, gen);
+    demote();
     if (blockIdx.x == 0 && tid == 0) {
         *a.pos = a.pos0 + a.n_steps;
         int live = 0;

@@ -492,7 +492,7 @@ void Session::launch_v3(int R_, int pos0, int n_steps, int logits_from, bool use
     last_decoder = 3;
     last_groups = 1;
     if (dec_version == 4) {
-        // <= 7 rows: the cluster/DSMEM decoder (decoder4.cu, 131 us per position at 3 rows); 8..24 rows (batched chunks of the small
+        // <= 7 rows: the cluster/DSMEM decoder (decoder4.cu; time per position at 3 rows: DESIGN.md section 6); 8..24 rows (batched chunks of the small
         // models): the head-fused tensor-core cluster decoder (decoder6.cu), whose packed weight slices are built on first use.
         // WB200_DEC6=force sends the small batches through decoder6.cu too (tests, A/B runs).
         if (!force_dec6 && launch_dec4(a, m->fp16_exact, st)) last_decoder = 4;
