@@ -163,13 +163,11 @@ def tiny_en():
 
 
 @pytest.mark.parametrize("kv", ["f32", "f16"])
-@pytest.mark.parametrize("hs", ["1", "2"])
-def test_tiny_en_cluster_decoder_one_chunk(tiny_en, kv, hs, monkeypatch):
-    """BASELINE config 2 through both cluster shapes of decoder6.cu: one CTA per head (6-CTA clusters) and two (12-CTA clusters,
-    keys and MLP slices split, softmax merge on the receiving side)."""
+def test_tiny_en_cluster_decoder_one_chunk(tiny_en, kv, monkeypatch):
+    """BASELINE config 2 through decoder6.cu (one CTA per head, 6-CTA clusters) with a single n-tile in the vocabulary
+    projection."""
     dims, sp, wh = tiny_en
-    monkeypatch.setenv("WB200_DEC6_HS", hs)
-    monkeypatch.setenv("WB200_DEC6", "force")     # 3 rows are decoder4.cu's range by default
+    monkeypatch.setenv("WB200_DECODER", "6")     # 3 rows are decoder4.cu's range by default
     waves, recs = _tiny_cases(kv, [0])
     sess = transcribe.Session(wh, max_windows=3, max_beams=1, max_text_len=105, kv_dtype=ffi.WB_KV_F16 if kv == "f16" else ffi.WB_KV_F32)
     got = sess.transcribe_windows(waves, sp, is_special_of(sp), beam_size=1, max_depth=100)

@@ -8,8 +8,8 @@ namespace wb {
 
 constexpr int DEC_KC = 8;   // top candidates a persistent decoder keeps per record (k <= 7)
 
-// ---- persistent cooperative decoder (decoder3.cu) ------------------------------------------------------
-struct Dec3Layer {
+// ---- persistent decoders (decoder3.cu .. decoder6.cu) -------------------------------------------------
+struct DecLayer {
     const float *ln1_g, *ln1_b, *ln2_g, *ln2_b, *ln3_g, *ln3_b;
     float ln1_eps, ln2_eps, ln3_eps;
     const void *Wqkv, *Wo, *Wcq, *Wco, *W1, *W2;     // [N][K] fp16 or fp32
@@ -33,12 +33,12 @@ struct Dec5Desc {
     int pad_[2] = {0, 0};          // sizeof % 16 == 0: the table is copied to shared memory in 16-byte words
 };
 static_assert(sizeof(Dec5Desc) % 16 == 0, "Dec5Desc must be a whole number of 16-byte words");
-struct Dec3Args {
+struct DecArgs {
     int R = 0, Rmax = 0, d = 0, H = 0, L = 0, V = 0, t_max = 0;
     int64_t Mcap = 0;
     int eps_outside = 1;
     float qk_scale = 1.0f;
-    const Dec3Layer* layers = nullptr;    // device array [L]
+    const DecLayer* layers = nullptr;    // device array [L]
     const float* tok_emb = nullptr;       // fp32 [V][d] (embedding lookup)
     const float* pos_emb = nullptr;
     const void* E = nullptr;              // logits matrix [V][d] fp16 or fp32
@@ -53,8 +53,7 @@ struct Dec3Args {
     float* lgbuf = nullptr;                 // decoder5.cu: [R][V] logits scratch (== logits_out when that is requested)
     int lg_slices = 1;                      // decoder5.cu: vocabulary slices per row in the softmax / candidate stage
     void *kc = nullptr, *vc = nullptr;    // [L][Rmax][t_max][d]  fp32 or fp16 (kv_half)
-    const void* ckv = nullptr;            // [L][Mcap][2d]
-    int ckv_hm = 0;                       // 1: head-major cross K/V (encoder.cu ckv_relayout_kernel), 0: GEMM row-major order
+    const void* ckv = nullptr;            // [L][Mcap][2d] cross K/V, head-major per window (encoder.cu ckv_relayout_kernel)
     int kv_half = 0;
     int kv_row0 = 0;                      // decoder5.cu row groups: local row r of this launch is cache row r + kv_row0 (ancestry entries are absolute)
     const int* row_window = nullptr;
@@ -84,23 +83,26 @@ struct Dec3Args {
     unsigned long long* trace = nullptr;  // optional: stage / barrier timestamps of CTA 0 (ns)
     int trace_cap = 0;
 };
-void launch_dec3(const Dec3Args& a, int n_ctas, bool w_half, cudaStream_t st);
-// cluster / DSMEM version (decoder4.cu); returns false when the configuration is not covered
-bool launch_dec4(const Dec3Args& a, bool w_half, cudaStream_t st);
-// batched tensor-core version (decoder5.cu); returns false when the configuration is not covered
-bool launch_dec5(const Dec3Args& a, int n_ctas, bool w_half, cudaStream_t st);
-size_t dec5_plane_uint4(int d);   // uint4 elements of one global activation plane
-// head-fused cluster decoder (decoder6.cu): greedy, d in {128, 384}, <= 24 rows; hs = CTAs per attention head (1 or 2)
-struct Dec6LayerSrc {   // device pointers of one decoder block (fp16 [N][K] weights, fp32 biases / LayerNorm parameters)
-    const __half *Wqkv, *Wo, *Wcq, *Wco, *W1, *W2;
-    const float *bqkv, *bo, *bcq, *bco, *b1, *b2;
-    const float *ln1_g, *ln1_b, *ln2_g, *ln2_b, *ln3_g, *ln3_b;
-    float ln1_eps, ln2_eps, ln3_eps;
+// Each launch_decN launches decoder N when it covers the configuration and reports whether it did.
+// grid-barrier FMA decoder (decoder3.cu): covers every configuration
+void launch_dec3(const DecArgs& a, int n_ctas, bool w_half, cudaStream_t st);
+// cluster / DSMEM decoder (decoder4.cu): greedy, d in {128, 384}, as many rows (<= 8) as co-resident 16-CTA clusters
+bool launch_dec4(const DecArgs& a, bool w_half, cudaStream_t st);
+// head-fused tensor-core cluster decoder (decoder6.cu): fp16-exact weights, greedy, d in {128, 384}, <= 24 rows, t_max <= 128
+struct Dec6Pack {   // this model's weights as per-CTA slices (built on the first launch)
+    DevBuf<uint8_t> pack;   // [L][CS][PACK] bytes
+    DevBuf<float> params;   // [L][CS][PARAMS] floats
 };
-bool dec6_supported(int d, int H);
-int dec6_pick_hs(int d, int R);
-void dec6_build_pack(int d, int hs, const std::vector<Dec6LayerSrc>& layers, DevBuf<uint8_t>& pack, DevBuf<float>& params, cudaStream_t st);
-bool launch_dec6(const Dec3Args& a, int hs, bool w_half, cudaStream_t st);
+bool launch_dec6(DecArgs a, const Model& m, Dec6Pack& pack, cudaStream_t st);
+// batched tensor-core decoder (decoder5.cu): fp16-exact weights, d % 256 == 0; more than 32 rows run as row groups of 32.
+// Returns the number of launches, 0 when the configuration is not covered.
+struct Dec5Tables {   // stage descriptors (Dec5Desc)
+    DevBuf<Dec5Desc> unsplit;   // the d x d projections unsplit
+    DevBuf<Dec5Desc> split;     // the same as K slabs (launches whose cross attention is not split over keys); may be empty
+};
+void dec5_build_tables(const Model& m, int n_sm, Dec5Tables& t);   // nothing unless the weights are fp16-exact
+int launch_dec5(const DecArgs& a, const Dec5Tables& t, int n_ctas, bool w_half, cudaStream_t st);
+size_t dec5_plane_uint4(int d);   // uint4 elements of one global activation plane
 
 void launch_dec_anc_identity(int* anc, int R, int t_max, cudaStream_t st);
 void launch_dec_reorder(const int* anc_old, int* anc_new, const int* parent, const int* pos_ptr, int R, int t_max,

@@ -28,7 +28,7 @@ namespace {
 // =====================================================================================================
 template <typename WT, int RC, int KC, typename KVT>
 __global__ void __launch_bounds__(NT, 1)
-dec3_kernel(const Dec3Args a) {
+dec3_kernel(const DecArgs a) {
     extern __shared__ __align__(16) float sm[];
     const int d = a.d, H = a.H, L = a.L, V = a.V, R = a.R, t_max = a.t_max;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -53,7 +53,7 @@ dec3_kernel(const Dec3Args a) {
         // embed: x[r] = tok_emb[token] + pos_emb[p] (mod.rs:141-146) is formed by EVERY CTA in shared memory for
         // the first LayerNorm (no extra barrier); rows are published to a.x by the CTAs r % grid for the residual adds.
         for (int l = 0; l < L; ++l) {
-            const Dec3Layer& W = a.layers[l];
+            const DecLayer& W = a.layers[l];
             KVT* kcl = reinterpret_cast<KVT*>(a.kc) + (size_t)l * a.Rmax * t_max * d;
             KVT* vcl = reinterpret_cast<KVT*>(a.vc) + (size_t)l * a.Rmax * t_max * d;
             // ================= P1: q | k | v = LN(x) Wqkv + b   (mod.rs:429-431)
@@ -152,12 +152,10 @@ dec3_kernel(const Dec3Args a) {
                     const int per = (T + S - 1) / S;
                     const int kb0 = sp * per;
                     const int nk = max(0, min(T, kb0 + per) - kb0);
-                    const KVT* kbase = ckvl + a.win_row_off[w] * (int64_t)(2 * d) + (a.ckv_hm ? ((int64_t)h * T + kb0) * 128 : kb0 * (int64_t)(2 * d) + h * 64);
-                    const int64_t ld = a.ckv_hm ? 128 : 2 * (int64_t)d;
-                    const int voff = a.ckv_hm ? 64 : d;
-                    auto kp = [&](int j) { return kbase + j * ld; };
-                    auto vp = [&](int j) { return kbase + j * ld + voff; };
-                    attn_cta(qs, nk, kp, vp, wm, wl, wo, ao, ML, a.ckv_hm ? kb0 : -1);
+                    const KVT* kbase = ckvl + a.win_row_off[w] * (int64_t)(2 * d) + ((int64_t)h * T + kb0) * 128;   // head-major K | V rows
+                    auto kp = [&](int j) { return kbase + j * 128; };
+                    auto vp = [&](int j) { return kbase + j * 128 + 64; };
+                    attn_cta(qs, nk, kp, vp, wm, wl, wo, ao, ML, kb0);
                     const int64_t o = ((int64_t)r * H + h) * S + sp;
                     if (tid < 64) a.part_o[o * 64 + tid] = ao[tid];
                     if (tid == 0) { a.part_m[o] = nk > 0 ? ML[0] : -INFINITY; a.part_l[o] = ML[1]; }
@@ -420,7 +418,7 @@ size_t dec3_smem_bytes(int d, int H, int S, int RC, int KC) {
 }
 
 template <typename WT, int RC, int KC, typename KVT>
-void launch_t(const Dec3Args& a, int n_ctas, cudaStream_t st) {
+void launch_t(const DecArgs& a, int n_ctas, cudaStream_t st) {
     const size_t smem = dec3_smem_bytes(a.d, a.H, a.n_splits, RC, KC);
     auto k = dec3_kernel<WT, RC, KC, KVT>;
     static PerDeviceConfig cfg;   // per instantiation
@@ -438,7 +436,7 @@ void launch_t(const Dec3Args& a, int n_ctas, cudaStream_t st) {
 
 }  // namespace
 
-void launch_dec3(const Dec3Args& a, int n_ctas, bool w_half, cudaStream_t st) {
+void launch_dec3(const DecArgs& a, int n_ctas, bool w_half, cudaStream_t st) {
     const bool big = a.R > 4;
     const bool wide = a.k > 1;
 #define WB_D3(WT)                                                        \

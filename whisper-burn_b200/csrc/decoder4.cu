@@ -16,10 +16,6 @@
 // Reference math: see decoder3.cu.  Greedy path only (beam steps use decoder3.cu).
 #include <cooperative_groups.h>
 
-#include <cstdio>
-#include <cstdlib>
-#include <mutex>
-
 #include "dec_common.cuh"
 
 namespace cg = cooperative_groups;
@@ -313,7 +309,7 @@ __device__ __forceinline__ void ln_warp(XRegs<PF>& x, const float* gb_s, float e
 
 template <int D, int RC, typename KVT>
 __global__ void __launch_bounds__(NT, 1)
-dec4_kernel(const Dec3Args a) {
+dec4_kernel(const DecArgs a) {
     extern __shared__ __align__(16) float sm[];
     cg::cluster_group cl = cg::this_cluster();
     constexpr int H = D / 64;
@@ -374,7 +370,7 @@ dec4_kernel(const Dec3Args a) {
     auto demote = [&]() {
         const size_t gt = (size_t)blockIdx.x * NT + tid, gn = (size_t)gridDim.x * NT;
         for (int l = 0; l < L; ++l) {
-            const Dec3Layer& W = a.layers[l];
+            const DecLayer& W = a.layers[l];
             l2_demote(W.Wqkv, (size_t)3 * D * D * 2, gt, gn);
             l2_demote(W.Wo, (size_t)D * D * 2, gt, gn);
             l2_demote(W.Wcq, (size_t)D * D * 2, gt, gn);
@@ -436,7 +432,7 @@ dec4_kernel(const Dec3Args a) {
             const int xnch = (CS - xh + H - 1) / H;              // CTAs working on head xh
             const int xw = __ldcg(a.row_window + row);
             const int xT = a.win_T[xw];
-            const int64_t xoff = a.win_row_off[xw] * (int64_t)(2 * D) + (a.ckv_hm ? (int64_t)xh * xT * 128 : (int64_t)xh * 64);
+            const int64_t xoff = a.win_row_off[xw] * (int64_t)(2 * D) + (int64_t)xh * xT * 128;   // head-major K | V block
             const int sub = lane >> 2, l4 = lane & 3;
             const bool self_fast = p + 1 <= NW * 16;             // self attention: every cached position fits one register batch
             constexpr int PF = D / 128;   // float4s of the row per lane
@@ -456,7 +452,7 @@ dec4_kernel(const Dec3Args a) {
             if (step == 0) ln_fetch<D, PF>(lnp, a.layers[0].ln1_g, a.layers[0].ln1_b, l2_policy_evict_last());   // later steps: fetched by the previous step's last layer
             __syncthreads();
             for (int l = 0; l < L; ++l) {
-                const Dec3Layer& W = a.layers[l];
+                const DecLayer& W = a.layers[l];
                 KVT* kcl = reinterpret_cast<KVT*>(a.kc) + (size_t)l * a.Rmax * t_max * D;
                 KVT* vcl = reinterpret_cast<KVT*>(a.vc) + (size_t)l * a.Rmax * t_max * D;
                 // ================= S1: q | k | v = LN1(x) Wqkv + b
@@ -601,9 +597,9 @@ dec4_kernel(const Dec3Args a) {
                 RowRegs<NR_D, VPL> w_cq;
                 auto pre_s4 = [&]() {
                     load_rows<NR_D, VPL>(reinterpret_cast<const __half*>(W.Wcq), W.bcq, D, rank * (D / CS) + warp, NW, w_cq, l2_policy_evict_last());
-                    if (a.ckv_hm)   // first batches of this layer's cross K/V: static data, two barriers ahead of its use
-                        attn_bulk_prefill<KV_STG, KVT, true>(reinterpret_cast<const KVT*>(a.ckv) + (size_t)l * a.Mcap * 2 * D + xoff, xT, xci * NW + warp,
-                                                             xnch * NW, ring + (size_t)warp * RINGW, kv_bar + warp * KV_STG, kv_count, ckv_policy());
+                    // first batches of this layer's cross K/V: static data, two barriers ahead of its use
+                    attn_bulk_prefill<KV_STG, KVT, true>(reinterpret_cast<const KVT*>(a.ckv) + (size_t)l * a.Mcap * 2 * D + xoff, xT, xci * NW + warp,
+                                                         xnch * NW, ring + (size_t)warp * RINGW, kv_bar + warp * KV_STG, kv_count, ckv_policy());
                 };
                 auto send_s3 = [&]() { put_slice<D / CS>(cl, stg_s, dl_s + rank * (D / CS), xbar + 2); };
                 D4_EXCHANGE(2, D * 4, send_s3, pre_s4);
@@ -632,18 +628,11 @@ dec4_kernel(const Dec3Args a) {
                 {
                     const int h = xh, ci = xci, nch = xnch, T = xT;
                     const KVT* kbase = reinterpret_cast<const KVT*>(a.ckv) + (size_t)l * a.Mcap * 2 * D + xoff;
-                    const int64_t ld = a.ckv_hm ? 128 : 2 * (int64_t)D;
-                    const int voff = a.ckv_hm ? 64 : D;
-                    auto kp = [&](int j) { return kbase + j * ld; };
-                    auto vp = [&](int j) { return kbase + j * ld + voff; };
-                    // keys j == ci*NW + warp (mod nch*NW)
+                    // keys j == ci*NW + warp (mod nch*NW); the contiguous head-major block arrives in 8-key batches by bulk copy into
+                    // this warp's ring (shared with the logits stage)
                     AttnAcc A;
-                    if (a.ckv_hm) {   // contiguous head-major block: 8-key batches by bulk copy into this warp's ring (shared with the logits stage)
-                        attn_warp_bulk<KV_STG, KVT, true>(q2_s + h * 64, kbase, T, ci * NW + warp, nch * NW, 0, ring + (size_t)warp * RINGW,
-                                                          kv_bar + warp * KV_STG, kv_count, A, true, ckv_policy());
-                    } else {
-                        attn_warp(q2_s + h * 64, T, ci * NW + warp, nch * NW, kp, vp, A, -1);
-                    }
+                    attn_warp_bulk<KV_STG, KVT, true>(q2_s + h * 64, kbase, T, ci * NW + warp, nch * NW, 0, ring + (size_t)warp * RINGW,
+                                                      kv_bar + warp * KV_STG, kv_count, A, true, ckv_policy());
                     if (l == L - 1 && want_logits) {   // the ring is free until the next position: first vocabulary half-tiles of this warp
                         __syncwarp();
                         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads of the ring before the bulk copies
@@ -652,7 +641,7 @@ dec4_kernel(const Dec3Args a) {
                     }
                     if (lane < 4) {
 #pragma unroll
-                        for (int c = 0; c < 16; ++c) wo[warp * 64 + (a.ckv_hm ? attn_bulk_dim<KVT>(lane, c) : lane * 16 + c)] = A.o[c];
+                        for (int c = 0; c < 16; ++c) wo[warp * 64 + attn_bulk_dim<KVT>(lane, c)] = A.o[c];
                     }
                     if (lane == 0) { wm[warp] = A.m; wl[warp] = A.l; }
                     __syncthreads();
@@ -710,7 +699,7 @@ dec4_kernel(const Dec3Args a) {
                 if (l == L - 1 && want_logits && rank == 0 && warp == 0) {   // this warp publishes the row: final LayerNorm next
                     ln_fetch<D, PF>(lnp, a.lnf_g, a.lnf_b, l2_policy_evict_last());
                 } else {   // LN1 of the next layer, or of layer 0 for the next position
-                    const Dec3Layer& Wn = a.layers[l + 1 < L ? l + 1 : 0];
+                    const DecLayer& Wn = a.layers[l + 1 < L ? l + 1 : 0];
                     ln_fetch<D, PF>(lnp, Wn.ln1_g, Wn.ln1_b, l2_policy_evict_last());
                 }
                 WB_FINE();
@@ -977,78 +966,22 @@ size_t dec4_smem() {
            (size_t)NW * std::max(LG_NBUF * LG_RB * D * 2, KV_STG * 8 * 128 * 4) + NW * LG_NBUF * 8 + NW * KV_STG * 8 + 8 * 8 + (size_t)2 * (D / 32) * 32 * 16 + 16;
 }
 
-struct LaunchState4 {
-    int clusters = 0;        // 0 unknown, > 0 co-resident clusters to launch, -1 unsupported
-    bool cooperative = true; // cooperative + cluster launch: the driver enforces the co-residency the grid barriers need
-};
-std::mutex g_mu4;
-
 template <int D, int RC, typename KVT>
-bool launch4_t(const Dec3Args& a, cudaStream_t st) {
-    auto k = dec4_kernel<D, RC, KVT>;
+bool launch4_t(const DecArgs& a, cudaStream_t st) {
+    const void* k = (const void*)dec4_kernel<D, RC, KVT>;
     const size_t smem = dec4_smem<D, RC>();
-    static LaunchState4 states[16];   // per device ordinal
-    int dev = 0;
-    WB_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 16) return false;
-    std::lock_guard<std::mutex> lock(g_mu4);
-    LaunchState4& S = states[dev];
-    cudaLaunchConfig_t cfg{};
-    cfg.blockDim = dim3(NT);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CS;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeCooperative;
-    attr[1].val.cooperative = 1;
-    cfg.attrs = attr;
-    if (S.clusters == 0) {
-        if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
-            cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) {
-            cudaGetLastError();
-            S.clusters = -1;
-            return false;
-        }
-        int n_clusters = 0;
-        cfg.gridDim = dim3(CS);
-        cfg.numAttrs = 1;
-        const cudaError_t oe = cudaOccupancyMaxActiveClusters(&n_clusters, k, &cfg);
-        if (getenv("WB200_VERBOSE")) fprintf(stderr, "[wb] dec4<D=%d,RC=%d>: smem %zu B, max active clusters %d (%s)\n", D, RC, smem, n_clusters, cudaGetErrorString(oe));
-        if (oe != cudaSuccess || n_clusters < 1) {
-            cudaGetLastError();
-            S.clusters = -1;
-            return false;
-        }
-        S.cooperative = getenv("WB200_NO_COOP") == nullptr;   // profilers cannot replay cooperative cluster launches
-        S.clusters = std::min(n_clusters, 8);   // every launched cluster must be co-resident (grid barriers)
-    }
-    if (S.clusters < 0 || a.R > S.clusters) return false;
-    cfg.gridDim = dim3(S.clusters * CS);
-    cudaError_t e = cudaErrorUnknown;
-    if (S.cooperative) {
-        cfg.numAttrs = 2;
-        e = cudaLaunchKernelEx(&cfg, k, a);
-        if (e != cudaSuccess) {   // cooperative + cluster rejected by this driver: plain cluster launch (co-residency from the occupancy query)
-            cudaGetLastError();
-            S.cooperative = false;
-        }
-    }
-    if (!S.cooperative) {
-        cfg.numAttrs = 1;
-        e = cudaLaunchKernelEx(&cfg, k, a);
-    }
-    WB_CUDA(e);
-    WB_LAUNCH_CHECK();
+    static ClusterLaunch cl;   // per instantiation
+    const int n_cl = std::min(cl.capacity(k, CS, NT, smem, "dec4"), 8);   // one cluster per row, at most 8
+    if (n_cl < 1 || a.R > n_cl) return false;
+    void* args[] = {(void*)&a};
+    cl.launch(k, CS, n_cl, NT, smem, args, st, "dec4");
     return true;
 }
 
 }  // namespace
 
-// Returns false when this configuration is not covered (caller falls back to decoder3.cu).
-bool launch_dec4(const Dec3Args& a, bool w_half, cudaStream_t st) {
+// Returns false when this configuration is not covered.
+bool launch_dec4(const DecArgs& a, bool w_half, cudaStream_t st) {
     if (!w_half || a.R > 8 || a.R < 1 || a.k != 1 || !a.greedy || a.use_cur_tok || a.anc != nullptr || a.logits_out != nullptr) return false;
     if (a.H * 64 != a.d || a.H > CS || a.E_tiled == nullptr) return false;
 #define WB_D4(DD)                                                                                         \

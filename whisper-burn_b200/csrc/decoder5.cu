@@ -20,7 +20,7 @@
 //     partial sums are folded into x, in a fixed order, by the LayerNorm stage that consumes x next (only CTA r
 //     touches row r there, so the fold is in place).  The d x d projections (out, cross query, cross out) run the same way
 //     as d/256 slabs of 256 columns when that still fits one round of the grid (small.en: 144 items instead of 48, a third of
-//     the staging per CTA); the cross query's partials are folded where the attention stage loads q (session.cu builds the
+//     the staging per CTA); the cross query's partials are folded where the attention stage loads q (dec5_build_tables builds the
 //     descriptors; the producers of the staged planes write them slab-major);
 //   * cross attention streams the unit's contiguous head-major K/V block (encoder.cu ckv_relayout_kernel) with 4 KB bulk
 //     copies (8 fp32 / 16 fp16 keys) into a per-warp mbarrier ring that aliases the (then dead) activation planes;
@@ -31,7 +31,7 @@
 // Code size matters: the layer loop must stay inside the instruction cache, so every building block (staging,
 // MMA tile, emit, attention) exists ONCE and the stages are driven by small descriptors (the first version
 // inlined six copies and ran 3x slower than its memory traffic explains).
-// Requirements: fp16-exact weights, d % 256 == 0, d <= 1280, R <= 32 per launch (the session runs larger batches -- beams of many
+// Requirements: fp16-exact weights, d % 256 == 0, d <= 1280, R <= 32 per launch (launch_dec5 runs larger batches -- beams of many
 // windows -- as row groups of 32, one launch each, a.kv_row0 = first cache row of the group).  Everything else falls back to decoder3.cu.
 #include <cooperative_groups.h>
 #include <cuda_fp16.h>
@@ -102,7 +102,7 @@ enum { SL_LN1 = 0, SL_QKV, SL_SELF, SL_OUT, SL_LN2, SL_CQ, SL_CROSS, SL_COUT, SL
 
 template <int NT8, typename KVT>
 __global__ void __launch_bounds__(NT, 1)
-dec5_kernel(const Dec3Args a) {
+dec5_kernel(const DecArgs a) {
     extern __shared__ __align__(16) float sm[];
     const int d = a.d, H = a.H, L = a.L, V = a.V, R = a.R, t_max = a.t_max;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -273,45 +273,33 @@ dec5_kernel(const Dec3Args a) {
                             *reinterpret_cast<float4*>(qs + grp * 64 + gt * 4) = q4;
                         }
                         bar_named(1 + grp, 128);
-                        int nk = p + 1, swz = -1;
-                        const KVT* kbase = nullptr;
-                        const int* anc = nullptr;
-                        if (is_cross) {
+                        int nk = p + 1;
+                        AttnAcc A;
+                        if (is_cross) {   // contiguous head-major block: 8-key batches by bulk copy into this warp's ring (aliases the planes, dead here)
                             const int w = __ldcg(a.row_window + r);
                             const int T = a.win_T[w];
                             const int per = (T + S - 1) / S;
                             const int kb0 = sp * per;
                             nk = max(0, min(T, kb0 + per) - kb0);
-                            swz = a.ckv_hm ? kb0 : -1;
-                            kbase = ckvl + a.win_row_off[w] * (int64_t)(2 * d) + (a.ckv_hm ? ((int64_t)h * T + kb0) * 128 : kb0 * (int64_t)(2 * d) + h * 64);
-                        } else {
-                            anc = a.anc ? a.anc + (int64_t)r * t_max : nullptr;
-                        }
-                        const int64_t ld = a.ckv_hm ? 128 : 2 * (int64_t)d;
-                        const int voff = a.ckv_hm ? 64 : d;
-                        auto kp = [&](int j) -> const KVT* {
-                            if (is_cross) return kbase + j * ld;
-                            const int rr = (anc && j < p) ? __ldcg(anc + j) : r + a.kv_row0;
-                            return kcl + ((int64_t)rr * t_max + j) * d + h * 64;
-                        };
-                        auto vp = [&](int j) -> const KVT* {
-                            if (is_cross) return kbase + j * ld + voff;
-                            const int rr = (anc && j < p) ? __ldcg(anc + j) : r + a.kv_row0;
-                            return vcl + ((int64_t)rr * t_max + j) * d + h * 64;
-                        };
-                        AttnAcc A;
-                        const bool bulk = is_cross && a.ckv_hm;
-                        if (bulk) {   // contiguous head-major block: 8-key batches by bulk copy into this warp's ring (aliases the planes, dead here)
-                            attn_warp_bulk<KV_STG, KVT>(qs + grp * 64, kbase, nk, wg, 4, swz, reinterpret_cast<unsigned char*>(sm) + warp * RING_W,
+                            const KVT* kbase = ckvl + a.win_row_off[w] * (int64_t)(2 * d) + ((int64_t)h * T + kb0) * 128;
+                            attn_warp_bulk<KV_STG, KVT>(qs + grp * 64, kbase, nk, wg, 4, kb0, reinterpret_cast<unsigned char*>(sm) + warp * RING_W,
                                                         kv_bar + warp * KV_STG, kv_count, A);
-                        } else if constexpr (sizeof(KVT) == 4) {
-                            attn_warp(qs + grp * 64, nk, wg, 4, kp, vp, A, swz);
                         } else {
-                            attn_warp_ring<RING_W / 2048>(qs + grp * 64, nk, wg, 4, kp, vp, reinterpret_cast<uint4*>(sm) + warp * (RING_W / 16), A, swz);
+                            const int* anc = a.anc ? a.anc + (int64_t)r * t_max : nullptr;
+                            auto kp = [&](int j) -> const KVT* {
+                                const int rr = (anc && j < p) ? __ldcg(anc + j) : r + a.kv_row0;
+                                return kcl + ((int64_t)rr * t_max + j) * d + h * 64;
+                            };
+                            auto vp = [&](int j) -> const KVT* {
+                                const int rr = (anc && j < p) ? __ldcg(anc + j) : r + a.kv_row0;
+                                return vcl + ((int64_t)rr * t_max + j) * d + h * 64;
+                            };
+                            if constexpr (sizeof(KVT) == 4) attn_warp(qs + grp * 64, nk, wg, 4, kp, vp, A);
+                            else attn_warp_ring<RING_W / 2048>(qs + grp * 64, nk, wg, 4, kp, vp, reinterpret_cast<uint4*>(sm) + warp * (RING_W / 16), A);
                         }
                         if (lane < 4) {
 #pragma unroll
-                            for (int c = 0; c < 16; ++c) wo[warp * 64 + (bulk ? attn_bulk_dim<KVT>(lane, c) : lane * 16 + c)] = A.o[c];
+                            for (int c = 0; c < 16; ++c) wo[warp * 64 + (is_cross ? attn_bulk_dim<KVT>(lane, c) : lane * 16 + c)] = A.o[c];
                         }
                         if (lane == 0) { wm[warp] = A.m; wl[warp] = A.l; }
                         bar_named(1 + grp, 128);
@@ -868,7 +856,7 @@ size_t dec5_smem_bytes(int d, int NT8, int L) {
 }
 
 template <int NT8, typename KVT>
-bool launch5_t(const Dec3Args& a, int n_ctas, cudaStream_t st) {
+bool launch5_t(const DecArgs& a, int n_ctas, cudaStream_t st) {
     const size_t smem = dec5_smem_bytes(a.d, NT8, a.L);
     auto k = dec5_kernel<NT8, KVT>;
     static PerDeviceConfig cfg;   // per instantiation
@@ -888,12 +876,11 @@ bool launch5_t(const Dec3Args& a, int n_ctas, cudaStream_t st) {
     return true;
 }
 
-}  // namespace
-
-size_t dec5_plane_uint4(int d) { return (size_t)PL_ROWS * d / 8; }   // uint4 per global plane (one K slab of d columns)
-
-// Returns false when this configuration is not covered (caller falls back to decoder3.cu).
-bool launch_dec5(const Dec3Args& a, int n_ctas, bool w_half, cudaStream_t st) {
+// one launch of <= 32 rows; false when the configuration is not covered.  The split stage table serves launches whose cross
+// attention is NOT split over keys (n_splits == 1: at least one (row, head) unit per SM, the batched shapes the split is for);
+// small batches keep the unsplit stages, whose cross-out staging merges the key-split partials over all d columns.
+bool launch5(DecArgs a, const Dec5Tables& t, int n_ctas, bool w_half, cudaStream_t st) {
+    a.d5 = (a.n_splits == 1 && t.split.p != nullptr) ? t.split.p : t.unsplit.p;
     if (!w_half || a.R < 1 || a.R > 32 || a.d % 256 != 0 || a.d > 1280 || a.H * 64 != a.d || n_ctas < 32) return false;
     if (a.lgbuf == nullptr || a.ypart == nullptr || a.att_pl == nullptr || a.hid_pl == nullptr || a.d5 == nullptr || a.lg_slices < 1 || a.k > DEC5_KC) return false;
     if (a.n_splits > 16 || (size_t)a.R * a.H * a.n_splits > (size_t)NW * ((a.R + 7) / 8) * 8 * RED_LD) return false;   // cross-merge weights live in the reduction buffer
@@ -904,6 +891,87 @@ bool launch_dec5(const Dec3Args& a, int n_ctas, bool w_half, cudaStream_t st) {
     if (nt8 == 3) return WB_D5(3);
     return WB_D5(4);
 #undef WB_D5
+}
+
+}  // namespace
+
+size_t dec5_plane_uint4(int d) { return (size_t)PL_ROWS * d / 8; }   // uint4 per global plane (one K slab of d columns)
+
+void dec5_build_tables(const Model& m, int n_sm, Dec5Tables& t) {
+    if (!m.fp16_exact) return;
+    const int d = m.dims.n_text_state, L = m.dims.n_text_layer, V = m.dims.n_vocab;
+    auto gemm = [&](Dec5Desc& q, const void* Wp, const float* bias, int N, int n_slabs, int stage, int emit, int src) {
+        q.kind = D5_KIND_GEMM; q.W = Wp; q.bias = bias; q.N = N; q.n_slabs = n_slabs; q.stage = stage; q.emit = emit; q.src = src; q.ks = d;
+    };
+    auto ln = [&](Dec5Desc& q, const LayerNormW& w, int stage) {
+        q.kind = D5_KIND_LN; q.g = w.g; q.b = w.b; q.eps = w.eps; q.stage = stage; q.ks = d;
+    };
+    // The d x d projections (out, cross query, cross out) have only d/16 feature tiles -- 48 of 132 CTAs busy for small.en, each
+    // staging all K columns of every row.  When d/256 slabs x d/16 tiles still fit ONE round of the grid, they run as K slabs of
+    // 256 columns (one 32-column chunk per warp): three times the CTAs, a third of the staging each; the partial sums go to
+    // ypart and are folded, in a fixed order, by the consumer (the next LayerNorm stage / the cross-attention query load).
+    const int psl = d / 256;
+    const bool can_split = d % 256 == 0 && psl >= 2 && psl <= 4 && (d / 16) * psl <= n_sm;
+    auto build = [&](bool split_dd, DevBuf<Dec5Desc>& dst) {
+        std::vector<Dec5Desc> ds((size_t)L * 16 + 16);
+        for (int l = 0; l < L; ++l) {
+            const DecBlockW& B = m.dec[(size_t)l];
+            Dec5Desc* q = ds.data() + (size_t)l * 16;
+            ln(q[0], B.attn_ln, l == 0 ? D5_ST_LN_EMB : D5_ST_LN_FOLD);
+            gemm(q[1], B.qkv.w16, B.qkv.b, 3 * d, 1, D5_ST_PLANES, D5_EM_QKV, 3);
+            q[2].kind = D5_KIND_ATTN;
+            gemm(q[3], B.out.w16, B.out.b, d, 1, D5_ST_PLANES, D5_EM_RESID, 1);
+            ln(q[4], B.cross_ln, D5_ST_LN_X);
+            gemm(q[5], B.cq.w16, B.cq.b, d, 1, D5_ST_PLANES, D5_EM_CQ, 3);
+            q[6].kind = D5_KIND_ATTN;
+            gemm(q[7], B.cout.w16, B.cout.b, d, 1, D5_ST_CROSS, D5_EM_RESID, 1);
+            ln(q[8], B.mlp_ln, D5_ST_LN_X);
+            gemm(q[9], B.mlp1.w16, B.mlp1.b, 4 * d, 1, D5_ST_PLANES, D5_EM_HID, 3);
+            gemm(q[10], B.mlp2.w16, B.mlp2.b, d, 4, D5_ST_PLANES, D5_EM_PART, 2);
+            // MLP2 K = 4d: 3 slabs of 4d/3 when that keeps the 8-warp K split (multiple of 256, <= 1280): d/16 tiles x 3 slabs
+            // = 144 items for small.en -> fewer rounds than 192 items
+            if ((4 * d) % 3 == 0 && (4 * d / 3) % 256 == 0 && 4 * d / 3 <= 1280) { q[10].n_slabs = 3; q[10].ks = 4 * d / 3; }
+            if (split_dd) {
+                for (int sl : {3, 5, 7}) { q[sl].n_slabs = psl; q[sl].ks = 256; q[sl].emit = D5_EM_PART; }
+                q[4].stage = D5_ST_LN_FOLD; q[4].n_fold = psl; q[4].ks = 256;   // folds the out projection, feeds the split cross query
+                q[8].stage = D5_ST_LN_FOLD; q[8].n_fold = psl;                  // folds the cross out projection
+            }
+            if (l > 0) q[0].n_fold = q[10].n_slabs;                             // folds MLP2 of the previous layer
+        }
+        ln(ds[(size_t)L * 16 + 11], m.dec_ln, D5_ST_LN_FOLD_NOPUB);
+        ds[(size_t)L * 16 + 11].n_fold = ds[(size_t)(L - 1) * 16 + 10].n_slabs;
+        gemm(ds[(size_t)L * 16 + 12], m.tok_emb16, nullptr, V, 1, D5_ST_PLANES, D5_EM_LOGITS, 3);
+        dst.alloc(ds.size());
+        WB_CUDA(cudaMemcpy(dst.p, ds.data(), ds.size() * sizeof(Dec5Desc), cudaMemcpyHostToDevice));
+    };
+    build(false, t.unsplit);
+    if (can_split) build(true, t.split);
+}
+
+int launch_dec5(const DecArgs& a, const Dec5Tables& t, int n_ctas, bool w_half, cudaStream_t st) {
+    if (a.R <= 32) return launch5(a, t, n_ctas, w_half, st) ? 1 : 0;
+    // more rows than one launch takes (beams of many windows, BASELINE configs[4]: 48 windows x 5 beams per GPU): row groups
+    // of 32, one launch each on the stream; rows are independent, ancestry entries stay absolute cache rows (kv_row0 = first
+    // cache row of the group)
+    if (!w_half || a.d % 256 != 0 || a.d > 1280 || a.k > DEC_KC) return 0;
+    int gi = 0;
+    for (int r0 = 0; r0 < a.R; r0 += 32, ++gi) {
+        const int Rg = std::min(32, a.R - r0), d = a.d;
+        DecArgs g = a;
+        g.R = Rg; g.kv_row0 = r0;
+        g.x += (int64_t)r0 * d; g.q += (int64_t)r0 * d; g.att += (int64_t)r0 * d; g.hid += (int64_t)r0 * 4 * d;
+        g.row_window += r0;
+        if (g.anc) g.anc += (int64_t)r0 * a.t_max;
+        g.tokens += (int64_t)r0 * a.t_max; g.cur_tok += r0; g.lengths += r0; g.finished += r0;
+        g.topk_id += (int64_t)r0 * a.k; g.topk_lp += (int64_t)r0 * a.k;
+        if (g.logits_out) { g.logits_out += (int64_t)r0 * a.V; g.lgbuf = g.logits_out; }
+        g.lg_slices = std::max(1, std::min(16, n_ctas / std::max(1, Rg)));
+        g.n_splits = std::max(1, std::min(16, n_ctas / std::max(1, Rg * a.H)));
+        g.steps_done += std::min(gi, 127); g.n_unfinished += std::min(gi, 127);
+        WB_CUDA(cudaMemsetAsync(a.bar, 0, 4 * sizeof(unsigned int), st));
+        if (!launch5(g, t, n_ctas, true, st)) fail(WB_ERR_UNSUPPORTED, "decoder5 rejected a row group");
+    }
+    return gi;
 }
 
 }  // namespace wb

@@ -5,17 +5,17 @@
 // the per-layer chain is cut from 8 cluster-wide stages (decoder4.cu) to THREE exchanges, and every linear layer runs on the
 // tensor cores (Hopper warpgroup MMA):
 //
-//   one thread-block cluster of CS = H * HS CTAs owns one batch row; CTA (h, hs) owns attention head h.
+//   one thread-block cluster of CS = H CTAs owns one batch row; CTA h owns attention head h.
 //   phase 1  x -> LN1 -> q_h | k_h | v_h (192 weight rows) -> causal self attention of head h -> the head's K-slice of the
 //            out projection: y = Wo[:, 64h..64h+64) . o_h   (a partial d-vector)
-//   phase 2  x -> LN2 -> cross query of head h -> cross attention of head h over its share of the window's keys
+//   phase 2  x -> LN2 -> cross query of head h -> cross attention of head h over the window's keys
 //            (head-major K/V block streamed by bulk copies) -> y = Wco[:, 64h..) . o_h (un-normalised, with its (max, sum))
 //   phase 3  x -> LN3 -> a 4d/CS slice of the MLP hidden layer (GELU) -> y = W2[:, slice] . hid_slice
 //   after each phase every CTA sends its partial record (y, max, sum) to ALL CTAs of the cluster with ONE bulk shared-memory ->
 //   distributed-shared-memory copy per destination (cp.async.bulk.shared::cluster.shared::cta) that signals the destination's
-//   mbarrier with complete_tx; the receiver adds bias + the weighted partials (softmax merge of the key splits happens here,
-//   in a fixed order, identically in every CTA) and owns a full copy of the residual stream again.  No hardware cluster barrier
-//   inside the step, no cross-thread release/acquire chains: data and its "ready" signal travel together.
+//   mbarrier with complete_tx; the receiver adds bias + the weighted partials (an attention record weighted by 1 / its
+//   softmax sum; in a fixed order, identically in every CTA) and owns a full copy of the residual stream again.  No hardware
+//   cluster barrier inside the step, no cross-thread release/acquire chains: data and its "ready" signal travel together.
 //
 //   Linear layers = swap-AB wgmma.mma_async (m64n8k16, fp16 operands, fp32 accumulate; M = weight rows): the weight slices of
 //   this CTA are pre-packed per (layer, CTA) as 128-row x 64-column slabs in the canonical K-major 128B-swizzled shared-memory
@@ -37,9 +37,7 @@
 // Everything else is handled by decoder5.cu / decoder3.cu.
 #include <cooperative_groups.h>
 
-#include <cstdio>
 #include <cstdlib>
-#include <mutex>
 
 #include "dec_common.cuh"
 #include "wgmma.cuh"
@@ -59,9 +57,9 @@ constexpr int NSLOT = 8;
 constexpr int LG_NBUF = 2;                // logits stage: ring slots per warp (aliases the weight ring)
 constexpr int BX_SLAB = 1024;             // B operand: 8 rows x 128 bytes (one swizzle atom) per 64-column slab
 
-template <int D, int HS>
+template <int D>
 struct Geo {
-    static constexpr int H = D / 64, CS = H * HS, NS = 4 * D / CS, SEND = D + 4;
+    static constexpr int H = D / 64, CS = H, NS = 4 * D / CS, SEND = D + 4;
     static constexpr int pad128(int n) { return (n + 127) / 128 * 128; }
     // packed weight segments of one (layer, rank), bytes: [tiles of 128 rows (the last one 64 rows when N % 128 == 64)][K / 64 slabs][rows x 128 B]
     static constexpr int OFF_QKV = 0, OFF_O = OFF_QKV + 192 * D * 2, OFF_CQ = OFF_O + D * 64 * 2, OFF_CO = OFF_CQ + 64 * D * 2,
@@ -339,7 +337,7 @@ __device__ __noinline__ void ln6(const float* x_s, const float* g, const float* 
 
 // merges the 8 per-warp attention records (wm, wl, wo) into the head's un-normalised output, written as the B operand of the
 // out projection, and its (max, sum) record
-__device__ __noinline__ void attn_merge6(const float* wm, const float* wl, const float* wo, uint8_t* bx, float* rec, float active) {
+__device__ __noinline__ void attn_merge6(const float* wm, const float* wl, const float* wo, uint8_t* bx, float* rec) {
     const int tid = threadIdx.x;
     bar_consumers();
     if (tid < 64) {
@@ -354,39 +352,24 @@ __device__ __noinline__ void attn_merge6(const float* wm, const float* wl, const
             o += sc * wo[w2 * 64 + tid];
         }
         bx_store(bx, tid, o);
-        if (tid == 0) { rec[0] = M; rec[1] = Ls; rec[2] = active; rec[3] = 0.0f; }
+        if (tid == 0) { rec[0] = M; rec[1] = Ls; }
     }
 }
 
 enum { MODE_SUM = 0, MODE_ATTN = 1 };
 
 // x += bias + sum over sources of weight * partial (fixed order, identical in every CTA of the cluster).  pr = the phase's
-// records [CS][D + 4] (y, max, sum, active); MODE_ATTN: softmax merge of the key splits of each head on the receiving side
-// (mod.rs:516-527 computed in pieces); MODE_SUM: plain sum.  Ends with a barrier.
-template <int D, int HS>
+// records [CS][D + 4] (y, max, sum, unused); MODE_ATTN: y is head h's un-normalised attention output projected by its slice
+// of the out projection, weight 1 / sum (mod.rs:516-527); MODE_SUM: plain sum.  Ends with a barrier.
+template <int D>
 __device__ __noinline__ void combine6(const float* pr, uint64_t* bar, uint32_t parity, int mode, const float* bias, float* x_s, float* wsrc_s) {
-    constexpr int H = D / 64, CS = H * HS, SEND = D + 4;
+    constexpr int CS = Geo<D>::CS, SEND = Geo<D>::SEND;
     const int tid = threadIdx.x;
     if (tid == 0) mbar_expect_tx(bar, CS * SEND * 4);
     mbar_wait(bar, parity);
     if (tid < CS) {
-        float wgt = 1.0f;
-        if (mode == MODE_ATTN) {
-            const int hh = tid % H;
-            float M = -INFINITY;
-#pragma unroll
-            for (int s = 0; s < HS; ++s)
-                if (pr[(hh + H * s) * SEND + D + 2] != 0.0f) M = fmaxf(M, pr[(hh + H * s) * SEND + D]);
-            float den = 0.0f;
-#pragma unroll
-            for (int s = 0; s < HS; ++s) {
-                const float* rec = pr + (hh + H * s) * SEND + D;
-                if (rec[2] != 0.0f && rec[0] > -INFINITY) den += expf(rec[0] - M) * rec[1];
-            }
-            const float* me = pr + tid * SEND + D;
-            wgt = (me[2] != 0.0f && me[0] > -INFINITY) ? __fdiv_rn(expf(me[0] - M), den) : 0.0f;
-        }
-        wsrc_s[tid] = wgt;
+        const float* me = pr + tid * SEND + D;
+        wsrc_s[tid] = mode == MODE_SUM ? 1.0f : me[0] > -INFINITY ? __fdiv_rn(1.0f, me[1]) : 0.0f;
     }
     bar_consumers();
 #pragma unroll 1
@@ -442,13 +425,13 @@ __device__ __noinline__ void self_attn6(const float* qkv_s, const KVT* kbase, co
     }
 }
 
-// cross attention of one head over keys [k_begin, k_end) of the window (mod.rs:482-490), the head-major K/V block arriving through
+// cross attention of one head over the T keys of the window (mod.rs:482-490), the head-major K/V block arriving through
 // the ring in chunks of KPC keys; 8 lanes per key.  A slot is released by the LAST of the 8 warps to finish with it (the slots'
 // empty barriers take one arrival, as the MMA warpgroup gives them for weight slabs).  (Waiting for several chunks at once to batch
 // the per-key latency chains was measured SLOWER, 6 -> 12 us per layer: the chunks arrive one per ~0.3 us and the batch waits for
 // the last one.)  Returns the ring counter.
 template <typename KVT>
-__device__ __noinline__ uint32_t cross_attn6(const Pipe P, uint32_t n, int* slot_cnt, const float* q2_s, int k_begin, int k_end, float* wm, float* wl, float* wo) {
+__device__ __noinline__ uint32_t cross_attn6(const Pipe P, uint32_t n, int* slot_cnt, const float* q2_s, int T, float* wm, float* wl, float* wo) {
     constexpr int ROWB = 128 * (int)sizeof(KVT), KPC = SLOT / ROWB;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, rg = lane >> 3, l8 = lane & 7;
     float q[8];
@@ -457,8 +440,8 @@ __device__ __noinline__ uint32_t cross_attn6(const Pipe P, uint32_t n, int* slot
     Softmax8 A;
     A.init();
 #pragma unroll 1
-    for (int k0 = k_begin; k0 < k_end; k0 += KPC) {
-        const int nk = min(KPC, k_end - k0);
+    for (int k0 = 0; k0 < T; k0 += KPC) {
+        const int nk = min(KPC, T - k0);
         const uint32_t slot = n % NSLOT;
         mbar_wait(P.full + slot, (n / NSLOT) & 1);
         const uint8_t* blk = P.ring + slot * SLOT;
@@ -497,18 +480,18 @@ __device__ __noinline__ uint32_t cross_attn6(const Pipe P, uint32_t n, int* slot
 }
 
 // =====================================================================================================================
-template <int D, int HS, int NT8, typename KVT>
+template <int D, int NT8, typename KVT>
 __global__ void __launch_bounds__(NTH6, 1)
-dec6_kernel(const Dec3Args a) {
-    using G = Geo<D, HS>;
-    constexpr int H = G::H, CS = G::CS, NS = G::NS, SEND = G::SEND, PARAMS = G::PARAMS;
+dec6_kernel(const DecArgs a) {
+    using G = Geo<D>;
+    constexpr int CS = G::CS, NS = G::NS, SEND = G::SEND, PARAMS = G::PARAMS;
     constexpr int KPC = SLOT / (128 * (int)sizeof(KVT));   // cross keys per ring chunk
     constexpr int ROWB = 128 * (int)sizeof(KVT);
     extern __shared__ __align__(1024) unsigned char smraw_[];
     uint8_t* smraw = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smraw_) + 1023) & ~(uintptr_t)1023);
     cg::cluster_group cl = cg::this_cluster();
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int rank = (int)cl.block_rank(), h = rank % H, hs = rank / H;
+    const int rank = (int)cl.block_rank(), h = rank;
     const int cluster_id = blockIdx.x / CS, n_clusters = gridDim.x / CS;
     const int L = a.L, V = a.V, R = a.R, t_max = a.t_max;
 
@@ -575,7 +558,6 @@ dec6_kernel(const Dec3Args a) {
                 for (int row = cluster_id; row < R; row += n_clusters) {
                     const int w = __ldg(a.row_window + row);
                     const int T = __ldg(a.win_T + w);
-                    const int per = (T + HS - 1) / HS, k_begin = min(T, hs * per), k_end = min(T, k_begin + per);
                     for (int l = 0; l < L; ++l) {
                         if (pw == 0) {
                             const uint32_t b = pl & 1, u = pl >> 1;
@@ -592,12 +574,13 @@ dec6_kernel(const Dec3Args a) {
                                 for (int sl = 0; sl < K / 64; ++sl, src += bytes) push(src, bytes);
                             }
                         };
-                        if (hs == 0) { seg(G::OFF_QKV, 192, D); seg(G::OFF_O, D, 64); }
+                        seg(G::OFF_QKV, 192, D);
+                        seg(G::OFF_O, D, 64);
                         seg(G::OFF_CQ, 64, D);
                         {
                             const KVT* kv = reinterpret_cast<const KVT*>(a.ckv) + (size_t)l * a.Mcap * 2 * D + __ldg(a.win_row_off + w) * (int64_t)(2 * D) +
-                                            ((int64_t)h * T + k_begin) * 128;
-                            for (int k0 = k_begin; k0 < k_end; k0 += KPC) push(kv + (int64_t)(k0 - k_begin) * 128, (uint32_t)(min(KPC, k_end - k0) * ROWB));
+                                            (int64_t)h * T * 128;
+                            for (int k0 = 0; k0 < T; k0 += KPC) push(kv + (int64_t)k0 * 128, (uint32_t)(min(KPC, T - k0) * ROWB));
                         }
                         seg(G::OFF_CO, D, 64);
                         seg(G::OFF_W1, NS, D);
@@ -633,7 +616,7 @@ dec6_kernel(const Dec3Args a) {
             }
         };
         auto combine = [&](int mode, const float* bias) {
-            combine6<D, HS>(part + (ph & 1) * CS * SEND, pbar + (ph & 1), (ph >> 1) & 1, mode, bias, x_s, wsrc_s);
+            combine6<D>(part + (ph & 1) * CS * SEND, pbar + (ph & 1), (ph >> 1) & 1, mode, bias, x_s, wsrc_s);
             ++ph;
         };
 
@@ -650,7 +633,6 @@ dec6_kernel(const Dec3Args a) {
                 }
                 const int w = __ldg(a.row_window + row);
                 const int T = __ldg(a.win_T + w);
-                const int per = (T + HS - 1) / HS, k_begin = min(T, hs * per), k_end = min(T, k_begin + per);
                 bar_consumers();
                 trace();
 #pragma unroll 1
@@ -668,31 +650,27 @@ dec6_kernel(const Dec3Args a) {
                     const float* prm = params + (pl & 1) * PARAMS;
                     ++pl;
                     float* ys = y_s + (ph & 1) * SEND;
-                    if (hs == 0) {
-                        ln6<D>(x_s, prm + G::P_LN1G, prm + G::P_LN1B, prm[G::P_EPS + 0], a.eps_outside, bx);
-                        KVT* kd = kcl + ((int64_t)row * t_max + p) * D + h * 64;
-                        KVT* vd = vcl + ((int64_t)row * t_max + p) * D + h * 64;
-                        c = gemv_epi6<KVT>(P, c, 192, S_D, GemvOut<KVT>{EM_QKV, prm + G::P_BQKV, scale, qkv_s, kd, vd});
-                        trace();   // [t2] q | k | v done
-                        self_attn6<KVT>(qkv_s, kcl + (int64_t)row * t_max * D + h * 64, vcl + (int64_t)row * t_max * D + h * 64, D, p, wm, wl, wo);
-                        attn_merge6(wm, wl, wo, bx, ys + D, 1.0f);
-                        trace();   // [t3] self attention done
-                        c = gemv_epi6<KVT>(P, c, D, 1, GemvOut<KVT>{EM_PLAIN, nullptr, 1.0f, ys, nullptr, nullptr});
-                    } else {
-                        for (int c2 = tid; c2 < SEND; c2 += 256) ys[c2] = 0.0f;    // inactive in this phase: weight 0, zeros
-                    }
+                    ln6<D>(x_s, prm + G::P_LN1G, prm + G::P_LN1B, prm[G::P_EPS + 0], a.eps_outside, bx);
+                    KVT* kd = kcl + ((int64_t)row * t_max + p) * D + h * 64;
+                    KVT* vd = vcl + ((int64_t)row * t_max + p) * D + h * 64;
+                    c = gemv_epi6<KVT>(P, c, 192, S_D, GemvOut<KVT>{EM_QKV, prm + G::P_BQKV, scale, qkv_s, kd, vd});
+                    trace();   // [t2] q | k | v done
+                    self_attn6<KVT>(qkv_s, kcl + (int64_t)row * t_max * D + h * 64, vcl + (int64_t)row * t_max * D + h * 64, D, p, wm, wl, wo);
+                    attn_merge6(wm, wl, wo, bx, ys + D);
+                    trace();   // [t3] self attention done
+                    c = gemv_epi6<KVT>(P, c, D, 1, GemvOut<KVT>{EM_PLAIN, nullptr, 1.0f, ys, nullptr, nullptr});
                     trace();   // [t4] out-projection slice done
                     send();
                     trace();   // [t5] sent
-                    // ================= phase 2: x += self-attention output; cross attention of head h over this CTA's keys (mod.rs:347)
+                    // ================= phase 2: x += self-attention output; cross attention of head h (mod.rs:347)
                     combine(MODE_ATTN, prm + G::P_BO);
                     trace();   // [t6] combined
                     ys = y_s + (ph & 1) * SEND;
                     ln6<D>(x_s, prm + G::P_LN2G, prm + G::P_LN2B, prm[G::P_EPS + 1], a.eps_outside, bx);
                     c = gemv_epi6<KVT>(P, c, 64, S_D, GemvOut<KVT>{EM_CQ, prm + G::P_BCQ, scale, q2_s, nullptr, nullptr});
                     trace();   // [t7] cross query done
-                    c.n = cross_attn6<KVT>(P, c.n, slot_cnt, q2_s, k_begin, k_end, wm, wl, wo);
-                    attn_merge6(wm, wl, wo, bx, ys + D, (k_end > k_begin) ? 1.0f : 0.0f);
+                    c.n = cross_attn6<KVT>(P, c.n, slot_cnt, q2_s, T, wm, wl, wo);
+                    attn_merge6(wm, wl, wo, bx, ys + D);
                     trace();   // [t8] cross attention done
                     c = gemv_epi6<KVT>(P, c, D, 1, GemvOut<KVT>{EM_PLAIN, nullptr, 1.0f, ys, nullptr, nullptr});
                     trace();   // [t9]
@@ -707,7 +685,6 @@ dec6_kernel(const Dec3Args a) {
                     for (int c2 = tid; c2 < NS; c2 += 256) bx_store(bx, c2, hid_s[c2]);   // every MMA of the W1 product has completed: the B operand may change
                     trace();   // [t12] hidden slice done
                     c = gemv_epi6<KVT>(P, c, D, S_NS, GemvOut<KVT>{EM_PLAIN, nullptr, 1.0f, ys, nullptr, nullptr});
-                    if (tid == 0) { ys[D] = 0.0f; ys[D + 1] = 1.0f; ys[D + 2] = 1.0f; ys[D + 3] = 0.0f; }
                     trace();   // [t13]
                     send();
                     trace();   // [t14]
@@ -1015,132 +992,74 @@ dec6_kernel(const Dec3Args a) {
     cl.sync();   // no CTA leaves while a peer may still address its shared memory
 }
 
-template <int D, int HS, int NT8>
+template <int D, int NT8>
 constexpr size_t dec6_smem() {
-    using G = Geo<D, HS>;
+    using G = Geo<D>;
     return 1024 + (size_t)NSLOT * SLOT + (size_t)(G::KMAX / 64) * BX_SLAB +
            sizeof(float) * ((size_t)2 * G::PARAMS + 2 * G::CS * G::SEND + 2 * G::SEND + D + 192 + 64 + G::NS + 16 + 8 + 8 + 512 + 4 + NSLOT) +
            8 * (size_t)(2 * NSLOT + 6 + NCW * LG_NBUF) + 64;
 }
 
-struct LaunchState {
-    int clusters = 0;        // 0 unknown, > 0 co-resident clusters to launch, -1 unsupported
-    bool cooperative = true;
-};
-std::mutex g_mu;
-
-template <int D, int HS, int NT8, typename KVT>
-bool launch6_t(const Dec3Args& a, cudaStream_t st) {
-    using G = Geo<D, HS>;
+template <int D, int NT8, typename KVT>
+bool launch6_t(const DecArgs& a, cudaStream_t st) {
+    using G = Geo<D>;
     static_assert((size_t)2 * NT8 * (D / 32) * 32 * 16 + (size_t)NCW * 8 * NT8 * 16 <= sizeof(float) * (2 * G::PARAMS + 2 * G::CS * G::SEND), "logits scratch must fit the aliased buffers");
-    auto k = dec6_kernel<D, HS, NT8, KVT>;
-    const size_t smem = dec6_smem<D, HS, NT8>();
-    static LaunchState state[16];   // per device ordinal
-    static bool wd_set[16] = {};
-    int dev = 0;
-    WB_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 16) return false;
-    std::lock_guard<std::mutex> lock(g_mu);
-    LaunchState& S = state[dev];
-    cudaLaunchConfig_t cfg{};
-    cfg.blockDim = dim3(NTH6);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = G::CS;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeCooperative;
-    attr[1].val.cooperative = 1;
-    cfg.attrs = attr;
-    if (S.clusters == 0) {
-        if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
-            (G::CS > 8 && cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess)) {
-            cudaGetLastError();
-            S.clusters = -1;
-            return false;
-        }
-        int n_clusters = 0;
-        cfg.gridDim = dim3(G::CS);
-        cfg.numAttrs = 1;
-        const cudaError_t oe = cudaOccupancyMaxActiveClusters(&n_clusters, k, &cfg);
-        if (getenv("WB200_VERBOSE")) fprintf(stderr, "[wb] dec6<D=%d,HS=%d,NT8=%d>: smem %zu B, max active clusters %d (%s)\n", D, HS, NT8, smem, n_clusters, cudaGetErrorString(oe));
-        if (oe != cudaSuccess || n_clusters < 1) {
-            cudaGetLastError();
-            S.clusters = -1;
-            return false;
-        }
-        S.clusters = n_clusters;
-    }
-    if (S.clusters < 0) return false;
-    if (!wd_set[dev]) {
+    const void* k = (const void*)dec6_kernel<D, NT8, KVT>;
+    const size_t smem = dec6_smem<D, NT8>();
+    static ClusterLaunch cl;   // per instantiation
+    const int n_cl = cl.capacity(k, G::CS, NTH6, smem, "dec6");
+    if (n_cl < 1) return false;
+    static PerDeviceConfig wd;
+    wd.ensure(1, [] {
         if (const char* e = getenv("WB200_WATCHDOG_MS")) {   // 0 = never trap
             const long long ms = atoll(e);
             const long long cyc = ms <= 0 ? (1LL << 62) : ms * 2000000LL;
             WB_CUDA(cudaMemcpyToSymbol(g_watchdog, &cyc, sizeof(cyc)));
         }
-        wd_set[dev] = true;
-    }
+        return true;
+    });
     // every launched cluster must be co-resident (grid barrier): launch what the device holds; rows beyond that are looped over
-    const int n_cl = S.clusters;
-    cfg.gridDim = dim3(n_cl * G::CS);
-    cudaError_t e = cudaErrorUnknown;
-    if (S.cooperative && getenv("WB200_NO_COOP")) S.cooperative = false;   // profilers cannot replay cooperative cluster launches
-    if (S.cooperative) {
-        cfg.numAttrs = 2;
-        e = cudaLaunchKernelEx(&cfg, k, a);
-        if (e != cudaSuccess) {   // cooperative + cluster rejected by this driver: plain cluster launch (co-residency from the occupancy query)
-            cudaGetLastError();
-            S.cooperative = false;
-            if (getenv("WB200_VERBOSE")) fprintf(stderr, "[wb] dec6: cooperative cluster launch rejected (%s), using a plain cluster launch\n", cudaGetErrorString(e));
-        }
-    }
-    if (!S.cooperative) {
-        cfg.numAttrs = 1;
-        e = cudaLaunchKernelEx(&cfg, k, a);
-    }
-    WB_CUDA(e);
-    WB_LAUNCH_CHECK();
+    void* args[] = {(void*)&a};
+    cl.launch(k, G::CS, n_cl, NTH6, smem, args, st, "dec6");
     return true;
 }
 
-}  // namespace
-
 // ---- host: packed weights / parameter blocks of a model (built once per session) ----------------------------------------------
-template <int D, int HS>
-static void build_pack_t(const std::vector<Dec6LayerSrc>& layers, DevBuf<uint8_t>& pack, DevBuf<float>& params, cudaStream_t st) {
-    using G = Geo<D, HS>;
-    const int L = (int)layers.size();
-    pack.alloc((size_t)L * G::CS * G::PACK);
-    params.alloc((size_t)L * G::CS * G::PARAMS);
+template <int D>
+void build_pack_t(const Model& m, Dec6Pack& pk, cudaStream_t st) {
+    using G = Geo<D>;
+    const int L = m.dims.n_text_layer;
+    pk.pack.alloc((size_t)L * G::CS * G::PACK);
+    pk.params.alloc((size_t)L * G::CS * G::PARAMS);
     std::vector<PackSeg> ps;
     std::vector<ParamSeg> qs;
     std::vector<float> eps_h((size_t)L * 4, 0.0f);
-    for (int l = 0; l < L; ++l) { eps_h[(size_t)l * 4] = layers[(size_t)l].ln1_eps; eps_h[(size_t)l * 4 + 1] = layers[(size_t)l].ln2_eps; eps_h[(size_t)l * 4 + 2] = layers[(size_t)l].ln3_eps; }
+    for (int l = 0; l < L; ++l) {
+        const DecBlockW& B = m.dec[(size_t)l];
+        eps_h[(size_t)l * 4] = B.attn_ln.eps; eps_h[(size_t)l * 4 + 1] = B.cross_ln.eps; eps_h[(size_t)l * 4 + 2] = B.mlp_ln.eps;
+    }
     DevBuf<float> eps_d;
     eps_d.alloc(eps_h.size());
     WB_CUDA(cudaMemcpyAsync(eps_d.p, eps_h.data(), eps_h.size() * sizeof(float), cudaMemcpyHostToDevice, st));
     for (int l = 0; l < L; ++l) {
-        const Dec6LayerSrc& S = layers[(size_t)l];
-        for (int r = 0; r < G::CS; ++r) {
-            const int h = r % G::H;
-            const int64_t base = ((int64_t)l * G::CS + r) * G::PACK;
-            const int64_t pb = ((int64_t)l * G::CS + r) * G::PARAMS;
+        const DecBlockW& B = m.dec[(size_t)l];
+        for (int h = 0; h < G::CS; ++h) {   // CTA h of a cluster owns attention head h
+            const int64_t base = ((int64_t)l * G::CS + h) * G::PACK;
+            const int64_t pb = ((int64_t)l * G::CS + h) * G::PARAMS;
             // q_h | k_h | v_h: three 64-row pieces of the fused [3d][d] matrix, d rows apart
-            ps.push_back(PackSeg{S.Wqkv, D, h * 64, 0, 192, D, 64, D, base + G::OFF_QKV});
-            ps.push_back(PackSeg{S.Wo, D, 0, h * 64, D, 64, D, 0, base + G::OFF_O});
-            ps.push_back(PackSeg{S.Wcq, D, h * 64, 0, 64, D, 64, 0, base + G::OFF_CQ});
-            ps.push_back(PackSeg{S.Wco, D, 0, h * 64, D, 64, D, 0, base + G::OFF_CO});
-            ps.push_back(PackSeg{S.W1, D, r * G::NS, 0, G::NS, D, G::NS, 0, base + G::OFF_W1});
-            ps.push_back(PackSeg{S.W2, 4 * D, 0, r * G::NS, D, G::NS, D, 0, base + G::OFF_W2});
-            qs.push_back(ParamSeg{S.ln1_g, D, pb + G::P_LN1G}); qs.push_back(ParamSeg{S.ln1_b, D, pb + G::P_LN1B});
-            qs.push_back(ParamSeg{S.ln2_g, D, pb + G::P_LN2G}); qs.push_back(ParamSeg{S.ln2_b, D, pb + G::P_LN2B});
-            qs.push_back(ParamSeg{S.ln3_g, D, pb + G::P_LN3G}); qs.push_back(ParamSeg{S.ln3_b, D, pb + G::P_LN3B});
-            qs.push_back(ParamSeg{S.bo, D, pb + G::P_BO}); qs.push_back(ParamSeg{S.bco, D, pb + G::P_BCO}); qs.push_back(ParamSeg{S.b2, D, pb + G::P_B2});
-            for (int part = 0; part < 3; ++part) qs.push_back(ParamSeg{S.bqkv + part * D + h * 64, 64, pb + G::P_BQKV + part * 64});
-            qs.push_back(ParamSeg{S.bcq + h * 64, 64, pb + G::P_BCQ});
-            qs.push_back(ParamSeg{S.b1 + r * G::NS, G::NS, pb + G::P_B1});
+            ps.push_back(PackSeg{B.qkv.w16, D, h * 64, 0, 192, D, 64, D, base + G::OFF_QKV});
+            ps.push_back(PackSeg{B.out.w16, D, 0, h * 64, D, 64, D, 0, base + G::OFF_O});
+            ps.push_back(PackSeg{B.cq.w16, D, h * 64, 0, 64, D, 64, 0, base + G::OFF_CQ});
+            ps.push_back(PackSeg{B.cout.w16, D, 0, h * 64, D, 64, D, 0, base + G::OFF_CO});
+            ps.push_back(PackSeg{B.mlp1.w16, D, h * G::NS, 0, G::NS, D, G::NS, 0, base + G::OFF_W1});
+            ps.push_back(PackSeg{B.mlp2.w16, 4 * D, 0, h * G::NS, D, G::NS, D, 0, base + G::OFF_W2});
+            qs.push_back(ParamSeg{B.attn_ln.g, D, pb + G::P_LN1G}); qs.push_back(ParamSeg{B.attn_ln.b, D, pb + G::P_LN1B});
+            qs.push_back(ParamSeg{B.cross_ln.g, D, pb + G::P_LN2G}); qs.push_back(ParamSeg{B.cross_ln.b, D, pb + G::P_LN2B});
+            qs.push_back(ParamSeg{B.mlp_ln.g, D, pb + G::P_LN3G}); qs.push_back(ParamSeg{B.mlp_ln.b, D, pb + G::P_LN3B});
+            qs.push_back(ParamSeg{B.out.b, D, pb + G::P_BO}); qs.push_back(ParamSeg{B.cout.b, D, pb + G::P_BCO}); qs.push_back(ParamSeg{B.mlp2.b, D, pb + G::P_B2});
+            for (int part = 0; part < 3; ++part) qs.push_back(ParamSeg{B.qkv.b + part * D + h * 64, 64, pb + G::P_BQKV + part * 64});
+            qs.push_back(ParamSeg{B.cq.b + h * 64, 64, pb + G::P_BCQ});
+            qs.push_back(ParamSeg{B.mlp1.b + h * G::NS, G::NS, pb + G::P_B1});
             qs.push_back(ParamSeg{eps_d.p + (size_t)l * 4, 4, pb + G::P_EPS});
         }
     }
@@ -1150,48 +1069,29 @@ static void build_pack_t(const std::vector<Dec6LayerSrc>& layers, DevBuf<uint8_t
     dqs.alloc(qs.size());
     WB_CUDA(cudaMemcpyAsync(dps.p, ps.data(), ps.size() * sizeof(PackSeg), cudaMemcpyHostToDevice, st));
     WB_CUDA(cudaMemcpyAsync(dqs.p, qs.data(), qs.size() * sizeof(ParamSeg), cudaMemcpyHostToDevice, st));
-    dec6_pack_kernel<<<dim3(32, (unsigned)std::min<size_t>(ps.size(), 1024)), 256, 0, st>>>(dps.p, (int)ps.size(), pack.p);
+    dec6_pack_kernel<<<dim3(32, (unsigned)std::min<size_t>(ps.size(), 1024)), 256, 0, st>>>(dps.p, (int)ps.size(), pk.pack.p);
     WB_LAUNCH_CHECK();
-    dec6_param_kernel<<<(unsigned)std::min<size_t>(qs.size(), 2048), 128, 0, st>>>(dqs.p, (int)qs.size(), params.p);
+    dec6_param_kernel<<<(unsigned)std::min<size_t>(qs.size(), 2048), 128, 0, st>>>(dqs.p, (int)qs.size(), pk.params.p);
     WB_LAUNCH_CHECK();
     WB_CUDA(cudaStreamSynchronize(st));   // the descriptor arrays go out of scope
 }
 
-bool dec6_supported(int d, int H) { return (d == 128 || d == 384) && H * 64 == d; }
+}  // namespace
 
-int dec6_pick_hs(int d, int R) {
-    const char* e = getenv("WB200_DEC6_HS");
-    if (e && (e[0] == '1' || e[0] == '2')) return e[0] - '0';
-    (void)d;
-    (void)R;
-    return 1;   // one CTA per head; WB200_DEC6_HS=2 selects the two-CTAs-per-head shape (keys and MLP slices split) for <= 8 rows:
-                // measured 150 vs 178 us per position at 3 rows, both behind decoder4.cu's 131 us, which therefore keeps <= 7 rows
-}
-
-void dec6_build_pack(int d, int hs, const std::vector<Dec6LayerSrc>& layers, DevBuf<uint8_t>& pack, DevBuf<float>& params, cudaStream_t st) {
-    if (d == 384 && hs == 1) build_pack_t<384, 1>(layers, pack, params, st);
-    else if (d == 384 && hs == 2) build_pack_t<384, 2>(layers, pack, params, st);
-    else if (d == 128 && hs == 1) build_pack_t<128, 1>(layers, pack, params, st);
-    else if (d == 128 && hs == 2) build_pack_t<128, 2>(layers, pack, params, st);
-    else fail(WB_ERR_UNSUPPORTED, "dec6: unsupported width");
-}
-
-// Returns false when this configuration is not covered (caller falls back to decoder5.cu / decoder3.cu).
-bool launch_dec6(const Dec3Args& a, int hs, bool w_half, cudaStream_t st) {
-    if (!w_half || a.R > 24 || a.R < 1 || a.k != 1 || !a.greedy || a.use_cur_tok || a.anc != nullptr || a.logits_out != nullptr) return false;
-    if (a.H * 64 != a.d || a.E_tiled == nullptr || a.d6_pack == nullptr || a.d6_params == nullptr || !a.ckv_hm || a.t_max > 128) return false;
-    if (hs == 2 && a.R > 8) return false;
-#define WB_D6(DD, HS_, NT8_) (a.kv_half ? launch6_t<DD, HS_, NT8_, __half>(a, st) : launch6_t<DD, HS_, NT8_, float>(a, st))
-    if (a.d == 384) {
-        if (hs == 2) return WB_D6(384, 2, 1);
-        return a.R <= 8 ? WB_D6(384, 1, 1) : WB_D6(384, 1, 3);
+// Returns false when this configuration is not covered.  The packed weights are built on the first launch.
+bool launch_dec6(DecArgs a, const Model& m, Dec6Pack& pk, cudaStream_t st) {
+    if (!m.fp16_exact || a.R > 24 || a.R < 1 || a.k != 1 || !a.greedy || a.use_cur_tok || a.anc != nullptr || a.logits_out != nullptr) return false;
+    if ((a.d != 128 && a.d != 384) || a.H * 64 != a.d || a.E_tiled == nullptr || a.t_max > 128) return false;
+    if (pk.pack.p == nullptr) {
+        if (a.d == 384) build_pack_t<384>(m, pk, st);
+        else build_pack_t<128>(m, pk, st);
     }
-    if (a.d == 128) {
-        if (hs == 2) return WB_D6(128, 2, 1);
-        return a.R <= 8 ? WB_D6(128, 1, 1) : WB_D6(128, 1, 3);
-    }
+    a.d6_pack = pk.pack.p;
+    a.d6_params = pk.params.p;
+#define WB_D6(DD, NT8_) (a.kv_half ? launch6_t<DD, NT8_, __half>(a, st) : launch6_t<DD, NT8_, float>(a, st))
+    if (a.d == 384) return a.R <= 8 ? WB_D6(384, 1) : WB_D6(384, 3);
+    return a.R <= 8 ? WB_D6(128, 1) : WB_D6(128, 3);
 #undef WB_D6
-    return false;
 }
 
 }  // namespace wb

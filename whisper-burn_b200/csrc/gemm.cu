@@ -30,7 +30,6 @@ struct GemmArgs {
     const float* A;
     const float* B;
     float* C;
-    __half* C16;   // when set, results are rounded to fp16 and stored here instead of C
     const float* bias;
     const float* residual;
     const float* pos;
@@ -139,12 +138,7 @@ gemm_f32_kernel(const GemmArgs g) {
             v[0] = __fadd_rn(r4.x, v[0]); v[1] = __fadd_rn(r4.y, v[1]);
             v[2] = __fadd_rn(r4.z, v[2]); v[3] = __fadd_rn(r4.w, v[3]);
         }
-        if (g.C16) {
-            *reinterpret_cast<__half2*>(g.C16 + co) = __floats2half2_rn(v[0], v[1]);
-            *reinterpret_cast<__half2*>(g.C16 + co + 2) = __floats2half2_rn(v[2], v[3]);
-        } else {
-            *reinterpret_cast<float4*>(g.C + co) = make_float4(v[0], v[1], v[2], v[3]);
-        }
+        *reinterpret_cast<float4*>(g.C + co) = make_float4(v[0], v[1], v[2], v[3]);
     }
 }
 
@@ -153,7 +147,7 @@ gemm_f32_kernel(const GemmArgs g) {
 void launch_gemm(const GemmParams& p, cudaStream_t st) {
     WB_REQUIRE(p.K % BK == 0 && p.N % 4 == 0 && p.lda % 4 == 0 && p.ldc % 4 == 0, "gemm: unsupported shape");
     GemmArgs a;
-    a.A = p.A; a.B = p.B; a.C = p.C; a.C16 = p.C16; a.bias = p.bias; a.residual = p.residual; a.pos = p.pos;
+    a.A = p.A; a.B = p.B; a.C = p.C; a.bias = p.bias; a.residual = p.residual; a.pos = p.pos;
     a.groups = p.groups; a.lda = p.lda; a.ldc = p.ldc; a.N = p.N; a.K = p.K; a.act = p.act;
     a.scale = p.scale; a.scale_cols = p.scale_cols;
     a.single = GemmGroup{0, 0, p.max_rows};

@@ -31,6 +31,10 @@ Session::Session(Model* model, int64_t max_w, int64_t max_b, int64_t max_text_le
     const int d = D.n_audio_state, H = D.n_text_head, L = D.n_text_layer, V = D.n_vocab;
     WB_REQUIRE(max_beams <= DEC_KC - 1, "session: max_beams must be <= 7 (candidates kept per record by the persistent decoders)");
     kmax = DEC_KC;
+    if (const char* e = getenv("WB200_DECODER"); e && e[0]) {   // run every launch on this decoder (comparisons, tests)
+        only_decoder = atoi(e);
+        WB_REQUIRE(only_decoder >= 3 && only_decoder <= 6, "session: WB200_DECODER must be 3, 4, 5 or 6");
+    }
 
     WB_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
     for (auto& e : ev) WB_CUDA(cudaEventCreate(&e));
@@ -68,9 +72,6 @@ Session::Session(Model* model, int64_t max_w, int64_t max_b, int64_t max_text_le
     topk_id.alloc((size_t)Rmax * kmax); topk_lp.alloc((size_t)Rmax * kmax);
     is_special.alloc(V);
     {
-        const char* e = getenv("WB200_DECODER");   // "3": force the grid-barrier FMA fallback (decoder3.cu) for A/B runs
-        if (e && e[0] == '3') dec_version = 3;
-        ckv_hm = true;                             // cross K/V head-major (encoder.cu ckv_relayout_kernel): what the persistent decoders stream
         ckv_tmp.alloc(Mcap * 2 * d);
         cudaDeviceProp prop;
         WB_CUDA(cudaGetDeviceProperties(&prop, m->device));
@@ -78,77 +79,25 @@ Session::Session(Model* model, int64_t max_w, int64_t max_b, int64_t max_text_le
         n_logit_ctas = 2 * prop.multiProcessorCount;
         // persistent decoder: per-layer pointer table, barrier words, larger split-KV partial buffers
         part_o.alloc((size_t)Rmax * H * 16 * 64); part_m.alloc((size_t)Rmax * H * 16); part_l.alloc((size_t)Rmax * H * 16);
-        datt.alloc((size_t)Rmax * d); steps_done.alloc(128); d3_bar.alloc(4);
-        WB_CUDA(cudaMemsetAsync(d3_bar.p, 0, 4 * sizeof(unsigned int), st));
-        { const char* e6 = getenv("WB200_DEC6"); use_dec6 = !(e6 && e6[0] == '0'); force_dec6 = e6 && e6[0] == 'f'; }
+        datt.alloc((size_t)Rmax * d); steps_done.alloc(128); dec_bar.alloc(4);
+        WB_CUDA(cudaMemsetAsync(dec_bar.p, 0, 4 * sizeof(unsigned int), st));
         {
             const bool h16 = m->fp16_exact;
             auto wp = [&](const LinearW& w) -> const void* { return h16 ? (const void*)w.w16 : (const void*)w.w32; };
-            std::vector<Dec3Layer> lay((size_t)L);
+            std::vector<DecLayer> lay((size_t)L);
             for (int l = 0; l < L; ++l) {
                 const DecBlockW& B = m->dec[(size_t)l];
-                Dec3Layer& y = lay[(size_t)l];
+                DecLayer& y = lay[(size_t)l];
                 y.ln1_g = B.attn_ln.g; y.ln1_b = B.attn_ln.b; y.ln1_eps = B.attn_ln.eps;
                 y.ln2_g = B.cross_ln.g; y.ln2_b = B.cross_ln.b; y.ln2_eps = B.cross_ln.eps;
                 y.ln3_g = B.mlp_ln.g; y.ln3_b = B.mlp_ln.b; y.ln3_eps = B.mlp_ln.eps;
                 y.Wqkv = wp(B.qkv); y.Wo = wp(B.out); y.Wcq = wp(B.cq); y.Wco = wp(B.cout); y.W1 = wp(B.mlp1); y.W2 = wp(B.mlp2);
                 y.bqkv = B.qkv.b; y.bo = B.out.b; y.bcq = B.cq.b; y.bco = B.cout.b; y.b1 = B.mlp1.b; y.b2 = B.mlp2.b;
             }
-            d3_layers.alloc((size_t)L);
-            WB_CUDA(cudaMemcpy(d3_layers.p, lay.data(), lay.size() * sizeof(Dec3Layer), cudaMemcpyHostToDevice));
-            if (h16) {   // decoder5.cu stage descriptors
-                auto gemm = [&](Dec5Desc& q, const void* Wp, const float* bias, int N, int n_slabs, int stage, int emit, int src) {
-                    q.kind = D5_KIND_GEMM; q.W = Wp; q.bias = bias; q.N = N; q.n_slabs = n_slabs; q.stage = stage; q.emit = emit; q.src = src; q.ks = d;
-                };
-                auto ln = [&](Dec5Desc& q, const LayerNormW& w, int stage) {
-                    q.kind = D5_KIND_LN; q.g = w.g; q.b = w.b; q.eps = w.eps; q.stage = stage; q.ks = d;
-                };
-                // The d x d projections (out, cross query, cross out) have only d/16 feature tiles -- 48 of 132 CTAs busy for small.en, each
-                // staging all K columns of every row.  When d/256 slabs x d/16 tiles still fit ONE round of the grid, they run as K slabs of
-                // 256 columns (one 32-column chunk per warp): three times the CTAs, a third of the staging each; the partial sums go to
-                // ypart and are folded, in a fixed order, by the consumer (the next LayerNorm stage / the cross-attention query load).
-                const int psl = d / 256;
-                const char* e_split = getenv("WB200_D5_SPLIT");
-                const bool can_split = !(e_split && e_split[0] == '0') && d % 256 == 0 && psl >= 2 && psl <= 4 && (d / 16) * psl <= n_sm;
-                // Two tables: the split one is used by launches whose cross attention is NOT split over keys (n_splits == 1, i.e. at
-                // least one (row, head) unit per SM: the batched shapes the split is for); small batches keep the unsplit stages, whose
-                // cross-out staging merges the key-split partials over all d columns (launch_v3 picks per launch).
-                auto build = [&](bool split_dd, DevBuf<Dec5Desc>& dst) {
-                    std::vector<Dec5Desc> ds((size_t)L * 16 + 16);
-                    for (int l = 0; l < L; ++l) {
-                        const DecBlockW& B = m->dec[(size_t)l];
-                        Dec5Desc* q = ds.data() + (size_t)l * 16;
-                        ln(q[0], B.attn_ln, l == 0 ? D5_ST_LN_EMB : D5_ST_LN_FOLD);
-                        gemm(q[1], B.qkv.w16, B.qkv.b, 3 * d, 1, D5_ST_PLANES, D5_EM_QKV, 3);
-                        q[2].kind = D5_KIND_ATTN;
-                        gemm(q[3], B.out.w16, B.out.b, d, 1, D5_ST_PLANES, D5_EM_RESID, 1);
-                        ln(q[4], B.cross_ln, D5_ST_LN_X);
-                        gemm(q[5], B.cq.w16, B.cq.b, d, 1, D5_ST_PLANES, D5_EM_CQ, 3);
-                        q[6].kind = D5_KIND_ATTN;
-                        gemm(q[7], B.cout.w16, B.cout.b, d, 1, D5_ST_CROSS, D5_EM_RESID, 1);
-                        ln(q[8], B.mlp_ln, D5_ST_LN_X);
-                        gemm(q[9], B.mlp1.w16, B.mlp1.b, 4 * d, 1, D5_ST_PLANES, D5_EM_HID, 3);
-                        gemm(q[10], B.mlp2.w16, B.mlp2.b, d, 4, D5_ST_PLANES, D5_EM_PART, 2);
-                        // MLP2 K = 4d: 3 slabs of 4d/3 when that keeps the 8-warp K split (multiple of 256, <= 1280): d/16 tiles x 3 slabs
-                        // = 144 items for small.en -> fewer rounds than 192 items
-                        if ((4 * d) % 3 == 0 && (4 * d / 3) % 256 == 0 && 4 * d / 3 <= 1280) { q[10].n_slabs = 3; q[10].ks = 4 * d / 3; }
-                        if (split_dd) {
-                            for (int sl : {3, 5, 7}) { q[sl].n_slabs = psl; q[sl].ks = 256; q[sl].emit = D5_EM_PART; }
-                            q[4].stage = D5_ST_LN_FOLD; q[4].n_fold = psl; q[4].ks = 256;   // folds the out projection, feeds the split cross query
-                            q[8].stage = D5_ST_LN_FOLD; q[8].n_fold = psl;                  // folds the cross out projection
-                        }
-                        if (l > 0) q[0].n_fold = q[10].n_slabs;                             // folds MLP2 of the previous layer
-                    }
-                    ln(ds[(size_t)L * 16 + 11], m->dec_ln, D5_ST_LN_FOLD_NOPUB);
-                    ds[(size_t)L * 16 + 11].n_fold = ds[(size_t)(L - 1) * 16 + 10].n_slabs;
-                    gemm(ds[(size_t)L * 16 + 12], m->tok_emb16, nullptr, V, 1, D5_ST_PLANES, D5_EM_LOGITS, 3);
-                    dst.alloc(ds.size());
-                    WB_CUDA(cudaMemcpy(dst.p, ds.data(), ds.size() * sizeof(Dec5Desc), cudaMemcpyHostToDevice));
-                };
-                build(false, d5_desc);
-                if (can_split) build(true, d5_desc_split);
-            }
+            dec_layers.alloc((size_t)L);
+            WB_CUDA(cudaMemcpy(dec_layers.p, lay.data(), lay.size() * sizeof(DecLayer), cudaMemcpyHostToDevice));
         }
+        dec5_build_tables(*m, n_sm, d5);
         ypart.alloc((size_t)4 * Rmax * d);   // decoder5.cu: MLP2 K-slab partial sums
         lg_m.alloc((size_t)n_logit_ctas * Rmax); lg_s.alloc((size_t)n_logit_ctas * Rmax);
         lg_v.alloc((size_t)n_logit_ctas * Rmax * DEC_KC); lg_i.alloc((size_t)n_logit_ctas * Rmax * DEC_KC);
@@ -380,31 +329,28 @@ void Session::run_encoder_f32() {
 }
 
 // cross keys (pre-scaled) | values of every decoder layer, projected once per window (mod.rs:484-485 hoisted out of the step loop)
+// into ckv_tmp, then re-laid out head-major per window (encoder.cu ckv_relayout_kernel): what the persistent decoders stream
 void Session::run_cross_kv() {
     const wb_dims& D = m->dims;
     const int d = D.n_text_state;
     const float qk_scale = (float)std::pow((double)d / (double)D.n_text_head, -0.25);
     for (int l = 0; l < D.n_text_layer; ++l) {
         const DecBlockW& B = m->dec[(size_t)l];
-        float* c32 = ckv_hm ? ckv_tmp.p : (kv_dtype == WB_KV_F16 ? nullptr : ckv.p + (size_t)l * Mcap * 2 * d);
         if (use_tc) {
             GemmF16Params p;
-            p.A_hi = xa_h.p; p.A_lo = xa_l.p; p.lda = d; p.B = B.ckv.w16; p.C = c32; p.ldc = 2 * d;
+            p.A_hi = xa_h.p; p.A_lo = xa_l.p; p.lda = d; p.B = B.ckv.w16; p.C = ckv_tmp.p; p.ldc = 2 * d;
             p.N = 2 * d; p.K = d; p.bias = B.ckv.b; p.scale = qk_scale; p.scale_cols = d; p.max_rows = (int)M_tot;
             GemmF16Plan& pl = *enc_plans[(size_t)2 + 4 * D.n_audio_layer + l];
             if (!pl.matches(p.max_rows, 1)) pl.build(p, 0, (int)M_tot);
             pl.launch(st);
         } else {
             GemmParams p;
-            p.A = xa.p; p.lda = d; p.B = B.ckv.w32; p.ldc = 2 * d;
-            if (c32) p.C = c32; else p.C16 = ckv16.p + (size_t)l * Mcap * 2 * d;
+            p.A = xa.p; p.lda = d; p.B = B.ckv.w32; p.C = ckv_tmp.p; p.ldc = 2 * d;
             p.N = 2 * d; p.K = d; p.bias = B.ckv.b; p.scale = qk_scale; p.scale_cols = d; p.max_rows = (int)M_tot;
             launch_gemm(p, st);
         }
-        if (ckv_hm) {
-            void* dst = kv_dtype == WB_KV_F16 ? (void*)(ckv16.p + (size_t)l * Mcap * 2 * d) : (void*)(ckv.p + (size_t)l * Mcap * 2 * d);
-            launch_ckv_relayout(ckv_tmp.p, dst, kv_dtype == WB_KV_F16, d_win_row_off.p, d_win_T.p, n_windows, M_tot, d, st);
-        }
+        void* dst = kv_dtype == WB_KV_F16 ? (void*)(ckv16.p + (size_t)l * Mcap * 2 * d) : (void*)(ckv.p + (size_t)l * Mcap * 2 * d);
+        launch_ckv_relayout(ckv_tmp.p, dst, kv_dtype == WB_KV_F16, d_win_row_off.p, d_win_T.p, n_windows, M_tot, d, st);   // head-major
     }
 }
 
@@ -452,28 +398,27 @@ void Session::begin(const int64_t* prompt, int64_t prompt_len, bool prefill) {
     WB_CUDA(cudaStreamSynchronize(st));
 }
 
-// One cooperative launch of the persistent decoder: n_steps positions starting at pos0.
-void Session::launch_v3(int R_, int pos0, int n_steps, int logits_from, bool use_cur_tok, int mask_mode, int k,
+// The persistent decoder for n_steps positions starting at pos0: the first of decoder4 -> decoder6 -> decoder5 -> decoder3
+// that covers the launch (each launch_decN decides that itself), or only the one WB200_DECODER names.
+void Session::launch_decoder(int R_, int pos0, int n_steps, int logits_from, bool use_cur_tok, int mask_mode, int k,
                         bool greedy, int eot) {
     const wb_dims& D = m->dims;
     const int d = D.n_text_state, H = D.n_text_head;
-    Dec3Args a;
+    DecArgs a;
     a.R = R_; a.Rmax = Rmax; a.d = d; a.H = H; a.L = D.n_text_layer; a.V = D.n_vocab; a.t_max = t_max; a.Mcap = Mcap;
     a.eps_outside = m->ln_eps_outside; a.qk_scale = (float)std::pow((double)d / (double)H, -0.25);
-    a.layers = d3_layers.p; a.tok_emb = m->tok_emb32; a.pos_emb = m->dec_pos;
+    a.layers = dec_layers.p; a.tok_emb = m->tok_emb32; a.pos_emb = m->dec_pos;
     a.E = m->fp16_exact ? (const void*)m->tok_emb16 : (const void*)m->tok_emb32;
     a.E_tiled = m->tok_emb16_tiled;
     a.lnf_g = m->dec_ln.g; a.lnf_b = m->dec_ln.b; a.lnf_eps = m->dec_ln.eps;
     a.x = dx.p; a.q = dq.p; a.att = datt.p; a.hid = dhid.p;
-    a.ypart = ypart.p; a.lgbuf = logits.p; a.att_pl = att_pl.p; a.hid_pl = hid_pl.p; a.d5 = d5_desc.p; a.ckv_hm = ckv_hm ? 1 : 0;   // a.d5: see pick_d5 below (needs n_splits)
+    a.ypart = ypart.p; a.lgbuf = logits.p; a.att_pl = att_pl.p; a.hid_pl = hid_pl.p;
     a.lg_slices = std::max(1, std::min(16, n_sm / std::max(1, R_)));
     a.kv_half = kv_dtype == WB_KV_F16 ? 1 : 0;
     if (a.kv_half) { a.kc = kc16.p; a.vc = vc16.p; a.ckv = ckv16.p; } else { a.kc = kc.p; a.vc = vc.p; a.ckv = ckv.p; }
     a.row_window = row_window.p; a.win_row_off = d_win_row_off.p; a.win_T = d_win_T.p;
     a.anc = anc_identity ? nullptr : (anc_cur == 0 ? anc0.p : anc1.p);
     a.n_splits = std::max(1, std::min(16, n_sm / std::max(1, R_ * H)));
-    auto pick_d5 = [&](int n_splits) { return (n_splits == 1 && d5_desc_split.p != nullptr) ? d5_desc_split.p : d5_desc.p; };
-    a.d5 = pick_d5(a.n_splits);
     a.part_o = part_o.p; a.part_m = part_m.p; a.part_l = part_l.p;
     a.tokens = tokens.p; a.cur_tok = cur_tok.p; a.use_cur_tok = use_cur_tok ? 1 : 0;
     a.pos0 = pos0; a.n_steps = n_steps; a.logits_from = logits_from;
@@ -481,75 +426,27 @@ void Session::launch_v3(int R_, int pos0, int n_steps, int logits_from, bool use
     a.k = k; a.greedy = greedy ? 1 : 0; a.eot = eot; a.lengths = lengths.p; a.finished = finished.p;
     a.topk_id = topk_id.p; a.topk_lp = topk_lp.p; a.logits_out = full_logits ? logits.p : nullptr;
     a.lg_m = lg_m.p; a.lg_s = lg_s.p; a.lg_v = lg_v.p; a.lg_i = lg_i.p;
-    a.pos = pos.p; a.n_unfinished = n_unfinished.p; a.steps_done = steps_done.p; a.bar = d3_bar.p;
+    a.pos = pos.p; a.n_unfinished = n_unfinished.p; a.steps_done = steps_done.p; a.bar = dec_bar.p;
     if (getenv("WB200_TRACE")) {
-        d3_trace.ensure(1 << 16);
-        WB_CUDA(cudaMemsetAsync(d3_trace.p, 0, sizeof(unsigned long long) * (1 << 16), st));
-        a.trace = d3_trace.p;
+        dec_trace.ensure(1 << 16);
+        WB_CUDA(cudaMemsetAsync(dec_trace.p, 0, sizeof(unsigned long long) * (1 << 16), st));
+        a.trace = dec_trace.p;
         a.trace_cap = 1 << 16;
     }
-    WB_CUDA(cudaMemsetAsync(d3_bar.p, 0, 4 * sizeof(unsigned int), st));   // monotonic barrier counters start at 0
-    last_decoder = 3;
+    WB_CUDA(cudaMemsetAsync(dec_bar.p, 0, 4 * sizeof(unsigned int), st));   // monotonic barrier counters start at 0
+    const bool h16 = m->fp16_exact;
+    auto allowed = [&](int n) { return only_decoder == 0 || only_decoder == n; };
+    int groups = 0;
     last_groups = 1;
-    if (dec_version == 4) {
-        // <= 7 rows: the cluster/DSMEM decoder (decoder4.cu; time per position at 3 rows: DESIGN.md section 6); 8..24 rows (batched chunks of the small
-        // models): the head-fused tensor-core cluster decoder (decoder6.cu), whose packed weight slices are built on first use.
-        // WB200_DEC6=force sends the small batches through decoder6.cu too (tests, A/B runs).
-        if (!force_dec6 && launch_dec4(a, m->fp16_exact, st)) last_decoder = 4;
-        if (last_decoder == 3 && use_dec6 && m->fp16_exact && greedy && k == 1 && !use_cur_tok && a.anc == nullptr && a.logits_out == nullptr && R_ <= 24 && ckv_hm &&
-            t_max <= 128 && dec6_supported(d, H)) {
-            const int hs = dec6_pick_hs(d, R_);
-            if (d6_pack[hs].p == nullptr) {
-                std::vector<Dec6LayerSrc> src((size_t)D.n_text_layer);
-                for (int l = 0; l < D.n_text_layer; ++l) {
-                    const DecBlockW& B = m->dec[(size_t)l];
-                    src[(size_t)l] = Dec6LayerSrc{B.qkv.w16, B.out.w16, B.cq.w16, B.cout.w16, B.mlp1.w16, B.mlp2.w16, B.qkv.b, B.out.b, B.cq.b, B.cout.b,
-                                                  B.mlp1.b, B.mlp2.b, B.attn_ln.g, B.attn_ln.b, B.cross_ln.g, B.cross_ln.b, B.mlp_ln.g, B.mlp_ln.b,
-                                                  B.attn_ln.eps, B.cross_ln.eps, B.mlp_ln.eps};
-                }
-                dec6_build_pack(d, hs, src, d6_pack[hs], d6_params[hs], st);
-            }
-            a.d6_pack = d6_pack[hs].p;
-            a.d6_params = d6_params[hs].p;
-            if (launch_dec6(a, hs, m->fp16_exact, st)) last_decoder = 6;
-        }
-        if (last_decoder == 3) {
-            if (launch_dec4(a, m->fp16_exact, st)) last_decoder = 4;
-            else if (launch_dec5(a, n_sm, m->fp16_exact, st)) last_decoder = 5;
-            else if (R_ > 32 && m->fp16_exact && d % 256 == 0 && d <= 1280 && k <= DEC_KC) {
-                // more rows than one launch of the batched tensor-core decoder takes (beams of many windows, BASELINE configs[4]:
-                // 48 windows x 5 beams per GPU): row groups of 32, one launch each on the session stream; rows are independent,
-                // ancestry entries stay absolute cache rows (a.kv_row0 = first cache row of the group)
-                bool ok = true;
-                int gi = 0;
-                for (int r0 = 0; r0 < R_ && ok; r0 += 32, ++gi) {
-                    const int Rg = std::min(32, R_ - r0);
-                    Dec3Args g = a;
-                    g.R = Rg; g.kv_row0 = r0;
-                    g.x += (int64_t)r0 * d; g.q += (int64_t)r0 * d; g.att += (int64_t)r0 * d; g.hid += (int64_t)r0 * 4 * d;
-                    g.row_window += r0;
-                    if (g.anc) g.anc += (int64_t)r0 * t_max;
-                    g.tokens += (int64_t)r0 * t_max; g.cur_tok += r0; g.lengths += r0; g.finished += r0;
-                    g.topk_id += (int64_t)r0 * k; g.topk_lp += (int64_t)r0 * k;
-                    if (g.logits_out) { g.logits_out += (int64_t)r0 * D.n_vocab; g.lgbuf = g.logits_out; }
-                    g.lg_slices = std::max(1, std::min(16, n_sm / std::max(1, Rg)));
-                    g.n_splits = std::max(1, std::min(16, n_sm / std::max(1, Rg * H)));
-                    g.d5 = pick_d5(g.n_splits);
-                    g.steps_done = steps_done.p + std::min(gi, 127); g.n_unfinished = n_unfinished.p + std::min(gi, 127);
-                    WB_CUDA(cudaMemsetAsync(d3_bar.p, 0, 4 * sizeof(unsigned int), st));
-                    ok = launch_dec5(g, n_sm, true, st);
-                }
-                if (!ok) fail(WB_ERR_UNSUPPORTED, "decoder5 rejected a row group");
-                last_decoder = 5;
-                last_groups = gi;
-            }
-        }
-    }
-    if (last_decoder == 3) launch_dec3(a, n_sm, m->fp16_exact, st);
+    if (allowed(4) && launch_dec4(a, h16, st)) last_decoder = 4;
+    else if (allowed(6) && launch_dec6(a, *m, d6, st)) last_decoder = 6;
+    else if (allowed(5) && (groups = launch_dec5(a, d5, n_sm, h16, st)) > 0) { last_decoder = 5; last_groups = groups; }
+    else if (allowed(3)) { launch_dec3(a, n_sm, h16, st); last_decoder = 3; }
+    else fail(WB_ERR_UNSUPPORTED, "WB200_DECODER=" + std::to_string(only_decoder) + ": decoder" + std::to_string(only_decoder) + " does not cover this launch");
     if (a.trace) {
         std::vector<unsigned long long> h(1 << 16);
         WB_CUDA(cudaStreamSynchronize(st));
-        WB_CUDA(cudaMemcpy(h.data(), d3_trace.p, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+        WB_CUDA(cudaMemcpy(h.data(), dec_trace.p, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
         FILE* f = fopen(getenv("WB200_TRACE"), "w");   // debugging aid: WB200_TRACE=<file> receives the stage time stamps of CTA 0
         if (f) {
             for (size_t i = 0; i < h.size(); ++i)
@@ -561,7 +458,7 @@ void Session::launch_v3(int R_, int pos0, int n_steps, int logits_from, bool use
 
 void Session::step_core(bool with_logits, int mask_mode, int k, bool greedy, int eot) {
     WB_REQUIRE(k >= 1 && k <= DEC_KC - 1, "step: k must be in [1, 7]");
-    launch_v3(R, host_pos, 1, with_logits ? 0 : INT_MAX, true, mask_mode, k, greedy, eot);
+    launch_decoder(R, host_pos, 1, with_logits ? 0 : INT_MAX, true, mask_mode, k, greedy, eot);
     ++host_pos;
 }
 
@@ -577,7 +474,7 @@ void Session::profile_decode(const int64_t* prompt, int64_t prompt_len, int n_st
     begin(prompt, prompt_len, false);
     const int total = (int)prompt_len - 1 + n_steps;
     WB_CUDA(cudaEventRecord(prof_ev[0], st));
-    launch_v3(R, 0, total, (int)prompt_len - 1, false, 2, 1, true, -1 /* never stop early */);
+    launch_decoder(R, 0, total, (int)prompt_len - 1, false, 2, 1, true, -1 /* never stop early */);
     WB_CUDA(cudaEventRecord(prof_ev[1], st));
     WB_CUDA(cudaStreamSynchronize(st));
     float t = 0.f;
@@ -637,7 +534,7 @@ void Session::greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_d
     // one launch: prompt prefill + every greedy step, early exit inside the kernel
     begin(prompt, prompt_len, /*prefill=*/false);
     const int n_steps = (int)prompt_len - 1 + max_depth;
-    if (max_depth > 0) launch_v3(R, 0, n_steps, (int)prompt_len - 1, false, 2, 1, true, (int)eot);
+    if (max_depth > 0) launch_decoder(R, 0, n_steps, (int)prompt_len - 1, false, 2, 1, true, (int)eot);
     std::vector<int> tk((size_t)R * t_max), len((size_t)R);
     int sdv[128] = {0};
     WB_CUDA(cudaMemcpyAsync(tk.data(), tokens.p, tk.size() * sizeof(int), cudaMemcpyDeviceToHost, st));

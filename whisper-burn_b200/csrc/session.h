@@ -43,18 +43,16 @@ struct Session {
     DevBuf<__half> mel_h, mel_l, h1_h, h1_l, xn_h, xn_l, qkv_h, qkv_l, att_h, att_l, hid_h, hid_l, xa_h, xa_l;
     std::vector<std::unique_ptr<GemmF16Plan>> enc_plans;   // conv1, conv2, per encoder layer qkv / out / mlp1 / mlp2, per decoder layer cross K|V
     bool conv_tc_ok = true;            // cleared if the driver rejects the overlapping-row tensor maps of the conv stems
-    bool use_tc = true;                // WB200_GEMM=simt forces the fp32 CUDA-core GEMM
+    bool use_tc = true;                // fp16-exact weights: tensor-core encoder; else the fp32 CUDA-core GEMM
     void run_encoder_f16();            // tensor-core encoder
     void run_encoder_f32();            // fp32 CUDA-core encoder (weights that are not fp16-exact)
     DevBuf<float> ckv;     // [L][Mcap][2d]  cross keys (scaled) | values, projected once per window
     DevBuf<float> ckv_tmp; // [Mcap][2d] one layer's projection in GEMM (row-major) order, before the head-major re-layout
-    bool ckv_hm = true;    // cross K/V stored head-major (what the persistent decoders stream)
     // ---- device: decode state
     DevBuf<float> kc, vc;  // [L][Rmax][t_max][d] self keys (scaled) / values
     DevBuf<__half> kc16, vc16, ckv16;   // fp16 caches (WB_KV_F16)
     DevBuf<float> dx, dq, dhid, logits;
-    DevBuf<Dec5Desc> d5_desc;         // decoder5.cu stage descriptors, d x d projections unsplit
-    DevBuf<Dec5Desc> d5_desc_split;   // the same with the d x d projections as K slabs (launches with unsplit cross attention); may be empty
+    Dec5Tables d5;                  // decoder5.cu stage descriptors
     DevBuf<uint4> att_pl, hid_pl;   // decoder5.cu activation planes
     DevBuf<float> part_o, part_m, part_l;
     DevBuf<int> tokens, lengths, cur_tok, finished, row_window, anc0, anc1, parent, pos, n_unfinished, topk_id;
@@ -74,18 +72,15 @@ struct Session {
     int64_t last_steps = 0;
     int last_groups = 1;         // row groups (launches) of the last decode
     int last_decoder = 0;        // which persistent decoder the last launch used (6, 5, 4 or 3); 0 = none yet
-    int dec_version = 4;         // 4 = best persistent decoder for the shape (decoder6 / decoder5 / decoder4), 3 = force the grid-barrier fallback (WB200_DECODER=3)
+    int only_decoder = 0;        // WB200_DECODER=3|4|5|6: every launch uses that decoder or fails; 0 = the first that covers it
     int n_sm = 0;
-    DevBuf<Dec3Layer> d3_layers;
-    DevBuf<uint8_t> d6_pack[3];     // decoder6.cu packed weight slices, index = CTAs per head (1, 2), built on first use
-    DevBuf<float> d6_params[3];
-    bool use_dec6 = true;           // WB200_DEC6=0 disables the head-fused cluster decoder
-    bool force_dec6 = false;        // WB200_DEC6=force: also for <= 7 rows (decoder4.cu's range)
-    DevBuf<unsigned int> d3_bar;
+    DevBuf<DecLayer> dec_layers;
+    Dec6Pack d6;                    // decoder6.cu packed weights
+    DevBuf<unsigned int> dec_bar;
     DevBuf<int> steps_done;
     DevBuf<float> datt;
-    DevBuf<unsigned long long> d3_trace;   // debug: WB200_TRACE=1
-    void launch_v3(int R_, int pos0, int n_steps, int logits_from, bool use_cur_tok, int mask_mode, int k, bool greedy,
+    DevBuf<unsigned long long> dec_trace;   // debug: WB200_TRACE=1
+    void launch_decoder(int R_, int pos0, int n_steps, int logits_from, bool use_cur_tok, int mask_mode, int k, bool greedy,
                    int eot);
     bool full_logits = false;    // also write raw logits [R][V] (stateless forward_decoder)
     int n_logit_ctas = 0;

@@ -6,6 +6,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
+#include <cstdio>
+#include <cstdlib>
 #include <map>
 #include <mutex>
 #include <stdexcept>
@@ -62,6 +65,82 @@ struct PerDeviceConfig {
         if (!configure()) return false;
         value[dev] = want;
         return true;
+    }
+};
+
+// Launches of a persistent cluster kernel (decoder4.cu, decoder6.cu), one object per kernel instance.  The kernel synchronises
+// its whole grid, so every cluster it launches must be co-resident: capacity() asks the device once how many clusters it holds,
+// launch() asks the driver to enforce that (cooperative cluster launch).  A driver that rejects the cooperative attribute gets
+// plain cluster launches from then on, whose co-residency rests on the occupancy query; so does WB200_NO_COOP (profilers
+// cannot replay cooperative cluster launches).
+struct ClusterLaunch {
+    std::mutex mu;
+    int clusters[16] = {};   // per device ordinal: 0 not queried, > 0 co-resident clusters, -1 the kernel does not fit
+    bool plain[16] = {};     // per device ordinal: launch without the cooperative attribute
+    static cudaLaunchConfig_t config(int cs, int n_clusters, int threads, size_t smem, cudaStream_t st, cudaLaunchAttribute (&attr)[2]) {
+        cudaLaunchConfig_t cfg{};
+        cfg.gridDim = dim3(n_clusters * cs);
+        cfg.blockDim = dim3(threads);
+        cfg.dynamicSmemBytes = smem;
+        cfg.stream = st;
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = cs;
+        attr[0].val.clusterDim.y = 1;
+        attr[0].val.clusterDim.z = 1;
+        attr[1].id = cudaLaunchAttributeCooperative;
+        attr[1].val.cooperative = 1;
+        cfg.attrs = attr;
+        cfg.numAttrs = 1;
+        return cfg;
+    }
+    // co-resident clusters of `cs` CTAs on the current device; 0 when the kernel does not fit it
+    int capacity(const void* k, int cs, int threads, size_t smem, const char* name) {
+        int dev = 0;
+        WB_CUDA(cudaGetDevice(&dev));
+        if (dev < 0 || dev >= 16) return 0;
+        std::lock_guard<std::mutex> lock(mu);
+        if (clusters[dev] == 0) {
+            clusters[dev] = -1;
+            if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
+                (cs > 8 && cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess)) {
+                cudaGetLastError();
+                return 0;
+            }
+            cudaLaunchAttribute attr[2];
+            const cudaLaunchConfig_t cfg = config(cs, 1, threads, smem, nullptr, attr);
+            int n = 0;
+            const cudaError_t e = cudaOccupancyMaxActiveClusters(&n, k, &cfg);
+            if (getenv("WB200_VERBOSE")) fprintf(stderr, "[wb] %s: cluster %d, smem %zu B, max active clusters %d (%s)\n", name, cs, smem, n, cudaGetErrorString(e));
+            if (e != cudaSuccess || n < 1) {
+                cudaGetLastError();
+                return 0;
+            }
+            clusters[dev] = n;
+            plain[dev] = getenv("WB200_NO_COOP") != nullptr;
+        }
+        return std::max(clusters[dev], 0);
+    }
+    // n_clusters clusters of `cs` CTAs; args as for cudaLaunchKernel
+    void launch(const void* k, int cs, int n_clusters, int threads, size_t smem, void** args, cudaStream_t st, const char* name) {
+        int dev = 0;
+        WB_CUDA(cudaGetDevice(&dev));
+        std::lock_guard<std::mutex> lock(mu);
+        cudaLaunchAttribute attr[2];
+        cudaLaunchConfig_t cfg = config(cs, n_clusters, threads, smem, st, attr);
+        if (!plain[dev]) {
+            cfg.numAttrs = 2;
+            const cudaError_t e = cudaLaunchKernelExC(&cfg, k, args);
+            if (e == cudaSuccess) {
+                WB_LAUNCH_CHECK();
+                return;
+            }
+            cudaGetLastError();
+            plain[dev] = true;
+            cfg.numAttrs = 1;
+            if (getenv("WB200_VERBOSE")) fprintf(stderr, "[wb] %s: cooperative cluster launch rejected (%s), using a plain cluster launch\n", name, cudaGetErrorString(e));
+        }
+        WB_CUDA(cudaLaunchKernelExC(&cfg, k, args));
+        WB_LAUNCH_CHECK();
     }
 };
 
@@ -176,7 +255,6 @@ struct GemmParams {
     int64_t lda = 0;
     const float* B = nullptr;      // [N][K]
     float* C = nullptr;
-    __half* C16 = nullptr;         // optional: store fp16-rounded results here instead of C (fp16 K/V cache)
     int64_t ldc = 0;
     int N = 0, K = 0;
     const float* bias = nullptr;   // [N] or null
