@@ -211,6 +211,11 @@ int wb_load_wav(const char* path, int strict_16k_mono, float* out, int64_t capac
 /* Diagnostics: which persistent decoder kernel the last decode launch used: 6 = head-fused cluster decoder (decoder6.cu),
  * 5 = batched tensor-core (decoder5.cu), 4 = cluster/DSMEM (decoder4.cu), 3 = grid-barrier FMA fallback (decoder3.cu), 0 = none yet. */
 int wb_session_last_decoder(const wb_session* s);
+/* Diagnostics: the candidates the last decoder launch selected at its last position, [n_rows][k] ids and log-probs, for rows
+ * 0 .. n_rows-1 of that launch.  Every decoder writes them, in greedy decoding too (k = 1: the chosen id and its log-prob), so
+ * a greedy run can be checked step by step.  WB_ERR_INVALID_ARG when k differs from that launch's k or n_rows exceeds its rows,
+ * WB_ERR_STATE before the first launch. */
+int wb_session_last_topk(wb_session* s, int64_t n_rows, int64_t k, int64_t* ids_out, float* lp_out);
 /* kernels launched by this library on this thread's sessions since the last reset */
 int64_t wb_kernel_launch_count(void);
 void wb_kernel_launch_count_reset(void);

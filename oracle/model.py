@@ -1,6 +1,7 @@
 """Oracle restatement of the Whisper model graph (reference: src/model/mod.rs).
 
-TEST INFRASTRUCTURE (see oracle/__init__.py).  PyTorch-CPU fp32; weights are a flat dict
+TEST INFRASTRUCTURE (see oracle/__init__.py).  PyTorch-CPU fp32, or float64 when the weights and inputs are float64
+(``as_dtype``): the same graph with the rounding of the GPU's fp32 arithmetic removed.  Weights are a flat dict
 keyed by the reference's own npy-tree paths (src/model/load.rs:19-310, python/dump.py:
 130-213), e.g. ``encoder/block_0/attn/query/weight`` with Linear weights in burn layout
 ``[d_in, d_out]`` (dump.py:141-145) and Conv1d weights ``[out, in, k]`` (load.rs:145-161).
@@ -65,6 +66,12 @@ def _f32(x: float) -> float:
     return float(np.float32(x))
 
 
+def as_dtype(w: dict, dtype: torch.dtype = torch.float64) -> dict:
+    """The weights in another float type (float64: the oracle then runs every op in float64).  The scalar constants stay the
+    fp32 values the GPU multiplies by (_f32)."""
+    return {k: v.to(dtype) for k, v in w.items()}
+
+
 # ---------------------------------------------------------------- third-party (burn) ops
 def linear(x: torch.Tensor, w: dict, path: str) -> torch.Tensor:
     """burn nn::Linear: x @ W[d_in,d_out] (+ b)."""
@@ -104,9 +111,9 @@ def log_softmax_last(x: torch.Tensor) -> torch.Tensor:
 
 
 # ---------------------------------------------------------------- mod.rs
-def attn_decoder_mask(n: int) -> torch.Tensor:
+def attn_decoder_mask(n: int, dtype: torch.dtype = torch.float32) -> torch.Tensor:
     """mod.rs:535-544: zeros with strict upper triangle = -inf."""
-    return torch.triu(torch.full((n, n), float("-inf"), dtype=torch.float32), diagonal=1)
+    return torch.triu(torch.full((n, n), float("-inf"), dtype=dtype), diagonal=1)
 
 
 def qkv_attention(q, k, v, mask, n_head: int, kv_f16: bool = False) -> torch.Tensor:
@@ -120,8 +127,8 @@ def qkv_attention(q, k, v, mask, n_head: int, kv_f16: bool = False) -> torch.Ten
     k = k.reshape(n_batch, n_ctx, n_head, n_hstate).transpose(1, 2).transpose(2, 3) * scale
     v = v.reshape(n_batch, n_ctx, n_head, n_hstate).transpose(1, 2)
     if kv_f16:
-        k = k.to(torch.float16).to(torch.float32)
-        v = v.to(torch.float16).to(torch.float32)
+        k = k.to(torch.float16).to(k.dtype)
+        v = v.to(torch.float16).to(v.dtype)
     qk = torch.matmul(q, k)
     if mask is not None:
         qk = qk + mask[0:n_qctx, 0:n_ctx]
@@ -185,7 +192,7 @@ def forward_decoder(w: dict, dims: WhisperDims, tokens: torch.Tensor, xa: torch.
     assert seq_len <= dims.n_text_ctx, f"Token sequence length {seq_len} must not exceed {dims.n_text_ctx}."
     x = F.embedding(tokens, w["decoder/token_embedding/weight"]) \
         + w["decoder/positional_embedding"][0:seq_len].unsqueeze(0)
-    mask = attn_decoder_mask(dims.n_text_ctx)
+    mask = attn_decoder_mask(dims.n_text_ctx, x.dtype)
     for i in range(dims.n_text_layer):
         p = f"decoder/block_{i}"
         x = x + self_attention(layer_norm(x, w, p + "/attn_ln", opts), w, p + "/attn", mask,

@@ -90,6 +90,30 @@ def _prefilter(lp: np.ndarray, k: int) -> np.ndarray:
     return np.nonzero(lp >= kth)[0]
 
 
+def masks_specials(max_seq_len: int) -> bool:
+    """transcribe.rs:271: the special tokens are masked out while the longest beam has at most 5 tokens."""
+    return not (max_seq_len > 5)
+
+
+def greedy_path_log_probs(w: dict, dims: model.WhisperDims, sp: SpecialTokens, xa: torch.Tensor, tokens: List[int],
+                          n_prompt: int = 4, opts: model.OracleOptions = model.DEFAULT_OPTS) -> torch.Tensor:
+    """Teacher-forced greedy scoring of one window: the log-softmax rows the greedy search (beam_size 1) evaluates when it
+    picks tokens[n_prompt], tokens[n_prompt + 1], ... on the path `tokens` (prompt first), with the special-token mask of
+    mels_to_tokens.  xa [1, T, d] is the window's encoder output; the rows [len(tokens) - n_prompt, V] come in the dtype of
+    the weights (float64 weights: a float64 reference of what the GPU computes along the same path)."""
+    dec = model.CachedDecoder(w, dims, xa, opts)
+    for t in tokens[:n_prompt - 1]:
+        dec.step(torch.tensor([t], dtype=torch.int64))
+    maskout = torch.from_numpy(sp.maskout())
+    rows = []
+    for i in range(n_prompt - 1, len(tokens) - 1):
+        logits = dec.step(torch.tensor([tokens[i]], dtype=torch.int64))
+        if masks_specials(i + 1):
+            logits = logits + maskout
+        rows.append(model.log_softmax_last(logits)[0])
+    return torch.stack(rows)
+
+
 def mels_to_tokens(w: dict, dims: model.WhisperDims, sp: SpecialTokens, mels: torch.Tensor,
                    beam_size: int = BEAM_SIZE, max_depth: int = MAX_DEPTH, use_cache: bool = True,
                    opts: model.OracleOptions = model.DEFAULT_OPTS, exact_topk: bool = False,
@@ -111,7 +135,7 @@ def mels_to_tokens(w: dict, dims: model.WhisperDims, sp: SpecialTokens, mels: to
             toks = [[t for t, _ in b.seq] + [0] * (max_seq_len - len(b.seq)) for b in beams]
             logits = model.forward_decoder(w, dims, torch.tensor(toks, dtype=torch.int64),
                                            encoder_output.repeat(len(beams), 1, 1), opts)
-            if not (max_seq_len > 5):
+            if masks_specials(max_seq_len):
                 logits = logits + maskout
             log_probs = model.log_softmax_last(logits)
             rows = [log_probs[i, len(b.seq) - 1].numpy() for i, b in enumerate(beams)]
@@ -131,7 +155,7 @@ def mels_to_tokens(w: dict, dims: model.WhisperDims, sp: SpecialTokens, mels: to
                 dec.reorder([prev.index(s[:-1]) for s in seqs])
             cache["rows"] = seqs
             logits = dec.step(torch.tensor([s[-1] for s in seqs], dtype=torch.int64))
-            if not (max_seq_len > 5):
+            if masks_specials(max_seq_len):
                 logits = logits + maskout
             log_probs = model.log_softmax_last(logits)
             rows = [None] * len(beams)

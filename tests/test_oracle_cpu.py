@@ -154,6 +154,45 @@ def test_wide_model_tokens_golden():
     assert transcribe.mels_to_tokens(w, dims, sp, mel, beam_size=5, max_depth=8) == gold["test-c_beam5_depth8_f32"][2]
 
 
+@pytest.mark.parametrize("kv", ["f32", "f16"])
+def test_float64_oracle_restates_the_float32_graph(kv):
+    """The oracle run on float64 weights and inputs is the same graph as the float32 oracle: encoder output, stateless
+    decoder logits and the teacher-forced greedy log-probs agree to float32 noise.  The GPU tests compare the kernels against
+    this float64 mode.  With the fp16 K/V cache the rounding keeps the input dtype; there the few K/V elements whose float32
+    and float64 values lie on opposite sides of an fp16 rounding boundary move by one fp16 ulp (2^-11 relative), which
+    shows as ~6e-5 in the logits and ~9e-5 in the log-probs of this model, so the bound is wider for f16."""
+    rel_tol, lp_tol = (5e-6, 1e-5) if kv == "f32" else (2e-4, 3e-4)
+    dims, _, w = synth.make_weights("test-a", seed=0)
+    w64 = model.as_dtype(w)
+    sp = synth.special_tokens(dims)
+    opts = model.OracleOptions(kv_dtype=kv)
+    raw = audio.prep_audio(torch.from_numpy(synth.waveform(20000, seed=3))[None])
+    mel = transcribe.pad_mel(raw, dims.n_audio_ctx)
+    enc = model.forward_encoder(w, dims, mel, opts)
+    enc64 = model.forward_encoder(w64, dims, mel.double(), opts)
+    assert enc64.dtype == torch.float64
+    assert float((enc64 - enc).abs().max() / enc64.abs().max()) < 5e-6       # the encoder has no K/V cache
+
+    toks = torch.tensor([sp.prompt() + [17, 300, 5, 911, 2]], dtype=torch.int64)
+    lg = model.forward_decoder(w, dims, toks, enc, opts)
+    lg64 = model.forward_decoder(w64, dims, toks, enc64, opts)
+    assert lg64.dtype == torch.float64
+    assert float((lg64 - lg).abs().max() / lg64.abs().max()) < rel_tol
+
+    path = transcribe.mels_to_tokens(w, dims, sp, raw, beam_size=1, max_depth=8, opts=opts)
+    lp = transcribe.greedy_path_log_probs(w, dims, sp, enc, path, opts=opts)
+    lp64 = transcribe.greedy_path_log_probs(w64, dims, sp, enc64, path, opts=opts)
+    assert lp64.dtype == torch.float64 and lp64.shape == (len(path) - 4, dims.n_vocab)
+    assert torch.isneginf(lp64[:2, sp.first_special:]).all() and torch.isfinite(lp64[2:]).all()   # mask on the first two steps
+    fin = torch.isfinite(lp64)
+    assert float((lp64 - lp)[fin].abs().max()) < lp_tol
+    # the path is the float32 greedy path: its tokens are the argmax of every row (up to float32 ties)
+    assert [int(i) for i in lp.argmax(dim=1)] == path[4:]
+    # and the cached scoring equals the stateless decoder's last-position log-softmax
+    full = model.log_softmax_last(model.forward_decoder(w64, dims, torch.tensor([path[:-1]]), enc64, opts)[0, 4 - 1:])
+    assert float((full - lp64)[2:].abs().max()) < 1e-9
+
+
 def test_repetition_heuristics_known_answers():
     """Hand-evaluated cases of transcribe.rs:385-447."""
     t = [0, 9] + [1, 2, 3] * 5

@@ -557,6 +557,13 @@ int wb_load_wav(const char* path, int strict_16k_mono, float* out, int64_t capac
 
 int wb_session_last_decoder(const wb_session* s) { return s ? s->impl->last_decoder : -1; }
 
+int wb_session_last_topk(wb_session* s, int64_t n_rows, int64_t k, int64_t* ids_out, float* lp_out) {
+    return guarded([&] {
+        WB_REQUIRE(s && ids_out && lp_out, "last_topk: null pointer");
+        s->impl->last_topk(n_rows, k, ids_out, lp_out);
+    });
+}
+
 // beam::beam_search (src/beam.rs:9-37) over a TABLE-driven `next`: the continuation log-prob of token v after a beam whose last
 // token is t and whose length is n is table[((t * 131 + n) % n_ctx) * n_vocab + v] (added to the beam's cumulative f64 log-prob);
 // a beam is finished when its last token is eot.  Host only: lets the CPU tests drive the complete C++ search (host/beam.hpp:

@@ -443,6 +443,8 @@ void Session::launch_decoder(int R_, int pos0, int n_steps, int logits_from, boo
     else if (allowed(5) && (groups = launch_dec5(a, d5, n_sm, h16, st)) > 0) { last_decoder = 5; last_groups = groups; }
     else if (allowed(3)) { launch_dec3(a, n_sm, h16, st); last_decoder = 3; }
     else fail(WB_ERR_UNSUPPORTED, "WB200_DECODER=" + std::to_string(only_decoder) + ": decoder" + std::to_string(only_decoder) + " does not cover this launch");
+    last_rows = R_;
+    last_k = k;
     if (a.trace) {
         std::vector<unsigned long long> h(1 << 16);
         WB_CUDA(cudaStreamSynchronize(st));
@@ -526,6 +528,17 @@ void Session::step_beams(int64_t n_rows, const int32_t* window_of_row, const int
         topk_ids_out[i] = hid_[i];
         topk_lp_out[i] = h_float[i];
     }
+}
+
+void Session::last_topk(int64_t n_rows, int64_t k, int64_t* ids_out, float* lp_out) {
+    if (last_decoder == 0) fail(WB_ERR_STATE, "last_topk: no decoder launch yet");
+    WB_REQUIRE(k == last_k, "last_topk: k differs from the last launch's k");
+    WB_REQUIRE(n_rows >= 1 && n_rows <= last_rows, "last_topk: n_rows exceeds the last launch's rows");
+    std::vector<int> ids((size_t)(n_rows * k));
+    WB_CUDA(cudaStreamSynchronize(st));
+    WB_CUDA(cudaMemcpy(ids.data(), topk_id.p, ids.size() * sizeof(int), cudaMemcpyDeviceToHost));
+    WB_CUDA(cudaMemcpy(lp_out, topk_lp.p, ids.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < ids.size(); ++i) ids_out[i] = ids[i];
 }
 
 void Session::greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_depth, int64_t eot,

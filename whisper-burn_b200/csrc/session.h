@@ -72,6 +72,7 @@ struct Session {
     int64_t last_steps = 0;
     int last_groups = 1;         // row groups (launches) of the last decode
     int last_decoder = 0;        // which persistent decoder the last launch used (6, 5, 4 or 3); 0 = none yet
+    int last_rows = 0, last_k = 0;   // rows and candidates per row of the last launch (its topk_id / topk_lp)
     int only_decoder = 0;        // WB200_DECODER=3|4|5|6: every launch uses that decoder or fails; 0 = the first that covers it
     int n_sm = 0;
     DevBuf<DecLayer> dec_layers;
@@ -109,6 +110,8 @@ struct Session {
     void step_core(bool with_logits, int mask_mode, int k, bool greedy, int eot);
     void step_beams(int64_t n_rows, const int32_t* window_of_row, const int32_t* parent_row, const int64_t* token,
                     int apply_mask, int k, int64_t* topk_ids_out, float* topk_lp_out);
+    // the [n_rows][k] candidates the last launch wrote at its last position
+    void last_topk(int64_t n_rows, int64_t k, int64_t* ids_out, float* lp_out);
     // greedy loop on the device; returns per-window token lists
     void greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_depth, int64_t eot,
                        std::vector<std::vector<int64_t>>& out);

@@ -137,6 +137,13 @@ class Session:
     def last_decoder(self) -> int:
         return int(ffi.lib().wb_session_last_decoder(self._h))
 
+    def last_topk(self, n_rows: int, k: int = 1):
+        """(ids [n_rows, k] int64, log-probs [n_rows, k] float32) the last decoder launch selected at its last position."""
+        ids = np.empty((n_rows, k), dtype=np.int64)
+        lps = np.empty((n_rows, k), dtype=np.float32)
+        ffi.check(ffi.lib().wb_session_last_topk(self._h, n_rows, k, ffi.i64ptr(ids), ffi.fptr(lps)))
+        return ids, lps
+
     def last_timings_ms(self):
         buf = np.zeros(4, dtype=np.float32)
         ffi.check(ffi.lib().wb_session_last_timings(self._h, ffi.fptr(buf)))
