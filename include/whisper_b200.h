@@ -153,7 +153,10 @@ int wb_session_step(wb_session* s, int64_t n_rows, const int32_t* window_of_row,
 /* ---- transcribe.rs (token side) ---------------------------------------------------------- */
 /* mels_to_text for a batch of independent windows: encode, then beam::beam_search with
  * beam_size / max_depth (reference: 5 / 100; greedy = beam_size 1).  tokens_out is
- * [n_windows, capacity]; each row gets prompt + generated ids (incl. EOT if reached). */
+ * [n_windows, capacity]; each row gets prompt + generated ids (incl. EOT if reached).
+ * Beam search (beam_size > 1) runs entirely on the GPU in one decoder launch (prefill + every search step, selection
+ * included) when the weights are fp16-exact, n_text_state is 128 or 384, n_windows * beam_size <= 24 and
+ * max_text_len <= 128; otherwise the host drives the search one batched device step per depth.  Both give the same ids. */
 int wb_transcribe_windows(wb_session* s, const float* const* waves, const int64_t* lens, int64_t n_windows,
                           int beam_size, int max_depth, const wb_special_ids* ids, const uint8_t* is_special,
                           int64_t* tokens_out, int64_t capacity, int64_t* lens_out);
@@ -199,6 +202,10 @@ int64_t wb_beam_get_top_elements(const double* scores, int64_t n, int64_t num, i
  * length of the best sequence written to seq_out, or -1 on bad arguments. */
 int64_t wb_beam_search_table(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token, int64_t eot,
                              int64_t beam_size, int64_t max_depth, int64_t* seq_out, int64_t capacity);
+/* The same search stepped by the fixed-capacity selection the on-device beam search runs (host/beam_fixed.hpp), on the CPU:
+ * each live beam contributes its beam_size best table entries.  beam_size <= 7.  Same return values; for tests. */
+int64_t wb_beam_search_table_fixed(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token, int64_t eot,
+                                   int64_t beam_size, int64_t max_depth, int64_t* seq_out, int64_t capacity);
 
 /* ---- transcribe binary helpers (host) ---------------------------------------------------------- */
 /* load_audio_waveform (src/bin/transcribe/main.rs:31-55): PCM int samples / (2^(bits-1) - 1), float samples as they

@@ -18,14 +18,16 @@ def get_top_elements(scores, num: int) -> list[int]:
     return [int(v) for v in out[:n]]
 
 
-def beam_search_table(table, first_token: int, eot: int, beam_size: int, max_depth: int) -> list[int]:
+def beam_search_table(table, first_token: int, eot: int, beam_size: int, max_depth: int, fixed: bool = False) -> list[int]:
     """beam::beam_search (beam.rs:9-37) in the library's C++ host code (host/beam.hpp) over a table-driven `next`:
-    log-prob of token v after a beam ending in t with length n = table[(t * 131 + n) % n_ctx][v]."""
+    log-prob of token v after a beam ending in t with length n = table[(t * 131 + n) % n_ctx][v].
+    fixed=True steps the search with the fixed-capacity selection the on-device search runs (host/beam_fixed.hpp)."""
     import ctypes as C
     t = np.ascontiguousarray(table, dtype=np.float64)
     out = np.zeros(max_depth + 2, dtype=np.int64)
-    n = ffi.lib().wb_beam_search_table(t.ctypes.data_as(C.POINTER(C.c_double)), t.shape[0], t.shape[1], first_token, eot, beam_size,
-                                      max_depth, ffi.i64ptr(out), out.shape[0])
+    fn = ffi.lib().wb_beam_search_table_fixed if fixed else ffi.lib().wb_beam_search_table
+    n = fn(t.ctypes.data_as(C.POINTER(C.c_double)), t.shape[0], t.shape[1], first_token, eot, beam_size, max_depth,
+           ffi.i64ptr(out), out.shape[0])
     if n < 0:
         raise ffi.WbError(ffi.WB_ERR_INVALID_ARG, "beam_search_table: bad arguments")
     return [int(v) for v in out[:n]]

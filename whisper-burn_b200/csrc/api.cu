@@ -7,6 +7,7 @@
 #include <new>
 
 #include "../host/beam.hpp"
+#include "../host/beam_fixed.hpp"
 #include "../host/repeat.hpp"
 #include "session.h"
 
@@ -590,6 +591,57 @@ int64_t wb_beam_search_table(const double* table, int64_t n_ctx, int64_t n_vocab
     if ((int64_t)best.size() > capacity) return -1;
     for (size_t i = 0; i < best.size(); ++i) seq_out[i] = best[i];
     return (int64_t)best.size();
+}
+
+// The same search as wb_beam_search_table, stepped by the fixed-capacity selection that decoder6.cu runs on the device
+// (host/beam_fixed.hpp).  Each live beam contributes its beam_size best table entries (get_top_elements over the whole
+// row, as the device contributes its top-k), and the step re-ranks them exactly as the reference does.
+int64_t wb_beam_search_table_fixed(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token, int64_t eot,
+                                   int64_t beam_size, int64_t max_depth, int64_t* seq_out, int64_t capacity) {
+    namespace fx = wb::beamfx;
+    if (!table || !seq_out || n_ctx < 1 || n_vocab < 1 || beam_size < 1 || beam_size > fx::MAX_BEAM || max_depth < 0) return -1;
+    const int B = (int)beam_size;
+    std::vector<fx::Head> heads(1);
+    std::vector<std::vector<int64_t>> seqs(1, std::vector<int64_t>{first_token});
+    heads[0] = fx::Head{0.0, first_token == eot ? 1 : 0, 0, 1, 0};
+    std::vector<double> scores((size_t)n_vocab);
+    for (int64_t depth = 0; depth < max_depth; ++depth) {
+        const int n = (int)heads.size();
+        if (fx::search_done(heads.data(), n)) break;
+        int step_row[fx::MAX_NODES], cand_id[fx::MAX_NODES * fx::MAX_BEAM];
+        double cand_lp[fx::MAX_NODES * fx::MAX_BEAM];
+        for (int b = 0; b < n; ++b) {
+            step_row[b] = b;
+            for (int i = 0; i < B; ++i) cand_id[b * B + i] = -1;
+            if (heads[(size_t)b].finished) continue;
+            const int64_t t = seqs[(size_t)b].back(), len = (int64_t)seqs[(size_t)b].size();
+            const double* row = table + ((t * 131 + len) % n_ctx) * n_vocab;
+            for (int64_t v = 0; v < n_vocab; ++v) scores[(size_t)v] = heads[(size_t)b].log_prob + row[v];
+            int top[fx::MAX_BEAM + 1];
+            const int nt = fx::top_elements(scores.data(), (int)n_vocab, B, top);
+            for (int i = 0; i < nt; ++i) {
+                cand_id[b * B + i] = top[i];
+                cand_lp[b * B + i] = row[top[i]];
+            }
+        }
+        fx::Pick out[fx::MAX_NODES];
+        const int n_out = fx::beam_step(heads.data(), n, step_row, cand_id, cand_lp, B, (int)eot, out);
+        std::vector<fx::Head> nh((size_t)n_out);
+        std::vector<std::vector<int64_t>> ns((size_t)n_out);
+        for (int i = 0; i < n_out; ++i) {
+            nh[(size_t)i] = out[i].head;
+            ns[(size_t)i] = seqs[(size_t)out[i].src];
+            if (out[i].token >= 0) ns[(size_t)i].push_back(out[i].token);
+        }
+        heads.swap(nh);
+        seqs.swap(ns);
+    }
+    const int best = fx::max_by_last(heads.data(), (int)heads.size());
+    if (best < 0) return 0;
+    const std::vector<int64_t>& s = seqs[(size_t)best];
+    if ((int64_t)s.size() > capacity) return -1;
+    for (size_t i = 0; i < s.size(); ++i) seq_out[i] = s[i];
+    return (int64_t)s.size();
 }
 
 int64_t wb_kernel_launch_count(void) { return wb::g_launch_count; }

@@ -2,6 +2,7 @@
 #pragma once
 #include <stdint.h>
 
+#include "../host/beam_fixed.hpp"
 #include "wb_internal.h"
 
 namespace wb {
@@ -82,13 +83,25 @@ struct DecArgs {
     const float* d6_params = nullptr;     // decoder6.cu: parameter blocks [L][CS][PARAMS] floats
     unsigned long long* trace = nullptr;  // optional: stage / barrier timestamps of CTA 0 (ns)
     int trace_cap = 0;
+    // decoder6.cu beam mode (beam > 1): prefill + the whole width-B search of n_win windows in one launch.  Row w * B + i is
+    // slot i of window w; anc (read at even depths) / anc_alt (odd depths) are the double-buffered ancestry tables.
+    int beam = 0, n_win = 0, max_depth = 0;
+    int* anc_alt = nullptr;
+    int* slot_live = nullptr;             // [R] the slot holds a live beam at the current position
+    beamfx::Head* bm_head = nullptr;      // [2][n_win][MAX_NODES] carried nodes, double-buffered by depth
+    int* bm_seq = nullptr;                // [2][n_win][MAX_NODES][t_max] their token sequences
+    int* bm_cnt = nullptr;                // [2][n_win] carried nodes per window
+    int* bm_win = nullptr;                // [n_win][2] current buffer, done
+    int* bm_out = nullptr;                // [n_win][t_max] best sequence of each window when the search ends
+    int* bm_out_len = nullptr;            // [n_win]
 };
 // Each launch_decN launches decoder N when it covers the configuration and reports whether it did.
 // grid-barrier FMA decoder (decoder3.cu): covers every configuration
 void launch_dec3(const DecArgs& a, int n_ctas, bool w_half, cudaStream_t st);
 // cluster / DSMEM decoder (decoder4.cu): greedy, d in {128, 384}, as many rows (<= 8) as co-resident 16-CTA clusters
 bool launch_dec4(const DecArgs& a, bool w_half, cudaStream_t st);
-// head-fused tensor-core cluster decoder (decoder6.cu): fp16-exact weights, greedy, d in {128, 384}, <= 24 rows, t_max <= 128
+// head-fused tensor-core cluster decoder (decoder6.cu): fp16-exact weights, d in {128, 384}, <= 24 rows, t_max <= 128; greedy,
+// or (a.beam > 1) the whole beam search
 struct Dec6Pack {   // this model's weights as per-CTA slices (built on the first launch)
     DevBuf<uint8_t> pack;   // [L][CS][PACK] bytes
     DevBuf<float> params;   // [L][CS][PARAMS] floats

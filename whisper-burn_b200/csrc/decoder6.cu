@@ -1,4 +1,4 @@
-// Head-fused cluster decoder for L2-resident models (d = 128 / 384: tiny.en and the test models), greedy path.
+// Head-fused cluster decoder for L2-resident models (d = 128 / 384: tiny.en and the test models), greedy path and beam search.
 //
 // Same math and single-launch structure as decoder3.cu (TextDecoder::forward src/model/mod.rs:131-157, blocks :345-350,
 // attention :428-533, MLP :376-382, search closure src/transcribe.rs:253-307; prefill + every greedy step in one kernel), but
@@ -33,8 +33,12 @@
 //   embedding, mma.sync swap-AB with fp16 hi/lo activation planes, fused mask / online softmax / arg-max), behind ONE grid
 //   barrier; the per-row finish is done by the LAST CTA to deliver its records (ticket), which then releases a flag.
 //
-// Requirements: fp16-exact weights, d in {128, 384}, greedy (k = 1), identity ancestry, R <= 24 rows, t_max <= 128.
-// Everything else is handled by decoder5.cu / decoder3.cu.
+// Beam mode (dec6_kernel<..., BEAM = true>, a.beam = B in 2..7): the same kernel runs the prefill and the whole width-B search of
+// R / B windows: row w * B + i is slot i of window w, self attention goes through the ancestry table, the vocabulary records
+// keep DEC_KC candidates, and the finisher selects the next beams on the device (finish_beam, host/beam_fixed.hpp).
+//
+// Requirements: fp16-exact weights, d in {128, 384}, R <= 24 rows, t_max <= 128; greedy (k = 1) with identity ancestry, or
+// the beam mode.  Everything else is handled by decoder5.cu / decoder3.cu.
 #include <cooperative_groups.h>
 
 #include <cstdlib>
@@ -384,8 +388,10 @@ __device__ __noinline__ void combine6(const float* pr, uint64_t* bar, uint32_t p
 
 // causal self attention of one head over positions 0..p (mod.rs:428-436 with the mask of :535-544 = "keys <= p"): 32 (warp, rg)
 // key slots, 8 lanes per key; keys < p come from the cache (L2), key p from shared memory.  Leaves per-warp records in wm/wl/wo.
-template <typename KVT>
-__device__ __noinline__ void self_attn6(const float* qkv_s, const KVT* kbase, const KVT* vbase, int ld, int p, float* wm, float* wl, float* wo) {
+// ANC (beam search): key j < p lives in cache row anc[j], i.e. at kbase + anc[j] * row_ld + j * ld (decoder3.cu addressing).
+template <typename KVT, bool ANC>
+__device__ __forceinline__ void self_attn6_body(const float* qkv_s, const KVT* kbase, const KVT* vbase, int ld, int p, const int* anc,
+                                                int64_t row_ld, float* wm, float* wl, float* wo) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, rg = lane >> 3, l8 = lane & 7;
     float q[8];
 #pragma unroll
@@ -398,8 +404,9 @@ __device__ __noinline__ void self_attn6(const float* qkv_s, const KVT* kbase, co
     for (int u = 0; u < 4; ++u) {                          // all loads first (t_max <= 128 -> at most 4 keys per slot)
         const int j = j0 + 32 * u;
         if (j < p) {
-            load_row8<KVT>(kbase + (int64_t)j * ld, l8, 0, kf[u], false);
-            load_row8<KVT>(vbase + (int64_t)j * ld, l8, 0, vf[u], false);
+            const int64_t off = ANC ? (int64_t)__ldcg(anc + j) * row_ld + (int64_t)j * ld : (int64_t)j * ld;
+            load_row8<KVT>(kbase + off, l8, 0, kf[u], false);
+            load_row8<KVT>(vbase + off, l8, 0, vf[u], false);
         } else if (j == p) {
 #pragma unroll
             for (int i = 0; i < 8; ++i) { kf[u][i] = qkv_s[64 + hdim<KVT>(l8, i)]; vf[u][i] = qkv_s[128 + hdim<KVT>(l8, i)]; }
@@ -423,6 +430,24 @@ __device__ __noinline__ void self_attn6(const float* qkv_s, const KVT* kbase, co
         for (int i = 0; i < 8; ++i) wo[warp * 64 + hdim<KVT>(l8, i)] = A.o[i];
         if (l8 == 0) { wm[warp] = A.m; wl[warp] = A.l; }
     }
+}
+template <typename KVT>
+__device__ __noinline__ void self_attn6(const float* qkv_s, const KVT* kbase, const KVT* vbase, int ld, int p, float* wm, float* wl, float* wo) {
+    self_attn6_body<KVT, false>(qkv_s, kbase, vbase, ld, p, nullptr, 0, wm, wl, wo);
+}
+template <typename KVT>
+__device__ __noinline__ void self_attn6_anc(const float* qkv_s, const KVT* kbase, const KVT* vbase, int ld, int p, const int* anc, int64_t row_ld,
+                                            float* wm, float* wl, float* wo) {
+    self_attn6_body<KVT, true>(qkv_s, kbase, vbase, ld, p, anc, row_ld, wm, wl, wo);
+}
+
+// beam mode: candidate list of one (warp, row) in the logits stage, sorted by (value desc, id asc); empty = (-inf, INT_MAX)
+__device__ __forceinline__ void cand_insert(float* lv, int* li, float v, int n) {
+    if (!(v > lv[DEC_KC - 1] || (v == lv[DEC_KC - 1] && n < li[DEC_KC - 1]))) return;
+    int k = DEC_KC - 1;
+    for (; k > 0 && (v > lv[k - 1] || (v == lv[k - 1] && n < li[k - 1])); --k) { lv[k] = lv[k - 1]; li[k] = li[k - 1]; }
+    lv[k] = v;
+    li[k] = n;
 }
 
 // cross attention of one head over the T keys of the window (mod.rs:482-490), the head-major K/V block arriving through
@@ -479,8 +504,207 @@ __device__ __noinline__ uint32_t cross_attn6(const Pipe P, uint32_t n, int* slot
     return n;
 }
 
+// ---- beam mode: the finisher's work at a search position p (depth = p - logits_from), by the last CTA to deliver its records.
+constexpr int BM_LIVE = 24;                                          // rows of a beam launch
+constexpr int BM_NX = 3 * BM_LIVE + 3 * NCW * beamfx::MAX_NODES;     // finish_beam's shared scratch (ints)
+//   (a) each live slot's B best candidates by the rounded log-prob (v - max) - lse, the lower id first on equal log-probs
+//       (decoder5.cu's rule), from the CTAs' records -> topk_id / topk_lp [row][B];
+//   (b) one warp per unfinished window: beamfx::beam_step on the carried nodes (lane 0), the new nodes' sequences (the warp);
+//       the next position's live slots w * B + i in carried order, each with its parent's cache row and its token;
+//   (c) the search ends when every window is done (its best carried node is finished) or at max_depth: then the best
+//       sequence of every window goes to bm_out and bar[3] is set; otherwise the next position's slots, tokens and ancestry
+//       table (anc_new[r][j] = anc_old[parent[r]][j] for j <= p, anc_new[r][p + 1] = r) are written.
+// Called by the 256 consumer threads; ends with a barrier of the consumers.
+__device__ __noinline__ void finish_beam(const DecArgs& a, int p, int depth, const int* anc_cur, uint8_t* scratch, const int* live, int* nx,
+                                         int* ctl) {
+    namespace fx = beamfx;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int R = a.R, B = a.beam, t_max = a.t_max, NW = a.n_win;
+    int* nx_par = nx;
+    int* nx_tok = nx_par + BM_LIVE;
+    int* nx_live = nx_tok + BM_LIVE;
+    int* pk_src = nx_live + BM_LIVE + warp * 3 * fx::MAX_NODES;   // this warp's picks: source, token, length
+    int* pk_tok = pk_src + fx::MAX_NODES;
+    int* pk_len = pk_tok + fx::MAX_NODES;
+    // ---- (a)
+    constexpr int RINGW = NSLOT * SLOT / NCW;
+    static_assert(160 * DEC_KC * 8 <= RINGW, "finisher candidate scratch");
+    for (int r = warp; r < R; r += NCW) {
+        if (!live[r]) continue;
+        const int NP = gridDim.x;   // <= 160 co-resident CTAs
+        float rm[5], rs[5];
+#pragma unroll
+        for (int k = 0; k < 5; ++k) {
+            const int c = min(lane + 32 * k, NP - 1);
+            rm[k] = __ldcg(a.lg_m + (int64_t)c * R + r);
+            rs[k] = __ldcg(a.lg_s + (int64_t)c * R + r);
+        }
+        float mx = -INFINITY;
+#pragma unroll
+        for (int k = 0; k < 5; ++k)
+            if (lane + 32 * k < NP) mx = fmaxf(mx, rm[k]);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        float se = 0.0f;
+#pragma unroll
+        for (int k = 0; k < 5; ++k)
+            if (lane + 32 * k < NP && rm[k] > -INFINITY) se += rs[k] * expf(rm[k] - mx);
+        se = warp_sum(se);
+        const float lse = logf(se);
+        // the row's NP * DEC_KC candidates as (log-prob, id) in this warp's share of the (idle) ring
+        float* cv = reinterpret_cast<float*>(scratch + (size_t)warp * RINGW);
+        int* ci = reinterpret_cast<int*>(cv + 160 * DEC_KC);
+        const int NC = NP * DEC_KC;
+        for (int q = lane; q < NC; q += 32) {
+            const int64_t o = ((int64_t)(q / DEC_KC) * R + r) * DEC_KC + q % DEC_KC;
+            ci[q] = __ldcg(a.lg_i + o);
+            cv[q] = __fsub_rn(__fsub_rn(__ldcg(a.lg_v + o), mx), lse);
+        }
+        __syncwarp();
+        float prev_v = INFINITY;
+        int prev_i = -1;
+        for (int kk = 0; kk < B; ++kk) {
+            float bv = -INFINITY;
+            int bi = INT_MAX;
+            for (int q = lane; q < NC; q += 32) {
+                const int idx = ci[q];
+                if (idx == INT_MAX) continue;
+                const float v = cv[q];
+                const bool after_prev = v < prev_v || (v == prev_v && idx > prev_i);
+                if (after_prev && (v > bv || (v == bv && idx < bi))) { bv = v; bi = idx; }
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+                const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+                if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+            }
+            if (lane == 0) {
+                a.topk_id[(int64_t)r * B + kk] = bi == INT_MAX ? -1 : bi;
+                a.topk_lp[(int64_t)r * B + kk] = bv;
+            }
+            prev_v = bv;
+            prev_i = bi;
+        }
+        __syncwarp();
+    }
+    bar_consumers();
+    // ---- (b)
+    for (int w = warp; w < NW; w += NCW) {
+        const int buf = __ldcg(a.bm_win + 2 * w);
+        if (__ldcg(a.bm_win + 2 * w + 1)) {   // done: its slots stay idle
+            if (lane < B) nx_live[w * B + lane] = 0;
+            continue;
+        }
+        const int nb = buf ^ 1;
+        int n_out = 0;
+        if (lane == 0) {
+            fx::Head in[fx::MAX_NODES];
+            int step_row[fx::MAX_NODES], cid[fx::MAX_NODES * fx::MAX_BEAM];
+            double clp[fx::MAX_NODES * fx::MAX_BEAM];
+            const int n_in = __ldcg(a.bm_cnt + buf * NW + w);
+            const fx::Head* hs = a.bm_head + ((size_t)buf * NW + w) * fx::MAX_NODES;
+            int li = 0;
+            for (int b = 0; b < n_in; ++b) {
+                in[b].log_prob = __ldcg(&hs[b].log_prob);
+                in[b].finished = __ldcg(&hs[b].finished);
+                in[b].row = __ldcg(&hs[b].row);
+                in[b].len = __ldcg(&hs[b].len);
+                in[b].pad = 0;
+                if (in[b].finished) continue;
+                const int r = w * B + li++;   // the li-th live node sat in slot r at this position
+                step_row[b] = r;
+                for (int i = 0; i < B; ++i) {
+                    cid[b * B + i] = __ldcg(a.topk_id + (int64_t)r * B + i);
+                    clp[b * B + i] = (double)__ldcg(a.topk_lp + (int64_t)r * B + i);
+                }
+            }
+            fx::Pick out[fx::MAX_NODES];
+            n_out = fx::beam_step(in, n_in, step_row, cid, clp, B, a.eot, out);
+            fx::Head* ho = a.bm_head + ((size_t)nb * NW + w) * fx::MAX_NODES;
+            int nl = 0;
+            for (int i = 0; i < n_out; ++i) {
+                ho[i] = out[i].head;
+                in[i] = out[i].head;   // (for the stop test below)
+                pk_src[i] = out[i].src;
+                pk_tok[i] = out[i].token;
+                pk_len[i] = out[i].head.len;
+                if (!out[i].head.finished) {
+                    const int s = w * B + nl++;
+                    nx_par[s] = out[i].head.row;
+                    nx_tok[s] = out[i].token;
+                    nx_live[s] = 1;
+                }
+            }
+            for (; nl < B; ++nl) nx_live[w * B + nl] = 0;
+            a.bm_cnt[nb * NW + w] = n_out;
+            a.bm_win[2 * w] = nb;
+            a.bm_win[2 * w + 1] = fx::search_done(in, n_out) ? 1 : 0;
+        }
+        n_out = __shfl_sync(0xffffffffu, n_out, 0);
+        __syncwarp();
+        const int* src = a.bm_seq + ((size_t)buf * NW + w) * fx::MAX_NODES * t_max;
+        int* dst = a.bm_seq + ((size_t)nb * NW + w) * fx::MAX_NODES * t_max;
+        for (int i = 0; i < n_out; ++i) {   // node i = its source's sequence (+ the token it appends)
+            const int s = pk_src[i], tk = pk_tok[i], ln = pk_len[i] - (tk >= 0 ? 1 : 0);
+            for (int j = lane; j < ln; j += 32) dst[i * t_max + j] = __ldcg(src + s * t_max + j);
+            if (lane == 0 && tk >= 0) dst[i * t_max + ln] = tk;
+        }
+        __syncwarp();
+    }
+    bar_consumers();
+    // ---- (c)
+    if (tid == 0) {
+        int open = 0;
+        for (int w = 0; w < NW; ++w) open += __ldcg(a.bm_win + 2 * w + 1) ? 0 : 1;
+        ctl[2] = (depth + 1 >= a.max_depth || open == 0) ? 1 : 0;
+        ctl[3] = open;
+    }
+    bar_consumers();
+    if (ctl[2] == 0) {
+        int* an = (depth & 1) ? const_cast<int*>(a.anc) : a.anc_alt;   // beam mode owns both tables (session anc0 / anc1)
+        if (tid < R) {
+            a.slot_live[tid] = nx_live[tid];
+            if (nx_live[tid]) a.tokens[(int64_t)tid * t_max + p + 1] = nx_tok[tid];
+        }
+        const int P = p + 2;
+        for (int q = tid; q < R * P; q += 256) {
+            const int r = q / P, j = q % P;
+            if (nx_live[r]) an[(int64_t)r * t_max + j] = j <= p ? __ldcg(anc_cur + (int64_t)nx_par[r] * t_max + j) : r;
+        }
+    } else {
+        for (int w = warp; w < NW; w += NCW) {
+            const int buf = __ldcg(a.bm_win + 2 * w);
+            const fx::Head* hs = a.bm_head + ((size_t)buf * NW + w) * fx::MAX_NODES;
+            int best = 0, len = 0;
+            if (lane == 0) {
+                const int n = __ldcg(a.bm_cnt + buf * NW + w);
+                fx::Head hn[fx::MAX_NODES];
+                for (int b = 0; b < n; ++b) { hn[b].log_prob = __ldcg(&hs[b].log_prob); hn[b].finished = __ldcg(&hs[b].finished); }
+                best = max(fx::max_by_last(hn, n), 0);
+                len = n > 0 ? __ldcg(&hs[best].len) : 0;
+                a.bm_out_len[w] = len;
+            }
+            best = __shfl_sync(0xffffffffu, best, 0);
+            len = __shfl_sync(0xffffffffu, len, 0);
+            const int* s = a.bm_seq + (((size_t)buf * NW + w) * fx::MAX_NODES + best) * t_max;
+            for (int j = lane; j < len; j += 32) a.bm_out[(int64_t)w * t_max + j] = __ldcg(s + j);
+        }
+        if (tid == 0) {
+            *a.steps_done = depth + 1;
+            *a.pos = p + 1;
+            *a.n_unfinished = ctl[3];
+            a.bar[3] = 1;
+        }
+    }
+    bar_consumers();
+}
+
 // =====================================================================================================================
-template <int D, int NT8, typename KVT>
+// BEAM: the beam search (a.beam = B > 1).  A slot without a live beam idles at a position (no layer work, empty records);
+// the finisher (last CTA to deliver its records) ranks each live slot's candidates, runs one beamfx::beam_step per
+// unfinished window, places the new live beams in slots w * B + i, and builds the next position's ancestry table.
+template <int D, int NT8, typename KVT, bool BEAM = false>
 __global__ void __launch_bounds__(NTH6, 1)
 dec6_kernel(const DecArgs a) {
     using G = Geo<D>;
@@ -518,6 +742,13 @@ dec6_kernel(const DecArgs a) {
     uint64_t* pfree = pfull + 2;              // [2] consumers are done with the parameter block
     uint64_t* pbar = pfree + 2;               // [2] partial records of a phase landed
     uint64_t* lg_bar = pbar + 2;              // [NCW][LG_NBUF] logits stage
+    // beam mode: live slots of a step, double-buffered by step parity (the producer may still read one step's set while the
+    // consumers publish the next): [2][BM_LIVE] flags, [2][BM_LIVE] compact list of live rows, [2] their count; then the
+    // finisher's scratch (finish_beam)
+    int* live_s = reinterpret_cast<int*>(lg_bar + NCW * LG_NBUF);
+    int* live_rows = live_s + 2 * BM_LIVE;
+    int* n_live_s = live_rows + 2 * BM_LIVE;
+    int* nx_s = n_live_s + 2;                 // [BM_NX]
     // logits-stage scratch aliases the (then dead) parameter / partial buffers
     uint4* pl_hi = reinterpret_cast<uint4*>(params);                        // [NT8][D/32][32] fp16 hi plane of the LayerNorm rows, fragment order
     uint4* pl_lo = pl_hi + NT8 * (D / 32) * 32;
@@ -531,6 +762,20 @@ dec6_kernel(const DecArgs a) {
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     for (int i = tid; i < (G::KMAX / 64) * BX_SLAB / 16; i += NTH6) reinterpret_cast<uint4*>(bx)[i] = make_uint4(0, 0, 0, 0);   // rows 2..7 stay zero
+    // beam mode: step 0's live slots (set by the host: slot 0 of every window) into buffer 0
+    auto snapshot_live = [&](int buf) {   // tid < R load, one barrier, tid 0 compacts; the caller's next barrier publishes
+        if (tid < R) live_s[buf * BM_LIVE + tid] = __ldcg(a.slot_live + tid);
+        bar_consumers();
+        if (tid == 0) {
+            int n = 0;
+            for (int r = 0; r < R; ++r)
+                if (live_s[buf * BM_LIVE + r]) live_rows[buf * BM_LIVE + n++] = r;
+            n_live_s[buf] = n;
+        }
+    };
+    if constexpr (BEAM) {
+        if (tid < 256) snapshot_live(0);
+    }
     cl.sync();   // every CTA's mbarriers exist before any peer signals them
     Pipe P;
     P.ring = ring_mem; P.full = full; P.empty = empty; P.bx = bx;
@@ -555,7 +800,9 @@ dec6_kernel(const DecArgs a) {
         };
         for (int step = 0; step < a.n_steps; ++step) {
             if (lane == 0) {
-                for (int row = cluster_id; row < R; row += n_clusters) {
+                const int n_iter = BEAM ? n_live_s[step & 1] : R;
+                for (int it = cluster_id; it < n_iter; it += n_clusters) {
+                    const int row = BEAM ? live_rows[(step & 1) * BM_LIVE + it] : it;
                     const int w = __ldg(a.row_window + row);
                     const int T = __ldg(a.win_T + w);
                     for (int l = 0; l < L; ++l) {
@@ -624,8 +871,12 @@ dec6_kernel(const DecArgs a) {
         for (int step = 0; step < a.n_steps; ++step) {
             const int p = a.pos0 + step;
             const bool want_logits = p >= a.logits_from;
+            const int depth = p - a.logits_from;   // beam mode: search depth (< 0 in the prefill)
+            const int n_iter = BEAM ? n_live_s[step & 1] : R;
+            const int* anc_cur = depth > 0 && (depth & 1) ? a.anc_alt : a.anc;   // the prefill reads the identity table of depth 0
 #pragma unroll 1
-            for (int row = cluster_id; row < R; row += n_clusters) {
+            for (int it = cluster_id; it < n_iter; it += n_clusters) {
+                const int row = BEAM ? live_rows[(step & 1) * BM_LIVE + it] : it;
                 // ---- embed (mod.rs:141-146): every CTA of the cluster builds its own copy of x
                 {
                     const int tok = __ldcg(a.tokens + (int64_t)row * t_max + p);
@@ -655,7 +906,10 @@ dec6_kernel(const DecArgs a) {
                     KVT* vd = vcl + ((int64_t)row * t_max + p) * D + h * 64;
                     c = gemv_epi6<KVT>(P, c, 192, S_D, GemvOut<KVT>{EM_QKV, prm + G::P_BQKV, scale, qkv_s, kd, vd});
                     trace();   // [t2] q | k | v done
-                    self_attn6<KVT>(qkv_s, kcl + (int64_t)row * t_max * D + h * 64, vcl + (int64_t)row * t_max * D + h * 64, D, p, wm, wl, wo);
+                    if constexpr (BEAM)
+                        self_attn6_anc<KVT>(qkv_s, kcl + h * 64, vcl + h * 64, D, p, anc_cur + (int64_t)row * t_max, (int64_t)t_max * D, wm, wl, wo);
+                    else
+                        self_attn6<KVT>(qkv_s, kcl + (int64_t)row * t_max * D + h * 64, vcl + (int64_t)row * t_max * D + h * 64, D, p, wm, wl, wo);
                     attn_merge6(wm, wl, wo, bx, ys + D);
                     trace();   // [t3] self attention done
                     c = gemv_epi6<KVT>(P, c, D, 1, GemvOut<KVT>{EM_PLAIN, nullptr, 1.0f, ys, nullptr, nullptr});
@@ -710,11 +964,12 @@ dec6_kernel(const DecArgs a) {
                 static_assert(LG_NBUF * (int)BLKB <= RINGW, "logits ring");
                 const __half* Et = reinterpret_cast<const __half*>(a.E_tiled);
                 const int v_tiles = (V + 15) / 16;
-                const bool idle_cta = cluster_id >= R;
-                const int n_idle_w = max(0, n_clusters - R) * CS * NCW;
+                const int R_act = BEAM ? n_live_s[step & 1] : R;   // clusters >= R_act had no row this step
+                const bool idle_cta = cluster_id >= R_act;
+                const int n_idle_w = max(0, n_clusters - R_act) * CS * NCW;
                 const int na = (n_idle_w > 0 && 2 * n_idle_w <= v_tiles) ? 1 : 0;   // = what an idle warp has in its ring when the barrier opens
                 const int tiles_a = na * n_idle_w, tiles_b = v_tiles - tiles_a;
-                const int iw = ((cluster_id - R) * CS + rank) * NCW + warp;                 // index among the idle warps
+                const int iw = ((cluster_id - R_act) * CS + rank) * NCW + warp;             // index among the idle warps
                 const int my_a = idle_cta ? na : 0;
                 const int my_tiles = my_a + (gw < tiles_b ? (tiles_b - gw + n_gw - 1) / n_gw : 0);
                 const int total = my_tiles * 2;
@@ -755,7 +1010,7 @@ dec6_kernel(const DecArgs a) {
                 for (int r = warp; r < 8 * NT8; r += NCW) {
                     constexpr int NV = D / 128;   // float4 per lane
                     float4 v[NV];
-                    if (r < R) {
+                    if (r < R && (!BEAM || live_s[(step & 1) * BM_LIVE + r])) {
 #pragma unroll
                         for (int i = 0; i < NV; ++i) v[i] = __ldcg(reinterpret_cast<const float4*>(a.x + (int64_t)r * D) + lane + 32 * i);
                         float sum = 0.0f;
@@ -802,6 +1057,17 @@ dec6_kernel(const DecArgs a) {
                     for (int j = 0; j < NT8; ++j)
 #pragma unroll
                         for (int e = 0; e < 2; ++e) { m_run[j][e] = -INFINITY; s_run[j][e] = 0.0f; bv[j][e] = -INFINITY; bi[j][e] = INT_MAX; }
+                    // beam mode: this warp's candidate list per batch row, behind its logits buffers in its share of the ring
+                    constexpr int LST = 8 * NT8 * DEC_KC;
+                    static_assert(!BEAM || LG_NBUF * (int)BLKB + LST * 8 <= RINGW, "beam candidate lists");
+                    float* cl_v = reinterpret_cast<float*>(wring + LG_NBUF * BLKB);
+                    int* cl_i = reinterpret_cast<int*>(cl_v + LST);
+                    unsigned int live_m = 0;   // live batch rows
+                    if constexpr (BEAM) {
+                        for (int i = lane; i < LST; i += 32) { cl_v[i] = -INFINITY; cl_i[i] = INT_MAX; }
+                        for (int r = 0; r < R; ++r) live_m |= live_s[(step & 1) * BM_LIVE + r] ? 1u << r : 0u;
+                        __syncwarp();
+                    }
                     if (!idle_cta) {
                         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the ring was last written by bulk copies and read through the generic proxy
 #pragma unroll
@@ -836,7 +1102,41 @@ dec6_kernel(const DecArgs a) {
                                 mma16816(al[j], a0.z, a8.z, a0.w, a8.w, bl.z, bl.w);
                             }
                         }
-                        if (half == 1) {
+                        if (BEAM && half == 1) {
+                            // as below, but every value is a candidate: the lanes of one g insert theirs into the warp's
+                            // per-row lists, g by g (the four lanes of one g own distinct rows)
+                            const int n0 = tile_of(it >> 1) * 16;
+                            float cv[NT8][4];
+#pragma unroll
+                            for (int j = 0; j < NT8; ++j)
+#pragma unroll
+                                for (int c = 0; c < 4; ++c) {
+                                    const int n = n0 + g + (c >> 1) * 8, e = c & 1, rr = j * 8 + 2 * t + e;
+                                    cv[j][c] = __int_as_float(0x7fffffff);   // NaN: never inserted
+                                    if (n < V && rr < R && ((live_m >> rr) & 1u)) {
+                                        const float raw = fmaf(al[j][c], 1.0f / 2048.0f, ah[j][c]);
+                                        const float v = (use_mask && a.is_special[n]) ? __fadd_rn(raw, -INFINITY) : raw;
+                                        if (v > -INFINITY) {
+                                            if (v > m_run[j][e]) { s_run[j][e] = s_run[j][e] * expf(m_run[j][e] - v) + 1.0f; m_run[j][e] = v; }
+                                            else s_run[j][e] += expf(v - m_run[j][e]);
+                                        }
+                                        cv[j][c] = v;
+                                    }
+                                }
+#pragma unroll 1
+                            for (int gi = 0; gi < 8; ++gi) {
+                                if (g == gi) {
+#pragma unroll
+                                    for (int j = 0; j < NT8; ++j)
+#pragma unroll
+                                        for (int c = 0; c < 4; ++c) {
+                                            const int rr = j * 8 + 2 * t + (c & 1);
+                                            cand_insert(cl_v + rr * DEC_KC, cl_i + rr * DEC_KC, cv[j][c], n0 + g + (c >> 1) * 8);
+                                        }
+                                }
+                                __syncwarp();
+                            }
+                        } else if (half == 1) {
                             // C fragment: c0,c1 -> (vocabulary row g, batch rows 2t, 2t+1), c2,c3 -> (row g+8, same batch rows)
                             const int n0 = tile_of(it >> 1) * 16;
 #pragma unroll
@@ -873,7 +1173,7 @@ dec6_kernel(const DecArgs a) {
                                 const float mn = fmaxf(m_run[j][e], m2);
                                 s_run[j][e] = (m_run[j][e] > -INFINITY ? s_run[j][e] * expf(m_run[j][e] - mn) : 0.0f) + (m2 > -INFINITY ? s2 * expf(m2 - mn) : 0.0f);
                                 m_run[j][e] = mn;
-                                if (v2 > bv[j][e] || (v2 == bv[j][e] && i2 < bi[j][e])) { bv[j][e] = v2; bi[j][e] = i2; }
+                                if (!BEAM && (v2 > bv[j][e] || (v2 == bv[j][e] && i2 < bi[j][e]))) { bv[j][e] = v2; bi[j][e] = i2; }
                             }
                             if (g == 0) {
                                 float* rec = red + (warp * 8 * NT8 + j * 8 + 2 * t + e) * 4;
@@ -881,7 +1181,34 @@ dec6_kernel(const DecArgs a) {
                             }
                         }
                     bar_consumers();
-                    if (tid < R) {
+                    if (BEAM && tid < R && ((live_m >> tid) & 1u)) {
+                        // the CTA's record of a live row: (max, sum) as below, and its DEC_KC best (value, id) from the 8 warps'
+                        // lists, merged into warp 0's list (each list is sorted: the first entry that stays out ends a list)
+                        float M = -INFINITY;
+                        for (int w2 = 0; w2 < NCW; ++w2) M = fmaxf(M, red[(w2 * 8 * NT8 + tid) * 4]);
+                        float Ssum = 0.0f;
+                        for (int w2 = 0; w2 < NCW; ++w2) {
+                            const float* rec = red + (w2 * 8 * NT8 + tid) * 4;
+                            if (rec[0] > -INFINITY) Ssum += rec[1] * expf(rec[0] - M);
+                        }
+                        float* acc_v = reinterpret_cast<float*>(ring_mem + LG_NBUF * BLKB) + tid * DEC_KC;
+                        int* acc_i = reinterpret_cast<int*>(reinterpret_cast<float*>(ring_mem + LG_NBUF * BLKB) + LST) + tid * DEC_KC;
+                        for (int w2 = 1; w2 < NCW; ++w2) {
+                            const float* sv = reinterpret_cast<const float*>(ring_mem + (size_t)w2 * RINGW + LG_NBUF * BLKB) + tid * DEC_KC;
+                            const int* si = reinterpret_cast<const int*>(reinterpret_cast<const float*>(ring_mem + (size_t)w2 * RINGW + LG_NBUF * BLKB) + LST) + tid * DEC_KC;
+                            for (int k = 0; k < DEC_KC; ++k) {
+                                const float v = sv[k];
+                                const int n = si[k];
+                                if (!(v > acc_v[DEC_KC - 1] || (v == acc_v[DEC_KC - 1] && n < acc_i[DEC_KC - 1]))) break;
+                                cand_insert(acc_v, acc_i, v, n);
+                            }
+                        }
+                        const int64_t o = (int64_t)blockIdx.x * R + tid;
+                        a.lg_m[o] = M;
+                        a.lg_s[o] = Ssum;
+#pragma unroll
+                        for (int k = 0; k < DEC_KC; ++k) { a.lg_v[o * DEC_KC + k] = acc_v[k]; a.lg_i[o * DEC_KC + k] = acc_i[k]; }
+                    } else if (!BEAM && tid < R) {
                         float M = -INFINITY;
                         for (int w2 = 0; w2 < NCW; ++w2) M = fmaxf(M, red[(w2 * 8 * NT8 + tid) * 4]);
                         float Ssum = 0.0f, best_v = -INFINITY;
@@ -910,6 +1237,9 @@ dec6_kernel(const DecArgs a) {
                 bar_consumers();
                 if (ctl[1]) {
                     __threadfence();
+                    if constexpr (BEAM) {
+                        finish_beam(a, p, depth, anc_cur, ring_mem, live_s + (step & 1) * BM_LIVE, nx_s, ctl);
+                    } else
                     for (int r = warp; r < R; r += NCW) {
                         // <= 160 co-resident CTAs: at most 5 records per lane, every load issued before any use (one L2 round trip)
                         const int NP = gridDim.x;
@@ -969,18 +1299,25 @@ dec6_kernel(const DecArgs a) {
                 }
                 bar_consumers();
                 trace();
-                int live = 0;
-                for (int r = 0; r < R; ++r) live += __ldcg(a.finished + r) ? 0 : 1;
-                if (live == 0) {
-                    stop = 1;
-                    if (blockIdx.x == 0 && tid == 0) { *a.pos = p + 1; *a.n_unfinished = 0; *a.steps_done = step + 1; }
+                if constexpr (BEAM) {
+                    stop = __ldcg(a.bar + 3) != 0;   // set by the finisher when the search ended
+                } else {
+                    int live = 0;
+                    for (int r = 0; r < R; ++r) live += __ldcg(a.finished + r) ? 0 : 1;
+                    if (live == 0) {
+                        stop = 1;
+                        if (blockIdx.x == 0 && tid == 0) { *a.pos = p + 1; *a.n_unfinished = 0; *a.steps_done = step + 1; }
+                    }
                 }
+            }
+            if constexpr (BEAM) {
+                if (!stop) snapshot_live((step + 1) & 1);   // the next position's live slots (the finisher placed them)
             }
             if (tid == 0) ctl[0] = stop;
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic accesses to the aliased buffers before the next step's bulk copies
             bar_all();   // hands the ring back to the producer; it reads the stop flag after this barrier
             if (stop) break;
-            if (step + 1 == a.n_steps && blockIdx.x == 0 && tid == 0) {
+            if (!BEAM && step + 1 == a.n_steps && blockIdx.x == 0 && tid == 0) {
                 *a.pos = a.pos0 + a.n_steps;
                 int live = 0;
                 for (int r = 0; r < R; ++r) live += __ldcg(a.finished + r) ? 0 : 1;
@@ -992,20 +1329,20 @@ dec6_kernel(const DecArgs a) {
     cl.sync();   // no CTA leaves while a peer may still address its shared memory
 }
 
-template <int D, int NT8>
+template <int D, int NT8, bool BEAM = false>
 constexpr size_t dec6_smem() {
     using G = Geo<D>;
     return 1024 + (size_t)NSLOT * SLOT + (size_t)(G::KMAX / 64) * BX_SLAB +
            sizeof(float) * ((size_t)2 * G::PARAMS + 2 * G::CS * G::SEND + 2 * G::SEND + D + 192 + 64 + G::NS + 16 + 8 + 8 + 512 + 4 + NSLOT) +
-           8 * (size_t)(2 * NSLOT + 6 + NCW * LG_NBUF) + 64;
+           8 * (size_t)(2 * NSLOT + 6 + NCW * LG_NBUF) + 64 + (BEAM ? sizeof(int) * (4 * BM_LIVE + 2 + BM_NX) : 0);
 }
 
-template <int D, int NT8, typename KVT>
+template <int D, int NT8, typename KVT, bool BEAM = false>
 bool launch6_t(const DecArgs& a, cudaStream_t st) {
     using G = Geo<D>;
     static_assert((size_t)2 * NT8 * (D / 32) * 32 * 16 + (size_t)NCW * 8 * NT8 * 16 <= sizeof(float) * (2 * G::PARAMS + 2 * G::CS * G::SEND), "logits scratch must fit the aliased buffers");
-    const void* k = (const void*)dec6_kernel<D, NT8, KVT>;
-    const size_t smem = dec6_smem<D, NT8>();
+    const void* k = (const void*)dec6_kernel<D, NT8, KVT, BEAM>;
+    const size_t smem = dec6_smem<D, NT8, BEAM>();
     static ClusterLaunch cl;   // per instantiation
     const int n_cl = cl.capacity(k, G::CS, NTH6, smem, "dec6");
     if (n_cl < 1) return false;
@@ -1079,8 +1416,14 @@ void build_pack_t(const Model& m, Dec6Pack& pk, cudaStream_t st) {
 }  // namespace
 
 // Returns false when this configuration is not covered.  The packed weights are built on the first launch.
+//   greedy: k = 1, identity ancestry (a.anc == nullptr);
+//   beam search (a.beam = B in 2..7): rows = n_win * B, prefill from position 0, ancestry tables anc / anc_alt, k = B.
 bool launch_dec6(DecArgs a, const Model& m, Dec6Pack& pk, cudaStream_t st) {
-    if (!m.fp16_exact || a.R > 24 || a.R < 1 || a.k != 1 || !a.greedy || a.use_cur_tok || a.anc != nullptr || a.logits_out != nullptr) return false;
+    const bool beam = a.beam > 1;
+    if (!m.fp16_exact || a.R > BM_LIVE || a.R < 1 || a.use_cur_tok || a.logits_out != nullptr) return false;
+    if (!beam && (a.k != 1 || !a.greedy || a.anc != nullptr)) return false;
+    if (beam && (a.beam > beamfx::MAX_BEAM || a.k != a.beam || a.greedy || a.R != a.n_win * a.beam || a.pos0 != 0 || a.max_depth < 1 ||
+                 a.anc == nullptr || a.anc_alt == nullptr || a.slot_live == nullptr || a.bm_head == nullptr)) return false;
     if ((a.d != 128 && a.d != 384) || a.H * 64 != a.d || a.E_tiled == nullptr || a.t_max > 128) return false;
     if (pk.pack.p == nullptr) {
         if (a.d == 384) build_pack_t<384>(m, pk, st);
@@ -1088,7 +1431,9 @@ bool launch_dec6(DecArgs a, const Model& m, Dec6Pack& pk, cudaStream_t st) {
     }
     a.d6_pack = pk.pack.p;
     a.d6_params = pk.params.p;
-#define WB_D6(DD, NT8_) (a.kv_half ? launch6_t<DD, NT8_, __half>(a, st) : launch6_t<DD, NT8_, float>(a, st))
+#define WB_D6(DD, NT8_)                                                                                                  \
+    (beam ? (a.kv_half ? launch6_t<DD, NT8_, __half, true>(a, st) : launch6_t<DD, NT8_, float, true>(a, st))             \
+          : (a.kv_half ? launch6_t<DD, NT8_, __half>(a, st) : launch6_t<DD, NT8_, float>(a, st)))
     if (a.d == 384) return a.R <= 8 ? WB_D6(384, 1) : WB_D6(384, 3);
     return a.R <= 8 ? WB_D6(128, 1) : WB_D6(128, 3);
 #undef WB_D6

@@ -400,8 +400,8 @@ void Session::begin(const int64_t* prompt, int64_t prompt_len, bool prefill) {
 
 // The persistent decoder for n_steps positions starting at pos0: the first of decoder4 -> decoder6 -> decoder5 -> decoder3
 // that covers the launch (each launch_decN decides that itself), or only the one WB200_DECODER names.
-void Session::launch_decoder(int R_, int pos0, int n_steps, int logits_from, bool use_cur_tok, int mask_mode, int k,
-                        bool greedy, int eot) {
+bool Session::launch_decoder(int R_, int pos0, int n_steps, int logits_from, bool use_cur_tok, int mask_mode, int k,
+                        bool greedy, int eot, int beam, int max_depth) {
     const wb_dims& D = m->dims;
     const int d = D.n_text_state, H = D.n_text_head;
     DecArgs a;
@@ -438,7 +438,13 @@ void Session::launch_decoder(int R_, int pos0, int n_steps, int logits_from, boo
     auto allowed = [&](int n) { return only_decoder == 0 || only_decoder == n; };
     int groups = 0;
     last_groups = 1;
-    if (allowed(4) && launch_dec4(a, h16, st)) last_decoder = 4;
+    if (beam > 1) {   // the whole search: only decoder6 has a beam mode
+        a.beam = beam; a.n_win = R_ / beam; a.max_depth = max_depth;
+        a.anc = anc0.p; a.anc_alt = anc1.p; a.slot_live = slot_live.p;
+        a.bm_head = bm_head.p; a.bm_seq = bm_seq.p; a.bm_cnt = bm_cnt.p; a.bm_win = bm_win.p; a.bm_out = bm_out.p; a.bm_out_len = bm_out_len.p;
+        if (!allowed(6) || !launch_dec6(a, *m, d6, st)) return false;
+        last_decoder = 6;
+    } else if (allowed(4) && launch_dec4(a, h16, st)) last_decoder = 4;
     else if (allowed(6) && launch_dec6(a, *m, d6, st)) last_decoder = 6;
     else if (allowed(5) && (groups = launch_dec5(a, d5, n_sm, h16, st)) > 0) { last_decoder = 5; last_groups = groups; }
     else if (allowed(3)) { launch_dec3(a, n_sm, h16, st); last_decoder = 3; }
@@ -456,6 +462,7 @@ void Session::launch_decoder(int R_, int pos0, int n_steps, int logits_from, boo
             fclose(f);
         }
     }
+    return true;
 }
 
 void Session::step_core(bool with_logits, int mask_mode, int k, bool greedy, int eot) {
@@ -561,6 +568,63 @@ void Session::greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_d
     out.assign((size_t)R, {});
     for (int r = 0; r < R; ++r)
         for (int i = 0; i < len[(size_t)r]; ++i) out[(size_t)r].push_back(tk[(size_t)r * t_max + i]);
+}
+
+bool Session::beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_size, int max_depth, int64_t eot,
+                          std::vector<std::vector<int64_t>>& out) {
+    namespace fx = beamfx;
+    if (!encoded) fail(WB_ERR_STATE, "session: decode before encode");
+    WB_REQUIRE(prompt_len >= 1 && prompt_len + max_depth <= t_max, "beam: prompt + max_depth exceeds the session's max_text_len");
+    const int B = beam_size, W = n_windows, Rb = W * B, V = m->dims.n_vocab;
+    if (B < 2 || B > fx::MAX_BEAM || max_depth < 1 || Rb > Rmax) return false;
+    for (int64_t i = 0; i < prompt_len; ++i) WB_REQUIRE(prompt[i] >= 0 && prompt[i] < V, "beam: prompt token out of range");
+    constexpr int MN = fx::MAX_NODES;
+    slot_live.ensure((size_t)Rmax);
+    bm_head.ensure((size_t)2 * W * MN); bm_seq.ensure((size_t)2 * W * MN * t_max);
+    bm_cnt.ensure((size_t)2 * W); bm_win.ensure((size_t)2 * W);
+    bm_out.ensure((size_t)W * t_max); bm_out_len.ensure((size_t)W);
+    // slot i of window w = row w * B + i; until the first search step only slot 0 holds a beam: the prompt, in its own cache row
+    std::vector<int> tk((size_t)Rb * t_max, 0), rw((size_t)Rb), live((size_t)Rb);
+    for (int r = 0; r < Rb; ++r) {
+        for (int64_t i = 0; i < prompt_len; ++i) tk[(size_t)r * t_max + i] = (int)prompt[i];
+        rw[(size_t)r] = r / B;
+        live[(size_t)r] = r % B == 0 ? 1 : 0;
+    }
+    std::vector<fx::Head> heads((size_t)W * MN, fx::Head{0.0, 0, 0, 0, 0});
+    std::vector<int> seq((size_t)W * MN * t_max, 0), cnt((size_t)2 * W, 0), win((size_t)2 * W, 0);   // depth-0 buffer; window: {buffer, done}
+    for (int w = 0; w < W; ++w) {
+        heads[(size_t)w * MN] = fx::Head{0.0, prompt[prompt_len - 1] == eot ? 1 : 0, w * B, (int)prompt_len, 0};
+        for (int64_t i = 0; i < prompt_len; ++i) seq[(size_t)w * MN * t_max + i] = (int)prompt[i];
+        cnt[(size_t)w] = 1;
+    }
+    WB_CUDA(cudaMemcpyAsync(tokens.p, tk.data(), tk.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    WB_CUDA(cudaMemcpyAsync(row_window.p, rw.data(), rw.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    WB_CUDA(cudaMemcpyAsync(slot_live.p, live.data(), live.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    WB_CUDA(cudaMemcpyAsync(bm_head.p, heads.data(), heads.size() * sizeof(fx::Head), cudaMemcpyHostToDevice, st));
+    WB_CUDA(cudaMemcpyAsync(bm_seq.p, seq.data(), seq.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    WB_CUDA(cudaMemcpyAsync(bm_cnt.p, cnt.data(), cnt.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    WB_CUDA(cudaMemcpyAsync(bm_win.p, win.data(), win.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    launch_dec_anc_identity(anc0.p, Rb, t_max, st);
+    const bool ran = launch_decoder(Rb, 0, (int)prompt_len - 1 + max_depth, (int)prompt_len - 1, false, 2, B, false, (int)eot, B, max_depth);
+    std::vector<int> res((size_t)W * t_max), res_len((size_t)W);
+    int sd = 0;
+    if (ran) {
+        WB_CUDA(cudaMemcpyAsync(res.data(), bm_out.p, res.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+        WB_CUDA(cudaMemcpyAsync(res_len.data(), bm_out_len.p, res_len.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+        WB_CUDA(cudaMemcpyAsync(&sd, steps_done.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    }
+    WB_CUDA(cudaStreamSynchronize(st));   // the host vectors above are in flight until here
+    if (!ran) return false;
+    // session state as the host search leaves it: rows, position, ancestry of the last position
+    R = Rb;
+    last_steps = sd;
+    host_pos = (int)prompt_len - 1 + sd;
+    anc_identity = false;
+    anc_cur = (sd - 1) & 1;
+    out.assign((size_t)W, {});
+    for (int w = 0; w < W; ++w)
+        for (int i = 0; i < res_len[(size_t)w]; ++i) out[(size_t)w].push_back(res[(size_t)w * t_max + i]);
+    return true;
 }
 
 }  // namespace wb

@@ -81,8 +81,12 @@ struct Session {
     DevBuf<int> steps_done;
     DevBuf<float> datt;
     DevBuf<unsigned long long> dec_trace;   // debug: WB200_TRACE=1
-    void launch_decoder(int R_, int pos0, int n_steps, int logits_from, bool use_cur_tok, int mask_mode, int k, bool greedy,
-                   int eot);
+    // beam > 1: the whole beam search in one decoder6 launch (beam_decode); returns false when decoder6 does not cover it
+    bool launch_decoder(int R_, int pos0, int n_steps, int logits_from, bool use_cur_tok, int mask_mode, int k, bool greedy,
+                   int eot, int beam = 0, int max_depth = 0);
+    // device beam search state (decoder6.cu beam mode), allocated on first use
+    DevBuf<int> slot_live, bm_seq, bm_cnt, bm_win, bm_out, bm_out_len;
+    DevBuf<beamfx::Head> bm_head;
     bool full_logits = false;    // also write raw logits [R][V] (stateless forward_decoder)
     int n_logit_ctas = 0;
     DevBuf<float> ypart, lg_m, lg_s, lg_v;
@@ -115,6 +119,10 @@ struct Session {
     // greedy loop on the device; returns per-window token lists
     void greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_depth, int64_t eot,
                        std::vector<std::vector<int64_t>>& out);
+    // the whole beam search (prefill + up to max_depth steps) of every encoded window in ONE decoder launch; false (nothing
+    // decoded) when no decoder covers it, and the caller runs the host search
+    bool beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_size, int max_depth, int64_t eot,
+                     std::vector<std::vector<int64_t>>& out);
 };
 
 // host pipeline (transcribe.cu)

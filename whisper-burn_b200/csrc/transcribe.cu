@@ -79,7 +79,13 @@ void transcribe_windows(Session& s, int beam_size, int max_depth, const wb_speci
         WB_CUDA(cudaEventRecord(s.ev[3], s.st));
         return;
     }
-    // ---- beam search, all windows in lock-step
+    // ---- beam search: on the device in one launch where decoder6 covers it (fp16-exact weights, d = 128 / 384,
+    // n_windows * beam_size <= 24, t_max <= 128), same selection rules and ids as the host search below
+    if (max_depth > 0 && s.beam_decode(prompt, 4, beam_size, max_depth, ids.eot, out)) {
+        WB_CUDA(cudaEventRecord(s.ev[3], s.st));
+        return;
+    }
+    // ---- otherwise the host search, all windows in lock-step
     const int64_t eot = ids.eot;
     auto is_finished = [eot](const std::vector<BeamSearchToken>& seq) { return !seq.empty() && seq.back().token == eot; };
     std::vector<std::vector<Node>> beams((size_t)W);
