@@ -1,5 +1,6 @@
-// Device helpers shared by the persistent decoders (decoder3.cu: grid-barrier version, decoder4.cu:
-// cluster / DSMEM version).  Internal; everything lives in an anonymous namespace of the including TU.
+// Device helpers shared by the persistent decoders decoder3.cu .. decoder6.cu: staging, GEMV and attention building blocks,
+// and the one definition of the candidate ranking, the softmax state, the per-(CTA, row) record and the per-row finish.
+// Internal; everything lives in an anonymous namespace of the including TU.
 #pragma once
 #include <algorithm>
 #include <type_traits>
@@ -853,6 +854,22 @@ __device__ __forceinline__ void store_frag(uint4* xhi, uint4* xlo, int nchunks, 
 }
 
 // ---- top candidates --------------------------------------------------------------------------------------
+// The ranking of vocabulary candidates, the only place it is written (DESIGN.md section 2): the higher value first, the
+// lower id on equal values.  An empty candidate is (-inf, INT_MAX).
+__device__ __forceinline__ bool cand_better(float v, int i, float bv, int bi) { return v > bv || (v == bv && i < bi); }
+
+// one xor-shuffle step of a warp arg-max: (bv, bi) becomes the better of this lane's and lane ^ off's
+__device__ __forceinline__ void cand_xor(float& bv, int& bi, int off) {
+    const float ov = __shfl_xor_sync(0xffffffffu, bv, off);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
+    if (cand_better(ov, oi, bv, bi)) { bv = ov; bi = oi; }
+}
+// arg-max over the warp: every lane ends with the warp's best (bv, bi)
+__device__ __forceinline__ void warp_best(float& bv, int& bi) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) cand_xor(bv, bi, o);
+}
+
 template <int KC>
 struct Cand {
     float v[KC];
@@ -861,20 +878,227 @@ struct Cand {
 #pragma unroll
         for (int k = 0; k < KC; ++k) { v[k] = -INFINITY; i[k] = INT_MAX; }
     }
-    __device__ __forceinline__ void push(float val, int idx) {   // keep the KC best by (value desc, index asc)
-        if (!(val > v[KC - 1] || (val == v[KC - 1] && idx < i[KC - 1]))) return;
+    __device__ __forceinline__ void push(float val, int idx) {   // keep the KC best
+        if (!cand_better(val, idx, v[KC - 1], i[KC - 1])) return;
         v[KC - 1] = val;
         i[KC - 1] = idx;
 #pragma unroll
         for (int k = KC - 1; k > 0; --k) {
-            const bool better = v[k] > v[k - 1] || (v[k] == v[k - 1] && i[k] < i[k - 1]);
-            if (better) {
+            if (cand_better(v[k], i[k], v[k - 1], i[k - 1])) {
                 const float tv = v[k]; v[k] = v[k - 1]; v[k - 1] = tv;
                 const int ti = i[k]; i[k] = i[k - 1]; i[k - 1] = ti;
             }
         }
     }
 };
+
+// The same list in shared memory, DEC_KC entries sorted best first; false when (v, n) stays out
+__device__ __forceinline__ bool cand_insert(float* lv, int* li, float v, int n) {
+    if (!cand_better(v, n, lv[DEC_KC - 1], li[DEC_KC - 1])) return false;
+    int k = DEC_KC - 1;
+    for (; k > 0 && cand_better(v, n, lv[k - 1], li[k - 1]); --k) { lv[k] = lv[k - 1]; li[k] = li[k - 1]; }
+    lv[k] = v;
+    li[k] = n;
+    return true;
+}
+
+// ---- softmax state: running max m and sum of exp(v - m) -----------------------------------------------
+// one more finite value v
+__device__ __forceinline__ void softmax_add(float& m, float& s, float v) {
+    if (v > m) { s = s * expf(m - v) + 1.0f; m = v; }
+    else s += expf(v - m);
+}
+// the state (m2, s2) of other values; an empty state has m = -inf
+__device__ __forceinline__ void softmax_merge(float& m, float& s, float m2, float s2) {
+    const float mn = fmaxf(m, m2);
+    s = (m > -INFINITY ? s * expf(m - mn) : 0.0f) + (m2 > -INFINITY ? s2 * expf(m2 - mn) : 0.0f);
+    m = mn;
+}
+
+// ---- one record per (CTA, row) --------------------------------------------------------------------------
+// The vocabulary stage leaves, per (CTA or slice c, row r), a record at o = c * R + r: lg_m / lg_s (max, sum-exp) and the
+// best candidates, lg_v / lg_i[o] for a top-1 record, lg_v / lg_i[o * KC + k] for a KC list.
+// (max, sum-exp) of n per-warp records rec[w * ld] = {max, sum-exp, ...}, folded in record order
+__device__ __forceinline__ float2 fold_softmax(const float* rec, int n, int ld) {
+    float M = -INFINITY;
+    for (int w = 0; w < n; ++w) M = fmaxf(M, rec[w * ld]);
+    float S = 0.0f;
+    for (int w = 0; w < n; ++w)
+        if (rec[w * ld] > -INFINITY) S += rec[w * ld + 1] * expf(rec[w * ld] - M);
+    return make_float2(M, S);
+}
+// the top-1 record o from n per-warp records rec[w * ld] = {max, sum-exp, best value, best id as float bits}
+__device__ __forceinline__ void fold_records_top1(const DecArgs& a, const float* rec, int n, int ld, int64_t o) {
+    const float2 ms = fold_softmax(rec, n, ld);
+    float bv = -INFINITY;
+    int bi = INT_MAX;
+    for (int w = 0; w < n; ++w) {
+        const int ci = __float_as_int(rec[w * ld + 3]);
+        if (cand_better(rec[w * ld + 2], ci, bv, bi)) { bv = rec[w * ld + 2]; bi = ci; }
+    }
+    a.lg_m[o] = ms.x;
+    a.lg_s[o] = ms.y;
+    a.lg_v[o] = bv;
+    a.lg_i[o] = bi;
+}
+// the KC-list record o from n per-warp records rec[w * ld] = {max, sum-exp, KC values, KC ids as float bits}, sorted
+// lists of which the first nk entries can matter
+template <int KC>
+__device__ __forceinline__ void fold_records(const DecArgs& a, const float* rec, int n, int ld, int nk, int64_t o) {
+    const float2 ms = fold_softmax(rec, n, ld);
+    Cand<KC> best;
+    best.init();
+    for (int w = 0; w < n; ++w)
+        for (int k = 0; k < nk; ++k) best.push(rec[w * ld + 2 + k], __float_as_int(rec[w * ld + 2 + KC + k]));
+    a.lg_m[o] = ms.x;
+    a.lg_s[o] = ms.y;
+#pragma unroll
+    for (int k = 0; k < KC; ++k) { a.lg_v[o * KC + k] = best.v[k]; a.lg_i[o * KC + k] = best.i[k]; }
+}
+
+// ---- per-row finish: log-probs (v - max) - lse of the candidates, lse from the NP records of the row (DESIGN.md section 2)
+// greedy bookkeeping of row r at position p (beam.rs:9-37 with beam_size 1): the token, the length, EOT
+__device__ __forceinline__ void greedy_commit(const DecArgs& a, int r, int p, int id) {
+    if (a.greedy && !__ldcg(a.finished + r)) {
+        a.tokens[(int64_t)r * a.t_max + p + 1] = id;
+        a.lengths[r] = p + 2;
+        if (id == a.eot) a.finished[r] = 1;
+    }
+}
+// rows whose search is still open: every row, or in a greedy search those that have not produced EOT
+__device__ __forceinline__ int rows_open(const DecArgs& a) {
+    int live = 0;
+    for (int r = 0; r < a.R; ++r) live += (a.greedy && __ldcg(a.finished + r)) ? 0 : 1;
+    return live;
+}
+// where a launch stopped: the next position, the searches still open and the steps run (written by one thread)
+__device__ __forceinline__ void decode_done(const DecArgs& a, int pos, int n_open, int steps) {
+    *a.pos = pos;
+    *a.n_unfinished = n_open;
+    *a.steps_done = steps;
+}
+
+// Warp per row: the max and lse of the row's NP <= 32 * NPL records, record lane + 32 k in rm[k] / rs[k] of this lane
+template <int NPL>
+__device__ __forceinline__ float row_lse(const float (&rm)[NPL], const float (&rs)[NPL], int NP, float& mx) {
+    const int lane = threadIdx.x & 31;
+    mx = -INFINITY;
+#pragma unroll
+    for (int k = 0; k < NPL; ++k)
+        if (lane + 32 * k < NP) mx = fmaxf(mx, rm[k]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    float se = 0.0f;
+#pragma unroll
+    for (int k = 0; k < NPL; ++k)
+        if (lane + 32 * k < NP && rm[k] > -INFINITY) se += rs[k] * expf(rm[k] - mx);
+    return logf(warp_sum(se));
+}
+// Warp per row, k = 1: the best candidate of row r from its NP <= 32 * NPL top-1 records, all loads issued before any use
+// (one L2 round trip) -> topk_id / topk_lp [r], then the greedy bookkeeping
+template <int NPL>
+__device__ __forceinline__ void finish_row_top1(const DecArgs& a, int r, int p, int NP) {
+    const int lane = threadIdx.x & 31, R = a.R;
+    float rm[NPL], rs[NPL], rv[NPL];
+    int ri[NPL];
+#pragma unroll
+    for (int k = 0; k < NPL; ++k) {
+        const int64_t o = (int64_t)min(lane + 32 * k, NP - 1) * R + r;
+        rm[k] = __ldcg(a.lg_m + o);
+        rs[k] = __ldcg(a.lg_s + o);
+        rv[k] = __ldcg(a.lg_v + o);
+        ri[k] = __ldcg(a.lg_i + o);
+    }
+    float mx;
+    const float lse = row_lse<NPL>(rm, rs, NP, mx);
+    float bv = -INFINITY;
+    int bi = INT_MAX;
+#pragma unroll
+    for (int k = 0; k < NPL; ++k)
+        if (lane + 32 * k < NP && ri[k] != INT_MAX && cand_better(rv[k], ri[k], bv, bi)) { bv = rv[k]; bi = ri[k]; }
+    warp_best(bv, bi);
+    if (lane == 0) {
+        a.topk_id[r] = bi == INT_MAX ? -1 : bi;
+        a.topk_lp[r] = __fsub_rn(__fsub_rn(bv, mx), lse);
+        greedy_commit(a, r, p, bi);
+    }
+}
+// CTA per row, the k best candidates of row r from its NP KC-list records -> topk_id / topk_lp [r][k]; candidate 0 goes
+// to the greedy bookkeeping.  s_f / s_i: NW floats / ints of shared scratch.  Called by the whole CTA.
+template <int KC>
+__device__ __forceinline__ void finish_row_topk(const DecArgs& a, int r, int p, int NP, float* s_f, int* s_i) {
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, R = a.R;
+    float mx = -INFINITY;
+    for (int c = tid; c < NP; c += NT) mx = fmaxf(mx, __ldcg(a.lg_m + (int64_t)c * R + r));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if (lane == 0) s_f[warp] = mx;
+    __syncthreads();
+    mx = s_f[0];
+#pragma unroll
+    for (int w = 1; w < NW; ++w) mx = fmaxf(mx, s_f[w]);
+    __syncthreads();
+    float se = 0.0f;
+    for (int c = tid; c < NP; c += NT) {
+        const float m = __ldcg(a.lg_m + (int64_t)c * R + r);
+        if (m > -INFINITY) se += __ldcg(a.lg_s + (int64_t)c * R + r) * expf(m - mx);
+    }
+    se = warp_sum(se);
+    if (lane == 0) s_f[warp] = se;
+    __syncthreads();
+    se = 0.0f;
+#pragma unroll
+    for (int w = 0; w < NW; ++w) se += s_f[w];
+    const float lse = logf(se);
+    __syncthreads();
+    float prev_v = INFINITY;
+    int prev_i = -1;
+    for (int kk = 0; kk < a.k; ++kk) {   // the best candidate ranked after the previous one
+        float bv = -INFINITY;
+        int bi = INT_MAX;
+        for (int c = tid; c < NP * KC; c += NT) {
+            const int part = c / KC, k = c % KC;
+            const int idx = __ldcg(a.lg_i + ((int64_t)part * R + r) * KC + k);
+            if (idx == INT_MAX) continue;
+            const float v = __fsub_rn(__fsub_rn(__ldcg(a.lg_v + ((int64_t)part * R + r) * KC + k), mx), lse);
+            if (cand_better(prev_v, prev_i, v, idx) && cand_better(v, idx, bv, bi)) { bv = v; bi = idx; }
+        }
+        warp_best(bv, bi);
+        if (lane == 0) { s_f[warp] = bv; s_i[warp] = bi; }
+        __syncthreads();
+        bv = s_f[0];
+        bi = s_i[0];
+#pragma unroll
+        for (int w = 1; w < NW; ++w)
+            if (cand_better(s_f[w], s_i[w], bv, bi)) { bv = s_f[w]; bi = s_i[w]; }
+        __syncthreads();
+        if (tid == 0) {
+            a.topk_id[(int64_t)r * a.k + kk] = bi == INT_MAX ? -1 : bi;
+            a.topk_lp[(int64_t)r * a.k + kk] = bv;
+            if (kk == 0) greedy_commit(a, r, p, bi);
+        }
+        prev_v = bv;
+        prev_i = bi;
+    }
+}
+
+// ---- ticket finish (decoder4, decoder6): every CTA takes a ticket after publishing its records; the CTA that takes the last
+// ticket of round n finishes the step and releases the flag the others wait on.  bar[1]: tickets, bar[2]: flag (the
+// rounds released so far); both zeroed by the host before the launch.  Called by one thread.
+__device__ __forceinline__ bool last_ticket(unsigned int* bar, unsigned int n) {
+    __threadfence();
+    return atomicAdd(bar + 1, 1u) == n * gridDim.x - 1;
+}
+__device__ __forceinline__ void release_flag(unsigned int* bar, unsigned int gen) {
+    __threadfence();
+    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(bar + 2), "r"(gen) : "memory");
+}
+// watchdog: SM clocks the wait may last before the kernel traps (fail loudly instead of hanging the GPU)
+__device__ __forceinline__ void wait_flag(const unsigned int* bar, unsigned int gen, long long watchdog) {
+    const long long t0 = clock64();
+    while (ld_acquire(bar + 2) < gen)
+        if (clock64() - t0 > watchdog) __trap();
+}
 
 
 }  // namespace

@@ -281,10 +281,7 @@ dec3_kernel(const DecArgs a) {
                                 const float raw = pick_row<RC>(acc[g], l8);
                                 if (a.logits_out) a.logits_out[(int64_t)(r0 + l8) * V + nn[g]] = raw;
                                 const float v = (use_mask && a.is_special[nn[g]]) ? __fadd_rn(raw, -INFINITY) : raw;
-                                if (v > -INFINITY) {
-                                    if (v > m_run) { s_run = s_run * expf(m_run - v) + 1.0f; m_run = v; }
-                                    else s_run += expf(v - m_run);
-                                }
+                                if (v > -INFINITY) softmax_add(m_run, s_run, v);
                                 cand.push(v, nn[g]);
                             }
                         }
@@ -299,117 +296,26 @@ dec3_kernel(const DecArgs a) {
                     for (int k = 0; k < KC; ++k) { rec[2 + k] = cand.v[k]; rec[2 + KC + k] = __int_as_float(cand.i[k]); }
                 }
                 __syncthreads();
-                if (tid < RC && r0 + tid < R) {
-                    float M = -INFINITY;
-                    for (int w = 0; w < NW * 4; ++w) M = fmaxf(M, red[(w * RC + tid) * (2 + 2 * KC)]);
-                    float Ssum = 0.0f;
-                    Cand<KC> best;
-                    best.init();
-                    for (int w = 0; w < NW * 4; ++w) {
-                        const float* rec = red + (w * RC + tid) * (2 + 2 * KC);
-                        if (rec[0] > -INFINITY) Ssum += rec[1] * expf(rec[0] - M);
-#pragma unroll
-                        for (int k = 0; k < KC; ++k) best.push(rec[2 + k], __float_as_int(rec[2 + KC + k]));
-                    }
-                    const int64_t o = (int64_t)blockIdx.x * R + r0 + tid;
-                    a.lg_m[o] = M;
-                    a.lg_s[o] = Ssum;
-#pragma unroll
-                    for (int k = 0; k < KC; ++k) { a.lg_v[o * KC + k] = best.v[k]; a.lg_i[o * KC + k] = best.i[k]; }
-                }
+                if (tid < RC && r0 + tid < R)
+                    fold_records<KC>(a, red + tid * (2 + 2 * KC), NW * 4, RC * (2 + 2 * KC), KC, (int64_t)blockIdx.x * R + r0 + tid);
                 __syncthreads();
             }
             WB_TRACE();
         grid_sync(a.bar, gen);
         WB_TRACE();
-            // ================= finish: log_softmax of the candidates, k best (ties -> lower id), greedy bookkeeping
-            for (int r = blockIdx.x; r < R; r += gridDim.x) {
-                float* s_f = wm;   // [NW] scratch
-                int* s_i = reinterpret_cast<int*>(wl);
-                const int NP = gridDim.x;
-                float mx = -INFINITY;
-                for (int c = tid; c < NP; c += NT) mx = fmaxf(mx, __ldcg(a.lg_m + (int64_t)c * R + r));
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-                if (lane == 0) s_f[warp] = mx;
-                __syncthreads();
-                mx = s_f[0];
-#pragma unroll
-                for (int w = 1; w < NW; ++w) mx = fmaxf(mx, s_f[w]);
-                __syncthreads();
-                float se = 0.0f;
-                for (int c = tid; c < NP; c += NT) {
-                    const float m = __ldcg(a.lg_m + (int64_t)c * R + r);
-                    if (m > -INFINITY) se += __ldcg(a.lg_s + (int64_t)c * R + r) * expf(m - mx);
-                }
-                se = warp_sum(se);
-                if (lane == 0) s_f[warp] = se;
-                __syncthreads();
-                se = 0.0f;
-#pragma unroll
-                for (int w = 0; w < NW; ++w) se += s_f[w];
-                const float lse = logf(se);
-                __syncthreads();
-                float prev_v = INFINITY;
-                int prev_i = -1;
-                for (int kk = 0; kk < a.k; ++kk) {
-                    float bv = -INFINITY;
-                    int bi = INT_MAX;
-                    for (int c = tid; c < NP * KC; c += NT) {
-                        const int part = c / KC, k = c % KC;
-                        const int idx = __ldcg(a.lg_i + ((int64_t)part * R + r) * KC + k);
-                        if (idx == INT_MAX) continue;
-                        const float v = __fsub_rn(__fsub_rn(__ldcg(a.lg_v + ((int64_t)part * R + r) * KC + k), mx), lse);
-                        const bool after_prev = v < prev_v || (v == prev_v && idx > prev_i);
-                        if (after_prev && (v > bv || (v == bv && idx < bi))) { bv = v; bi = idx; }
-                    }
-#pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) {
-                        const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-                        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-                        if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-                    }
-                    if (lane == 0) { s_f[warp] = bv; s_i[warp] = bi; }
-                    __syncthreads();
-                    bv = s_f[0];
-                    bi = s_i[0];
-#pragma unroll
-                    for (int w = 1; w < NW; ++w)
-                        if (s_f[w] > bv || (s_f[w] == bv && s_i[w] < bi)) { bv = s_f[w]; bi = s_i[w]; }
-                    __syncthreads();
-                    if (tid == 0) {
-                        a.topk_id[(int64_t)r * a.k + kk] = bi == INT_MAX ? -1 : bi;
-                        a.topk_lp[(int64_t)r * a.k + kk] = bv;
-                        if (kk == 0 && a.greedy && !__ldcg(a.finished + r)) {   // beam.rs:9-37 with beam_size 1
-                            a.tokens[(int64_t)r * t_max + p + 1] = bi;
-                            a.lengths[r] = p + 2;
-                            if (bi == a.eot) a.finished[r] = 1;
-                        }
-                    }
-                    prev_v = bv;
-                    prev_i = bi;
-                }
-            }
+            // ================= finish: log_softmax of the candidates, k best, greedy bookkeeping
+            for (int r = blockIdx.x; r < R; r += gridDim.x) finish_row_topk<KC>(a, r, p, gridDim.x, wm, reinterpret_cast<int*>(wl));
             WB_TRACE();
         grid_sync(a.bar, gen);
         WB_TRACE();
-            if (a.greedy) {   // stop as soon as every search has produced EOT (beam.rs:22-27)
-                int live = 0;
-                for (int r = 0; r < R; ++r) live += __ldcg(a.finished + r) ? 0 : 1;
-                if (live == 0) {
-                    if (blockIdx.x == 0 && tid == 0) { *a.pos = p + 1; *a.n_unfinished = 0; *a.steps_done = step + 1; }
-                    return;
-                }
+            // stop as soon as every search has produced EOT (beam.rs:22-27)
+            if (a.greedy && rows_open(a) == 0) {
+                if (blockIdx.x == 0 && tid == 0) decode_done(a, p + 1, 0, step + 1);
+                return;
             }
         }
     }
-    if (blockIdx.x == 0 && tid == 0) {
-        *a.pos = a.pos0 + a.n_steps;
-        int live = 0;
-        for (int r = 0; r < R; ++r) live += (a.greedy && __ldcg(a.finished + r)) ? 0 : 1;
-        *a.n_unfinished = live;
-        *a.steps_done = a.n_steps;
-    }
+    if (blockIdx.x == 0 && tid == 0) decode_done(a, a.pos0 + a.n_steps, rows_open(a), a.n_steps);
 }
 
 size_t dec3_smem_bytes(int d, int H, int S, int RC, int KC) {

@@ -316,7 +316,6 @@ dec4_kernel(const DecArgs a) {
     constexpr int VPL = (D / 8 + 31) / 32;        // vectors per lane for K = D
     constexpr int VPL4 = (4 * D / 8 + 31) / 32;   // K = 4D
     constexpr int NR_QKV = 3 * D / (CS * NW), NR_D = D / (CS * NW), NR_H = 4 * D / (CS * NW);
-    constexpr int KC = 2;
     const int L = a.L, V = a.V, R = a.R, t_max = a.t_max;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int rank = (int)cl.block_rank();
@@ -339,7 +338,7 @@ dec4_kernel(const DecArgs a) {
     float* stg_s = ML + 4;            // [STG_N] this CTA's slice of a stage output, staged for the 16-byte sends
     float* xb = stg_s + STG_N;        // [2][D] residual row x, two copies used alternately (read one, write the other)
     float* xn_s = xb + 2 * D;         // [D]   LayerNorm output (written identically by every warp)
-    float* red = xn_s + D;            // [NW][8 rows][m, s, best value, best id] logits merge scratch (sized [NW*4][RC][2 + 2*KC])
+    float* red = xn_s + D;            // [NW][8 rows][m, s, best value, best id] logits merge scratch (sized [NW*4][RC][6])
     constexpr int RINGW = (LG_NBUF * LG_RB * D * 2 > KV_STG * 8 * 128 * 4) ? LG_NBUF * LG_RB * D * 2 : KV_STG * 8 * 128 * 4;   // bytes of a warp's ring (logits rows / cross K/V batches)
     constexpr int LG_PITCH = D * 2;                                        // bytes per staged vocabulary row (rows contiguous: one bulk copy per block)
     uint8_t* ring = reinterpret_cast<uint8_t*>(red + NW * 4 * RC * 6);      // [NW][LG_NBUF][LG_RB][LG_PITCH]
@@ -811,11 +810,8 @@ dec4_kernel(const DecArgs a) {
                         if (n < V && 2 * t + e < R) {   // RC == 4: R <= 4, i.e. lanes t < 2
                             const float raw = fmaf(al[c], 1.0f / 2048.0f, ah[c]);
                             const float v = (use_mask && ((sp01 >> ((c >> 1) * 8)) & 0xffu)) ? __fadd_rn(raw, -INFINITY) : raw;
-                            if (v > -INFINITY) {
-                                if (v > m_run[e]) { s_run[e] = s_run[e] * expf(m_run[e] - v) + 1.0f; m_run[e] = v; }
-                                else s_run[e] += expf(v - m_run[e]);
-                            }
-                            if (v > bv[e] || (v == bv[e] && n < bi[e])) { bv[e] = v; bi[e] = n; }
+                            if (v > -INFINITY) softmax_add(m_run[e], s_run[e], v);
+                            if (cand_better(v, n, bv[e], bi[e])) { bv[e] = v; bi[e] = n; }
                         }
                     }
                 }
@@ -829,13 +825,8 @@ dec4_kernel(const DecArgs a) {
             for (int e = 0; e < 2; ++e) {
 #pragma unroll
                 for (int off = 4; off < 32; off <<= 1) {
-                    const float m2 = __shfl_xor_sync(0xffffffffu, m_run[e], off), s2 = __shfl_xor_sync(0xffffffffu, s_run[e], off);
-                    const float v2 = __shfl_xor_sync(0xffffffffu, bv[e], off);
-                    const int i2 = __shfl_xor_sync(0xffffffffu, bi[e], off);
-                    const float mn = fmaxf(m_run[e], m2);
-                    s_run[e] = (m_run[e] > -INFINITY ? s_run[e] * expf(m_run[e] - mn) : 0.0f) + (m2 > -INFINITY ? s2 * expf(m2 - mn) : 0.0f);
-                    m_run[e] = mn;
-                    if (v2 > bv[e] || (v2 == bv[e] && i2 < bi[e])) { bv[e] = v2; bi[e] = i2; }
+                    softmax_merge(m_run[e], s_run[e], __shfl_xor_sync(0xffffffffu, m_run[e], off), __shfl_xor_sync(0xffffffffu, s_run[e], off));
+                    cand_xor(bv[e], bi[e], off);
                 }
                 if (g == 0) {
                     float* rec = red + (warp * 8 + 2 * t + e) * 4;
@@ -843,121 +834,37 @@ dec4_kernel(const DecArgs a) {
                 }
             }
             __syncthreads();
-            if (tid < R) {
-                float M = -INFINITY;
-                for (int w2 = 0; w2 < NW; ++w2) M = fmaxf(M, red[(w2 * 8 + tid) * 4]);
-                float Ssum = 0.0f, best_v = -INFINITY;
-                int best_i = INT_MAX;
-                for (int w2 = 0; w2 < NW; ++w2) {
-                    const float* rec = red + (w2 * 8 + tid) * 4;
-                    if (rec[0] > -INFINITY) Ssum += rec[1] * expf(rec[0] - M);
-                    const int ci = __float_as_int(rec[3]);
-                    if (rec[2] > best_v || (rec[2] == best_v && ci < best_i)) { best_v = rec[2]; best_i = ci; }
-                }
-                const int64_t o = (int64_t)blockIdx.x * R + tid;
-                a.lg_m[o] = M;
-                a.lg_s[o] = Ssum;
-                a.lg_v[o * KC] = best_v;
-                a.lg_i[o * KC] = best_i;
-#pragma unroll
-                for (int k = 1; k < KC; ++k) { a.lg_v[o * KC + k] = -INFINITY; a.lg_i[o * KC + k] = INT_MAX; }
-            }
+            if (tid < R) fold_records_top1(a, red + tid * 4, NW, 8 * 4, (int64_t)blockIdx.x * R + tid);
         }
         WB_TRACE();
-        // ================= finish (greedy: beam.rs:9-37 with beam_size 1) by the LAST CTA to deliver its records: every CTA
-        // takes a ticket after publishing its records; the holder of the last ticket of this step merges them (one warp
-        // per row) and releases a flag the others wait on -- one flag wait instead of two grid barriers around the finish.
+        // ================= finish (greedy: beam.rs:9-37 with beam_size 1) by the LAST CTA to deliver its records, one warp
+        // per row -- one flag wait instead of two grid barriers around the finish.
         ++lstep;
         __syncthreads();
-        if (tid == 0) {
-            __threadfence();
-            const unsigned int ticket = atomicAdd(a.bar + 1, 1u);
-            reinterpret_cast<int*>(ML)[2] = (ticket == lstep * gridDim.x - 1) ? 1 : 0;
-        }
+        if (tid == 0) reinterpret_cast<int*>(ML)[2] = last_ticket(a.bar, lstep);
         __syncthreads();
         WB_TRACE();
         if (reinterpret_cast<int*>(ML)[2]) {
             __threadfence();
-            for (int r = warp; r < R; r += NW) {
-                const int NP = gridDim.x;   // <= 128 co-resident CTAs: at most 4 records per lane, all loads issued before any use
-                float rm[4], rs[4], rv[4];
-                int ri[4];
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const int c = min(lane + 32 * k, NP - 1);
-                    rm[k] = __ldcg(a.lg_m + (int64_t)c * R + r);
-                    rs[k] = __ldcg(a.lg_s + (int64_t)c * R + r);
-                    rv[k] = __ldcg(a.lg_v + ((int64_t)c * R + r) * KC);
-                    ri[k] = __ldcg(a.lg_i + ((int64_t)c * R + r) * KC);
-                }
-                float mx = -INFINITY;
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    if (lane + 32 * k < NP) mx = fmaxf(mx, rm[k]);
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-                float se = 0.0f, bv = -INFINITY;
-                int bi = INT_MAX;
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    if (lane + 32 * k < NP) {
-                        if (rm[k] > -INFINITY) se += rs[k] * expf(rm[k] - mx);
-                        if (ri[k] != INT_MAX && (rv[k] > bv || (rv[k] == bv && ri[k] < bi))) { bv = rv[k]; bi = ri[k]; }
-                    }
-                }
-                se = warp_sum(se);
-                const float lse = logf(se);
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) {
-                    const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-                    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-                    if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-                }
-                if (lane == 0) {
-                    a.topk_id[r] = bi == INT_MAX ? -1 : bi;
-                    a.topk_lp[r] = __fsub_rn(__fsub_rn(bv, mx), lse);
-                    if (!__ldcg(a.finished + r)) {
-                        a.tokens[(int64_t)r * t_max + p + 1] = bi;
-                        a.lengths[r] = p + 2;
-                        if (bi == a.eot) a.finished[r] = 1;
-                    }
-                }
-            }
+            // <= 128 co-resident CTAs: at most 4 records per lane
+            for (int r = warp; r < R; r += NW) finish_row_top1<4>(a, r, p, gridDim.x);
             __syncthreads();
-            if (tid == 0) {
-                __threadfence();
-                asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(a.bar + 2), "r"(lstep) : "memory");
-            }
+            if (tid == 0) release_flag(a.bar, lstep);
         }
         WB_TRACE();
-        if (tid == 0) {
-            const long long t0 = clock64();
-            while (ld_acquire(a.bar + 2) < lstep) {
-                if (clock64() - t0 > 40000000000LL) __trap();   // ~20 s of SM clocks: fail loudly instead of hanging the GPU
-            }
-        }
+        if (tid == 0) wait_flag(a.bar, lstep, 40000000000LL);   // ~20 s of SM clocks
         __syncthreads();
         WB_TRACE();
-        {
-            int live = 0;
-            for (int r = 0; r < R; ++r) live += __ldcg(a.finished + r) ? 0 : 1;
-            if (live == 0) {
-                if (blockIdx.x == 0 && tid == 0) { *a.pos = p + 1; *a.n_unfinished = 0; *a.steps_done = step + 1; }
-                demote();   // every CTA is past the flag: no evict_last load is left
-                return;
-            }
+        if (rows_open(a) == 0) {
+            if (blockIdx.x == 0 && tid == 0) decode_done(a, p + 1, 0, step + 1);
+            demote();   // every CTA is past the flag: no evict_last load is left
+            return;
         }
     }
     // after a prefill position clusters run independently: all of them finish their loads before any line is demoted
     if (a.n_steps > 0 && a.pos0 + a.n_steps - 1 < a.logits_from) grid_sync(a.bar, gen);
     demote();
-    if (blockIdx.x == 0 && tid == 0) {
-        *a.pos = a.pos0 + a.n_steps;
-        int live = 0;
-        for (int r = 0; r < R; ++r) live += __ldcg(a.finished + r) ? 0 : 1;
-        *a.n_unfinished = live;
-        *a.steps_done = a.n_steps;
-    }
+    if (blockIdx.x == 0 && tid == 0) decode_done(a, a.pos0 + a.n_steps, rows_open(a), a.n_steps);
 }
 
 template <int D, int RC>

@@ -615,22 +615,17 @@ dec5_kernel(const DecArgs a) {
                             }
 #pragma unroll 1
                             for (int off = 1; off < 32; off <<= 1) {
-                                const float m2 = __shfl_xor_sync(0xffffffffu, m_run, off), s2 = __shfl_xor_sync(0xffffffffu, s_run, off);
-                                const float v2 = __shfl_xor_sync(0xffffffffu, bv, off);
-                                const int i2 = __shfl_xor_sync(0xffffffffu, bi, off);
-                                const float mn = fmaxf(m_run, m2);
-                                s_run = (m_run > -INFINITY ? s_run * expf(m_run - mn) : 0.0f) + (m2 > -INFINITY ? s2 * expf(m2 - mn) : 0.0f);
-                                m_run = mn;
-                                if (v2 > bv || (v2 == bv && i2 < bi)) { bv = v2; bi = i2; }
+                                softmax_merge(m_run, s_run, __shfl_xor_sync(0xffffffffu, m_run, off), __shfl_xor_sync(0xffffffffu, s_run, off));
+                                cand_xor(bv, bi, off);
                             }
                             if (pass == 0 && lane == 0) { rec[0] = m_run; rec[1] = s_run; rec[2] = bv; rec[3] = __int_as_float(bi); }
                         }
-                        if (tid == 0) {
+                        if (tid == 0) {   // the top-1 record
                             const int64_t o = (int64_t)sl * R + r;
                             a.lg_m[o] = m_run;
                             a.lg_s[o] = s_run;
-                            a.lg_v[o * KC] = bv;
-                            a.lg_i[o * KC] = bi;
+                            a.lg_v[o] = bv;
+                            a.lg_i[o] = bi;
                         }
                         __syncthreads();
                     }
@@ -707,148 +702,30 @@ dec5_kernel(const DecArgs a) {
                         for (int k = 0; k < KC; ++k) { rec[2 + k] = cand.v[k]; rec[2 + KC + k] = __int_as_float(cand.i[k]); }
                     }
                     __syncthreads();
-                    if (tid == 0) {
-                        float M = -INFINITY;
-                        for (int w = 0; w < NW; ++w) M = fmaxf(M, red[w * (2 + 2 * KC)]);
-                        float Ssum = 0.0f;
-                        Cand<KC> best;
-                        best.init();
-                        for (int w = 0; w < NW; ++w) {
-                            const float* rc = red + w * (2 + 2 * KC);
-                            if (rc[0] > -INFINITY) Ssum += rc[1] * expf(rc[0] - M);
-                            for (int k = 0; k < a.k; ++k) best.push(rc[2 + k], __float_as_int(rc[2 + KC + k]));
-                        }
-                        const int64_t o = (int64_t)sl * R + r;
-                        a.lg_m[o] = M;
-                        a.lg_s[o] = Ssum;
-#pragma unroll
-                        for (int k = 0; k < KC; ++k) { a.lg_v[o * KC + k] = best.v[k]; a.lg_i[o * KC + k] = best.i[k]; }
-                    }
+                    if (tid == 0) fold_records<KC>(a, red, NW, 2 + 2 * KC, a.k, (int64_t)sl * R + r);
                     __syncthreads();
                 }
             }
             WB_TRACE();
             grid_sync(a.bar, gen);
             WB_TRACE();
-            // ================= finish: log_softmax of the candidates, k best (ties -> lower id), greedy bookkeeping
-            if (a.k == 1) {   // greedy: one warp per row over the NSL <= 16 slice records (beam.rs:9-37 with beam_size 1)
-                for (int r = blockIdx.x; r < R; r += gridDim.x) {
-                    if (warp == 0) {
-                        const bool have = lane < NSL;
-                        const float m = have ? __ldcg(a.lg_m + (int64_t)lane * R + r) : -INFINITY;
-                        const float sv = have ? __ldcg(a.lg_s + (int64_t)lane * R + r) : 0.0f;
-                        float bv = have ? __ldcg(a.lg_v + ((int64_t)lane * R + r) * KC) : -INFINITY;
-                        int bi = have ? __ldcg(a.lg_i + ((int64_t)lane * R + r) * KC) : INT_MAX;
-                        float mx = m;
-#pragma unroll
-                        for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-                        const float se = warp_sum(m > -INFINITY ? sv * expf(m - mx) : 0.0f);
-                        const float lse = logf(se);
-#pragma unroll
-                        for (int o = 16; o > 0; o >>= 1) {
-                            const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-                            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-                            if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-                        }
-                        if (lane == 0) {
-                            a.topk_id[r] = bi == INT_MAX ? -1 : bi;
-                            a.topk_lp[r] = __fsub_rn(__fsub_rn(bv, mx), lse);
-                            if (a.greedy && !__ldcg(a.finished + r)) {
-                                a.tokens[(int64_t)r * t_max + p + 1] = bi;
-                                a.lengths[r] = p + 2;
-                                if (bi == a.eot) a.finished[r] = 1;
-                            }
-                        }
-                    }
-                }
+            // ================= finish: log_softmax of the candidates, k best, greedy bookkeeping
+            if (a.k == 1) {   // greedy: one warp per row over the NSL <= 16 slice records
+                for (int r = blockIdx.x; r < R; r += gridDim.x)
+                    if (warp == 0) finish_row_top1<1>(a, r, p, NSL);
             } else
-            for (int r = blockIdx.x; r < R; r += gridDim.x) {
-                float* s_f = wm;   // [NW] scratch
-                int* s_i = reinterpret_cast<int*>(wl);
-                const int NP = NSL;
-                float mx = -INFINITY;
-                for (int c = tid; c < NP; c += NT) mx = fmaxf(mx, __ldcg(a.lg_m + (int64_t)c * R + r));
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-                if (lane == 0) s_f[warp] = mx;
-                __syncthreads();
-                mx = s_f[0];
-#pragma unroll
-                for (int w = 1; w < NW; ++w) mx = fmaxf(mx, s_f[w]);
-                __syncthreads();
-                float se = 0.0f;
-                for (int c = tid; c < NP; c += NT) {
-                    const float m = __ldcg(a.lg_m + (int64_t)c * R + r);
-                    if (m > -INFINITY) se += __ldcg(a.lg_s + (int64_t)c * R + r) * expf(m - mx);
-                }
-                se = warp_sum(se);
-                if (lane == 0) s_f[warp] = se;
-                __syncthreads();
-                se = 0.0f;
-#pragma unroll
-                for (int w = 0; w < NW; ++w) se += s_f[w];
-                const float lse = logf(se);
-                __syncthreads();
-                float prev_v = INFINITY;
-                int prev_i = -1;
-                for (int kk = 0; kk < a.k; ++kk) {
-                    float bv = -INFINITY;
-                    int bi = INT_MAX;
-                    for (int c = tid; c < NP * KC; c += NT) {
-                        const int part = c / KC, k = c % KC;
-                        const int idx = __ldcg(a.lg_i + ((int64_t)part * R + r) * KC + k);
-                        if (idx == INT_MAX) continue;
-                        const float v = __fsub_rn(__fsub_rn(__ldcg(a.lg_v + ((int64_t)part * R + r) * KC + k), mx), lse);
-                        const bool after_prev = v < prev_v || (v == prev_v && idx > prev_i);
-                        if (after_prev && (v > bv || (v == bv && idx < bi))) { bv = v; bi = idx; }
-                    }
-#pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) {
-                        const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-                        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-                        if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-                    }
-                    if (lane == 0) { s_f[warp] = bv; s_i[warp] = bi; }
-                    __syncthreads();
-                    bv = s_f[0];
-                    bi = s_i[0];
-#pragma unroll
-                    for (int w = 1; w < NW; ++w)
-                        if (s_f[w] > bv || (s_f[w] == bv && s_i[w] < bi)) { bv = s_f[w]; bi = s_i[w]; }
-                    __syncthreads();
-                    if (tid == 0) {
-                        a.topk_id[(int64_t)r * a.k + kk] = bi == INT_MAX ? -1 : bi;
-                        a.topk_lp[(int64_t)r * a.k + kk] = bv;
-                        if (kk == 0 && a.greedy && !__ldcg(a.finished + r)) {   // beam.rs:9-37 with beam_size 1
-                            a.tokens[(int64_t)r * t_max + p + 1] = bi;
-                            a.lengths[r] = p + 2;
-                            if (bi == a.eot) a.finished[r] = 1;
-                        }
-                    }
-                    prev_v = bv;
-                    prev_i = bi;
-                }
-            }
+            for (int r = blockIdx.x; r < R; r += gridDim.x) finish_row_topk<KC>(a, r, p, NSL, wm, reinterpret_cast<int*>(wl));
             WB_TRACE();
             grid_sync(a.bar, gen);
             WB_TRACE();
-            if (a.greedy) {   // stop as soon as every search has produced EOT (beam.rs:22-27)
-                int live = 0;
-                for (int r = 0; r < R; ++r) live += __ldcg(a.finished + r) ? 0 : 1;
-                if (live == 0) {
-                    if (blockIdx.x == 0 && tid == 0) { *a.pos = p + 1; *a.n_unfinished = 0; *a.steps_done = step + 1; }
-                    return;
-                }
+            // stop as soon as every search has produced EOT (beam.rs:22-27)
+            if (a.greedy && rows_open(a) == 0) {
+                if (blockIdx.x == 0 && tid == 0) decode_done(a, p + 1, 0, step + 1);
+                return;
             }
         }
     }
-    if (blockIdx.x == 0 && tid == 0) {
-        *a.pos = a.pos0 + a.n_steps;
-        int live = 0;
-        for (int r = 0; r < R; ++r) live += (a.greedy && __ldcg(a.finished + r)) ? 0 : 1;
-        *a.n_unfinished = live;
-        *a.steps_done = a.n_steps;
-    }
+    if (blockIdx.x == 0 && tid == 0) decode_done(a, a.pos0 + a.n_steps, rows_open(a), a.n_steps);
 }
 
 size_t dec5_smem_bytes(int d, int NT8, int L) {

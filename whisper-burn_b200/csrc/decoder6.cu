@@ -441,15 +441,6 @@ __device__ __noinline__ void self_attn6_anc(const float* qkv_s, const KVT* kbase
     self_attn6_body<KVT, true>(qkv_s, kbase, vbase, ld, p, anc, row_ld, wm, wl, wo);
 }
 
-// beam mode: candidate list of one (warp, row) in the logits stage, sorted by (value desc, id asc); empty = (-inf, INT_MAX)
-__device__ __forceinline__ void cand_insert(float* lv, int* li, float v, int n) {
-    if (!(v > lv[DEC_KC - 1] || (v == lv[DEC_KC - 1] && n < li[DEC_KC - 1]))) return;
-    int k = DEC_KC - 1;
-    for (; k > 0 && (v > lv[k - 1] || (v == lv[k - 1] && n < li[k - 1])); --k) { lv[k] = lv[k - 1]; li[k] = li[k - 1]; }
-    lv[k] = v;
-    li[k] = n;
-}
-
 // cross attention of one head over the T keys of the window (mod.rs:482-490), the head-major K/V block arriving through
 // the ring in chunks of KPC keys; 8 lanes per key.  A slot is released by the LAST of the 8 warps to finish with it (the slots'
 // empty barriers take one arrival, as the MMA warpgroup gives them for weight slabs).  (Waiting for several chunks at once to batch
@@ -507,8 +498,8 @@ __device__ __noinline__ uint32_t cross_attn6(const Pipe P, uint32_t n, int* slot
 // ---- beam mode: the finisher's work at a search position p (depth = p - logits_from), by the last CTA to deliver its records.
 constexpr int BM_LIVE = 24;                                          // rows of a beam launch
 constexpr int BM_NX = 3 * BM_LIVE + 3 * NCW * beamfx::MAX_NODES;     // finish_beam's shared scratch (ints)
-//   (a) each live slot's B best candidates by the rounded log-prob (v - max) - lse, the lower id first on equal log-probs
-//       (decoder5.cu's rule), from the CTAs' records -> topk_id / topk_lp [row][B];
+//   (a) each live slot's B best candidates by the rounded log-prob (v - max) - lse, ranked by cand_better, from the CTAs'
+//       records -> topk_id / topk_lp [row][B];
 //   (b) one warp per unfinished window: beamfx::beam_step on the carried nodes (lane 0), the new nodes' sequences (the warp);
 //       the next position's live slots w * B + i in carried order, each with its parent's cache row and its token;
 //   (c) the search ends when every window is done (its best carried node is finished) or at max_depth: then the best
@@ -539,18 +530,8 @@ __device__ __noinline__ void finish_beam(const DecArgs& a, int p, int depth, con
             rm[k] = __ldcg(a.lg_m + (int64_t)c * R + r);
             rs[k] = __ldcg(a.lg_s + (int64_t)c * R + r);
         }
-        float mx = -INFINITY;
-#pragma unroll
-        for (int k = 0; k < 5; ++k)
-            if (lane + 32 * k < NP) mx = fmaxf(mx, rm[k]);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-        float se = 0.0f;
-#pragma unroll
-        for (int k = 0; k < 5; ++k)
-            if (lane + 32 * k < NP && rm[k] > -INFINITY) se += rs[k] * expf(rm[k] - mx);
-        se = warp_sum(se);
-        const float lse = logf(se);
+        float mx;
+        const float lse = row_lse<5>(rm, rs, NP, mx);
         // the row's NP * DEC_KC candidates as (log-prob, id) in this warp's share of the (idle) ring
         float* cv = reinterpret_cast<float*>(scratch + (size_t)warp * RINGW);
         int* ci = reinterpret_cast<int*>(cv + 160 * DEC_KC);
@@ -563,22 +544,16 @@ __device__ __noinline__ void finish_beam(const DecArgs& a, int p, int depth, con
         __syncwarp();
         float prev_v = INFINITY;
         int prev_i = -1;
-        for (int kk = 0; kk < B; ++kk) {
+        for (int kk = 0; kk < B; ++kk) {   // the best candidate ranked after the previous one
             float bv = -INFINITY;
             int bi = INT_MAX;
             for (int q = lane; q < NC; q += 32) {
                 const int idx = ci[q];
                 if (idx == INT_MAX) continue;
                 const float v = cv[q];
-                const bool after_prev = v < prev_v || (v == prev_v && idx > prev_i);
-                if (after_prev && (v > bv || (v == bv && idx < bi))) { bv = v; bi = idx; }
+                if (cand_better(prev_v, prev_i, v, idx) && cand_better(v, idx, bv, bi)) { bv = v; bi = idx; }
             }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-                const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-                if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-            }
+            warp_best(bv, bi);
             if (lane == 0) {
                 a.topk_id[(int64_t)r * B + kk] = bi == INT_MAX ? -1 : bi;
                 a.topk_lp[(int64_t)r * B + kk] = bv;
@@ -691,9 +666,7 @@ __device__ __noinline__ void finish_beam(const DecArgs& a, int p, int depth, con
             for (int j = lane; j < len; j += 32) a.bm_out[(int64_t)w * t_max + j] = __ldcg(s + j);
         }
         if (tid == 0) {
-            *a.steps_done = depth + 1;
-            *a.pos = p + 1;
-            *a.n_unfinished = ctl[3];
+            decode_done(a, p + 1, ctl[3], depth + 1);
             a.bar[3] = 1;
         }
     }
@@ -1116,10 +1089,7 @@ dec6_kernel(const DecArgs a) {
                                     if (n < V && rr < R && ((live_m >> rr) & 1u)) {
                                         const float raw = fmaf(al[j][c], 1.0f / 2048.0f, ah[j][c]);
                                         const float v = (use_mask && a.is_special[n]) ? __fadd_rn(raw, -INFINITY) : raw;
-                                        if (v > -INFINITY) {
-                                            if (v > m_run[j][e]) { s_run[j][e] = s_run[j][e] * expf(m_run[j][e] - v) + 1.0f; m_run[j][e] = v; }
-                                            else s_run[j][e] += expf(v - m_run[j][e]);
-                                        }
+                                        if (v > -INFINITY) softmax_add(m_run[j][e], s_run[j][e], v);
                                         cv[j][c] = v;
                                     }
                                 }
@@ -1147,11 +1117,8 @@ dec6_kernel(const DecArgs a) {
                                     if (n < V && j * 8 + 2 * t + e < R) {
                                         const float raw = fmaf(al[j][c], 1.0f / 2048.0f, ah[j][c]);
                                         const float v = (use_mask && a.is_special[n]) ? __fadd_rn(raw, -INFINITY) : raw;
-                                        if (v > -INFINITY) {
-                                            if (v > m_run[j][e]) { s_run[j][e] = s_run[j][e] * expf(m_run[j][e] - v) + 1.0f; m_run[j][e] = v; }
-                                            else s_run[j][e] += expf(v - m_run[j][e]);
-                                        }
-                                        if (v > bv[j][e] || (v == bv[j][e] && n < bi[j][e])) { bv[j][e] = v; bi[j][e] = n; }
+                                        if (v > -INFINITY) softmax_add(m_run[j][e], s_run[j][e], v);
+                                        if (cand_better(v, n, bv[j][e], bi[j][e])) { bv[j][e] = v; bi[j][e] = n; }
                                     }
                                 }
                         }
@@ -1167,13 +1134,9 @@ dec6_kernel(const DecArgs a) {
                         for (int e = 0; e < 2; ++e) {
 #pragma unroll
                             for (int off = 4; off < 32; off <<= 1) {
-                                const float m2 = __shfl_xor_sync(0xffffffffu, m_run[j][e], off), s2 = __shfl_xor_sync(0xffffffffu, s_run[j][e], off);
-                                const float v2 = __shfl_xor_sync(0xffffffffu, bv[j][e], off);
-                                const int i2 = __shfl_xor_sync(0xffffffffu, bi[j][e], off);
-                                const float mn = fmaxf(m_run[j][e], m2);
-                                s_run[j][e] = (m_run[j][e] > -INFINITY ? s_run[j][e] * expf(m_run[j][e] - mn) : 0.0f) + (m2 > -INFINITY ? s2 * expf(m2 - mn) : 0.0f);
-                                m_run[j][e] = mn;
-                                if (!BEAM && (v2 > bv[j][e] || (v2 == bv[j][e] && i2 < bi[j][e]))) { bv[j][e] = v2; bi[j][e] = i2; }
+                                softmax_merge(m_run[j][e], s_run[j][e], __shfl_xor_sync(0xffffffffu, m_run[j][e], off),
+                                              __shfl_xor_sync(0xffffffffu, s_run[j][e], off));
+                                if (!BEAM) cand_xor(bv[j][e], bi[j][e], off);
                             }
                             if (g == 0) {
                                 float* rec = red + (warp * 8 * NT8 + j * 8 + 2 * t + e) * 4;
@@ -1182,132 +1145,50 @@ dec6_kernel(const DecArgs a) {
                         }
                     bar_consumers();
                     if (BEAM && tid < R && ((live_m >> tid) & 1u)) {
-                        // the CTA's record of a live row: (max, sum) as below, and its DEC_KC best (value, id) from the 8 warps'
+                        // the CTA's record of a live row: (max, sum-exp) of the 8 warps, and its DEC_KC best (value, id) from their
                         // lists, merged into warp 0's list (each list is sorted: the first entry that stays out ends a list)
-                        float M = -INFINITY;
-                        for (int w2 = 0; w2 < NCW; ++w2) M = fmaxf(M, red[(w2 * 8 * NT8 + tid) * 4]);
-                        float Ssum = 0.0f;
-                        for (int w2 = 0; w2 < NCW; ++w2) {
-                            const float* rec = red + (w2 * 8 * NT8 + tid) * 4;
-                            if (rec[0] > -INFINITY) Ssum += rec[1] * expf(rec[0] - M);
-                        }
+                        const float2 ms = fold_softmax(red + tid * 4, NCW, 8 * NT8 * 4);
                         float* acc_v = reinterpret_cast<float*>(ring_mem + LG_NBUF * BLKB) + tid * DEC_KC;
                         int* acc_i = reinterpret_cast<int*>(reinterpret_cast<float*>(ring_mem + LG_NBUF * BLKB) + LST) + tid * DEC_KC;
                         for (int w2 = 1; w2 < NCW; ++w2) {
                             const float* sv = reinterpret_cast<const float*>(ring_mem + (size_t)w2 * RINGW + LG_NBUF * BLKB) + tid * DEC_KC;
                             const int* si = reinterpret_cast<const int*>(reinterpret_cast<const float*>(ring_mem + (size_t)w2 * RINGW + LG_NBUF * BLKB) + LST) + tid * DEC_KC;
-                            for (int k = 0; k < DEC_KC; ++k) {
-                                const float v = sv[k];
-                                const int n = si[k];
-                                if (!(v > acc_v[DEC_KC - 1] || (v == acc_v[DEC_KC - 1] && n < acc_i[DEC_KC - 1]))) break;
-                                cand_insert(acc_v, acc_i, v, n);
-                            }
+                            for (int k = 0; k < DEC_KC; ++k)
+                                if (!cand_insert(acc_v, acc_i, sv[k], si[k])) break;
                         }
                         const int64_t o = (int64_t)blockIdx.x * R + tid;
-                        a.lg_m[o] = M;
-                        a.lg_s[o] = Ssum;
+                        a.lg_m[o] = ms.x;
+                        a.lg_s[o] = ms.y;
 #pragma unroll
                         for (int k = 0; k < DEC_KC; ++k) { a.lg_v[o * DEC_KC + k] = acc_v[k]; a.lg_i[o * DEC_KC + k] = acc_i[k]; }
                     } else if (!BEAM && tid < R) {
-                        float M = -INFINITY;
-                        for (int w2 = 0; w2 < NCW; ++w2) M = fmaxf(M, red[(w2 * 8 * NT8 + tid) * 4]);
-                        float Ssum = 0.0f, best_v = -INFINITY;
-                        int best_i = INT_MAX;
-                        for (int w2 = 0; w2 < NCW; ++w2) {
-                            const float* rec = red + (w2 * 8 * NT8 + tid) * 4;
-                            if (rec[0] > -INFINITY) Ssum += rec[1] * expf(rec[0] - M);
-                            const int ci = __float_as_int(rec[3]);
-                            if (rec[2] > best_v || (rec[2] == best_v && ci < best_i)) { best_v = rec[2]; best_i = ci; }
-                        }
-                        const int64_t o = (int64_t)blockIdx.x * R + tid;
-                        a.lg_m[o] = M;
-                        a.lg_s[o] = Ssum;
-                        a.lg_v[o] = best_v;
-                        a.lg_i[o] = best_i;
+                        fold_records_top1(a, red + tid * 4, NCW, 8 * NT8 * 4, (int64_t)blockIdx.x * R + tid);
                     }
                 }
                 trace();
                 // ================= finish (greedy: beam.rs:9-37 with beam_size 1) by the LAST CTA to deliver its records
                 bar_consumers();
-                if (tid == 0) {
-                    __threadfence();
-                    const unsigned int ticket = atomicAdd(a.bar + 1, 1u);
-                    ctl[1] = (ticket == gen * gridDim.x - 1) ? 1 : 0;
-                }
+                if (tid == 0) ctl[1] = last_ticket(a.bar, gen);
                 bar_consumers();
                 if (ctl[1]) {
                     __threadfence();
                     if constexpr (BEAM) {
                         finish_beam(a, p, depth, anc_cur, ring_mem, live_s + (step & 1) * BM_LIVE, nx_s, ctl);
-                    } else
-                    for (int r = warp; r < R; r += NCW) {
-                        // <= 160 co-resident CTAs: at most 5 records per lane, every load issued before any use (one L2 round trip)
-                        const int NP = gridDim.x;
-                        float rm[5], rs[5], rv[5];
-                        int ri[5];
-#pragma unroll
-                        for (int k = 0; k < 5; ++k) {
-                            const int c = min(lane + 32 * k, NP - 1);
-                            rm[k] = __ldcg(a.lg_m + (int64_t)c * R + r);
-                            rs[k] = __ldcg(a.lg_s + (int64_t)c * R + r);
-                            rv[k] = __ldcg(a.lg_v + (int64_t)c * R + r);
-                            ri[k] = __ldcg(a.lg_i + (int64_t)c * R + r);
-                        }
-                        float mx = -INFINITY;
-#pragma unroll
-                        for (int k = 0; k < 5; ++k)
-                            if (lane + 32 * k < NP) mx = fmaxf(mx, rm[k]);
-#pragma unroll
-                        for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-                        float se = 0.0f, bvv = -INFINITY;
-                        int bii = INT_MAX;
-#pragma unroll
-                        for (int k = 0; k < 5; ++k) {
-                            if (lane + 32 * k < NP) {
-                                if (rm[k] > -INFINITY) se += rs[k] * expf(rm[k] - mx);
-                                if (ri[k] != INT_MAX && (rv[k] > bvv || (rv[k] == bvv && ri[k] < bii))) { bvv = rv[k]; bii = ri[k]; }
-                            }
-                        }
-                        se = warp_sum(se);
-                        const float lse = logf(se);
-#pragma unroll
-                        for (int o = 16; o > 0; o >>= 1) {
-                            const float ov = __shfl_xor_sync(0xffffffffu, bvv, o);
-                            const int oi = __shfl_xor_sync(0xffffffffu, bii, o);
-                            if (ov > bvv || (ov == bvv && oi < bii)) { bvv = ov; bii = oi; }
-                        }
-                        if (lane == 0) {
-                            a.topk_id[r] = bii == INT_MAX ? -1 : bii;
-                            a.topk_lp[r] = __fsub_rn(__fsub_rn(bvv, mx), lse);
-                            if (!__ldcg(a.finished + r)) {
-                                a.tokens[(int64_t)r * t_max + p + 1] = bii;
-                                a.lengths[r] = p + 2;
-                                if (bii == a.eot) a.finished[r] = 1;
-                            }
-                        }
+                    } else {
+                        // <= 160 co-resident CTAs: at most 5 records per lane
+                        for (int r = warp; r < R; r += NCW) finish_row_top1<5>(a, r, p, gridDim.x);
                     }
                     bar_consumers();
-                    if (tid == 0) {
-                        __threadfence();
-                        asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(a.bar + 2), "r"(gen) : "memory");
-                    }
+                    if (tid == 0) release_flag(a.bar, gen);
                 }
-                if (tid == 0) {
-                    const long long t0 = clock64(), wd = g_watchdog;
-                    while (ld_acquire(a.bar + 2) < gen)
-                        if (clock64() - t0 > wd) __trap();
-                }
+                if (tid == 0) wait_flag(a.bar, gen, g_watchdog);
                 bar_consumers();
                 trace();
                 if constexpr (BEAM) {
                     stop = __ldcg(a.bar + 3) != 0;   // set by the finisher when the search ended
-                } else {
-                    int live = 0;
-                    for (int r = 0; r < R; ++r) live += __ldcg(a.finished + r) ? 0 : 1;
-                    if (live == 0) {
-                        stop = 1;
-                        if (blockIdx.x == 0 && tid == 0) { *a.pos = p + 1; *a.n_unfinished = 0; *a.steps_done = step + 1; }
-                    }
+                } else if (rows_open(a) == 0) {
+                    stop = 1;
+                    if (blockIdx.x == 0 && tid == 0) decode_done(a, p + 1, 0, step + 1);
                 }
             }
             if constexpr (BEAM) {
@@ -1317,13 +1198,7 @@ dec6_kernel(const DecArgs a) {
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic accesses to the aliased buffers before the next step's bulk copies
             bar_all();   // hands the ring back to the producer; it reads the stop flag after this barrier
             if (stop) break;
-            if (!BEAM && step + 1 == a.n_steps && blockIdx.x == 0 && tid == 0) {
-                *a.pos = a.pos0 + a.n_steps;
-                int live = 0;
-                for (int r = 0; r < R; ++r) live += __ldcg(a.finished + r) ? 0 : 1;
-                *a.n_unfinished = live;
-                *a.steps_done = a.n_steps;
-            }
+            if (!BEAM && step + 1 == a.n_steps && blockIdx.x == 0 && tid == 0) decode_done(a, a.pos0 + a.n_steps, rows_open(a), a.n_steps);
         }
     }
     cl.sync();   // no CTA leaves while a peer may still address its shared memory
