@@ -44,11 +44,12 @@ def pool_waves(gold, n):
     return [chunk[off:off + m] for off, m in (gold["pool"][i % len(gold["pool"])] for i in range(n))]
 
 
-def decode(wh, waves, sp, b, depth, kv, host=False, monkeypatch=None):
+def decode(wh, waves, sp, b, depth, kv, host=False, monkeypatch=None, max_text_len=None):
     if host:
         monkeypatch.setenv("WB200_DECODER", "3")   # the host search on the FMA decoder: a second reference
     try:
-        sess = transcribe.Session(wh, max_windows=len(waves), max_beams=7, max_text_len=4 + depth + 1, kv_dtype=KV[kv])
+        sess = transcribe.Session(wh, max_windows=len(waves), max_beams=7, max_text_len=max_text_len or 4 + depth + 1,
+                                  kv_dtype=KV[kv])
     finally:
         if host:
             monkeypatch.delenv("WB200_DECODER", raising=False)
@@ -87,6 +88,31 @@ def test_device_beam_tiny_en_vs_oracle_and_host(tiny, gold, monkeypatch, kv):
     assert got == gold["tiny_en"][kv]["5"]
     host, hs = decode(wh, waves, sp, 5, gold["depth_tiny_en"], kv, host=True, monkeypatch=monkeypatch)
     assert hs.last_decoder() == 3 and host == got and hs.last_steps() == sess.last_steps()
+
+
+DEEP = 124   # 4 + 124 = 128, the longest text decoder6 holds: the last step attends over 127 keys
+
+
+@pytest.mark.parametrize("kv", ["f32", "f16"])
+@pytest.mark.parametrize("b", [2, 5, 7])
+def test_device_beam_test_a_deep_vs_oracle_and_host(small, gold, monkeypatch, b, kv):
+    """test-a at max_depth 124 (max_text_len 128): self attention through all four of decoder6's 32-key slots, the keys read
+    through the ancestry tables, beam sequences copied to 128 ids.  EOT is declared to be the last vocabulary id, which
+    these searches never emit, so every window runs all 124 steps.  The same ids as the live oracle and as the host search
+    on decoder3, and the same number of steps."""
+    dims, w_t, sp, wh = small
+    sp2 = o_tr.SpecialTokens(sp.sot, sp.lang, sp.transcribe, sp.notimestamps, sp.n_vocab - 1, sp.first_special, sp.n_vocab)
+    waves = pool_waves(gold, min(len(gold["pool"]), 24 // b))
+    got, sess = decode(wh, waves, sp2, b, DEEP, kv, max_text_len=4 + DEEP)
+    assert sess.last_decoder() == 6 and sess.last_steps() == DEEP
+    host, hs = decode(wh, waves, sp2, b, DEEP, kv, host=True, monkeypatch=monkeypatch, max_text_len=4 + DEEP)
+    assert hs.last_decoder() == 3 and hs.last_steps() == DEEP
+    assert host == got
+    opts = o_model.OracleOptions(kv_dtype=kv)
+    for i, wave in enumerate(waves):
+        want = o_tr.mels_to_tokens(w_t, dims, sp2, o_audio.prep_audio(torch.from_numpy(wave)[None]), beam_size=b,
+                                   max_depth=DEEP, opts=opts)
+        assert len(want) == 4 + DEEP and got[i] == want, f"window {i}"
 
 
 def test_device_beam_live_oracle(small):

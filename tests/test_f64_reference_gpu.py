@@ -11,13 +11,30 @@ compared on the log-probs it selects, and the encoder on its output, at the shap
   * windows whose encoder lengths fall on the cross-attention split edges, T in {6, 64, 65, 750}, mixed within one batch
     (T = (min(n // 160, 1490) + 10 - 1) // 2 + 1 for n samples).
 
-The float64 reference runs on the GPU's own encoder output, so the decoder checks do not include encoder error.  Greedy-only
-decoders (decoder4, decoder6) are read back with wb_session_last_topk after greedy runs to depth s = 1 .. DEPTH.
+The float64 reference runs on the GPU's own encoder output, so the decoder checks do not include encoder error.  Greedy
+decoders are read back with wb_session_last_topk after greedy runs to each checked depth s: s = 1 .. DEPTH at the shapes
+above, and at depth the steps on either side of every key count where a decoder's self attention changes how it walks the
+keys.  Step s is chosen from the logits at position p = s + 2, over n = s + 3 keys; for each edge E the deep cases check
+n = E - 1, E, E + 1 and the last step the session allows (n = max_text_len - 1):
+
+  * decoder4: up to 128 keys one register batch from the cp.async ring; from 129 keys the long path (key p read back from
+    the cache, attn_cta in 128-key turns): E = 128, 256, 384 at max_text_len 448;
+  * decoder6: 32 key slots x 4 keys, slot u from 32 u keys on; max_text_len 128 (the most it covers): E = 32, 64, 96;
+  * decoder5: fp32 K/V attn_warp in 64-key turns, fp16 K/V attn_warp_ring in 32-key turns through 8 stages (a stage is
+    first reused from 257 keys on): E = 64, 128, 256 for both at max_text_len 448, with 1, 9, 17 and 33 rows (row groups);
+  * decoder3: attn_cta in 128-key turns: E = 128, 256 at max_text_len 448;
+  * the default selection on both sides of decoder6's t_max <= 128 (d = 384, 9 rows: decoder6 at 128, decoder3 at 129).
+
+The deep cases use V = 2051 (the vocabulary tails are covered at depth 10) and declare EOT to be an id the windows never emit,
+so every row runs to the last checked step; check_greedy asserts that it does.
 
 Tolerances are absolute on log-probs (|log-prob| ~ 7.6 for V = 2051, ~10.9 for V = 51864) and separate for the fp32 and the
 fp16 K/V cache: at an fp16 rounding boundary a float64 value can round to the neighbour of the one the GPU's float32 value
 rounds to.  Each constant states the worst error measured on one H100 80GB HBM3 and the margin over it."""
 import functools
+import multiprocessing
+import os
+from concurrent.futures import ProcessPoolExecutor
 
 import numpy as np
 import pytest
@@ -44,6 +61,7 @@ LOGITS_REL_TOL = 2e-5
 ENC_REL_TOL = 2e-5
 
 DEPTH = 10                                       # greedy steps per window: 2 with the special-token mask, 8 without
+SHALLOW_STEPS = tuple(range(1, DEPTH + 1))
 N_OF_T = {6: 400, 64: 18720, 65: 19040, 750: 480000}   # waveform samples giving each encoder length
 T_ORDER = (750, 6, 65, 64)
 
@@ -67,6 +85,22 @@ def _weights(d, H, V, n_text_layer, exact):
     if not exact:   # no longer fp16-representable: the fp32 encoder (gemm.cu) and decoder3<float>
         w_np = {k: (v * np.float32(1.0001) if v.ndim else v) for k, v in w_np.items()}
     return dims, w_np, o_model.as_dtype(synth.to_torch(w_np))
+
+
+def _greedy_ref_rows(model_key, sp, xa, tokens, kv, steps):
+    """In a worker process: the float64 log-prob rows of the greedy steps `steps` along `tokens` (greedy_path_log_probs on
+    the weights _weights(*model_key) and the window's encoder output xa [T, d])."""
+    dims, _, w64 = _weights(*model_key)
+    ref = o_tr.greedy_path_log_probs(w64, dims, sp, torch.from_numpy(xa)[None], tokens, opts=o_model.OracleOptions(kv_dtype=kv))
+    return {s: ref[s - 1].numpy() for s in steps}
+
+
+@functools.lru_cache(maxsize=1)
+def _ref_pool():
+    """Worker processes for the float64 reference: scoring one row is a few hundred small sequential float64 steps, so rows
+    run side by side, one torch thread each."""
+    return ProcessPoolExecutor(max(1, min(8, (os.cpu_count() or 2) - 1)), mp_context=multiprocessing.get_context("spawn"),
+                               initializer=torch.set_num_threads, initargs=(1,))
 
 
 def make_model(d, H, V, exact=True, n_text_layer=2):
@@ -99,19 +133,50 @@ def use_decoder(monkeypatch, n):
         monkeypatch.delenv("WB200_DECODER", raising=False)
 
 
+def edge_steps(edges, max_text_len):
+    """The greedy steps whose self attention runs over E - 1, E and E + 1 keys for every edge E, and the last step a session
+    of max_text_len allows (step s attends over n = s + 3 keys: the 4-id prompt and s - 1 generated ids)."""
+    last = max_text_len - 4
+    return tuple(sorted({s for e in edges for s in (e - 4, e - 3, e - 2) if s <= last} | {last}))
+
+
+def default_decoder(d, rows, t_max):
+    """The decoder the default selection picks for a greedy launch of fp16-exact weights that decoder4 does not take (more
+    rows than co-resident 16-CTA clusters, or more than 8): decoder6 for d = 128 / 384, <= 24 rows and t_max <= 128, else
+    decoder5 where d % 256 == 0, else decoder3."""
+    if d in (128, 384) and rows <= 24 and t_max <= 128:
+        return 6
+    return 5 if d % 256 == 0 else 3
+
+
 # ---------------------------------------------------------------- a. greedy, per step, top-1 against float64
-def check_greedy(dims, wh, w64, kv, n_rows, decoder, seed, depth=DEPTH):
-    """Greedy-decodes n_rows windows to depth 1 .. depth (one launch each) and checks the top-1 (id, log-prob) of every row at
-    every step against float64 on the GPU's own path.  Returns the worst |log-prob error|."""
+def check_greedy(dims, wh, kv, n_rows, decoder, seed, steps=SHALLOW_STEPS, max_text_len=None, full_depth=False):
+    """Greedy-decodes n_rows windows once to the deepest step of `steps` and once to each step s of `steps`, and checks the
+    top-1 (id, log-prob) of every row at every step s against float64 on the GPU's own path.  max_text_len defaults to the
+    deepest step plus the prompt and one.  full_depth: EOT is declared to be a special id past the named ones that no row
+    emits (the largest one not emitted by an earlier full-depth launch that a row stopped in), and every row must reach the
+    deepest step.  Returns the worst |log-prob error|."""
+    depth = max(steps)
     sp = synth.special_tokens(dims)
     bitmap = sp.is_special_bitmap()
     Ts, waves = windows(n_rows, seed)
-    sess = transcribe.Session(wh, max_windows=n_rows, max_beams=1, max_text_len=4 + depth + 1, kv_dtype=kv_code(kv))
-    full = sess.transcribe_windows(waves, sp, bitmap, beam_size=1, max_depth=depth)
+    sess = transcribe.Session(wh, max_windows=n_rows, max_beams=1, max_text_len=max_text_len or 4 + depth + 1,
+                              kv_dtype=kv_code(kv))
+    full = sess.transcribe_windows(waves, sp, bitmap, beam_size=1, max_depth=depth) if not full_depth else None
+    eot = sp.n_vocab
+    while full is None or (full_depth and any(len(t) < 4 + depth for t in full)):
+        eot = max(set(range(sp.first_special, eot)) - {i for t in full or [] for i in t})
+        sp = o_tr.SpecialTokens(sp.sot, sp.lang, sp.transcribe, sp.notimestamps, eot, sp.first_special, sp.n_vocab)
+        full = sess.transcribe_windows(waves, sp, bitmap, beam_size=1, max_depth=depth)
     assert sess.last_decoder() == decoder
+    if full_depth:
+        assert sess.last_steps() == depth and [len(t) for t in full] == [4 + depth] * n_rows
     xa = encoder_outputs64(sess, Ts)
+    key = (dims.n_text_state, dims.n_text_head, dims.n_vocab, dims.n_text_layer, wh.weights_fp16_exact)
+    refs = [_ref_pool().submit(_greedy_ref_rows, key, sp, xa[r][0].numpy(), full[r], kv,
+                               [s for s in steps if 4 + s <= len(full[r])]) for r in range(n_rows)]
     got = [dict() for _ in range(n_rows)]      # step -> (id, log-prob) of every row that produced a token at that step
-    for s in range(1, depth + 1):
+    for s in steps:
         toks = sess.transcribe_windows(waves, sp, bitmap, beam_size=1, max_depth=s)
         assert sess.last_decoder() == decoder
         ids, lps = sess.last_topk(n_rows, 1)
@@ -121,18 +186,17 @@ def check_greedy(dims, wh, w64, kv, n_rows, decoder, seed, depth=DEPTH):
                 assert int(ids[r, 0]) == toks[r][-1]
                 got[r][s] = float(lps[r, 0])
     tol = GREEDY_LP_TOL[kv]
-    opts = o_model.OracleOptions(kv_dtype=kv)
     worst = 0.0
     for r in range(n_rows):
-        ref = o_tr.greedy_path_log_probs(w64, dims, sp, xa[r], full[r], opts=opts).numpy()
-        assert sorted(got[r]) == list(range(1, len(full[r]) - 4 + 1))
+        ref = refs[r].result()
+        assert sorted(got[r]) == sorted(ref)
         for s, lp in got[r].items():
             tok = full[r][4 + s - 1]
-            err = abs(lp - ref[s - 1, tok])
+            err = abs(lp - ref[s][tok])
             worst = max(worst, err)
-            assert err < tol, f"row {r} (T = {Ts[r]}) step {s}: log-prob {lp} vs float64 {ref[s - 1, tok]}"
-            gap = ref[s - 1].max() - ref[s - 1, tok]       # the GPU id is the float64 argmax up to a near-tie
-            assert gap < tol, f"row {r} step {s}: id {tok} is {gap} below the float64 argmax {int(ref[s - 1].argmax())}"
+            assert err < tol, f"row {r} (T = {Ts[r]}) step {s}: log-prob {lp} vs float64 {ref[s][tok]}"
+            gap = ref[s].max() - ref[s][tok]       # the GPU id is the float64 argmax up to a near-tie
+            assert gap < tol, f"row {r} step {s}: id {tok} is {gap} below the float64 argmax {int(ref[s].argmax())}"
     return worst
 
 
@@ -157,24 +221,40 @@ def test_last_topk_argument_checks(monkeypatch):
 DEC4_CASES = [(d, rows, kv) for d in (128, 384) for rows in (1, 4, 5, 8) for kv in ("f32", "f16")]
 
 
-@pytest.mark.parametrize("d,rows,kv", DEC4_CASES)
-def test_decoder4_greedy_steps_vs_float64(d, rows, kv, monkeypatch):
-    """decoder4.cu, dec4_kernel<d, RC, KVT>: RC = 4 for <= 4 rows, 8 for 5 to 8 rows."""
-    dims, wh, w64 = make_model(d, d // 64, 2051 if d == 128 else 51864)
+def check_decoder4(d, V, rows, kv, seed, what, monkeypatch, **greedy_args):
+    """check_greedy on decoder4, or, where decoder4 does not cover the rows, on the decoder the default selection picks for
+    them at this max_text_len (default_decoder), followed by a skip."""
+    dims, wh, _ = make_model(d, d // 64, V)
     use_decoder(monkeypatch, 4)
     try:
-        worst = check_greedy(dims, wh, w64, kv, rows, 4, seed=300 + rows)
+        worst = check_greedy(dims, wh, kv, rows, 4, seed, **greedy_args)
     except ffi.WbError as e:
         if e.code != ffi.WB_ERR_UNSUPPORTED or rows <= 4:
             raise
         # decoder4 runs one 16-CTA cluster per row and needs all of them co-resident; where the GPU holds fewer, the default
-        # selection must send these rows to decoder6, and they must pass there
+        # selection must send these rows on, and they must pass there
+        steps = greedy_args.get("steps", SHALLOW_STEPS)
+        fallback = default_decoder(d, rows, greedy_args.get("max_text_len") or 4 + max(steps) + 1)
         use_decoder(monkeypatch, 0)
-        worst = check_greedy(dims, wh, w64, kv, rows, 6, seed=300 + rows)
-        report(f"decoder6 (default for decoder4's rows) d={d} rows={rows} kv={kv}", worst, GREEDY_LP_TOL[kv])
+        worst = check_greedy(dims, wh, kv, rows, fallback, seed, **greedy_args)
+        report(f"decoder{fallback} (default for decoder4's rows) {what} d={d} rows={rows} kv={kv}", worst, GREEDY_LP_TOL[kv])
         pytest.skip(f"decoder4 does not cover {rows} rows: fewer than {rows} co-resident 16-CTA clusters fit on this GPU "
-                    f"(checked on decoder6 instead)")
-    report(f"decoder4 d={d} rows={rows} kv={kv}", worst, GREEDY_LP_TOL[kv])
+                    f"(checked on decoder{fallback} instead)")
+    report(f"decoder4 {what} d={d} rows={rows} kv={kv}", worst, GREEDY_LP_TOL[kv])
+
+
+@pytest.mark.parametrize("d,rows,kv", DEC4_CASES)
+def test_decoder4_greedy_steps_vs_float64(d, rows, kv, monkeypatch):
+    """decoder4.cu, dec4_kernel<d, RC, KVT>: RC = 4 for <= 4 rows, 8 for 5 to 8 rows."""
+    check_decoder4(d, 2051 if d == 128 else 51864, rows, kv, 300 + rows, "", monkeypatch)
+
+
+@pytest.mark.parametrize("d,rows,kv", DEC4_CASES)
+def test_decoder4_deep_greedy_steps_vs_float64(d, rows, kv, monkeypatch):
+    """decoder4 at max_text_len 448: the register batch up to 128 keys, the long path (key p read back from the cache after
+    the cluster barrier, attn_cta over row * t_max addressing) from 129 keys on, across its 128-key turns."""
+    check_decoder4(d, 2051, rows, kv, 1300 + rows, "deep", monkeypatch, steps=edge_steps((128, 256, 384), 448),
+                   max_text_len=448, full_depth=True)
 
 
 DEC6_CASES = [(d, rows, kv) for d in (128, 384) for rows in (1, 8, 9, 24) for kv in ("f32", "f16")]
@@ -183,10 +263,20 @@ DEC6_CASES = [(d, rows, kv) for d in (128, 384) for rows in (1, 8, 9, 24) for kv
 @pytest.mark.parametrize("d,rows,kv", DEC6_CASES)
 def test_decoder6_greedy_steps_vs_float64(d, rows, kv, monkeypatch):
     """decoder6.cu, dec6_kernel<d, NT8, KVT>: NT8 = 1 for <= 8 rows, 3 for 9 to 24 rows."""
-    dims, wh, w64 = make_model(d, d // 64, 2051 if d == 128 else 51864)
+    dims, wh, _ = make_model(d, d // 64, 2051 if d == 128 else 51864)
     use_decoder(monkeypatch, 6)
-    worst = check_greedy(dims, wh, w64, kv, rows, 6, seed=400 + rows)
+    worst = check_greedy(dims, wh, kv, rows, 6, seed=400 + rows)
     report(f"decoder6 d={d} rows={rows} kv={kv}", worst, GREEDY_LP_TOL[kv])
+
+
+@pytest.mark.parametrize("d,rows,kv", DEC6_CASES)
+def test_decoder6_deep_greedy_steps_vs_float64(d, rows, kv, monkeypatch):
+    """decoder6 at max_text_len 128, the most it covers: all four key slots of self_attn6_body (slot u from 32 u keys on)."""
+    dims, wh, _ = make_model(d, d // 64, 2051)
+    use_decoder(monkeypatch, 6)
+    worst = check_greedy(dims, wh, kv, rows, 6, 1400 + rows, steps=edge_steps((32, 64, 96), 128), max_text_len=128,
+                         full_depth=True)
+    report(f"decoder6 deep d={d} rows={rows} kv={kv}", worst, GREEDY_LP_TOL[kv])
 
 
 # (d, rows): nt8 = 1..4, row groups of 32 (33 rows = 32 + 1), the split d x d stage table (n_splits == 1 with d >= 512),
@@ -198,10 +288,24 @@ DEC5_CASES = [(d, rows, kv) for d, rows in ((256, 1), (256, 9), (256, 33), (512,
 @pytest.mark.parametrize("d,rows,kv", DEC5_CASES)
 def test_decoder5_greedy_steps_vs_float64(d, rows, kv, monkeypatch):
     """decoder5.cu, dec5_kernel<NT8, KVT> with NT8 = ceil(rows / 8) per row group, chosen by the default selection."""
-    dims, wh, w64 = make_model(d, d // 64, 51865 if d == 1280 else 2051)
+    dims, wh, _ = make_model(d, d // 64, 51865 if d == 1280 else 2051)
     use_decoder(monkeypatch, 0)
-    worst = check_greedy(dims, wh, w64, kv, rows, 5, seed=500 + rows)
+    worst = check_greedy(dims, wh, kv, rows, 5, seed=500 + rows)
     report(f"decoder5 d={d} rows={rows} kv={kv}", worst, GREEDY_LP_TOL[kv])
+
+
+DEC5_DEEP_CASES = [(d, rows, kv) for d, rows in ((256, 1), (256, 9), (256, 33), (512, 17)) for kv in ("f32", "f16")]
+
+
+@pytest.mark.parametrize("d,rows,kv", DEC5_DEEP_CASES)
+def test_decoder5_deep_greedy_steps_vs_float64(d, rows, kv, monkeypatch):
+    """decoder5 at max_text_len 448: fp32 K/V attn_warp (64-key turns), fp16 K/V attn_warp_ring (32-key turns, 8 stages,
+    the first stage reused from 257 keys on); 33 rows run as row groups of 32 + 1 (cache rows offset by kv_row0)."""
+    dims, wh, _ = make_model(d, d // 64, 2051)
+    use_decoder(monkeypatch, 0)
+    worst = check_greedy(dims, wh, kv, rows, 5, 1500 + rows, steps=edge_steps((64, 128, 256), 448), max_text_len=448,
+                         full_depth=True)
+    report(f"decoder5 deep d={d} rows={rows} kv={kv}", worst, GREEDY_LP_TOL[kv])
 
 
 DEC3_CASES = [(d, exact, rows, kv) for d in (128, 192, 384) for exact in (True, False) for rows in (3, 6)
@@ -211,10 +315,37 @@ DEC3_CASES = [(d, exact, rows, kv) for d in (128, 192, 384) for exact in (True, 
 @pytest.mark.parametrize("d,exact,rows,kv", DEC3_CASES)
 def test_decoder3_greedy_steps_vs_float64(d, exact, rows, kv, monkeypatch):
     """decoder3.cu, dec3_kernel<WT, RC, 2, KVT>: RC = 4 for <= 4 rows, 8 above; WT = __half (fp16-exact weights) or float."""
-    dims, wh, w64 = make_model(d, d // 64, 51864 if d == 384 else 2051, exact=exact)
+    dims, wh, _ = make_model(d, d // 64, 51864 if d == 384 else 2051, exact=exact)
     use_decoder(monkeypatch, 3)
-    worst = check_greedy(dims, wh, w64, kv, rows, 3, seed=600 + rows)
+    worst = check_greedy(dims, wh, kv, rows, 3, seed=600 + rows)
     report(f"decoder3 d={d} {'fp16' if exact else 'fp32'} weights rows={rows} kv={kv}", worst, GREEDY_LP_TOL[kv])
+
+
+DEC3_DEEP_CASES = [(d, exact, rows, kv) for d in (128, 384) for exact in (True, False) for rows in (3, 6)
+                   for kv in ("f32", "f16")]
+
+
+@pytest.mark.parametrize("d,exact,rows,kv", DEC3_DEEP_CASES)
+def test_decoder3_deep_greedy_steps_vs_float64(d, exact, rows, kv, monkeypatch):
+    """decoder3 at max_text_len 448: attn_cta over 128-key turns."""
+    dims, wh, _ = make_model(d, d // 64, 2051, exact=exact)
+    use_decoder(monkeypatch, 3)
+    worst = check_greedy(dims, wh, kv, rows, 3, 1600 + rows, steps=edge_steps((128, 256), 448), max_text_len=448,
+                         full_depth=True)
+    report(f"decoder3 deep d={d} {'fp16' if exact else 'fp32'} weights rows={rows} kv={kv}", worst, GREEDY_LP_TOL[kv])
+
+
+@pytest.mark.parametrize("kv", ["f32", "f16"])
+@pytest.mark.parametrize("max_text_len,decoder", [(128, 6), (129, 3)])
+def test_default_selection_at_t_max_edge_vs_float64(max_text_len, decoder, kv, monkeypatch):
+    """9 rows of a d = 384 model (more than decoder4 ever takes) with the default selection: decoder6 up to t_max = 128;
+    above, decoder5 needs d % 256 == 0, so decoder3 runs them."""
+    assert default_decoder(384, 9, max_text_len) == decoder
+    dims, wh, _ = make_model(384, 6, 2051)
+    use_decoder(monkeypatch, 0)
+    worst = check_greedy(dims, wh, kv, 9, decoder, 1700, steps=edge_steps((32, 64, 96, 128), max_text_len),
+                         max_text_len=max_text_len, full_depth=True)
+    report(f"default selection max_text_len={max_text_len} decoder{decoder} d=384 rows=9 kv={kv}", worst, GREEDY_LP_TOL[kv])
 
 
 # ---------------------------------------------------------------- b. wb_session_step, k = 7, with beams
