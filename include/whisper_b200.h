@@ -54,6 +54,17 @@ extern "C" {
 #define WB_KV_F32 0            /* reference numerics */
 #define WB_KV_F16 1            /* fp16 K/V cache (north_star); rounding restated by the oracle's kv_dtype="f16" */
 
+/* Window modes of a session: the most mel frames one window gives the encoder.  Everything else of the reference's
+ * windowing (10 zero frames appended, 3 s overlap, overlap merge, prompt, beam rules) is the same in both.
+ *   REFERENCE: n_audio_ctx mel frames, as the reference (transcribe.rs:32-34, 161-177): a window keeps at most
+ *              n_audio_ctx - 10 frames, so T <= n_audio_ctx / 2 encoder positions (750 for Whisper: a 30 s chunk is
+ *              3 windows).  The default, and the mode the reference's outputs are compared in.
+ *   NATIVE:    2 * n_audio_ctx mel frames: a window keeps at most 2 * n_audio_ctx - 10 frames, T <= n_audio_ctx
+ *              (1500 for Whisper: the 30 s context the models were trained on; 480 000 samples give one window of
+ *              T = 1500, the last 0.1 s clipped as in the reference).  Buffers sized per window double. */
+#define WB_WINDOWS_REFERENCE 0
+#define WB_WINDOWS_NATIVE 1
+
 typedef struct wb_model wb_model;
 typedef struct wb_session wb_session;
 
@@ -76,6 +87,10 @@ int wb_device_count(int* n_out);
 /* ---- audio.rs ---------------------------------------------------------------------- */
 /* audio.rs:12-17 */
 int64_t wb_max_waveform_samples(int64_t n_frame_max);
+/* Samples of one window in a window mode (transcribe.rs:32-34 with that mode's frame limit): the window_len of
+ * wb_window_bounds.  WB_WINDOWS_REFERENCE gives wb_max_waveform_samples(n_audio_ctx - 10) (238 559 for Whisper),
+ * WB_WINDOWS_NATIVE wb_max_waveform_samples(2 * n_audio_ctx - 10) (478 559).  -1 for an unknown mode or n_audio_ctx <= 10. */
+int64_t wb_window_samples(int64_t n_audio_ctx, int window_mode);
 /* audio.rs:34-56: wave [n_batch, n_samples] -> mel_out [n_batch, 80, n_samples/160] (f32, row-major).
  * The max of audio.rs:50 is taken over the whole call (all batches), as in the reference.
  * WB_ERR_INVALID_ARG if n_samples < 400 (audio.rs:292). */
@@ -122,9 +137,16 @@ int wb_forward_decoder(wb_model* m, const int64_t* tokens, int64_t n_batch, int6
 /* A session holds, for up to max_windows audio windows x max_beams live beams each: encoder
  * output, per-layer cross K/V (computed once per window), per-layer self K/V for
  * max_text_len positions, and all workspaces.  max_beams <= 7 and k <= 7 in wb_session_step (the decoders keep 8 candidates per
- * record; the reference searches with width 5, src/transcribe.rs:232); larger values are rejected with WB_ERR_INVALID_ARG. */
+ * record; the reference searches with width 5, src/transcribe.rs:232); larger values are rejected with WB_ERR_INVALID_ARG.
+ * wb_session_create makes a WB_WINDOWS_REFERENCE session; wb_session_create_windows takes the window mode (WB_WINDOWS_*),
+ * which sets the frame limit of every call below: encode_waveforms clips windows at limit - 10 frames, encode_mels takes
+ * n_ctx <= limit, get_mel / get_encoder_output return up to limit / (limit - 1) / 2 + 1 rows per window, and
+ * waveform(s)_to_tokens cut windows of wb_window_samples(n_audio_ctx, mode) samples.  A native session holds twice the
+ * per-window encoder and cross K/V memory of a reference one. */
 int wb_session_create(wb_model* m, int64_t max_windows, int64_t max_beams, int64_t max_text_len,
                       int kv_dtype, wb_session** out);
+int wb_session_create_windows(wb_model* m, int64_t max_windows, int64_t max_beams, int64_t max_text_len,
+                              int kv_dtype, int window_mode, wb_session** out);
 void wb_session_destroy(wb_session* s);
 /* prep_audio + mel padding of mels_to_text (transcribe.rs:161-177) + forward_encoder + cross
  * K/V for n_windows waveforms; waves[i] has lens[i] samples (ragged; each >= 400). */
@@ -133,7 +155,8 @@ int wb_session_encode_waveforms(wb_session* s, const float* const* waves, const 
 /* same, windows already on the device, concatenated: window i = wave_dev[offsets[i] .. +lens[i]) */
 int wb_session_encode_waveforms_dev(wb_session* s, const float* wave_dev, const int64_t* offsets,
                                     const int64_t* lens, int64_t n_windows);
-/* forward_encoder + cross K/V from caller-provided mels [n_windows, n_mels, n_ctx] (no padding added) */
+/* forward_encoder + cross K/V from caller-provided mels [n_windows, n_mels, n_ctx] (no padding added); n_ctx up to the
+ * session's frame limit (n_audio_ctx, or 2 * n_audio_ctx in WB_WINDOWS_NATIVE), WB_ERR_INVALID_ARG above it */
 int wb_session_encode_mels(wb_session* s, const float* mel, int64_t n_windows, int64_t n_mels, int64_t n_ctx);
 /* copies the session's padded mel [n_windows, 80, n_ctx] / encoder output [n_ctx_enc, d] of one window */
 int wb_session_get_mel(wb_session* s, int64_t window, float* mel_out, int64_t capacity, int64_t* n_ctx_out);

@@ -309,15 +309,25 @@ int wb_forward_decoder(wb_model* m, const int64_t* tokens, int64_t n_batch, int6
     });
 }
 
-int wb_session_create(wb_model* m, int64_t max_windows, int64_t max_beams, int64_t max_text_len, int kv_dtype,
-                      wb_session** out) {
+int64_t wb_window_samples(int64_t n_audio_ctx, int window_mode) {
+    if (n_audio_ctx <= wb::MEL_PADDING || n_audio_ctx > INT32_MAX / 2 || (window_mode != WB_WINDOWS_REFERENCE && window_mode != WB_WINDOWS_NATIVE)) return -1;
+    return wb::window_samples((int)n_audio_ctx, window_mode);
+}
+
+int wb_session_create_windows(wb_model* m, int64_t max_windows, int64_t max_beams, int64_t max_text_len, int kv_dtype,
+                              int window_mode, wb_session** out) {
     return guarded([&] {
         WB_REQUIRE(m && out, "session_create: null pointer");
         std::unique_ptr<wb_session> s(new wb_session());
         s->model = m;
-        s->impl.reset(new wb::Session(&m->impl, max_windows, max_beams, max_text_len, kv_dtype));
+        s->impl.reset(new wb::Session(&m->impl, max_windows, max_beams, max_text_len, kv_dtype, window_mode));
         *out = s.release();
     });
+}
+
+int wb_session_create(wb_model* m, int64_t max_windows, int64_t max_beams, int64_t max_text_len, int kv_dtype,
+                      wb_session** out) {
+    return wb_session_create_windows(m, max_windows, max_beams, max_text_len, kv_dtype, WB_WINDOWS_REFERENCE, out);
 }
 
 void wb_session_destroy(wb_session* s) { delete s; }
@@ -443,7 +453,7 @@ static void waveforms_to_tokens(wb::Session& S, const float* const* waveforms, c
     // the frontend tables (mel filterbank, DFT bins) are the 16 kHz ones: the reference builds them from the caller's rate
     // (audio.rs:44, 67-143) but its binary only ever passes 16 kHz (src/bin/transcribe/main.rs:38-41 asserts it)
     WB_REQUIRE(sample_rate == 16000, "waveform_to_tokens: only 16 kHz input is supported (frontend tables are built for 16 kHz)");
-    const int64_t window_len = wb_max_waveform_samples(S.m->dims.n_audio_ctx - wb::MEL_PADDING);   // transcribe.rs:32-34
+    const int64_t window_len = wb::window_samples(S.m->dims.n_audio_ctx, S.window_mode);   // transcribe.rs:32-34
     std::vector<const float*> ptrs;
     std::vector<int64_t> lens;
     std::vector<int> owner;

@@ -13,7 +13,17 @@
 
 namespace wb {
 
-Session::Session(Model* model, int64_t max_w, int64_t max_b, int64_t max_text_len, int kv) : m(model) {
+int window_mel_frames(int n_audio_ctx, int window_mode) {
+    WB_REQUIRE(window_mode == WB_WINDOWS_REFERENCE || window_mode == WB_WINDOWS_NATIVE,
+               "window_mode must be WB_WINDOWS_REFERENCE or WB_WINDOWS_NATIVE");
+    return window_mode == WB_WINDOWS_NATIVE ? 2 * n_audio_ctx : n_audio_ctx;
+}
+
+int64_t window_samples(int n_audio_ctx, int window_mode) {
+    return wb_max_waveform_samples(window_mel_frames(n_audio_ctx, window_mode) - MEL_PADDING);   // transcribe.rs:32-34
+}
+
+Session::Session(Model* model, int64_t max_w, int64_t max_b, int64_t max_text_len, int kv, int mode) : m(model) {
     if (!m || !m->finalized) fail(WB_ERR_STATE, "session: model not finalized");
     const wb_dims& D = m->dims;
     WB_REQUIRE(max_w >= 1 && max_b >= 1 && max_w * max_b <= 4096, "session: bad max_windows / max_beams");
@@ -24,9 +34,11 @@ Session::Session(Model* model, int64_t max_w, int64_t max_b, int64_t max_text_le
     max_beams = (int)max_b;
     t_max = (int)max_text_len;
     kv_dtype = kv;
+    window_mode = mode;
+    mel_limit = window_mel_frames(D.n_audio_ctx, mode);
     Rmax = max_windows * max_beams;
-    TmS = D.n_audio_ctx + 2;
-    Tcap = (D.n_audio_ctx - 1) / 2 + 1;
+    TmS = mel_limit + 2;
+    Tcap = (mel_limit - 1) / 2 + 1;
     Mcap = (int64_t)max_windows * Tcap;
     const int d = D.n_audio_state, H = D.n_text_head, L = D.n_text_layer, V = D.n_vocab;
     WB_REQUIRE(max_beams <= DEC_KC - 1, "session: max_beams must be <= 7 (candidates kept per record by the persistent decoders)");
@@ -155,7 +167,6 @@ static void set_geometry(Session& s, const std::vector<int>& Tm) {
 
 void Session::encode_from_device_wave(const float* wave_dev, const int64_t* offsets, const int64_t* lens, int64_t n) {
     WB_REQUIRE(n >= 1 && n <= max_windows, "encode: n_windows out of range for this session");
-    const wb_dims& D = m->dims;
     std::vector<LogMelWindow> lw((size_t)n);
     std::vector<int> Tm((size_t)n);
     win_F.resize((size_t)n);
@@ -164,7 +175,7 @@ void Session::encode_from_device_wave(const float* wave_dev, const int64_t* offs
         WB_REQUIRE(lens[w] >= N_FFT, "prep_audio: waveform shorter than n_fft (audio.rs:292)");
         WB_REQUIRE(lens[w] < (int64_t)1 << 30, "prep_audio: waveform too long");
         const int F = (int)(lens[w] / HOP);                        // frames after dropping the last one
-        const int keep = std::min(F, D.n_audio_ctx - MEL_PADDING);  // transcribe.rs:173
+        const int keep = std::min(F, mel_limit - MEL_PADDING);      // transcribe.rs:173
         win_F[(size_t)w] = F;
         Tm[(size_t)w] = keep + MEL_PADDING;
         lw[(size_t)w] = LogMelWindow{offsets[w], (int)lens[w], F, keep, (int)w, ((int64_t)w * TmS + 1) * N_MELS};
@@ -199,7 +210,8 @@ void Session::encode_waveforms_host(const float* const* waves, const int64_t* le
 void Session::encode_mels_host(const float* mel, int64_t n, int64_t n_mels, int64_t n_ctx) {
     const wb_dims& D = m->dims;
     WB_REQUIRE(n_mels == D.n_mels, "Audio mel spectrum size must be n_mels (mod.rs:231-235)");
-    WB_REQUIRE(n_ctx >= 1 && n_ctx <= D.n_audio_ctx, "Audio length cannot exceed n_audio_ctx (mod.rs:236-241)");
+    WB_REQUIRE(n_ctx >= 1 && n_ctx <= mel_limit, "Audio length cannot exceed the session's mel frame limit: n_audio_ctx, "
+                                                 "2 * n_audio_ctx in native windowing (mod.rs:236-241)");
     WB_REQUIRE(n >= 1 && n <= max_windows, "encode: n_windows out of range for this session");
     std::vector<int> Tm((size_t)n, (int)n_ctx);
     set_geometry(*this, Tm);

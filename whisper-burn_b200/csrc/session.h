@@ -10,13 +10,22 @@ namespace wb {
 
 constexpr int MEL_PADDING = 10;   // transcribe.rs:33
 
+// The most mel frames one window gives the encoder (whisper_b200.h WB_WINDOWS_*): n_audio_ctx in the reference's windowing
+// (transcribe.rs:32-34, 161-177), 2 * n_audio_ctx in native windowing (conv2 has stride 2, so T <= n_audio_ctx encoder
+// positions).  Every other limit of a window follows from it: the waveform window is max_waveform_samples(limit - MEL_PADDING),
+// a window keeps at most limit - MEL_PADDING frames.  Throws WB_ERR_INVALID_ARG on an unknown mode.
+int window_mel_frames(int n_audio_ctx, int window_mode);
+int64_t window_samples(int n_audio_ctx, int window_mode);
+
 struct Session {
     Model* m = nullptr;
     cudaStream_t st = nullptr;
     int max_windows = 0, max_beams = 0, t_max = 0, kv_dtype = WB_KV_F32;
+    int window_mode = WB_WINDOWS_REFERENCE;
+    int mel_limit = 0;   // window_mel_frames(n_audio_ctx, window_mode)
     int Rmax = 0;        // max_windows * max_beams decode rows
-    int TmS = 0;         // rows per window in the token-major mel / conv1 buffers (n_audio_ctx + 2 halo rows)
-    int Tcap = 0;        // max encoder positions per window
+    int TmS = 0;         // rows per window in the token-major mel / conv1 buffers (mel_limit + 2 halo rows)
+    int Tcap = 0;        // max encoder positions per window: (mel_limit - 1) / 2 + 1
     int64_t Mcap = 0;    // max packed encoder rows
     int kmax = 8;        // candidates per row the step API can return (k <= 7)
 
@@ -94,7 +103,8 @@ struct Session {
     std::vector<cudaEvent_t> prof_ev;   // wb_session_profile_decode: launch begin / end
     void profile_decode(const int64_t* prompt, int64_t prompt_len, int n_steps, int64_t eot, float* logits_ms, float* step_ms);
 
-    Session(Model* model, int64_t max_windows, int64_t max_beams, int64_t max_text_len, int kv_dtype);
+    Session(Model* model, int64_t max_windows, int64_t max_beams, int64_t max_text_len, int kv_dtype,
+            int window_mode = WB_WINDOWS_REFERENCE);
     ~Session();
     Session(const Session&) = delete;
     Session& operator=(const Session&) = delete;

@@ -17,6 +17,7 @@ class WbError(RuntimeError):
 
 WB_OK, WB_ERR_INVALID_ARG, WB_ERR_CUDA, WB_ERR_OOM, WB_ERR_STATE, WB_ERR_UNSUPPORTED = range(6)
 WB_KV_F32, WB_KV_F16 = 0, 1
+WB_WINDOWS_REFERENCE, WB_WINDOWS_NATIVE = 0, 1
 
 
 class Dims(C.Structure):
@@ -44,6 +45,7 @@ SYMBOLS = {
     "wb_last_error": (C.c_char_p, []),
     "wb_device_count": (C.c_int, [C.POINTER(C.c_int)]),
     "wb_max_waveform_samples": (C.c_int64, [C.c_int64]),
+    "wb_window_samples": (C.c_int64, [C.c_int64, C.c_int]),
     "wb_prep_audio": (C.c_int, [C.c_int, _F, C.c_int64, C.c_int64, _F, _I64]),
     "wb_prep_audio_dev": (C.c_int, [C.c_int, _P, C.c_int64, C.c_int64, _P, _I64]),
     "wb_model_create": (C.c_int, [C.POINTER(Dims), C.c_int, C.POINTER(_P)]),
@@ -58,6 +60,7 @@ SYMBOLS = {
     "wb_forward_encoder": (C.c_int, [_P, _F, C.c_int64, C.c_int64, C.c_int64, _F]),
     "wb_forward_decoder": (C.c_int, [_P, _I64, C.c_int64, C.c_int64, _F, C.c_int64, _F]),
     "wb_session_create": (C.c_int, [_P, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.POINTER(_P)]),
+    "wb_session_create_windows": (C.c_int, [_P, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_int, C.POINTER(_P)]),
     "wb_session_destroy": (None, [_P]),
     "wb_session_encode_waveforms": (C.c_int, [_P, C.POINTER(_F), _I64, C.c_int64]),
     "wb_session_encode_waveforms_dev": (C.c_int, [_P, _P, _I64, _I64, C.c_int64]),

@@ -11,15 +11,35 @@ from . import ffi
 from .model import Whisper
 
 
+WINDOW_MODES = {"reference": ffi.WB_WINDOWS_REFERENCE, "native": ffi.WB_WINDOWS_NATIVE}
+
+
+def window_samples(n_audio_ctx: int, mode: str = "reference") -> int:
+    """Samples of one window (transcribe.rs:32-34) in a window mode: "reference" clips a window at n_audio_ctx mel frames,
+    "native" at 2 * n_audio_ctx (the encoder's full n_audio_ctx positions)."""
+    n = int(ffi.lib().wb_window_samples(n_audio_ctx, WINDOW_MODES[mode]))
+    if n < 0:
+        raise ValueError(f"window_samples: n_audio_ctx {n_audio_ctx} out of range")
+    return n
+
+
 class Session:
-    """KV-cached decoding session (wb_session): encoder output, cross/self K/V, workspaces."""
+    """KV-cached decoding session (wb_session): encoder output, cross/self K/V, workspaces.
+    windows="reference" (default) gives the encoder at most n_audio_ctx mel frames per window, as the reference does;
+    "native" gives it 2 * n_audio_ctx frames, i.e. n_audio_ctx encoder positions (one 30 s window of T = 1500)."""
 
     def __init__(self, whisper: Whisper, max_windows: int, max_beams: int = 5, max_text_len: int = 104,
-                 kv_dtype: int = ffi.WB_KV_F32):
+                 kv_dtype: int = ffi.WB_KV_F32, windows: str = "reference"):
+        if windows not in WINDOW_MODES:
+            raise ValueError(f"windows must be one of {sorted(WINDOW_MODES)}, not {windows!r}")
         self.whisper = whisper
         self.max_windows = max_windows
+        self.windows = windows
+        n_ctx = whisper.config.n_audio_ctx
+        self.max_mel_frames = 2 * n_ctx if windows == "native" else n_ctx
         self._h = C.c_void_p()
-        ffi.check(ffi.lib().wb_session_create(whisper.handle, max_windows, max_beams, max_text_len, kv_dtype, C.byref(self._h)))
+        ffi.check(ffi.lib().wb_session_create_windows(whisper.handle, max_windows, max_beams, max_text_len, kv_dtype,
+                                                      WINDOW_MODES[windows], C.byref(self._h)))
 
     def close(self):
         if getattr(self, "_h", None):
@@ -45,7 +65,7 @@ class Session:
         ffi.check(ffi.lib().wb_session_encode_mels(self._h, ffi.fptr(mels), n, n_mels, n_ctx))
 
     def get_mel(self, window: int) -> np.ndarray:
-        cap = 80 * (self.whisper.config.n_audio_ctx + 2)
+        cap = 80 * self.max_mel_frames
         buf = np.empty(cap, dtype=np.float32)
         n = C.c_int64(0)
         ffi.check(ffi.lib().wb_session_get_mel(self._h, window, ffi.fptr(buf), cap, C.byref(n)))
@@ -53,7 +73,7 @@ class Session:
 
     def get_encoder_output(self, window: int) -> np.ndarray:
         d = self.whisper.config.n_audio_state
-        cap = d * self.whisper.config.n_audio_ctx
+        cap = d * ((self.max_mel_frames - 1) // 2 + 1)
         buf = np.empty(cap, dtype=np.float32)
         n = C.c_int64(0)
         ffi.check(ffi.lib().wb_session_get_encoder_output(self._h, window, ffi.fptr(buf), cap, C.byref(n)))
