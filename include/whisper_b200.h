@@ -65,6 +65,22 @@ extern "C" {
 #define WB_WINDOWS_REFERENCE 0
 #define WB_WINDOWS_NATIVE 1
 
+/* Search rules of a session (wb_session_set_search): how wb_transcribe_windows[_dev] and wb_waveform(s)_to_tokens pick tokens.
+ *   BEAM:        the reference's beam::beam_search (transcribe.rs:232-309) with beam_size / max_depth; greedy is beam_size 1.
+ *                The special ids are masked while a sequence has at most 5 tokens.  The default.
+ *   GREEDY_LOOP: the greedy loop the reference leaves commented out (transcribe.rs:314-380).  At each step the arg-max of
+ *                the raw logits (no special-token mask; is_special is ignored and may be NULL) is appended, then
+ *                - EOT test: when exp(eot_logit - token_logit) > 0.5 (f64 on the two f32 logits) the window ends, with EOT
+ *                  appended unless the arg-max was EOT;
+ *                - repetition cut: when find_repeated_tokens_index(tokens, 5, 4) (the whole sequence, prompt included)
+ *                  finds (first, end), the sequence is cut to `end` tokens and EOT appended;
+ *                - context stop: a sequence of min(n_text_ctx, 4 + max_depth) tokens gets EOT appended.
+ *                beam_size must be 1 (WB_ERR_INVALID_ARG otherwise), and every window ends in EOT, so an output row holds
+ *                up to 4 + max_depth + 1 ids.  max_depth = n_text_ctx - 4 on a session with max_text_len = n_text_ctx is
+ *                the reference's loop exactly.  Windowing and the overlap merge are those of both window modes. */
+#define WB_SEARCH_BEAM 0
+#define WB_SEARCH_GREEDY_LOOP 1
+
 typedef struct wb_model wb_model;
 typedef struct wb_session wb_session;
 
@@ -148,6 +164,8 @@ int wb_session_create(wb_model* m, int64_t max_windows, int64_t max_beams, int64
 int wb_session_create_windows(wb_model* m, int64_t max_windows, int64_t max_beams, int64_t max_text_len,
                               int kv_dtype, int window_mode, wb_session** out);
 void wb_session_destroy(wb_session* s);
+/* Sets the search rule (WB_SEARCH_*) of the session's decode calls; WB_ERR_INVALID_ARG on an unknown rule. */
+int wb_session_set_search(wb_session* s, int rule);
 /* prep_audio + mel padding of mels_to_text (transcribe.rs:161-177) + forward_encoder + cross
  * K/V for n_windows waveforms; waves[i] has lens[i] samples (ragged; each >= 400). */
 int wb_session_encode_waveforms(wb_session* s, const float* const* waves, const int64_t* lens,

@@ -25,6 +25,8 @@ pub mod ffi {
         pub n_mels: i32, pub n_audio_ctx: i32, pub n_audio_state: i32, pub n_audio_head: i32, pub n_audio_layer: i32,
         pub n_vocab: i32, pub n_text_ctx: i32, pub n_text_state: i32, pub n_text_head: i32, pub n_text_layer: i32,
     }
+    pub const WB_SEARCH_BEAM: c_int = 0;          // search rules of a session (wb_session_set_search)
+    pub const WB_SEARCH_GREEDY_LOOP: c_int = 1;
     #[repr(C)]
     #[derive(Clone, Copy, Debug)]
     pub struct wb_special_ids { pub sot: i64, pub lang: i64, pub transcribe: i64, pub notimestamps: i64, pub eot: i64 }
@@ -45,6 +47,7 @@ pub mod ffi {
         pub fn wb_forward_decoder(m: *mut c_void, tokens: *const i64, n_batch: i64, seq_len: i64, enc: *const f32, n_enc_ctx: i64, logits_out: *mut f32) -> c_int;
         pub fn wb_session_create(m: *mut c_void, max_windows: i64, max_beams: i64, max_text_len: i64, kv_dtype: c_int, out: *mut *mut c_void) -> c_int;
         pub fn wb_session_destroy(s: *mut c_void);
+        pub fn wb_session_set_search(s: *mut c_void, rule: c_int) -> c_int;
         pub fn wb_session_encode_mels(s: *mut c_void, mel: *const f32, n_windows: i64, n_mels: i64, n_ctx: i64) -> c_int;
         pub fn wb_session_begin(s: *mut c_void, prompt: *const i64, prompt_len: i64) -> c_int;
         pub fn wb_session_step(s: *mut c_void, n_rows: i64, window_of_row: *const i32, parent_row: *const i32, token: *const i64, apply_special_mask: c_int,
@@ -252,6 +255,31 @@ pub mod transcribe {
         whisper.with_session(n_windows.min(64), BEAM_SIZE, 4 + MAX_DEPTH + 1, |s| {
             check(unsafe { ffi::wb_waveform_to_tokens(s, waveform.as_ptr(), waveform.len() as i64, sample_rate as i64, BEAM_SIZE as c_int,
                                                       MAX_DEPTH as c_int, &sp.ids, sp.is_special.as_ptr(), out.as_mut_ptr(), cap as i64, &mut n) })
+        })?;
+        let tokens: Vec<usize> = out[..n as usize].iter().map(|&t| t as usize).collect();
+        Ok((bpe.decode(&tokens[..], true)?, tokens))
+    }
+
+    /// The greedy loop the reference leaves commented out in `mels_to_text` (src/transcribe.rs:314-380), with waveform_to_text's
+    /// signature and windowing: per window the arg-max of the raw logits (no special-token mask) until the EOT probability stop,
+    /// the repetition cut of find_repeated_tokens_index(tokens, 5, 4) or n_text_ctx tokens, all on the GPU in one decoder launch
+    /// per batch of windows (WB_SEARCH_GREEDY_LOOP with max_depth = n_text_ctx - 4: the reference's loop exactly).
+    pub fn waveform_to_text_greedy_loop(whisper: &model::Whisper, bpe: &Gpt2Tokenizer, lang: Language, waveform: Vec<f32>, sample_rate: usize)
+            -> token::Result<(String, Vec<usize>)> {
+        let sp = SpecialTokens::from_tokenizer(bpe, lang);
+        let window = audio::max_waveform_samples(whisper.encoder_ctx_size() - 10);            // transcribe.rs:32-34
+        let shift = window.saturating_sub(sample_rate * 3).max(1);                             // transcribe.rs:120-123
+        let n_windows = waveform.len().saturating_sub(1) / shift + 1;
+        let n_ctx = whisper.decoder_ctx_size();
+        let cap = n_windows * (n_ctx + 1) + 16;
+        let mut out = vec![0i64; cap];
+        let mut n = 0i64;
+        whisper.with_session(n_windows.min(64), 1, n_ctx, |s| {
+            check(unsafe { ffi::wb_session_set_search(s, ffi::WB_SEARCH_GREEDY_LOOP) })?;
+            let r = check(unsafe { ffi::wb_waveform_to_tokens(s, waveform.as_ptr(), waveform.len() as i64, sample_rate as i64, 1,
+                                                              (n_ctx - 4) as c_int, &sp.ids, std::ptr::null(), out.as_mut_ptr(), cap as i64, &mut n) });
+            check(unsafe { ffi::wb_session_set_search(s, ffi::WB_SEARCH_BEAM) })?;   // the cached session's other callers search by beam
+            r
         })?;
         let tokens: Vec<usize> = out[..n as usize].iter().map(|&t| t as usize).collect();
         Ok((bpe.decode(&tokens[..], true)?, tokens))

@@ -70,6 +70,11 @@ void copy_tokens_out(const std::vector<std::vector<int64_t>>& toks, int64_t* tok
     }
 }
 
+// the decode calls need the is_special bitmap, except under the greedy loop, which masks nothing
+bool special_given(const wb_session* s, const uint8_t* is_special) {
+    return is_special != nullptr || (s && s->impl->search == WB_SEARCH_GREEDY_LOOP);
+}
+
 void collect_timings(wb::Session& s) {
     WB_CUDA(cudaStreamSynchronize(s.st));
     cudaEventElapsedTime(&s.last_ms[0], s.ev[0], s.ev[1]);
@@ -332,6 +337,14 @@ int wb_session_create(wb_model* m, int64_t max_windows, int64_t max_beams, int64
 
 void wb_session_destroy(wb_session* s) { delete s; }
 
+int wb_session_set_search(wb_session* s, int rule) {
+    return guarded([&] {
+        WB_REQUIRE(s, "set_search: null pointer");
+        WB_REQUIRE(rule == WB_SEARCH_BEAM || rule == WB_SEARCH_GREEDY_LOOP, "set_search: unknown search rule");
+        s->impl->search = rule;
+    });
+}
+
 int wb_session_encode_waveforms(wb_session* s, const float* const* waves, const int64_t* lens, int64_t n_windows) {
     return guarded([&] {
         WB_REQUIRE(s && waves && lens, "encode: null pointer");
@@ -410,7 +423,7 @@ int wb_transcribe_windows(wb_session* s, const float* const* waves, const int64_
                           int beam_size, int max_depth, const wb_special_ids* ids, const uint8_t* is_special,
                           int64_t* tokens_out, int64_t capacity, int64_t* lens_out) {
     return guarded([&] {
-        WB_REQUIRE(s && waves && lens && ids && is_special && tokens_out && lens_out, "transcribe: null pointer");
+        WB_REQUIRE(s && waves && lens && ids && special_given(s, is_special) && tokens_out && lens_out, "transcribe: null pointer");
         s->impl->encode_waveforms_host(waves, lens, n_windows);
         std::vector<std::vector<int64_t>> toks;
         wb::transcribe_windows(*s->impl, beam_size, max_depth, *ids, is_special, toks);
@@ -423,7 +436,7 @@ int wb_transcribe_windows_dev(wb_session* s, const float* wave_dev, const int64_
                               int64_t n_windows, int beam_size, int max_depth, const wb_special_ids* ids,
                               const uint8_t* is_special, int64_t* tokens_out, int64_t capacity, int64_t* lens_out) {
     return guarded([&] {
-        WB_REQUIRE(s && wave_dev && offsets && lens && ids && is_special && tokens_out && lens_out, "transcribe: null pointer");
+        WB_REQUIRE(s && wave_dev && offsets && lens && ids && special_given(s, is_special) && tokens_out && lens_out, "transcribe: null pointer");
         s->impl->encode_from_device_wave(wave_dev, offsets, lens, n_windows);
         std::vector<std::vector<int64_t>> toks;
         wb::transcribe_windows(*s->impl, beam_size, max_depth, *ids, is_special, toks);
@@ -488,7 +501,7 @@ int wb_waveform_to_tokens(wb_session* s, const float* waveform, int64_t n_sample
                           int max_depth, const wb_special_ids* ids, const uint8_t* is_special, int64_t* tokens_out,
                           int64_t capacity, int64_t* n_tokens_out) {
     return guarded([&] {
-        WB_REQUIRE(s && waveform && ids && is_special && tokens_out && n_tokens_out, "waveform_to_tokens: null pointer");
+        WB_REQUIRE(s && waveform && ids && special_given(s, is_special) && tokens_out && n_tokens_out, "waveform_to_tokens: null pointer");
         std::vector<std::vector<int64_t>> out;
         waveforms_to_tokens(*s->impl, &waveform, &n_samples, 1, sample_rate, beam_size, max_depth, *ids, is_special, out);
         WB_REQUIRE((int64_t)out[0].size() <= capacity, "tokens_out capacity too small");
@@ -501,7 +514,7 @@ int wb_waveforms_to_tokens(wb_session* s, const float* const* waveforms, const i
                            int64_t sample_rate, int beam_size, int max_depth, const wb_special_ids* ids,
                            const uint8_t* is_special, int64_t* tokens_out, int64_t capacity, int64_t* n_tokens_out) {
     return guarded([&] {
-        WB_REQUIRE(s && waveforms && n_samples && ids && is_special && tokens_out && n_tokens_out, "waveforms_to_tokens: null pointer");
+        WB_REQUIRE(s && waveforms && n_samples && ids && special_given(s, is_special) && tokens_out && n_tokens_out, "waveforms_to_tokens: null pointer");
         WB_REQUIRE(n_waveforms >= 1, "waveforms_to_tokens: n_waveforms must be >= 1");
         std::vector<std::vector<int64_t>> out;
         waveforms_to_tokens(*s->impl, waveforms, n_samples, n_waveforms, sample_rate, beam_size, max_depth, *ids, is_special, out);

@@ -8,6 +8,7 @@
 #include <cuda_fp16.h>
 #include <climits>
 
+#include "../host/loop_rules.hpp"
 #include "decoder.h"
 #include "wb_internal.h"
 
@@ -965,6 +966,30 @@ __device__ __forceinline__ void greedy_commit(const DecArgs& a, int r, int p, in
         if (id == a.eot) a.finished[r] = 1;
     }
 }
+// The greedy loop's rules (DecArgs::loop_rules, host/loop_rules.hpp) for row r after greedy_commit put `id` at p + 1: the EOT
+// test on the raw logits of `id` (`top`) and of EOT, then the repetition cut over tokens[0, p + 2), lane l taking windows
+// i = l (mod 32).  Only for a row that was open before the commit.  The EOT test only finishes the row: the host appends the
+// EOT that follows (Session::greedy_decode).  The cut writes EOT at `end` and finishes the row.  Called by a whole warp.
+__device__ __forceinline__ void loop_finish(const DecArgs& a, int r, int p, int id, float top) {
+    if (id == a.eot) return;   // finished by greedy_commit; the EOT test holds and appends nothing
+    const int lane = threadIdx.x & 31;
+    if (loop::eot_stop(__ldcg(a.eot_logit + r), top)) {
+        if (lane == 0) a.finished[r] = 1;
+        return;
+    }
+    int* row = a.tokens + (int64_t)r * a.t_max;
+    const int n = p + 2;
+    auto tok = [&](int j) { return j == p + 1 ? id : __ldcg(row + j); };
+    const int end = loop::repeat_cut(n, [&](int base) {
+        const int i = base + lane;
+        return __ballot_sync(0xffffffffu, i + 2 * loop::REPEAT_WINDOW <= n && loop::window_repeats(tok, n, i));
+    });
+    if (end >= 0 && lane == 0) {
+        row[end] = a.eot;
+        a.lengths[r] = end + 1;
+        a.finished[r] = 1;
+    }
+}
 // rows whose search is still open: every row, or in a greedy search those that have not produced EOT
 __device__ __forceinline__ int rows_open(const DecArgs& a) {
     int live = 0;
@@ -1009,6 +1034,7 @@ __device__ __forceinline__ void finish_row_top1(const DecArgs& a, int r, int p, 
         rv[k] = __ldcg(a.lg_v + o);
         ri[k] = __ldcg(a.lg_i + o);
     }
+    const bool loop_open = a.loop_rules && !__ldcg(a.finished + r);   // read before the commit below
     float mx;
     const float lse = row_lse<NPL>(rm, rs, NP, mx);
     float bv = -INFINITY;
@@ -1022,12 +1048,15 @@ __device__ __forceinline__ void finish_row_top1(const DecArgs& a, int r, int p, 
         a.topk_lp[r] = __fsub_rn(__fsub_rn(bv, mx), lse);
         greedy_commit(a, r, p, bi);
     }
+    if (loop_open) loop_finish(a, r, p, bi, bv);   // bv: the raw logit of bi (no mask in loop mode)
 }
 // CTA per row, the k best candidates of row r from its NP KC-list records -> topk_id / topk_lp [r][k]; candidate 0 goes
 // to the greedy bookkeeping.  s_f / s_i: NW floats / ints of shared scratch.  Called by the whole CTA.
 template <int KC>
 __device__ __forceinline__ void finish_row_topk(const DecArgs& a, int r, int p, int NP, float* s_f, int* s_i) {
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, R = a.R;
+    const bool loop_open = a.loop_rules && !__ldcg(a.finished + r);   // read before the commit below
+    int id0 = -1;
     float mx = -INFINITY;
     for (int c = tid; c < NP; c += NT) mx = fmaxf(mx, __ldcg(a.lg_m + (int64_t)c * R + r));
 #pragma unroll
@@ -1077,9 +1106,12 @@ __device__ __forceinline__ void finish_row_topk(const DecArgs& a, int r, int p, 
             a.topk_lp[(int64_t)r * a.k + kk] = bv;
             if (kk == 0) greedy_commit(a, r, p, bi);
         }
+        if (kk == 0) id0 = bi;
         prev_v = bv;
         prev_i = bi;
     }
+    // the raw logit of candidate 0 is the row's max mx: the records' maxima run over the same values as their candidates
+    if (loop_open && warp == 0) loop_finish(a, r, p, id0, mx);
 }
 
 // ---- ticket finish (decoder4, decoder6): every CTA takes a ticket after publishing its records; the CTA that takes the last

@@ -72,6 +72,11 @@ struct DecArgs {
     int mask_mode = 0;
     int k = 1, greedy = 0, eot = -1;
     int *lengths = nullptr, *finished = nullptr;
+    // greedy loop (WB_SEARCH_GREEDY_LOOP, host/loop_rules.hpp): the row finish also applies the EOT test and the repetition
+    // cut (dec_common.cuh loop_finish); the vocabulary stage stores each row's raw EOT logit in eot_logit [R].  The context
+    // stop is the launch's n_steps.
+    int loop_rules = 0;
+    float* eot_logit = nullptr;
     int *topk_id = nullptr;
     float* topk_lp = nullptr;
     float* logits_out = nullptr;

@@ -254,6 +254,7 @@ dec3_kernel(const DecArgs a) {
             // ================= logits = LN(x) tok_emb^T (mod.rs:155-156) + mask + online softmax + candidates.
             // 8 lanes per vocabulary row, 8 rows per warp step; lane (sub, l8) tracks batch row l8.
             const bool use_mask = a.is_special != nullptr && (a.mask_mode == 1 || (a.mask_mode == 2 && p + 1 <= 5));
+            const int eot_cap = a.loop_rules ? a.eot : -1;   // the id whose logit the greedy loop's EOT test reads
             const WT* E = reinterpret_cast<const WT*>(a.E);
             const int sub = lane >> 3, l8 = lane & 7;
             for (int r0 = 0; r0 < R; r0 += RC) {
@@ -283,6 +284,7 @@ dec3_kernel(const DecArgs a) {
                                 const float v = (use_mask && a.is_special[nn[g]]) ? __fadd_rn(raw, -INFINITY) : raw;
                                 if (v > -INFINITY) softmax_add(m_run, s_run, v);
                                 cand.push(v, nn[g]);
+                                if (nn[g] == eot_cap) a.eot_logit[r0 + l8] = v;
                             }
                         }
                     }

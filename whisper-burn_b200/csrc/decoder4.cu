@@ -757,6 +757,7 @@ dec4_kernel(const DecArgs a) {
         // ================= logits (all CTAs): LN(x) tok_emb^T + mask + online softmax + candidates
         {
             const bool use_mask = a.is_special != nullptr && (a.mask_mode == 1 || (a.mask_mode == 2 && p + 1 <= 5));
+            const int eot_cap = a.loop_rules ? a.eot : -1;   // the id whose logit the greedy loop's EOT test reads
             // the published rows: fp16 hi / lo planes in MMA fragment order (decoder5.cu); rows >= R are never used
             for (int i = tid; i < 2 * (D / 32) * 32; i += NT) cp_async16(pl_hi + i, gpl_hi + i);   // pl_lo follows pl_hi in both spaces
             cp_async_wait_all();
@@ -812,6 +813,7 @@ dec4_kernel(const DecArgs a) {
                             const float v = (use_mask && ((sp01 >> ((c >> 1) * 8)) & 0xffu)) ? __fadd_rn(raw, -INFINITY) : raw;
                             if (v > -INFINITY) softmax_add(m_run[e], s_run[e], v);
                             if (cand_better(v, n, bv[e], bi[e])) { bv[e] = v; bi[e] = n; }
+                            if (n == eot_cap) a.eot_logit[2 * t + e] = v;
                         }
                     }
                 }

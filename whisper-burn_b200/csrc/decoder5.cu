@@ -575,6 +575,8 @@ dec5_kernel(const DecArgs a) {
                         const float* row = a.lgbuf + (int64_t)r * V;
                         float m_run = -INFINITY, s_run = 0.0f, bv = -INFINITY;
                         int bi = INT_MAX;
+                        // the id whose logit the greedy loop's EOT test reads, when this slice holds it
+                        const int eot_cap = a.loop_rules && a.eot >= n_begin && a.eot < n_end ? a.eot : -1;
 #pragma unroll 1
                         for (int n0 = n_begin + tid; n0 < n_end; n0 += NT * 8) {
                             float val[8];
@@ -592,6 +594,7 @@ dec5_kernel(const DecArgs a) {
                                 if (n0 + i * NT >= n_end) val[i] = -INFINITY;
                                 bm = fmaxf(bm, val[i]);
                                 if (val[i] > bv) { bv = val[i]; bi = n0 + i * NT; }   // indices grow: ties keep the lower id
+                                if (n0 + i * NT == eot_cap) a.eot_logit[r] = val[i];
                             }
                             if (bm > -INFINITY) {
                                 const float mn = fmaxf(m_run, bm);
@@ -840,6 +843,7 @@ int launch_dec5(const DecArgs& a, const Dec5Tables& t, int n_ctas, bool w_half, 
         g.row_window += r0;
         if (g.anc) g.anc += (int64_t)r0 * a.t_max;
         g.tokens += (int64_t)r0 * a.t_max; g.cur_tok += r0; g.lengths += r0; g.finished += r0;
+        if (g.eot_logit) g.eot_logit += r0;
         g.topk_id += (int64_t)r0 * a.k; g.topk_lp += (int64_t)r0 * a.k;
         if (g.logits_out) { g.logits_out += (int64_t)r0 * a.V; g.lgbuf = g.logits_out; }
         g.lg_slices = std::max(1, std::min(16, n_ctas / std::max(1, Rg)));

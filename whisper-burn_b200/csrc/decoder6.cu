@@ -979,6 +979,7 @@ dec6_kernel(const DecArgs a) {
                 trace();
                 // ================= logits (all CTAs): LN(x) tok_emb^T + mask + online softmax + arg-max (mod.rs:155-156, transcribe.rs:271-276)
                 const bool use_mask = a.is_special != nullptr && (a.mask_mode == 1 || (a.mask_mode == 2 && p + 1 <= 5));
+                const int eot_cap = !BEAM && a.loop_rules ? a.eot : -1;   // the id whose logit the greedy loop's EOT test reads
                 // LayerNorm rows straight into fp16 hi / lo planes in MMA fragment order (decoder5.cu); rows >= R are zero
                 for (int r = warp; r < 8 * NT8; r += NCW) {
                     constexpr int NV = D / 128;   // float4 per lane
@@ -1119,6 +1120,7 @@ dec6_kernel(const DecArgs a) {
                                         const float v = (use_mask && a.is_special[n]) ? __fadd_rn(raw, -INFINITY) : raw;
                                         if (v > -INFINITY) softmax_add(m_run[j][e], s_run[j][e], v);
                                         if (cand_better(v, n, bv[j][e], bi[j][e])) { bv[j][e] = v; bi[j][e] = n; }
+                                        if (n == eot_cap) a.eot_logit[j * 8 + 2 * t + e] = v;
                                     }
                                 }
                         }

@@ -82,6 +82,7 @@ Session::Session(Model* model, int64_t max_w, int64_t max_b, int64_t max_text_le
     row_window.alloc(Rmax); anc0.alloc((size_t)Rmax * t_max); anc1.alloc((size_t)Rmax * t_max); parent.alloc(Rmax);
     pos.alloc(1); n_unfinished.alloc(128);
     topk_id.alloc((size_t)Rmax * kmax); topk_lp.alloc((size_t)Rmax * kmax);
+    eot_logit.alloc(Rmax);
     is_special.alloc(V);
     {
         ckv_tmp.alloc(Mcap * 2 * d);
@@ -413,7 +414,7 @@ void Session::begin(const int64_t* prompt, int64_t prompt_len, bool prefill) {
 // The persistent decoder for n_steps positions starting at pos0: the first of decoder4 -> decoder6 -> decoder5 -> decoder3
 // that covers the launch (each launch_decN decides that itself), or only the one WB200_DECODER names.
 bool Session::launch_decoder(int R_, int pos0, int n_steps, int logits_from, bool use_cur_tok, int mask_mode, int k,
-                        bool greedy, int eot, int beam, int max_depth) {
+                        bool greedy, int eot, int beam, int max_depth, bool loop_rules) {
     const wb_dims& D = m->dims;
     const int d = D.n_text_state, H = D.n_text_head;
     DecArgs a;
@@ -436,6 +437,7 @@ bool Session::launch_decoder(int R_, int pos0, int n_steps, int logits_from, boo
     a.pos0 = pos0; a.n_steps = n_steps; a.logits_from = logits_from;
     a.is_special = have_special ? is_special.p : nullptr; a.mask_mode = mask_mode;
     a.k = k; a.greedy = greedy ? 1 : 0; a.eot = eot; a.lengths = lengths.p; a.finished = finished.p;
+    a.loop_rules = loop_rules ? 1 : 0; a.eot_logit = eot_logit.p;
     a.topk_id = topk_id.p; a.topk_lp = topk_lp.p; a.logits_out = full_logits ? logits.p : nullptr;
     a.lg_m = lg_m.p; a.lg_s = lg_s.p; a.lg_v = lg_v.p; a.lg_i = lg_i.p;
     a.pos = pos.p; a.n_unfinished = n_unfinished.p; a.steps_done = steps_done.p; a.bar = dec_bar.p;
@@ -561,12 +563,14 @@ void Session::last_topk(int64_t n_rows, int64_t k, int64_t* ids_out, float* lp_o
 }
 
 void Session::greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_depth, int64_t eot,
-                            std::vector<std::vector<int64_t>>& out) {
+                            std::vector<std::vector<int64_t>>& out, bool loop_rules) {
     WB_REQUIRE(prompt_len + max_depth <= t_max, "greedy: prompt + max_depth exceeds the session's max_text_len");
-    // one launch: prompt prefill + every greedy step, early exit inside the kernel
+    // one launch: prompt prefill + every greedy step, early exit inside the kernel.  The beam rule masks the special ids while
+    // a sequence has at most 5 tokens (mask_mode 2); the greedy loop masks nothing, and its context stop, at
+    // prompt_len + max_depth <= t_max <= n_text_ctx tokens, is the end of the launch.
     begin(prompt, prompt_len, /*prefill=*/false);
     const int n_steps = (int)prompt_len - 1 + max_depth;
-    if (max_depth > 0) launch_decoder(R, 0, n_steps, (int)prompt_len - 1, false, 2, 1, true, (int)eot);
+    if (max_depth > 0) launch_decoder(R, 0, n_steps, (int)prompt_len - 1, false, loop_rules ? 0 : 2, 1, true, (int)eot, 0, 0, loop_rules);
     std::vector<int> tk((size_t)R * t_max), len((size_t)R);
     int sdv[128] = {0};
     WB_CUDA(cudaMemcpyAsync(tk.data(), tokens.p, tk.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -578,8 +582,12 @@ void Session::greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_d
     last_steps = max_depth > 0 ? sd - ((int)prompt_len - 1) : 0;
     host_pos = (int)prompt_len - 1 + (int)last_steps;
     out.assign((size_t)R, {});
-    for (int r = 0; r < R; ++r)
+    for (int r = 0; r < R; ++r) {
         for (int i = 0; i < len[(size_t)r]; ++i) out[(size_t)r].push_back(tk[(size_t)r * t_max + i]);
+        // the greedy loop always ends in EOT: the EOT test's EOT and the context stop's are appended here (the latter may
+        // not fit the token buffer)
+        if (loop_rules && out[(size_t)r].back() != eot) out[(size_t)r].push_back(eot);
+    }
 }
 
 bool Session::beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_size, int max_depth, int64_t eot,

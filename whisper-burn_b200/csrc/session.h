@@ -22,6 +22,7 @@ struct Session {
     cudaStream_t st = nullptr;
     int max_windows = 0, max_beams = 0, t_max = 0, kv_dtype = WB_KV_F32;
     int window_mode = WB_WINDOWS_REFERENCE;
+    int search = WB_SEARCH_BEAM;   // wb_session_set_search: the rule transcribe_windows decodes by
     int mel_limit = 0;   // window_mel_frames(n_audio_ctx, window_mode)
     int Rmax = 0;        // max_windows * max_beams decode rows
     int TmS = 0;         // rows per window in the token-major mel / conv1 buffers (mel_limit + 2 halo rows)
@@ -66,6 +67,7 @@ struct Session {
     DevBuf<float> part_o, part_m, part_l;
     DevBuf<int> tokens, lengths, cur_tok, finished, row_window, anc0, anc1, parent, pos, n_unfinished, topk_id;
     DevBuf<float> topk_lp;
+    DevBuf<float> eot_logit;   // [Rmax] raw EOT logit of each row at the current position (greedy loop)
     DevBuf<uint8_t> is_special;
     bool have_special = false;
     int anc_cur = 0;       // which ancestry table is current
@@ -92,7 +94,7 @@ struct Session {
     DevBuf<unsigned long long> dec_trace;   // debug: WB200_TRACE=1
     // beam > 1: the whole beam search in one decoder6 launch (beam_decode); returns false when decoder6 does not cover it
     bool launch_decoder(int R_, int pos0, int n_steps, int logits_from, bool use_cur_tok, int mask_mode, int k, bool greedy,
-                   int eot, int beam = 0, int max_depth = 0);
+                   int eot, int beam = 0, int max_depth = 0, bool loop_rules = false);
     // device beam search state (decoder6.cu beam mode), allocated on first use
     DevBuf<int> slot_live, bm_seq, bm_cnt, bm_win, bm_out, bm_out_len;
     DevBuf<beamfx::Head> bm_head;
@@ -126,9 +128,10 @@ struct Session {
                     int apply_mask, int k, int64_t* topk_ids_out, float* topk_lp_out);
     // the [n_rows][k] candidates the last launch wrote at its last position
     void last_topk(int64_t n_rows, int64_t k, int64_t* ids_out, float* lp_out);
-    // greedy loop on the device; returns per-window token lists
+    // greedy search on the device in one launch; returns per-window token lists.  loop_rules: the reference's greedy loop
+    // (WB_SEARCH_GREEDY_LOOP) instead of beam_size 1
     void greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_depth, int64_t eot,
-                       std::vector<std::vector<int64_t>>& out);
+                       std::vector<std::vector<int64_t>>& out, bool loop_rules = false);
     // the whole beam search (prefill + up to max_depth steps) of every encoded window in ONE decoder launch; false (nothing
     // decoded) when no decoder covers it, and the caller runs the host search
     bool beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_size, int max_depth, int64_t eot,

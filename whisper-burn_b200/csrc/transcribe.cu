@@ -65,6 +65,8 @@ using Node = beam::BeamNode<BeamSearchToken>;
 
 void transcribe_windows(Session& s, int beam_size, int max_depth, const wb_special_ids& ids, const uint8_t* is_special,
                         std::vector<std::vector<int64_t>>& out) {
+    const bool loop = s.search == WB_SEARCH_GREEDY_LOOP;
+    WB_REQUIRE(!loop || beam_size == 1, "transcribe: the greedy loop takes beam_size 1");
     WB_REQUIRE(beam_size >= 1 && beam_size <= s.max_beams, "transcribe: beam_size exceeds the session's max_beams");
     WB_REQUIRE(max_depth >= 0, "transcribe: negative max_depth");
     const int V = s.m->dims.n_vocab;
@@ -74,8 +76,8 @@ void transcribe_windows(Session& s, int beam_size, int max_depth, const wb_speci
     WB_REQUIRE(4 + max_depth <= s.t_max, "transcribe: 4 + max_depth exceeds the session's max_text_len");
     s.set_special(is_special);
     const int W = s.n_windows;
-    if (beam_size == 1) {
-        s.greedy_decode(prompt, 4, max_depth, ids.eot, out);
+    if (beam_size == 1) {   // greedy: beam_size 1 of the search, or the greedy loop (transcribe.rs:314-380)
+        s.greedy_decode(prompt, 4, max_depth, ids.eot, out, loop);
         WB_CUDA(cudaEventRecord(s.ev[3], s.st));
         return;
     }

@@ -18,6 +18,7 @@ class WbError(RuntimeError):
 WB_OK, WB_ERR_INVALID_ARG, WB_ERR_CUDA, WB_ERR_OOM, WB_ERR_STATE, WB_ERR_UNSUPPORTED = range(6)
 WB_KV_F32, WB_KV_F16 = 0, 1
 WB_WINDOWS_REFERENCE, WB_WINDOWS_NATIVE = 0, 1
+WB_SEARCH_BEAM, WB_SEARCH_GREEDY_LOOP = 0, 1
 
 
 class Dims(C.Structure):
@@ -62,6 +63,7 @@ SYMBOLS = {
     "wb_session_create": (C.c_int, [_P, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.POINTER(_P)]),
     "wb_session_create_windows": (C.c_int, [_P, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_int, C.POINTER(_P)]),
     "wb_session_destroy": (None, [_P]),
+    "wb_session_set_search": (C.c_int, [_P, C.c_int]),
     "wb_session_encode_waveforms": (C.c_int, [_P, C.POINTER(_F), _I64, C.c_int64]),
     "wb_session_encode_waveforms_dev": (C.c_int, [_P, _P, _I64, _I64, C.c_int64]),
     "wb_session_encode_mels": (C.c_int, [_P, _F, C.c_int64, C.c_int64, C.c_int64]),

@@ -12,6 +12,7 @@ from .model import Whisper
 
 
 WINDOW_MODES = {"reference": ffi.WB_WINDOWS_REFERENCE, "native": ffi.WB_WINDOWS_NATIVE}
+SEARCH_RULES = {"beam": ffi.WB_SEARCH_BEAM, "greedy_loop": ffi.WB_SEARCH_GREEDY_LOOP}
 
 
 def window_samples(n_audio_ctx: int, mode: str = "reference") -> int:
@@ -23,15 +24,25 @@ def window_samples(n_audio_ctx: int, mode: str = "reference") -> int:
     return n
 
 
+def _special(is_special: Optional[np.ndarray]):
+    """The is_special bitmap as a pointer argument (None: NULL, which the greedy loop accepts)."""
+    return None if is_special is None else ffi.u8ptr(np.ascontiguousarray(is_special, dtype=np.uint8))
+
+
 class Session:
     """KV-cached decoding session (wb_session): encoder output, cross/self K/V, workspaces.
     windows="reference" (default) gives the encoder at most n_audio_ctx mel frames per window, as the reference does;
-    "native" gives it 2 * n_audio_ctx frames, i.e. n_audio_ctx encoder positions (one 30 s window of T = 1500)."""
+    "native" gives it 2 * n_audio_ctx frames, i.e. n_audio_ctx encoder positions (one 30 s window of T = 1500).
+    search="beam" (default) decodes with the reference's beam search (greedy = beam_size 1); "greedy_loop" with the greedy
+    loop it leaves commented out (transcribe.rs:314-380: no special-token mask, EOT-probability stop, repetition cut, context
+    stop; beam_size must be 1 and is_special may be None)."""
 
     def __init__(self, whisper: Whisper, max_windows: int, max_beams: int = 5, max_text_len: int = 104,
-                 kv_dtype: int = ffi.WB_KV_F32, windows: str = "reference"):
+                 kv_dtype: int = ffi.WB_KV_F32, windows: str = "reference", search: str = "beam"):
         if windows not in WINDOW_MODES:
             raise ValueError(f"windows must be one of {sorted(WINDOW_MODES)}, not {windows!r}")
+        if search not in SEARCH_RULES:
+            raise ValueError(f"search must be one of {sorted(SEARCH_RULES)}, not {search!r}")
         self.whisper = whisper
         self.max_windows = max_windows
         self.windows = windows
@@ -40,6 +51,8 @@ class Session:
         self._h = C.c_void_p()
         ffi.check(ffi.lib().wb_session_create_windows(whisper.handle, max_windows, max_beams, max_text_len, kv_dtype,
                                                       WINDOW_MODES[windows], C.byref(self._h)))
+        self.search = search
+        ffi.check(ffi.lib().wb_session_set_search(self._h, SEARCH_RULES[search]))
 
     def close(self):
         if getattr(self, "_h", None):
@@ -107,9 +120,9 @@ class Session:
         out = np.zeros((len(ws), cap), dtype=np.int64)
         out_len = np.zeros(len(ws), dtype=np.int64)
         ids = ffi.SpecialIds(special.sot, special.lang, special.transcribe, special.notimestamps, special.eot)
-        sp = np.ascontiguousarray(is_special, dtype=np.uint8)
+        sp = _special(is_special)
         ffi.check(ffi.lib().wb_transcribe_windows(self._h, ptrs, ffi.i64ptr(lens), len(ws), beam_size, max_depth,
-                                                 C.byref(ids), ffi.u8ptr(sp), ffi.i64ptr(out), cap, ffi.i64ptr(out_len)))
+                                                 C.byref(ids), sp, ffi.i64ptr(out), cap, ffi.i64ptr(out_len)))
         return [[int(t) for t in out[i, :out_len[i]]] for i in range(len(ws))]
 
     def transcribe_windows_dev(self, wave_dev_ptr: int, offsets, lens, special, is_special: np.ndarray,
@@ -121,9 +134,9 @@ class Session:
         out = np.zeros((len(ln), cap), dtype=np.int64)
         out_len = np.zeros(len(ln), dtype=np.int64)
         ids = ffi.SpecialIds(special.sot, special.lang, special.transcribe, special.notimestamps, special.eot)
-        sp = np.ascontiguousarray(is_special, dtype=np.uint8)
+        sp = _special(is_special)
         ffi.check(ffi.lib().wb_transcribe_windows_dev(self._h, C.c_void_p(wave_dev_ptr), ffi.i64ptr(offs), ffi.i64ptr(ln),
-                                                     len(ln), beam_size, max_depth, C.byref(ids), ffi.u8ptr(sp),
+                                                     len(ln), beam_size, max_depth, C.byref(ids), sp,
                                                      ffi.i64ptr(out), cap, ffi.i64ptr(out_len)))
         return [[int(t) for t in out[i, :out_len[i]]] for i in range(len(ln))]
 
@@ -134,9 +147,9 @@ class Session:
         out = np.zeros(cap, dtype=np.int64)
         n = C.c_int64(0)
         ids = ffi.SpecialIds(special.sot, special.lang, special.transcribe, special.notimestamps, special.eot)
-        sp = np.ascontiguousarray(is_special, dtype=np.uint8)
+        sp = _special(is_special)
         ffi.check(ffi.lib().wb_waveform_to_tokens(self._h, ffi.fptr(w), len(w), sample_rate, beam_size, max_depth,
-                                                 C.byref(ids), ffi.u8ptr(sp), ffi.i64ptr(out), cap, C.byref(n)))
+                                                 C.byref(ids), sp, ffi.i64ptr(out), cap, C.byref(n)))
         return [int(t) for t in out[:n.value]]
 
     def waveforms_to_tokens(self, waveforms: Sequence[np.ndarray], special, is_special: np.ndarray, sample_rate: int = 16000,
@@ -149,9 +162,9 @@ class Session:
         ptrs = (C.c_void_p * len(ws))(*[w.ctypes.data for w in ws])
         lens = np.array([len(w) for w in ws], dtype=np.int64)
         ids = ffi.SpecialIds(special.sot, special.lang, special.transcribe, special.notimestamps, special.eot)
-        sp = np.ascontiguousarray(is_special, dtype=np.uint8)
+        sp = _special(is_special)
         ffi.check(ffi.lib().wb_waveforms_to_tokens(self._h, ptrs, ffi.i64ptr(lens), len(ws), sample_rate, beam_size, max_depth,
-                                                  C.byref(ids), ffi.u8ptr(sp), ffi.i64ptr(out), cap, ffi.i64ptr(n)))
+                                                  C.byref(ids), sp, ffi.i64ptr(out), cap, ffi.i64ptr(n)))
         return [[int(t) for t in out[i, :n[i]]] for i in range(len(ws))]
 
     def last_decoder(self) -> int:
