@@ -217,6 +217,19 @@ int wb_waveform_to_tokens(wb_session* s, const float* waveform, int64_t n_sample
 int wb_waveforms_to_tokens(wb_session* s, const float* const* waveforms, const int64_t* n_samples, int64_t n_waveforms,
                            int64_t sample_rate, int beam_size, int max_depth, const wb_special_ids* ids,
                            const uint8_t* is_special, int64_t* tokens_out, int64_t capacity, int64_t* n_tokens_out);
+/* Per-token log-probs of the last wb_transcribe_windows[_dev] (index = window) or wb_waveform(s)_to_tokens (index = waveform)
+ * call on this session, aligned with the ids that call wrote: n_out = that row's id count.  WB_ERR_STATE before the first such
+ * call, WB_ERR_INVALID_ARG for an index out of range or capacity < n_out.  out == NULL only sets n_out.
+ * The values (float32; the reference's BeamSearchToken.log_prob, transcribe.rs:142-146, holds the same f32 widened to f64):
+ *   - the 4 prompt ids: 0.0 (transcribe.rs:205-208);
+ *   - WB_SEARCH_BEAM, beam_size >= 2: the f32 log_softmax value the search scored the id with, special-id mask included
+ *     while sequences have <= 5 tokens (transcribe.rs:291-299).  The left-to-right f64 sum of a row is the cumulative
+ *     log-prob the search chose the row by;
+ *   - WB_SEARCH_BEAM, beam_size 1: the same, the value wb_session_last_topk reports for that position;
+ *   - WB_SEARCH_GREEDY_LOOP: log_softmax of the unmasked logits at the arg-max id; NaN for an EOT a rule appended (EOT test,
+ *     repetition cut, context stop);
+ *   - wb_waveform(s)_to_tokens: each log-prob travels with its id through the overlap merge (transcribe.rs:56-63). */
+int wb_session_last_logprobs(wb_session* s, int64_t index, float* out, int64_t capacity, int64_t* n_out);
 /* transcribe.rs:114-138: number of windows and their [start, end) bounds */
 int64_t wb_window_count(int64_t n_samples, int64_t sample_rate, int64_t window_len);
 int wb_window_bounds(int64_t n_samples, int64_t sample_rate, int64_t window_len, int64_t* starts, int64_t* ends);

@@ -57,6 +57,7 @@ pub mod ffi {
         pub fn wb_find_repeated_tokens_index(tokens: *const i64, n: i64, window_size: i64, min_repeat_count: i64, first_repeat_index: *mut i64, end: *mut i64) -> c_int;
         pub fn wb_waveform_to_tokens(s: *mut c_void, waveform: *const f32, n_samples: i64, sample_rate: i64, beam_size: c_int, max_depth: c_int,
                                      ids: *const wb_special_ids, is_special: *const u8, tokens_out: *mut i64, capacity: i64, n_tokens_out: *mut i64) -> c_int;
+        pub fn wb_session_last_logprobs(s: *mut c_void, index: i64, out: *mut f32, capacity: i64, n_out: *mut i64) -> c_int;
     }
 }
 
@@ -258,6 +259,30 @@ pub mod transcribe {
         })?;
         let tokens: Vec<usize> = out[..n as usize].iter().map(|&t| t as usize).collect();
         Ok((bpe.decode(&tokens[..], true)?, tokens))
+    }
+
+    /// src/transcribe.rs:142-146: a token with the log-prob the search scored it with (0.0 for the prompt, :205-208).
+    #[derive(Clone, Copy, Debug, PartialEq)]
+    pub struct BeamSearchToken { pub token: usize, pub log_prob: f64 }
+
+    /// waveform_to_text's windowing, beam width and depth, returning the merged tokens with the `BeamSearchToken.log_prob`
+    /// each was chosen with (wb_session_last_logprobs: f32 values, which the reference's f64 holds exactly) instead of text.
+    pub fn waveform_to_tokens_with_log_probs(whisper: &model::Whisper, bpe: &Gpt2Tokenizer, lang: Language, waveform: Vec<f32>,
+                                             sample_rate: usize) -> token::Result<Vec<BeamSearchToken>> {
+        let sp = SpecialTokens::from_tokenizer(bpe, lang);
+        let window = audio::max_waveform_samples(whisper.encoder_ctx_size() - 10);            // transcribe.rs:32-34
+        let shift = window.saturating_sub(sample_rate * 3).max(1);                             // transcribe.rs:120-123
+        let n_windows = waveform.len().saturating_sub(1) / shift + 1;
+        let cap = n_windows * (4 + MAX_DEPTH + 1) + 16;
+        let (mut out, mut lps) = (vec![0i64; cap], vec![0f32; cap]);
+        let (mut n, mut n_lp) = (0i64, 0i64);
+        whisper.with_session(n_windows.min(64), BEAM_SIZE, 4 + MAX_DEPTH + 1, |s| {
+            check(unsafe { ffi::wb_waveform_to_tokens(s, waveform.as_ptr(), waveform.len() as i64, sample_rate as i64, BEAM_SIZE as c_int,
+                                                      MAX_DEPTH as c_int, &sp.ids, sp.is_special.as_ptr(), out.as_mut_ptr(), cap as i64, &mut n) })?;
+            check(unsafe { ffi::wb_session_last_logprobs(s, 0, lps.as_mut_ptr(), cap as i64, &mut n_lp) })
+        })?;
+        assert_eq!(n, n_lp, "one log-prob per token");
+        Ok((0..n as usize).map(|i| BeamSearchToken { token: out[i] as usize, log_prob: lps[i] as f64 }).collect())
     }
 
     /// The greedy loop the reference leaves commented out in `mels_to_text` (src/transcribe.rs:314-380), with waveform_to_text's

@@ -29,6 +29,10 @@ struct wb_model {
 struct wb_session {
     std::unique_ptr<wb::Session> impl;
     wb_model* model;
+    // per output row of the last transcribe / waveform(s)_to_tokens call, the log-prob of each id (wb_session_last_logprobs);
+    // empty with have_logprobs == false until a call succeeds
+    std::vector<std::vector<float>> logprobs;
+    bool have_logprobs = false;
 };
 
 namespace {
@@ -424,11 +428,13 @@ int wb_transcribe_windows(wb_session* s, const float* const* waves, const int64_
                           int64_t* tokens_out, int64_t capacity, int64_t* lens_out) {
     return guarded([&] {
         WB_REQUIRE(s && waves && lens && ids && special_given(s, is_special) && tokens_out && lens_out, "transcribe: null pointer");
+        s->have_logprobs = false;
         s->impl->encode_waveforms_host(waves, lens, n_windows);
         std::vector<std::vector<int64_t>> toks;
-        wb::transcribe_windows(*s->impl, beam_size, max_depth, *ids, is_special, toks);
+        wb::transcribe_windows(*s->impl, beam_size, max_depth, *ids, is_special, toks, s->logprobs);
         copy_tokens_out(toks, tokens_out, capacity, lens_out);
         collect_timings(*s->impl);
+        s->have_logprobs = true;
     });
 }
 
@@ -437,11 +443,13 @@ int wb_transcribe_windows_dev(wb_session* s, const float* wave_dev, const int64_
                               const uint8_t* is_special, int64_t* tokens_out, int64_t capacity, int64_t* lens_out) {
     return guarded([&] {
         WB_REQUIRE(s && wave_dev && offsets && lens && ids && special_given(s, is_special) && tokens_out && lens_out, "transcribe: null pointer");
+        s->have_logprobs = false;
         s->impl->encode_from_device_wave(wave_dev, offsets, lens, n_windows);
         std::vector<std::vector<int64_t>> toks;
-        wb::transcribe_windows(*s->impl, beam_size, max_depth, *ids, is_special, toks);
+        wb::transcribe_windows(*s->impl, beam_size, max_depth, *ids, is_special, toks, s->logprobs);
         copy_tokens_out(toks, tokens_out, capacity, lens_out);
         collect_timings(*s->impl);
+        s->have_logprobs = true;
     });
 }
 
@@ -459,10 +467,11 @@ int wb_window_bounds(int64_t n_samples, int64_t sample_rate, int64_t window_len,
 
 // windows of ALL waveforms are decoded together in batches of the session's capacity (they are independent,
 // SURVEY.md F9), then each waveform's windows are merged in order exactly like the reference's sequential
-// loop (transcribe.rs:42-71)
+// loop (transcribe.rs:42-71); each id's log-prob travels with it through the merge into out_lp
 static void waveforms_to_tokens(wb::Session& S, const float* const* waveforms, const int64_t* n_samples, int64_t n_waveforms,
                                 int64_t sample_rate, int beam_size, int max_depth, const wb_special_ids& ids,
-                                const uint8_t* is_special, std::vector<std::vector<int64_t>>& out) {
+                                const uint8_t* is_special, std::vector<std::vector<int64_t>>& out,
+                                std::vector<std::vector<float>>& out_lp) {
     // the frontend tables (mel filterbank, DFT bins) are the 16 kHz ones: the reference builds them from the caller's rate
     // (audio.rs:44, 67-143) but its binary only ever passes 16 kHz (src/bin/transcribe/main.rs:38-41 asserts it)
     WB_REQUIRE(sample_rate == 16000, "waveform_to_tokens: only 16 kHz input is supported (frontend tables are built for 16 kHz)");
@@ -477,20 +486,27 @@ static void waveforms_to_tokens(wb::Session& S, const float* const* waveforms, c
             owner.push_back((int)w);
         }
     out.assign((size_t)n_waveforms, {});
+    out_lp.assign((size_t)n_waveforms, {});
     for (size_t b0 = 0; b0 < ptrs.size(); b0 += (size_t)S.max_windows) {
         const size_t nb = std::min(ptrs.size() - b0, (size_t)S.max_windows);
         S.encode_waveforms_host(ptrs.data() + b0, lens.data() + b0, (int64_t)nb);
         std::vector<std::vector<int64_t>> toks;
-        wb::transcribe_windows(S, beam_size, max_depth, ids, is_special, toks);
+        std::vector<std::vector<float>> lps;
+        wb::transcribe_windows(S, beam_size, max_depth, ids, is_special, toks, lps);
         for (size_t i = 0; i < nb; ++i) {
             std::vector<int64_t>& tokens = out[(size_t)owner[b0 + i]];
+            std::vector<float>& tlp = out_lp[(size_t)owner[b0 + i]];
             const auto& nt = toks[i];
+            const auto& nl = lps[i];
             int64_t pi = 0, ci = 0;
             if (wb::find_chunk_overlap(tokens.data(), (int64_t)tokens.size(), nt.data(), (int64_t)nt.size(), 40, 3, &pi, &ci)) {
                 tokens.resize((size_t)pi);                                    // transcribe.rs:59-60
                 tokens.insert(tokens.end(), nt.begin() + ci, nt.end());
+                tlp.resize((size_t)pi);
+                tlp.insert(tlp.end(), nl.begin() + ci, nl.end());
             } else {
                 tokens.insert(tokens.end(), nt.begin(), nt.end());
+                tlp.insert(tlp.end(), nl.begin(), nl.end());
             }
         }
     }
@@ -502,11 +518,13 @@ int wb_waveform_to_tokens(wb_session* s, const float* waveform, int64_t n_sample
                           int64_t capacity, int64_t* n_tokens_out) {
     return guarded([&] {
         WB_REQUIRE(s && waveform && ids && special_given(s, is_special) && tokens_out && n_tokens_out, "waveform_to_tokens: null pointer");
+        s->have_logprobs = false;
         std::vector<std::vector<int64_t>> out;
-        waveforms_to_tokens(*s->impl, &waveform, &n_samples, 1, sample_rate, beam_size, max_depth, *ids, is_special, out);
+        waveforms_to_tokens(*s->impl, &waveform, &n_samples, 1, sample_rate, beam_size, max_depth, *ids, is_special, out, s->logprobs);
         WB_REQUIRE((int64_t)out[0].size() <= capacity, "tokens_out capacity too small");
         std::memcpy(tokens_out, out[0].data(), out[0].size() * sizeof(int64_t));
         *n_tokens_out = (int64_t)out[0].size();
+        s->have_logprobs = true;
     });
 }
 
@@ -516,13 +534,29 @@ int wb_waveforms_to_tokens(wb_session* s, const float* const* waveforms, const i
     return guarded([&] {
         WB_REQUIRE(s && waveforms && n_samples && ids && special_given(s, is_special) && tokens_out && n_tokens_out, "waveforms_to_tokens: null pointer");
         WB_REQUIRE(n_waveforms >= 1, "waveforms_to_tokens: n_waveforms must be >= 1");
+        s->have_logprobs = false;
         std::vector<std::vector<int64_t>> out;
-        waveforms_to_tokens(*s->impl, waveforms, n_samples, n_waveforms, sample_rate, beam_size, max_depth, *ids, is_special, out);
+        waveforms_to_tokens(*s->impl, waveforms, n_samples, n_waveforms, sample_rate, beam_size, max_depth, *ids, is_special, out,
+                            s->logprobs);
         for (int64_t w = 0; w < n_waveforms; ++w) {
             WB_REQUIRE((int64_t)out[(size_t)w].size() <= capacity, "tokens_out capacity (per waveform) too small");
             std::memcpy(tokens_out + w * capacity, out[(size_t)w].data(), out[(size_t)w].size() * sizeof(int64_t));
             n_tokens_out[w] = (int64_t)out[(size_t)w].size();
         }
+        s->have_logprobs = true;
+    });
+}
+
+int wb_session_last_logprobs(wb_session* s, int64_t index, float* out, int64_t capacity, int64_t* n_out) {
+    return guarded([&] {
+        WB_REQUIRE(s && n_out, "last_logprobs: null pointer");
+        if (!s->have_logprobs) wb::fail(WB_ERR_STATE, "last_logprobs: no transcribe or waveform(s)_to_tokens call yet");
+        WB_REQUIRE(index >= 0 && index < (int64_t)s->logprobs.size(), "last_logprobs: index out of range");
+        const std::vector<float>& v = s->logprobs[(size_t)index];
+        *n_out = (int64_t)v.size();
+        if (!out) return;   // size query
+        WB_REQUIRE(capacity >= (int64_t)v.size(), "last_logprobs: capacity too small");
+        std::memcpy(out, v.data(), v.size() * sizeof(float));
     });
 }
 

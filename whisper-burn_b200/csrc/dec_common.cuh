@@ -958,10 +958,12 @@ __device__ __forceinline__ void fold_records(const DecArgs& a, const float* rec,
 }
 
 // ---- per-row finish: log-probs (v - max) - lse of the candidates, lse from the NP records of the row (DESIGN.md section 2)
-// greedy bookkeeping of row r at position p (beam.rs:9-37 with beam_size 1): the token, the length, EOT
-__device__ __forceinline__ void greedy_commit(const DecArgs& a, int r, int p, int id) {
+// greedy bookkeeping of row r at position p (beam.rs:9-37 with beam_size 1): the token and its rounded log-prob lp, the
+// length, EOT
+__device__ __forceinline__ void greedy_commit(const DecArgs& a, int r, int p, int id, float lp) {
     if (a.greedy && !__ldcg(a.finished + r)) {
         a.tokens[(int64_t)r * a.t_max + p + 1] = id;
+        a.token_lp[(int64_t)r * a.t_max + p + 1] = lp;
         a.lengths[r] = p + 2;
         if (id == a.eot) a.finished[r] = 1;
     }
@@ -969,7 +971,8 @@ __device__ __forceinline__ void greedy_commit(const DecArgs& a, int r, int p, in
 // The greedy loop's rules (DecArgs::loop_rules, host/loop_rules.hpp) for row r after greedy_commit put `id` at p + 1: the EOT
 // test on the raw logits of `id` (`top`) and of EOT, then the repetition cut over tokens[0, p + 2), lane l taking windows
 // i = l (mod 32).  Only for a row that was open before the commit.  The EOT test only finishes the row: the host appends the
-// EOT that follows (Session::greedy_decode).  The cut writes EOT at `end` and finishes the row.  Called by a whole warp.
+// EOT that follows (Session::greedy_decode).  The cut writes EOT at `end`, with a NaN log-prob (no step chose it), and
+// finishes the row.  Called by a whole warp.
 __device__ __forceinline__ void loop_finish(const DecArgs& a, int r, int p, int id, float top) {
     if (id == a.eot) return;   // finished by greedy_commit; the EOT test holds and appends nothing
     const int lane = threadIdx.x & 31;
@@ -986,6 +989,7 @@ __device__ __forceinline__ void loop_finish(const DecArgs& a, int r, int p, int 
     });
     if (end >= 0 && lane == 0) {
         row[end] = a.eot;
+        a.token_lp[(int64_t)r * a.t_max + end] = __int_as_float(0x7fffffff);
         a.lengths[r] = end + 1;
         a.finished[r] = 1;
     }
@@ -1045,8 +1049,9 @@ __device__ __forceinline__ void finish_row_top1(const DecArgs& a, int r, int p, 
     warp_best(bv, bi);
     if (lane == 0) {
         a.topk_id[r] = bi == INT_MAX ? -1 : bi;
-        a.topk_lp[r] = __fsub_rn(__fsub_rn(bv, mx), lse);
-        greedy_commit(a, r, p, bi);
+        const float lp = __fsub_rn(__fsub_rn(bv, mx), lse);
+        a.topk_lp[r] = lp;
+        greedy_commit(a, r, p, bi, lp);
     }
     if (loop_open) loop_finish(a, r, p, bi, bv);   // bv: the raw logit of bi (no mask in loop mode)
 }
@@ -1104,7 +1109,7 @@ __device__ __forceinline__ void finish_row_topk(const DecArgs& a, int r, int p, 
         if (tid == 0) {
             a.topk_id[(int64_t)r * a.k + kk] = bi == INT_MAX ? -1 : bi;
             a.topk_lp[(int64_t)r * a.k + kk] = bv;
-            if (kk == 0) greedy_commit(a, r, p, bi);
+            if (kk == 0) greedy_commit(a, r, p, bi, bv);
         }
         if (kk == 0) id0 = bi;
         prev_v = bv;

@@ -65,6 +65,7 @@ struct DecArgs {
     float *part_o = nullptr, *part_m = nullptr, *part_l = nullptr;   // [R][H][S][64], [R][H][S]
     // tokens / control
     int* tokens = nullptr;                // [Rmax][t_max]
+    float* token_lp = nullptr;            // [Rmax][t_max] log-prob of each committed token (greedy_commit), NaN where a rule put EOT
     const int* cur_tok = nullptr;
     int use_cur_tok = 0;
     int pos0 = 0, n_steps = 1, logits_from = 0;
@@ -95,9 +96,11 @@ struct DecArgs {
     int* slot_live = nullptr;             // [R] the slot holds a live beam at the current position
     beamfx::Head* bm_head = nullptr;      // [2][n_win][MAX_NODES] carried nodes, double-buffered by depth
     int* bm_seq = nullptr;                // [2][n_win][MAX_NODES][t_max] their token sequences
+    float* bm_seq_lp = nullptr;           // [2][n_win][MAX_NODES][t_max] the log-prob each token was scored with (0 for the prompt)
     int* bm_cnt = nullptr;                // [2][n_win] carried nodes per window
     int* bm_win = nullptr;                // [n_win][2] current buffer, done
     int* bm_out = nullptr;                // [n_win][t_max] best sequence of each window when the search ends
+    float* bm_out_lp = nullptr;           // [n_win][t_max] its log-probs
     int* bm_out_len = nullptr;            // [n_win]
 };
 // Each launch_decN launches decoder N when it covers the configuration and reports whether it did.

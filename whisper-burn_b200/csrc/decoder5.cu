@@ -842,7 +842,7 @@ int launch_dec5(const DecArgs& a, const Dec5Tables& t, int n_ctas, bool w_half, 
         g.x += (int64_t)r0 * d; g.q += (int64_t)r0 * d; g.att += (int64_t)r0 * d; g.hid += (int64_t)r0 * 4 * d;
         g.row_window += r0;
         if (g.anc) g.anc += (int64_t)r0 * a.t_max;
-        g.tokens += (int64_t)r0 * a.t_max; g.cur_tok += r0; g.lengths += r0; g.finished += r0;
+        g.tokens += (int64_t)r0 * a.t_max; g.token_lp += (int64_t)r0 * a.t_max; g.cur_tok += r0; g.lengths += r0; g.finished += r0;
         if (g.eot_logit) g.eot_logit += r0;
         g.topk_id += (int64_t)r0 * a.k; g.topk_lp += (int64_t)r0 * a.k;
         if (g.logits_out) { g.logits_out += (int64_t)r0 * a.V; g.lgbuf = g.logits_out; }

@@ -500,10 +500,11 @@ constexpr int BM_LIVE = 24;                                          // rows of 
 constexpr int BM_NX = 3 * BM_LIVE + 3 * NCW * beamfx::MAX_NODES;     // finish_beam's shared scratch (ints)
 //   (a) each live slot's B best candidates by the rounded log-prob (v - max) - lse, ranked by cand_better, from the CTAs'
 //       records -> topk_id / topk_lp [row][B];
-//   (b) one warp per unfinished window: beamfx::beam_step on the carried nodes (lane 0), the new nodes' sequences (the warp);
-//       the next position's live slots w * B + i in carried order, each with its parent's cache row and its token;
+//   (b) one warp per unfinished window: beamfx::beam_step on the carried nodes (lane 0), the new nodes' sequences and the
+//       log-probs their tokens were scored with (bm_seq / bm_seq_lp, the warp); the next position's live slots w * B + i in
+//       carried order, each with its parent's cache row and its token;
 //   (c) the search ends when every window is done (its best carried node is finished) or at max_depth: then the best
-//       sequence of every window goes to bm_out and bar[3] is set; otherwise the next position's slots, tokens and ancestry
+//       sequence of every window goes to bm_out / bm_out_lp and bar[3] is set; otherwise the next position's slots, tokens and ancestry
 //       table (anc_new[r][j] = anc_old[parent[r]][j] for j <= p, anc_new[r][p + 1] = r) are written.
 // Called by the 256 consumer threads; ends with a barrier of the consumers.
 __device__ __noinline__ void finish_beam(const DecArgs& a, int p, int depth, const int* anc_cur, uint8_t* scratch, const int* live, int* nx,
@@ -597,6 +598,7 @@ __device__ __noinline__ void finish_beam(const DecArgs& a, int p, int depth, con
             fx::Pick out[fx::MAX_NODES];
             n_out = fx::beam_step(in, n_in, step_row, cid, clp, B, a.eot, out);
             fx::Head* ho = a.bm_head + ((size_t)nb * NW + w) * fx::MAX_NODES;
+            float* lp_dst = a.bm_seq_lp + ((size_t)nb * NW + w) * fx::MAX_NODES * t_max;
             int nl = 0;
             for (int i = 0; i < n_out; ++i) {
                 ho[i] = out[i].head;
@@ -604,6 +606,7 @@ __device__ __noinline__ void finish_beam(const DecArgs& a, int p, int depth, con
                 pk_src[i] = out[i].src;
                 pk_tok[i] = out[i].token;
                 pk_len[i] = out[i].head.len;
+                if (out[i].token >= 0) lp_dst[i * t_max + out[i].head.len - 1] = (float)out[i].lp;   // exact: a widened f32
                 if (!out[i].head.finished) {
                     const int s = w * B + nl++;
                     nx_par[s] = out[i].head.row;
@@ -620,9 +623,16 @@ __device__ __noinline__ void finish_beam(const DecArgs& a, int p, int depth, con
         __syncwarp();
         const int* src = a.bm_seq + ((size_t)buf * NW + w) * fx::MAX_NODES * t_max;
         int* dst = a.bm_seq + ((size_t)nb * NW + w) * fx::MAX_NODES * t_max;
-        for (int i = 0; i < n_out; ++i) {   // node i = its source's sequence (+ the token it appends)
+        const float* src_lp = a.bm_seq_lp + ((size_t)buf * NW + w) * fx::MAX_NODES * t_max;
+        float* dst_lp = a.bm_seq_lp + ((size_t)nb * NW + w) * fx::MAX_NODES * t_max;
+        for (int i = 0; i < n_out; ++i) {   // node i = its source's sequence (+ the token it appends, its log-prob written above)
             const int s = pk_src[i], tk = pk_tok[i], ln = pk_len[i] - (tk >= 0 ? 1 : 0);
-            for (int j = lane; j < ln; j += 32) dst[i * t_max + j] = __ldcg(src + s * t_max + j);
+            for (int j = lane; j < ln; j += 32) {   // both loads before either store: one L2 round trip per position
+                const int t = __ldcg(src + s * t_max + j);
+                const float l = __ldcg(src_lp + s * t_max + j);
+                dst[i * t_max + j] = t;
+                dst_lp[i * t_max + j] = l;
+            }
             if (lane == 0 && tk >= 0) dst[i * t_max + ln] = tk;
         }
         __syncwarp();
@@ -662,8 +672,13 @@ __device__ __noinline__ void finish_beam(const DecArgs& a, int p, int depth, con
             }
             best = __shfl_sync(0xffffffffu, best, 0);
             len = __shfl_sync(0xffffffffu, len, 0);
-            const int* s = a.bm_seq + (((size_t)buf * NW + w) * fx::MAX_NODES + best) * t_max;
-            for (int j = lane; j < len; j += 32) a.bm_out[(int64_t)w * t_max + j] = __ldcg(s + j);
+            const size_t o = (((size_t)buf * NW + w) * fx::MAX_NODES + best) * t_max;
+            for (int j = lane; j < len; j += 32) {
+                const int t = __ldcg(a.bm_seq + o + j);
+                const float l = __ldcg(a.bm_seq_lp + o + j);
+                a.bm_out[(int64_t)w * t_max + j] = t;
+                a.bm_out_lp[(int64_t)w * t_max + j] = l;
+            }
         }
         if (tid == 0) {
             decode_done(a, p + 1, ctl[3], depth + 1);

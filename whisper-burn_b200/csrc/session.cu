@@ -78,7 +78,7 @@ Session::Session(Model* model, int64_t max_w, int64_t max_b, int64_t max_text_le
     WB_CUDA(cudaMemsetAsync(hid_pl.p, 0, 8 * dec5_plane_uint4(d) * sizeof(uint4), st));
     dq.alloc((size_t)Rmax * d); dhid.alloc((size_t)Rmax * 4 * d);
     logits.alloc((size_t)Rmax * V);
-    tokens.alloc((size_t)Rmax * t_max); lengths.alloc(Rmax); cur_tok.alloc(Rmax); finished.alloc(Rmax);
+    tokens.alloc((size_t)Rmax * t_max); token_lp.alloc((size_t)Rmax * t_max); lengths.alloc(Rmax); cur_tok.alloc(Rmax); finished.alloc(Rmax);
     row_window.alloc(Rmax); anc0.alloc((size_t)Rmax * t_max); anc1.alloc((size_t)Rmax * t_max); parent.alloc(Rmax);
     pos.alloc(1); n_unfinished.alloc(128);
     topk_id.alloc((size_t)Rmax * kmax); topk_lp.alloc((size_t)Rmax * kmax);
@@ -433,7 +433,7 @@ bool Session::launch_decoder(int R_, int pos0, int n_steps, int logits_from, boo
     a.anc = anc_identity ? nullptr : (anc_cur == 0 ? anc0.p : anc1.p);
     a.n_splits = std::max(1, std::min(16, n_sm / std::max(1, R_ * H)));
     a.part_o = part_o.p; a.part_m = part_m.p; a.part_l = part_l.p;
-    a.tokens = tokens.p; a.cur_tok = cur_tok.p; a.use_cur_tok = use_cur_tok ? 1 : 0;
+    a.tokens = tokens.p; a.token_lp = token_lp.p; a.cur_tok = cur_tok.p; a.use_cur_tok = use_cur_tok ? 1 : 0;
     a.pos0 = pos0; a.n_steps = n_steps; a.logits_from = logits_from;
     a.is_special = have_special ? is_special.p : nullptr; a.mask_mode = mask_mode;
     a.k = k; a.greedy = greedy ? 1 : 0; a.eot = eot; a.lengths = lengths.p; a.finished = finished.p;
@@ -456,6 +456,7 @@ bool Session::launch_decoder(int R_, int pos0, int n_steps, int logits_from, boo
         a.beam = beam; a.n_win = R_ / beam; a.max_depth = max_depth;
         a.anc = anc0.p; a.anc_alt = anc1.p; a.slot_live = slot_live.p;
         a.bm_head = bm_head.p; a.bm_seq = bm_seq.p; a.bm_cnt = bm_cnt.p; a.bm_win = bm_win.p; a.bm_out = bm_out.p; a.bm_out_len = bm_out_len.p;
+        a.bm_seq_lp = bm_seq_lp.p; a.bm_out_lp = bm_out_lp.p;
         if (!allowed(6) || !launch_dec6(a, *m, d6, st)) return false;
         last_decoder = 6;
     } else if (allowed(4) && launch_dec4(a, h16, st)) last_decoder = 4;
@@ -563,7 +564,7 @@ void Session::last_topk(int64_t n_rows, int64_t k, int64_t* ids_out, float* lp_o
 }
 
 void Session::greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_depth, int64_t eot,
-                            std::vector<std::vector<int64_t>>& out, bool loop_rules) {
+                            std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp, bool loop_rules) {
     WB_REQUIRE(prompt_len + max_depth <= t_max, "greedy: prompt + max_depth exceeds the session's max_text_len");
     // one launch: prompt prefill + every greedy step, early exit inside the kernel.  The beam rule masks the special ids while
     // a sequence has at most 5 tokens (mask_mode 2); the greedy loop masks nothing, and its context stop, at
@@ -572,8 +573,10 @@ void Session::greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_d
     const int n_steps = (int)prompt_len - 1 + max_depth;
     if (max_depth > 0) launch_decoder(R, 0, n_steps, (int)prompt_len - 1, false, loop_rules ? 0 : 2, 1, true, (int)eot, 0, 0, loop_rules);
     std::vector<int> tk((size_t)R * t_max), len((size_t)R);
+    std::vector<float> lp((size_t)R * t_max);
     int sdv[128] = {0};
     WB_CUDA(cudaMemcpyAsync(tk.data(), tokens.p, tk.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+    WB_CUDA(cudaMemcpyAsync(lp.data(), token_lp.p, lp.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
     WB_CUDA(cudaMemcpyAsync(len.data(), lengths.p, len.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
     if (max_depth > 0) WB_CUDA(cudaMemcpyAsync(sdv, steps_done.p, sizeof(int) * std::min(last_groups, 128), cudaMemcpyDeviceToHost, st));
     WB_CUDA(cudaStreamSynchronize(st));
@@ -582,16 +585,25 @@ void Session::greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_d
     last_steps = max_depth > 0 ? sd - ((int)prompt_len - 1) : 0;
     host_pos = (int)prompt_len - 1 + (int)last_steps;
     out.assign((size_t)R, {});
+    out_lp.assign((size_t)R, {});
     for (int r = 0; r < R; ++r) {
-        for (int i = 0; i < len[(size_t)r]; ++i) out[(size_t)r].push_back(tk[(size_t)r * t_max + i]);
+        for (int i = 0; i < len[(size_t)r]; ++i) {
+            out[(size_t)r].push_back(tk[(size_t)r * t_max + i]);
+            out_lp[(size_t)r].push_back(i < prompt_len ? 0.0f : lp[(size_t)r * t_max + i]);   // transcribe.rs:205-208
+        }
+        // a repetition cut that ends inside the prompt (the loop masks nothing) leaves its EOT in a prompt position
+        if (loop_rules && max_depth > 0 && len[(size_t)r] <= prompt_len) out_lp[(size_t)r].back() = std::nanf("");
         // the greedy loop always ends in EOT: the EOT test's EOT and the context stop's are appended here (the latter may
-        // not fit the token buffer)
-        if (loop_rules && out[(size_t)r].back() != eot) out[(size_t)r].push_back(eot);
+        // not fit the token buffer); no step chose them, so their log-prob is NaN
+        if (loop_rules && out[(size_t)r].back() != eot) {
+            out[(size_t)r].push_back(eot);
+            out_lp[(size_t)r].push_back(std::nanf(""));
+        }
     }
 }
 
 bool Session::beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_size, int max_depth, int64_t eot,
-                          std::vector<std::vector<int64_t>>& out) {
+                          std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp) {
     namespace fx = beamfx;
     if (!encoded) fail(WB_ERR_STATE, "session: decode before encode");
     WB_REQUIRE(prompt_len >= 1 && prompt_len + max_depth <= t_max, "beam: prompt + max_depth exceeds the session's max_text_len");
@@ -600,9 +612,9 @@ bool Session::beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_si
     for (int64_t i = 0; i < prompt_len; ++i) WB_REQUIRE(prompt[i] >= 0 && prompt[i] < V, "beam: prompt token out of range");
     constexpr int MN = fx::MAX_NODES;
     slot_live.ensure((size_t)Rmax);
-    bm_head.ensure((size_t)2 * W * MN); bm_seq.ensure((size_t)2 * W * MN * t_max);
+    bm_head.ensure((size_t)2 * W * MN); bm_seq.ensure((size_t)2 * W * MN * t_max); bm_seq_lp.ensure((size_t)2 * W * MN * t_max);
     bm_cnt.ensure((size_t)2 * W); bm_win.ensure((size_t)2 * W);
-    bm_out.ensure((size_t)W * t_max); bm_out_len.ensure((size_t)W);
+    bm_out.ensure((size_t)W * t_max); bm_out_lp.ensure((size_t)W * t_max); bm_out_len.ensure((size_t)W);
     // slot i of window w = row w * B + i; until the first search step only slot 0 holds a beam: the prompt, in its own cache row
     std::vector<int> tk((size_t)Rb * t_max, 0), rw((size_t)Rb), live((size_t)Rb);
     for (int r = 0; r < Rb; ++r) {
@@ -622,14 +634,17 @@ bool Session::beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_si
     WB_CUDA(cudaMemcpyAsync(slot_live.p, live.data(), live.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     WB_CUDA(cudaMemcpyAsync(bm_head.p, heads.data(), heads.size() * sizeof(fx::Head), cudaMemcpyHostToDevice, st));
     WB_CUDA(cudaMemcpyAsync(bm_seq.p, seq.data(), seq.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    WB_CUDA(cudaMemsetAsync(bm_seq_lp.p, 0, seq.size() * sizeof(float), st));   // the prompt's log-probs (transcribe.rs:205-208)
     WB_CUDA(cudaMemcpyAsync(bm_cnt.p, cnt.data(), cnt.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     WB_CUDA(cudaMemcpyAsync(bm_win.p, win.data(), win.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     launch_dec_anc_identity(anc0.p, Rb, t_max, st);
     const bool ran = launch_decoder(Rb, 0, (int)prompt_len - 1 + max_depth, (int)prompt_len - 1, false, 2, B, false, (int)eot, B, max_depth);
     std::vector<int> res((size_t)W * t_max), res_len((size_t)W);
+    std::vector<float> res_lp((size_t)W * t_max);
     int sd = 0;
     if (ran) {
         WB_CUDA(cudaMemcpyAsync(res.data(), bm_out.p, res.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+        WB_CUDA(cudaMemcpyAsync(res_lp.data(), bm_out_lp.p, res_lp.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
         WB_CUDA(cudaMemcpyAsync(res_len.data(), bm_out_len.p, res_len.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
         WB_CUDA(cudaMemcpyAsync(&sd, steps_done.p, sizeof(int), cudaMemcpyDeviceToHost, st));
     }
@@ -642,8 +657,12 @@ bool Session::beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_si
     anc_identity = false;
     anc_cur = (sd - 1) & 1;
     out.assign((size_t)W, {});
+    out_lp.assign((size_t)W, {});
     for (int w = 0; w < W; ++w)
-        for (int i = 0; i < res_len[(size_t)w]; ++i) out[(size_t)w].push_back(res[(size_t)w * t_max + i]);
+        for (int i = 0; i < res_len[(size_t)w]; ++i) {
+            out[(size_t)w].push_back(res[(size_t)w * t_max + i]);
+            out_lp[(size_t)w].push_back(res_lp[(size_t)w * t_max + i]);
+        }
     return true;
 }
 

@@ -67,6 +67,7 @@ struct Session {
     DevBuf<float> part_o, part_m, part_l;
     DevBuf<int> tokens, lengths, cur_tok, finished, row_window, anc0, anc1, parent, pos, n_unfinished, topk_id;
     DevBuf<float> topk_lp;
+    DevBuf<float> token_lp;    // [Rmax][t_max] log-prob of each token the greedy decoders commit (DecArgs::token_lp)
     DevBuf<float> eot_logit;   // [Rmax] raw EOT logit of each row at the current position (greedy loop)
     DevBuf<uint8_t> is_special;
     bool have_special = false;
@@ -97,6 +98,7 @@ struct Session {
                    int eot, int beam = 0, int max_depth = 0, bool loop_rules = false);
     // device beam search state (decoder6.cu beam mode), allocated on first use
     DevBuf<int> slot_live, bm_seq, bm_cnt, bm_win, bm_out, bm_out_len;
+    DevBuf<float> bm_seq_lp, bm_out_lp;
     DevBuf<beamfx::Head> bm_head;
     bool full_logits = false;    // also write raw logits [R][V] (stateless forward_decoder)
     int n_logit_ctas = 0;
@@ -128,19 +130,21 @@ struct Session {
                     int apply_mask, int k, int64_t* topk_ids_out, float* topk_lp_out);
     // the [n_rows][k] candidates the last launch wrote at its last position
     void last_topk(int64_t n_rows, int64_t k, int64_t* ids_out, float* lp_out);
-    // greedy search on the device in one launch; returns per-window token lists.  loop_rules: the reference's greedy loop
-    // (WB_SEARCH_GREEDY_LOOP) instead of beam_size 1
+    // greedy search on the device in one launch; returns per-window token lists and the log-prob of each token (0 for the
+    // prompt, NaN for an EOT a rule appended).  loop_rules: the reference's greedy loop (WB_SEARCH_GREEDY_LOOP) instead of
+    // beam_size 1
     void greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_depth, int64_t eot,
-                       std::vector<std::vector<int64_t>>& out, bool loop_rules = false);
+                       std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp, bool loop_rules = false);
     // the whole beam search (prefill + up to max_depth steps) of every encoded window in ONE decoder launch; false (nothing
     // decoded) when no decoder covers it, and the caller runs the host search
     bool beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_size, int max_depth, int64_t eot,
-                     std::vector<std::vector<int64_t>>& out);
+                     std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp);
 };
 
-// host pipeline (transcribe.cu)
+// host pipeline (transcribe.cu): per window the ids and the log-prob each was chosen with (BeamSearchToken.log_prob)
 void transcribe_windows(Session& s, int beam_size, int max_depth, const wb_special_ids& ids,
-                        const uint8_t* is_special, std::vector<std::vector<int64_t>>& out);
+                        const uint8_t* is_special, std::vector<std::vector<int64_t>>& out,
+                        std::vector<std::vector<float>>& out_lp);
 std::vector<std::pair<int64_t, int64_t>> window_bounds(int64_t n_samples, int64_t sample_rate, int64_t window_len);
 bool find_chunk_overlap(const int64_t* prev, int64_t n_prev, const int64_t* curr, int64_t n_curr, int64_t max_n_offsets,
                         int64_t min_n_overlaps, int64_t* prev_index, int64_t* curr_index);

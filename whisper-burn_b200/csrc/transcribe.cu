@@ -64,7 +64,7 @@ using Node = beam::BeamNode<BeamSearchToken>;
 }  // namespace
 
 void transcribe_windows(Session& s, int beam_size, int max_depth, const wb_special_ids& ids, const uint8_t* is_special,
-                        std::vector<std::vector<int64_t>>& out) {
+                        std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp) {
     const bool loop = s.search == WB_SEARCH_GREEDY_LOOP;
     WB_REQUIRE(!loop || beam_size == 1, "transcribe: the greedy loop takes beam_size 1");
     WB_REQUIRE(beam_size >= 1 && beam_size <= s.max_beams, "transcribe: beam_size exceeds the session's max_beams");
@@ -77,13 +77,13 @@ void transcribe_windows(Session& s, int beam_size, int max_depth, const wb_speci
     s.set_special(is_special);
     const int W = s.n_windows;
     if (beam_size == 1) {   // greedy: beam_size 1 of the search, or the greedy loop (transcribe.rs:314-380)
-        s.greedy_decode(prompt, 4, max_depth, ids.eot, out, loop);
+        s.greedy_decode(prompt, 4, max_depth, ids.eot, out, out_lp, loop);
         WB_CUDA(cudaEventRecord(s.ev[3], s.st));
         return;
     }
     // ---- beam search: on the device in one launch where decoder6 covers it (fp16-exact weights, d = 128 / 384,
     // n_windows * beam_size <= 24, t_max <= 128), same selection rules and ids as the host search below
-    if (max_depth > 0 && s.beam_decode(prompt, 4, beam_size, max_depth, ids.eot, out)) {
+    if (max_depth > 0 && s.beam_decode(prompt, 4, beam_size, max_depth, ids.eot, out, out_lp)) {
         WB_CUDA(cudaEventRecord(s.ev[3], s.st));
         return;
     }
@@ -161,10 +161,14 @@ void transcribe_windows(Session& s, int beam_size, int max_depth, const wb_speci
     }
     s.last_steps = steps;
     out.assign((size_t)W, {});
+    out_lp.assign((size_t)W, {});
     for (int w = 0; w < W; ++w) {
         const int best = beam::max_by_last(beams[(size_t)w]);
         if (best >= 0)
-            for (const auto& t : beams[(size_t)w][(size_t)best].seq) out[(size_t)w].push_back(t.token);
+            for (const auto& t : beams[(size_t)w][(size_t)best].seq) {
+                out[(size_t)w].push_back(t.token);
+                out_lp[(size_t)w].push_back((float)t.log_prob);   // exact: a widened f32 (transcribe.rs:291-299)
+            }
     }
     WB_CUDA(cudaEventRecord(s.ev[3], s.st));
 }

@@ -36,6 +36,7 @@ struct Pick {          // one node of the next carried list
     Head head;
     int src;           // the input node it extends (token >= 0) or carries unchanged (token < 0)
     int token;
+    double lp;         // the appended token's own log-prob (the candidate's cand_lp); 0 when token < 0
 };
 
 // get_top_elements (beam.rs:81-110) over scores s[0..n), num <= MAX_BEAM: writes the kept indices in output order to top
@@ -80,7 +81,7 @@ WB_HD inline bool search_done(const Head* h, int n) {
 WB_HD inline int beam_step(const Head* in, int n_in, const int* step_row, const int* cand_id, const double* cand_lp, int beam_size,
                            int eot, Pick* out) {
     double ns[MAX_CONT], fs[MAX_NODES];
-    int nsrc[MAX_CONT], ntok[MAX_CONT], fsrc[MAX_NODES];
+    int nsrc[MAX_CONT], nslot[MAX_CONT], fsrc[MAX_NODES];   // a continuation: its node, its candidate slot, its score
     int n_new = 0, n_fin = 0;
     for (int b = 0; b < n_in; ++b) {
         if (in[b].finished) {
@@ -88,26 +89,23 @@ WB_HD inline int beam_step(const Head* in, int n_in, const int* step_row, const 
             fs[n_fin++] = in[b].log_prob;
             continue;
         }
-        // this beam's continuations in ascending token id (insertion sort of <= 7)
-        int id[MAX_BEAM];
-        double lp[MAX_BEAM];
+        // this beam's continuations in ascending token id (insertion sort of its <= 7 candidate slots)
+        int slot[MAX_BEAM];
         int nc = 0;
         for (int i = 0; i < beam_size; ++i) {
-            const int t = cand_id[b * beam_size + i];
+            const int s = b * beam_size + i, t = cand_id[s];
             if (t < 0) continue;
-            const double l = cand_lp[b * beam_size + i];
             int k = nc++;
-            for (; k > 0 && id[k - 1] > t; --k) { id[k] = id[k - 1]; lp[k] = lp[k - 1]; }
-            id[k] = t;
-            lp[k] = l;
+            for (; k > 0 && cand_id[slot[k - 1]] > t; --k) slot[k] = slot[k - 1];
+            slot[k] = s;
         }
         double sc[MAX_BEAM];
-        for (int i = 0; i < nc; ++i) sc[i] = in[b].log_prob + lp[i];   // transcribe.rs:291-299
+        for (int i = 0; i < nc; ++i) sc[i] = in[b].log_prob + cand_lp[slot[i]];   // transcribe.rs:291-299
         int top[MAX_BEAM + 1];
         const int nt = top_elements(sc, nc, beam_size, top);
         for (int i = 0; i < nt; ++i) {
             nsrc[n_new] = b;
-            ntok[n_new] = id[top[i]];
+            nslot[n_new] = slot[top[i]];
             ns[n_new++] = sc[top[i]];
         }
     }
@@ -118,9 +116,10 @@ WB_HD inline int beam_step(const Head* in, int n_in, const int* step_row, const 
         const int c = top[i], b = nsrc[c];
         Pick& o = out[n_out++];
         o.src = b;
-        o.token = ntok[c];
+        o.token = cand_id[nslot[c]];
+        o.lp = cand_lp[nslot[c]];
         o.head.log_prob = ns[c];
-        o.head.finished = ntok[c] == eot ? 1 : 0;
+        o.head.finished = o.token == eot ? 1 : 0;
         o.head.row = step_row[b];
         o.head.len = in[b].len + 1;
         o.head.pad = 0;
@@ -131,6 +130,7 @@ WB_HD inline int beam_step(const Head* in, int n_in, const int* step_row, const 
         Pick& o = out[n_out++];
         o.src = b;
         o.token = -1;
+        o.lp = 0.0;
         o.head = in[b];
     }
     return n_out;

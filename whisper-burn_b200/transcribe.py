@@ -167,6 +167,16 @@ class Session:
                                                   C.byref(ids), sp, ffi.i64ptr(out), cap, ffi.i64ptr(n)))
         return [[int(t) for t in out[i, :n[i]]] for i in range(len(ws))]
 
+    def last_logprobs(self, index: int) -> np.ndarray:
+        """float32 log-prob of each id of row `index` (window or waveform) of the last transcribe_windows[_dev] /
+        waveform(s)_to_tokens call: 0 for the prompt, the log-prob the search chose the id with, NaN for an EOT the greedy
+        loop's rules appended (wb_session_last_logprobs)."""
+        n = C.c_int64(0)
+        ffi.check(ffi.lib().wb_session_last_logprobs(self._h, index, None, 0, C.byref(n)))
+        out = np.empty(n.value, dtype=np.float32)
+        ffi.check(ffi.lib().wb_session_last_logprobs(self._h, index, ffi.fptr(out), n.value, C.byref(n)))
+        return out
+
     def last_decoder(self) -> int:
         return int(ffi.lib().wb_session_last_decoder(self._h))
 
