@@ -11,6 +11,7 @@
 #include "../host/loop_rules.hpp"
 #include "decoder.h"
 #include "wb_internal.h"
+#include "prims.cuh"
 
 namespace wb {
 
@@ -19,10 +20,6 @@ namespace {
 constexpr int NT = 256;
 constexpr int NW = 8;
 
-__device__ __forceinline__ float gelu_erf(float x) {
-    const float t = __fadd_rn(erff(__fdiv_rn(x, 1.41421356237309504880f)), 1.0f);
-    return __fdiv_rn(__fmul_rn(x, t), 2.0f);
-}
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -68,19 +65,6 @@ __device__ __forceinline__ unsigned int ldg_l2(const uint8_t* p, uint64_t pol) {
     unsigned int v;
     asm("ld.global.nc.L2::cache_hint.u8 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
     return v;
-}
-// 16-byte cp.async (L2 only) with an L2 policy; completion with cp.async.wait_all / wait_group like the plain form
-__device__ __forceinline__ void cp_async16_l2(void* dst, const void* src, uint64_t pol) {
-    asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src),
-                 "l"(pol)
-                 : "memory");
-}
-// 1-D bulk copy global -> shared (TMA engine) with an L2 policy, completion counted on an mbarrier of this CTA
-__device__ __forceinline__ void bulk_g2s_l2(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t pol) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
-                     (uint32_t)__cvta_generic_to_shared(dst)),
-                 "l"(src), "r"(bytes), "r"((uint32_t)__cvta_generic_to_shared(bar)), "l"(pol)
-                 : "memory");
 }
 // Back to normal priority: the 128-byte lines of [p, p + bytes) that are resident, line i handled by thread (i - first) % nthreads
 // == tid of the calling grid (p need not be aligned: applypriority addresses the line that contains the address)
@@ -515,8 +499,8 @@ __device__ __forceinline__ void attn_warp_ring(const float* q_smem, int n_keys, 
             const uint4* vp = reinterpret_cast<const uint4*>(vptr(j)) + blk * NV;
 #pragma unroll
             for (int c = 0; c < NV; ++c) {
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(dst + c * 32)), "l"(kp + c) : "memory");
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(dst + (NV + c) * 32)), "l"(vp + c) : "memory");
+                cp_async16(dst + c * 32, kp + c);
+                cp_async16(dst + (NV + c) * 32, vp + c);
             }
         }
         asm volatile("cp.async.commit_group;" ::: "memory");   // always: keeps the group count uniform
@@ -564,23 +548,9 @@ __device__ __forceinline__ void attn_warp_ring(const float* q_smem, int n_keys, 
             for (int c = 0; c < 16; ++c) A.o[c] = fmaf(e, vf[c], A.o[c] * corr);
         }
     }
-    asm volatile("cp.async.wait_all;" ::: "memory");
+    cp_async_wait_all();
     __syncwarp();
-#pragma unroll
-    for (int off = 4; off < 32; off <<= 1) {   // merge the 8 key sub-groups
-        const float m2 = __shfl_xor_sync(0xffffffffu, A.m, off);
-        const float l2 = __shfl_xor_sync(0xffffffffu, A.l, off);
-        const float mn = fmaxf(A.m, m2);
-        const float c1 = A.m > -INFINITY ? expf(A.m - mn) : 0.0f;
-        const float c2 = m2 > -INFINITY ? expf(m2 - mn) : 0.0f;
-        A.l = A.l * c1 + l2 * c2;
-#pragma unroll
-        for (int c = 0; c < 16; ++c) {
-            const float o2 = __shfl_xor_sync(0xffffffffu, A.o[c], off);
-            A.o[c] = A.o[c] * c1 + o2 * c2;
-        }
-        A.m = mn;
-    }
+    attn_merge_subs(A);
 }
 
 // Bulk-copy variant for the head-major cross K/V layout (encoder.cu ckv_relayout_kernel): the unit's keys are ONE contiguous
@@ -603,34 +573,30 @@ struct AttnBulkGeom {
     static constexpr int STGB = 4096;                    // bytes per batch / ring stage
     static constexpr int KPB = STGB / ROWB;              // keys per batch: 8 (fp32) or 16 (fp16)
 };
+// Batch bb of the unit's keys, the cnt-th batch through this warp's ring: its bytes expected on the stage's mbarrier and one bulk
+// copy into the stage.  L2H: the copy carries the L2 policy l2pol (l2_policy_*).  Called by one lane.
+template <int NSTG, typename KT, bool L2H>
+__device__ __forceinline__ void attn_bulk_issue(const KT* base, int n_keys, int bb, unsigned int cnt, unsigned char* ring, uint64_t* mbar,
+                                                uint64_t l2pol) {
+    constexpr int ROWB = AttnBulkGeom<KT>::ROWB, STGB = AttnBulkGeom<KT>::STGB, KPB = AttnBulkGeom<KT>::KPB;
+    const int slot = (int)(cnt % NSTG);
+    const uint32_t bytes = (uint32_t)min(KPB, n_keys - bb * KPB) * ROWB;
+    mbar_expect_tx(mbar + slot, bytes);
+    if constexpr (L2H) bulk_g2s_l2(ring + slot * STGB, base + (int64_t)bb * KPB * 128, bytes, mbar + slot, l2pol);
+    else bulk_g2s(ring + slot * STGB, base + (int64_t)bb * KPB * 128, bytes, mbar + slot);
+}
 // The first NSTG-1 batches of attn_warp_bulk, issued ahead of time (the K/V rows are static: nothing to wait for); the
 // matching attn_warp_bulk call passes prefilled = true and the SAME base / n_keys / wslot / nwarps / ring_count.
-// L2H: the bulk copies carry the L2 policy l2pol (l2_policy_*).
 template <int NSTG, typename KT, bool L2H = false>
 __device__ __forceinline__ void attn_bulk_prefill(const KT* base, int n_keys, int wslot, int nwarps, unsigned char* ring, uint64_t* mbar,
                                                   unsigned int ring_count, uint64_t l2pol = 0) {
-    constexpr int ROWB = AttnBulkGeom<KT>::ROWB, STGB = AttnBulkGeom<KT>::STGB, KPB = AttnBulkGeom<KT>::KPB;
+    constexpr int KPB = AttnBulkGeom<KT>::KPB;
     if ((threadIdx.x & 31) != 0) return;
     const int n_batches = (n_keys + KPB - 1) / KPB;
     const int n_it = n_batches > wslot ? (n_batches - wslot + nwarps - 1) / nwarps : 0;
 #pragma unroll
-    for (int it = 0; it < NSTG - 1; ++it) {
-        if (it < n_it) {
-            const int bb = wslot + it * nwarps;
-            const int slot = (int)((ring_count + (unsigned int)it) % NSTG);
-            const uint32_t bytes = (uint32_t)min(KPB, n_keys - bb * KPB) * ROWB;
-            const uint32_t mb = (uint32_t)__cvta_generic_to_shared(mbar + slot);
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mb), "r"(bytes) : "memory");
-            if constexpr (L2H) {
-                bulk_g2s_l2(ring + slot * STGB, base + (int64_t)bb * KPB * 128, bytes, mbar + slot, l2pol);
-            } else {
-                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                                 (uint32_t)__cvta_generic_to_shared(ring + slot * STGB)),
-                             "l"(base + (int64_t)bb * KPB * 128), "r"(bytes), "r"(mb)
-                             : "memory");
-            }
-        }
-    }
+    for (int it = 0; it < NSTG - 1; ++it)
+        if (it < n_it) attn_bulk_issue<NSTG, KT, L2H>(base, n_keys, wslot + it * nwarps, ring_count + (unsigned int)it, ring, mbar, l2pol);
 }
 template <int NSTG, typename KT, bool L2H = false>
 __device__ __forceinline__ void attn_warp_bulk(const float* q_smem, const KT* base, int n_keys, int wslot, int nwarps, int swz,
@@ -649,22 +615,7 @@ __device__ __forceinline__ void attn_warp_bulk(const float* q_smem, const KT* ba
     const int n_batches = (n_keys + KPB - 1) / KPB;
     const int n_it = n_batches > wslot ? (n_batches - wslot + nwarps - 1) / nwarps : 0;
     auto issue = [&](int it) {
-        if (it < n_it && lane == 0) {
-            const int bb = wslot + it * nwarps;
-            const unsigned int cnt = ring_count + (unsigned int)it;
-            const int slot = (int)(cnt % NSTG);
-            const uint32_t bytes = (uint32_t)min(KPB, n_keys - bb * KPB) * ROWB;
-            const uint32_t mb = (uint32_t)__cvta_generic_to_shared(mbar + slot);
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mb), "r"(bytes) : "memory");
-            if constexpr (L2H) {
-                bulk_g2s_l2(ring + slot * STGB, base + (int64_t)bb * KPB * 128, bytes, mbar + slot, l2pol);
-            } else {
-                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                                 (uint32_t)__cvta_generic_to_shared(ring + slot * STGB)),
-                             "l"(base + (int64_t)bb * KPB * 128), "r"(bytes), "r"(mb)
-                             : "memory");
-            }
-        }
+        if (it < n_it && lane == 0) attn_bulk_issue<NSTG, KT, L2H>(base, n_keys, wslot + it * nwarps, ring_count + (unsigned int)it, ring, mbar, l2pol);
     };
     auto load16 = [&](const unsigned char* p16, int par, float (&f)[16]) {   // this lane's 16 dims of one K or V row
 #pragma unroll
@@ -692,13 +643,7 @@ __device__ __forceinline__ void attn_warp_bulk(const float* q_smem, const KT* ba
         issue(it + NSTG - 1);
         const unsigned int cnt = ring_count + (unsigned int)it;
         const int slot = (int)(cnt % NSTG);
-        {
-            const uint32_t mb = (uint32_t)__cvta_generic_to_shared(mbar + slot), parity = (cnt / NSTG) & 1;
-            uint32_t done = 0;
-            while (!done) {
-                asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}" : "=r"(done) : "r"(mb), "r"(parity) : "memory");
-            }
-        }
+        mbar_wait(mbar + slot, (cnt / NSTG) & 1);
         const int bb = wslot + it * nwarps;
         const int j0 = bb * KPB + sub;
         if (j0 < n_keys) {
@@ -767,21 +712,7 @@ __device__ __forceinline__ void attn_warp_bulk(const float* q_smem, const KT* ba
     }
     ring_count += (unsigned int)n_it;
     __syncwarp();
-#pragma unroll
-    for (int off = 4; off < 32; off <<= 1) {   // merge the 8 key sub-groups (same l4 = same dims)
-        const float m2 = __shfl_xor_sync(0xffffffffu, A.m, off);
-        const float l2 = __shfl_xor_sync(0xffffffffu, A.l, off);
-        const float mn = fmaxf(A.m, m2);
-        const float c1 = A.m > -INFINITY ? expf(A.m - mn) : 0.0f;
-        const float c2 = m2 > -INFINITY ? expf(m2 - mn) : 0.0f;
-        A.l = A.l * c1 + l2 * c2;
-#pragma unroll
-        for (int c = 0; c < 16; ++c) {
-            const float o2 = __shfl_xor_sync(0xffffffffu, A.o[c], off);
-            A.o[c] = A.o[c] * c1 + o2 * c2;
-        }
-        A.m = mn;
-    }
+    attn_merge_subs(A);   // same l4 = same dims
 }
 
 // block-level merge of the 8 warps' partial attention results; out[64] / ML valid after the trailing __syncthreads()
@@ -822,24 +753,7 @@ __device__ __forceinline__ void attn_cta(const float* q_smem, int n_keys, KF&& k
     attn_cta_tail(A, wm, wl, wo, out, ML);
 }
 
-// ---- tensor-core helpers (mma.sync m16n8k16, fp16 hi/lo split of fp32 activations; see decoder5.cu) -------------
-__device__ __forceinline__ void mma16816(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
-
-// 4 consecutive fp32 values -> fp16 hi and fp16 (residual * 2048); x == hi + lo / 2048 up to 2^-23 |x|
-__device__ __forceinline__ void split4(const float4 v, uint2& hi, uint2& lo) {
-    const __half2 h01 = __floats2half2_rn(v.x, v.y), h23 = __floats2half2_rn(v.z, v.w);
-    const float2 f01 = __half22float2(h01), f23 = __half22float2(h23);
-    const __half2 l01 = __floats2half2_rn((v.x - f01.x) * 2048.0f, (v.y - f01.y) * 2048.0f);
-    const __half2 l23 = __floats2half2_rn((v.z - f23.x) * 2048.0f, (v.w - f23.y) * 2048.0f);
-    hi = make_uint2(h2_bits(h01), h2_bits(h23));
-    lo = make_uint2(h2_bits(l01), h2_bits(l23));
-}
-
+// ---- activation planes of the mma.sync products (fp16 hi/lo split of prims.cuh; see decoder5.cu) -------------
 // Fragment-order planes: element (row, col) of an activation matrix [rows][K] lives in the uint4
 //   ((row / 8) * (K / 32) + col / 32) * 32 + (row % 8) * 4 + (col % 32) / 8,   half (col % 8)
 // i.e. lane (g = row % 8, t) of the MMA finds the 8 halves x[row][chunk*32 + t*8 .. +8) in ONE 16-byte word.
@@ -848,7 +762,7 @@ __device__ __forceinline__ int plane_idx(int nchunks, int row, int col) {
 }
 __device__ __forceinline__ void store_frag(uint4* xhi, uint4* xlo, int nchunks, int row, int col, const float4 v) {
     uint2 hi, lo;
-    split4(v, hi, lo);
+    hl_split4(v, hi, lo);
     const int idx = plane_idx(nchunks, row, col), half = (col & 7) >> 2;
     reinterpret_cast<uint2*>(xhi + idx)[half] = hi;
     reinterpret_cast<uint2*>(xlo + idx)[half] = lo;

@@ -74,32 +74,6 @@ constexpr int KV_STG = 4;                  // cross attention: stages (8 keys ea
 #endif
 __device__ __forceinline__ uint64_t ckv_policy() { return D4_L2_CKV_KEEP ? l2_policy_evict_last() : l2_policy_evict_first(); }
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "LG_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra LG_DONE;\n"
-        "bra LG_WAIT;\n"
-        "LG_DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
-// 16-byte asynchronous copy global -> shared (L2 only), lane-private destination: completion with cp_async_wait_all()
-__device__ __forceinline__ void cp_async16(void* dst, const void* src) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
-
 __device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
 __device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 
@@ -195,11 +169,6 @@ __device__ __forceinline__ void dot_rows1(const RowRegs<NR, VPL>& r, const float
     }
 }
 
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-    return r;
-}
 // 16 bytes -> shared memory of another CTA of the cluster, completing 16 transaction bytes on that CTA's mbarrier
 __device__ __forceinline__ void st_async_v4(uint32_t raddr, const float4& v, uint32_t rbar) {
     asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v4.f32 [%0], {%1, %2, %3, %4}, [%5];" ::"r"(raddr), "f"(v.x),
@@ -232,10 +201,7 @@ __device__ __forceinline__ void xwait(uint64_t* bar, uint32_t bytes, uint32_t pa
     uint32_t done = 0;
     int spins = 0;
     while (!done) {
-        asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
-                     : "=r"(done)
-                     : "r"(mb), "r"(parity)
-                     : "memory");
+        done = mbar_try_wait(mb, parity);
         if (!done && ++spins > (1 << 24)) __trap();   // a lost message must not hang the GPU
     }
 }
@@ -352,7 +318,7 @@ dec4_kernel(const DecArgs a) {
         for (int j = 0; j < LG_NBUF; ++j) mbar_init(lg_bar + warp * LG_NBUF + j, 1);
         if (warp == 0)
             for (int j = 0; j < 8; ++j) mbar_init(xbar + j, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_fence_init();
     }
     cl.sync();                   // every CTA's stage barriers exist before the first remote store can target them
     unsigned int lc = 0;         // layers this CTA has run: phase parity of the stage barriers (each is used once per layer)
@@ -634,7 +600,7 @@ dec4_kernel(const DecArgs a) {
                                                       kv_bar + warp * KV_STG, kv_count, A, true, ckv_policy());
                     if (l == L - 1 && want_logits) {   // the ring is free until the next position: first vocabulary half-tiles of this warp
                         __syncwarp();
-                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads of the ring before the bulk copies
+                        fence_proxy_async();   // generic reads of the ring before the bulk copies
 #pragma unroll
                         for (int j = 0; j < LG_NBUF; ++j) issue(j);
                     }
@@ -809,7 +775,7 @@ dec4_kernel(const DecArgs a) {
                         const int n = n0 + g + (c >> 1) * 8, e = c & 1;
                         if constexpr (RC == 4) al[c] = __shfl_xor_sync(0xffffffffu, ah[c], 2);   // lo product of rows 2t, 2t+1: columns 2t+4, 2t+5 = lane t + 2
                         if (n < V && 2 * t + e < R) {   // RC == 4: R <= 4, i.e. lanes t < 2
-                            const float raw = fmaf(al[c], 1.0f / 2048.0f, ah[c]);
+                            const float raw = hl_join(ah[c], al[c]);
                             const float v = (use_mask && ((sp01 >> ((c >> 1) * 8)) & 0xffu)) ? __fadd_rn(raw, -INFINITY) : raw;
                             if (v > -INFINITY) softmax_add(m_run[e], s_run[e], v);
                             if (cand_better(v, n, bv[e], bi[e])) { bv[e] = v; bi[e] = n; }

@@ -58,15 +58,11 @@ enum { EM_QKV = D5_EM_QKV, EM_RESID = D5_EM_RESID, EM_CQ = D5_EM_CQ, EM_HID = D5
 
 using GemmDesc = Dec5Desc;   // host-built stage descriptors (decoder.h): no switch in the kernel, so the compiler cannot clone the stage body per case
 
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 __device__ __forceinline__ void bar_named(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 __device__ __forceinline__ void store_plane_elem(uint4* phi, uint4* plo, int nchunks, int row, int col, float v) {
-    const __half h = __float2half_rn(v);
-    const __half l = __float2half_rn((v - __half2float(h)) * 2048.0f);
+    __half h, l;
+    hl_split(v, h, l);
     const int idx = plane_idx(nchunks, row, col);
     reinterpret_cast<__half*>(phi + idx)[col & 7] = h;
     reinterpret_cast<__half*>(plo + idx)[col & 7] = l;
@@ -122,8 +118,8 @@ dec5_kernel(const DecArgs a) {
     uint64_t* kv_bar = reinterpret_cast<uint64_t*>(ds + L * 16 + 16);   // [NW][KV_STG] cross-attention K/V ring: one mbarrier per stage
     constexpr int KV_STG = RING_W / AttnBulkGeom<KVT>::STGB;               // 4 stages of 4 KB: 8 fp32 keys or 16 fp16 keys each
     if (lane == 0) {
-        for (int j = 0; j < KV_STG; ++j) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"((uint32_t)__cvta_generic_to_shared(kv_bar + warp * KV_STG + j)));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        for (int j = 0; j < KV_STG; ++j) mbar_init(kv_bar + warp * KV_STG + j, 1);
+        mbar_fence_init();
     }
     unsigned int kv_count = 0;   // batches this warp has pushed through its K/V ring
     __syncthreads();
@@ -248,7 +244,7 @@ dec5_kernel(const DecArgs a) {
                     // ================= attention: self (causal over the row's ancestry) / cross (split over keys).
                     // Two (row, head[, split]) units per CTA at a time, 4 warps each (named barriers).
                     const bool is_cross = slot == SL_CROSS;
-                    if (is_cross) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the ring aliases the planes written through the generic proxy
+                    if (is_cross) fence_proxy_async();   // the ring aliases the planes written through the generic proxy
                     const int U = is_cross ? R * H * S : R * H;
                     const int grp = warp >> 2, wg = warp & 3, gt = tid & 127;
                     const KVT* ckvl = reinterpret_cast<const KVT*>(a.ckv) + (size_t)l * a.Mcap * 2 * d;
@@ -436,10 +432,10 @@ dec5_kernel(const DecArgs a) {
 #pragma unroll
                                 for (int j = 0; j < NT8; ++j) {
                                     const int r0 = j * 8 + 2 * t;
-                                    my[r0 * RED_LD + g] = fmaf(al[j][0], 1.0f / 2048.0f, ah[j][0]);
-                                    my[(r0 + 1) * RED_LD + g] = fmaf(al[j][1], 1.0f / 2048.0f, ah[j][1]);
-                                    my[r0 * RED_LD + g + 8] = fmaf(al[j][2], 1.0f / 2048.0f, ah[j][2]);
-                                    my[(r0 + 1) * RED_LD + g + 8] = fmaf(al[j][3], 1.0f / 2048.0f, ah[j][3]);
+                                    my[r0 * RED_LD + g] = hl_join(ah[j][0], al[j][0]);
+                                    my[(r0 + 1) * RED_LD + g] = hl_join(ah[j][1], al[j][1]);
+                                    my[r0 * RED_LD + g + 8] = hl_join(ah[j][2], al[j][2]);
+                                    my[(r0 + 1) * RED_LD + g + 8] = hl_join(ah[j][3], al[j][3]);
                                 }
                             }
                             __syncthreads();
@@ -526,7 +522,7 @@ dec5_kernel(const DecArgs a) {
 #pragma unroll
                                         for (int c = 0; c < 4; ++c) {
                                             const int n = n0 + g + (c >> 1) * 8, r = r0 + (c & 1);
-                                            if (n < V && r < R) a.lgbuf[(int64_t)r * V + n] = fmaf(al[j][c], 1.0f / 2048.0f, ah[j][c]);
+                                            if (n < V && r < R) a.lgbuf[(int64_t)r * V + n] = hl_join(ah[j][c], al[j][c]);
                                         }
                                     }
                                 }

@@ -21,7 +21,7 @@
 //   this CTA are pre-packed per (layer, CTA) as 128-row x 64-column slabs in the canonical K-major 128B-swizzled shared-memory
 //   image (dec6_pack_kernel), so a slab is ONE 16 KB bulk copy (TMA engine) into a ring slot and IS the A operand of two
 //   m64 MMAs; the activation is the B operand: 8 rows of which row 0 = fp16(x) and row 1 = fp16((x - hi) * 2048) (the
-//   decoder5.cu split: exact products, fp32 accumulation), the rest zero.  The two consumer warpgroups take the 128-row output
+//   hi/lo split of prims.cuh: exact products, fp32 accumulation), the rest zero.  The two consumer warpgroups take the 128-row output
 //   tiles in turn (ping-pong: one group's epilogue overlaps the other's MMAs); the accumulator lives in the registers of the
 //   group, columns 0 and 1 of a row in one thread, which combines hi + lo / 2048 after a shuffle that gives every lane one row
 //   and applies bias / scale / GELU.  Weights do not depend on activations, so they never wait for the chain: a PRODUCER warp
@@ -77,33 +77,12 @@ struct Geo {
 };
 
 // ---- small PTX helpers -------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t s32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s32(bar)), "r"(count)); }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(s32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s32(bar)) : "memory"); }
 __device__ long long g_watchdog = 20000000000LL;   // SM clocks a wait may last before the kernel traps (fail loudly instead of hanging the GPU); host-settable
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    const long long WATCHDOG = g_watchdog;
-    const uint32_t b = s32(bar);
-    const long long t0 = clock64();
-    for (;;) {
-        uint32_t done;
-        asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}" : "=r"(done) : "r"(b), "r"(parity) : "memory");
-        if (done) return;
-        if (clock64() - t0 > WATCHDOG) __trap();
-    }
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(s32(dst)), "l"(src), "r"(bytes), "r"(s32(bar)) : "memory");
-}
 // local shared memory -> the same offset in CTA `rank` of the cluster, completion on that CTA's mbarrier
 __device__ __forceinline__ void bulk_s2peer(void* dst_local, const void* src, uint32_t bytes, uint64_t* bar_local, uint32_t rank) {
-    uint32_t rd, rb;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rd) : "r"(s32(dst_local)), "r"(rank));
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rb) : "r"(s32(bar_local)), "r"(rank));
-    asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(rd), "r"(s32(src)), "r"(bytes), "r"(rb) : "memory");
+    const uint32_t rd = mapa_u32(smem_u32(dst_local), rank);
+    const uint32_t rb = mapa_u32(smem_u32(bar_local), rank);
+    asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(rd), "r"(smem_u32(src)), "r"(bytes), "r"(rb) : "memory");
 }
 __device__ __forceinline__ void bar_consumers() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 __device__ __forceinline__ void bar_all() { asm volatile("bar.sync 2, %0;" ::"n"(NTH6) : "memory"); }
@@ -215,9 +194,10 @@ __global__ void dec6_param_kernel(const ParamSeg* segs, int n_segs, float* dst) 
 
 // the B operand of the next linear layer: value v of column k -> fp16 hi in row 0, fp16 (residual * 2048) in row 1
 __device__ __forceinline__ void bx_store(uint8_t* bx, int k, float v) {
-    const __half h = __float2half_rn(v);
+    __half h, l;
+    hl_split(v, h, l);
     *reinterpret_cast<__half*>(bx + sw128_off(0, k, BX_SLAB)) = h;
-    *reinterpret_cast<__half*>(bx + sw128_off(1, k, BX_SLAB)) = __float2half_rn((v - __half2float(h)) * 2048.0f);
+    *reinterpret_cast<__half*>(bx + sw128_off(1, k, BX_SLAB)) = l;
 }
 
 struct Pipe {        // shared-memory handles of the ring / tensor-core pipeline
@@ -246,10 +226,10 @@ struct GemvOut {
 template <typename KVT>
 __device__ __noinline__ Counters gemv_epi6(const Pipe P, Counters c, int N, int n_slabs, const GemvOut<KVT> o) {
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes of the B operand -> tensor-core (async proxy) reads
+    fence_proxy_async();   // generic writes of the B operand -> tensor-core (async proxy) reads
     bar_consumers();
     const int n_tiles = (N + 127) >> 7;
-    const uint32_t ring0 = s32(P.ring), bx0 = s32(P.bx);
+    const uint32_t ring0 = smem_u32(P.ring), bx0 = smem_u32(P.bx);
 #pragma unroll 1
     for (int t = 0; t < n_tiles; ++t) {
         const uint32_t T = c.tile + (uint32_t)t, g = T & 1;
@@ -262,7 +242,7 @@ __device__ __noinline__ Counters gemv_epi6(const Pipe P, Counters c, int N, int 
 #pragma unroll 1
         for (int s = 0; s < n_slabs; ++s, ++n) {
             const uint32_t slot = n % NSLOT;
-            mbar_wait(P.full + slot, (n / NSLOT) & 1);
+            mbar_wait_bounded(P.full + slot, (n / NSLOT) & 1, g_watchdog);
             // rows 64..127 of a slab start 8 swizzle atoms (8192 bytes) in; K step = 32 bytes -> +2 in the (>> 4) address field.
             // A 64-row slab leaves the second half of its slot stale: that MMA runs anyway (no branch between the MMAs, which
             // would serialise them) and its rows are discarded.
@@ -293,7 +273,7 @@ __device__ __noinline__ Counters gemv_epi6(const Pipe P, Counters c, int N, int 
         const float lo = sel == 0 ? lv[0] : sel == 1 ? lv[1] : sel == 2 ? lv[2] : lv[3];
         const int row = t * 128 + 64 * (lane >> 4) + 16 * (warp & 3) + 8 * ((lane >> 3) & 1) + (lane & 7);
         if (row < N && (!half_tile || lane < 16)) {
-            const float s = fmaf(lo, 1.0f / 2048.0f, hi);
+            const float s = hl_join(hi, lo);
             if (o.mode == EM_PLAIN) {
                 o.out[row] = s;
             } else if (o.mode == EM_QKV) {       // mod.rs:429-431; q and k carry (d/H)^-0.25 each (:500-503)
@@ -370,7 +350,7 @@ __device__ __noinline__ void combine6(const float* pr, uint64_t* bar, uint32_t p
     constexpr int CS = Geo<D>::CS, SEND = Geo<D>::SEND;
     const int tid = threadIdx.x;
     if (tid == 0) mbar_expect_tx(bar, CS * SEND * 4);
-    mbar_wait(bar, parity);
+    mbar_wait_bounded(bar, parity, g_watchdog);
     if (tid < CS) {
         const float* me = pr + tid * SEND + D;
         wsrc_s[tid] = mode == MODE_SUM ? 1.0f : me[0] > -INFINITY ? __fdiv_rn(1.0f, me[1]) : 0.0f;
@@ -459,7 +439,7 @@ __device__ __noinline__ uint32_t cross_attn6(const Pipe P, uint32_t n, int* slot
     for (int k0 = 0; k0 < T; k0 += KPC) {
         const int nk = min(KPC, T - k0);
         const uint32_t slot = n % NSLOT;
-        mbar_wait(P.full + slot, (n / NSLOT) & 1);
+        mbar_wait_bounded(P.full + slot, (n / NSLOT) & 1, g_watchdog);
         const uint8_t* blk = P.ring + slot * SLOT;
 #pragma unroll 2
         for (int kk = warp * 4 + rg; kk < nk; kk += 32) {
@@ -747,7 +727,7 @@ dec6_kernel(const DecArgs a) {
         for (int i = 0; i < 2; ++i) { mbar_init(pfull + i, 1); mbar_init(pfree + i, NCW); mbar_init(pbar + i, 1); }
         for (int i = 0; i < NCW * LG_NBUF; ++i) mbar_init(lg_bar + i, 1);
         ctl[0] = 0; ctl[1] = 0;
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_fence_init();
     }
     for (int i = tid; i < (G::KMAX / 64) * BX_SLAB / 16; i += NTH6) reinterpret_cast<uint4*>(bx)[i] = make_uint4(0, 0, 0, 0);   // rows 2..7 stay zero
     // beam mode: step 0's live slots (set by the host: slot 0 of every window) into buffer 0
@@ -780,7 +760,7 @@ dec6_kernel(const DecArgs a) {
         auto push = [&](const void* src, uint32_t bytes) {
             if (n % NPROD == pw) {
                 const uint32_t slot = n % NSLOT;
-                if (n >= NSLOT) mbar_wait(empty + slot, ((n / NSLOT) - 1) & 1);
+                if (n >= NSLOT) mbar_wait_bounded(empty + slot, ((n / NSLOT) - 1) & 1, g_watchdog);
                 mbar_expect_tx(full + slot, bytes);
                 bulk_g2s(ring_mem + slot * SLOT, src, bytes, full + slot);
             }
@@ -796,7 +776,7 @@ dec6_kernel(const DecArgs a) {
                     for (int l = 0; l < L; ++l) {
                         if (pw == 0) {
                             const uint32_t b = pl & 1, u = pl >> 1;
-                            if (u >= 1) mbar_wait(pfree + b, (u - 1) & 1);
+                            if (u >= 1) mbar_wait_bounded(pfree + b, (u - 1) & 1, g_watchdog);
                             mbar_expect_tx(pfull + b, PARAMS * 4);
                             bulk_g2s(params + b * PARAMS, gparams + ((size_t)l * CS + rank) * PARAMS, PARAMS * 4, pfull + b);
                         }
@@ -843,7 +823,7 @@ dec6_kernel(const DecArgs a) {
         };
         // sends y_s[ph & 1] (D values + max, sum, active) to every CTA of the cluster
         auto send = [&]() {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            fence_proxy_async();
             bar_consumers();
             if (tid < CS) {   // one issuing thread per destination
                 const uint32_t b = ph & 1;
@@ -885,7 +865,7 @@ dec6_kernel(const DecArgs a) {
                         if (lane == 0) mbar_arrive(pfree + ((pl + 1) & 1));               // previous layer's parameters are dead now
                     }
                     trace();   // [t1] records of the previous phase combined
-                    mbar_wait(pfull + (pl & 1), (pl >> 1) & 1);
+                    mbar_wait_bounded(pfull + (pl & 1), (pl >> 1) & 1, g_watchdog);
                     const float* prm = params + (pl & 1) * PARAMS;
                     ++pl;
                     float* ys = y_s + (ph & 1) * SEND;
@@ -973,7 +953,7 @@ dec6_kernel(const DecArgs a) {
                     }
                 };
                 if (idle_cta) {
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                    fence_proxy_async();
 #pragma unroll
                     for (int j = 0; j < LG_NBUF; ++j) issue(j);
                 }
@@ -1058,7 +1038,7 @@ dec6_kernel(const DecArgs a) {
                         __syncwarp();
                     }
                     if (!idle_cta) {
-                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the ring was last written by bulk copies and read through the generic proxy
+                        fence_proxy_async();   // the ring was last written by bulk copies and read through the generic proxy
 #pragma unroll
                         for (int j = 0; j < LG_NBUF; ++j) issue(j);
                     }
@@ -1067,7 +1047,7 @@ dec6_kernel(const DecArgs a) {
                     for (int it = 0; it < total; ++it) {
                         const unsigned int cnt = lg_count + (unsigned int)it;
                         const int slot = (int)(cnt % LG_NBUF);
-                        mbar_wait(wbar + slot, (cnt / LG_NBUF) & 1);
+                        mbar_wait_bounded(wbar + slot, (cnt / LG_NBUF) & 1, g_watchdog);
                         const uint8_t* blk = wring + (size_t)slot * BLKB;
                         const int half = it & 1;
                         if (half == 0) {
@@ -1103,7 +1083,7 @@ dec6_kernel(const DecArgs a) {
                                     const int n = n0 + g + (c >> 1) * 8, e = c & 1, rr = j * 8 + 2 * t + e;
                                     cv[j][c] = __int_as_float(0x7fffffff);   // NaN: never inserted
                                     if (n < V && rr < R && ((live_m >> rr) & 1u)) {
-                                        const float raw = fmaf(al[j][c], 1.0f / 2048.0f, ah[j][c]);
+                                        const float raw = hl_join(ah[j][c], al[j][c]);
                                         const float v = (use_mask && a.is_special[n]) ? __fadd_rn(raw, -INFINITY) : raw;
                                         if (v > -INFINITY) softmax_add(m_run[j][e], s_run[j][e], v);
                                         cv[j][c] = v;
@@ -1131,7 +1111,7 @@ dec6_kernel(const DecArgs a) {
                                 for (int c = 0; c < 4; ++c) {
                                     const int n = n0 + g + (c >> 1) * 8, e = c & 1;
                                     if (n < V && j * 8 + 2 * t + e < R) {
-                                        const float raw = fmaf(al[j][c], 1.0f / 2048.0f, ah[j][c]);
+                                        const float raw = hl_join(ah[j][c], al[j][c]);
                                         const float v = (use_mask && a.is_special[n]) ? __fadd_rn(raw, -INFINITY) : raw;
                                         if (v > -INFINITY) softmax_add(m_run[j][e], s_run[j][e], v);
                                         if (cand_better(v, n, bv[j][e], bi[j][e])) { bv[j][e] = v; bi[j][e] = n; }
@@ -1212,7 +1192,7 @@ dec6_kernel(const DecArgs a) {
                 if (!stop) snapshot_live((step + 1) & 1);   // the next position's live slots (the finisher placed them)
             }
             if (tid == 0) ctl[0] = stop;
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic accesses to the aliased buffers before the next step's bulk copies
+            fence_proxy_async();   // generic accesses to the aliased buffers before the next step's bulk copies
             bar_all();   // hands the ring back to the producer; it reads the stop flag after this barrier
             if (stop) break;
             if (!BEAM && step + 1 == a.n_steps && blockIdx.x == 0 && tid == 0) decode_done(a, a.pos0 + a.n_steps, rows_open(a), a.n_steps);

@@ -2,8 +2,8 @@
 //
 // Flash-attention structure (one CTA = 64 queries of one (window, head), 4 warps x 16 query rows, key/value tiles of 64
 // positions streamed through a double-buffered cp.async ring), but at fp32-class accuracy: the reference computes in f32 and the
-// parity bar is 2e-5 of scale, so every operand is a PAIR of fp16 planes  x = hi + lo / 2048  (hi = fp16(x),
-// lo = fp16((x - hi) * 2048): 22 mantissa bits, the decoder5.cu split) and every product is three mma.sync.m16n8k16 terms
+// parity bar is 2e-5 of scale, so every operand is a PAIR of fp16 planes  x = hi + lo / 2048  (the hi/lo split of prims.cuh)
+// and every product is three mma.sync.m16n8k16 terms
 //     Q.K^T = Qh.Kh + (Qh.Kl + Ql.Kh) / 2048          P.V = Ph.Vh + (Ph.Vl + Pl.Vh) / 2048
 // (the dropped lo.lo term is 2^-22 relative) with fp32 accumulation in two accumulators (main / correction) and the softmax in
 // fp32 exactly as burn's activation::softmax composes it (exp(x - max) / sum, online over the key tiles).
@@ -11,6 +11,7 @@
 // the output leaves as the fp16 planes [rows][d] the out-projection GEMM consumes.
 #include <cuda_fp16.h>
 
+#include "prims.cuh"
 #include "wb_internal.h"
 
 namespace wb {
@@ -22,7 +23,6 @@ constexpr int AT_THREADS = 128;
 constexpr int TILE_B = 64 * 128;                       // one [64][64] fp16 tile = 8 KB (rows of 128 bytes)
 constexpr size_t AT_SMEM = 2 * TILE_B + 2 * 4 * TILE_B;   // Q hi/lo + 2 stages x (K hi, K lo, V hi, V lo) = 80 KB
 
-__device__ __forceinline__ uint32_t s_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void cp16(uint32_t dst, const void* src, bool ok) {
     const int sz = ok ? 16 : 0;   // zero-fill out-of-range rows
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(sz) : "memory");
@@ -35,20 +35,13 @@ __device__ __forceinline__ void ldsm4(uint32_t addr, uint32_t& a, uint32_t& b, u
 __device__ __forceinline__ void ldsm4t(uint32_t addr, uint32_t& a, uint32_t& b, uint32_t& c, uint32_t& d) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d) : "r"(addr));
 }
-__device__ __forceinline__ void mma(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint32_t pack2(__half a, __half b) {
-    const __half2 h = __halves2half2(a, b);
-    return *reinterpret_cast<const uint32_t*>(&h);
-}
-// two fp32 values -> fp16 hi pair and fp16 (residual * 2048) pair
+__device__ __forceinline__ void mma(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) { mma16816(c, a[0], a[1], a[2], a[3], b0, b1); }
+// two fp32 values -> fp16 hi pair and fp16 lo pair, as the A / B fragment registers of an MMA
 __device__ __forceinline__ void split2(float x, float y, uint32_t& hi, uint32_t& lo) {
-    const __half hx = __float2half_rn(x), hy = __float2half_rn(y);
-    hi = pack2(hx, hy);
-    lo = pack2(__float2half_rn((x - __half2float(hx)) * 2048.0f), __float2half_rn((y - __half2float(hy)) * 2048.0f));
+    __half2 h, l;
+    hl_split_pair(x, y, h, l);
+    hi = h2_bits(h);
+    lo = h2_bits(l);
 }
 
 __global__ void __launch_bounds__(AT_THREADS)
@@ -63,7 +56,7 @@ enc_attn_tc_kernel(const __half* __restrict__ qkv_hi, const __half* __restrict__
     const int64_t ld = 3 * (int64_t)d;
     const __half* bh = qkv_hi + win.row_off * ld + h * HD;
     const __half* bl = qkv_lo + win.row_off * ld + h * HD;
-    const uint32_t sQ = s_addr(sm), sKV = sQ + 2 * TILE_B;
+    const uint32_t sQ = smem_u32(sm), sKV = sQ + 2 * TILE_B;
 
     // ---- Q tile (hi, lo) and the first K/V tiles
     auto load_tile = [&](uint32_t dst, const __half* src, int row0) {   // [64][64] halves from rows row0.. of a [.][3d] plane
@@ -137,7 +130,7 @@ enc_attn_tc_kernel(const __half* __restrict__ qkv_hi, const __half* __restrict__
         for (int i = 0; i < 8; ++i)
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-                float v = fmaf(s_c[i][j], 1.0f / 2048.0f, s_m[i][j]);
+                float v = hl_join(s_m[i][j], s_c[i][j]);
                 if (k0 + i * 8 + 2 * t + (j & 1) >= T) v = -INFINITY;
                 s_m[i][j] = v;
                 mx[j >> 1] = fmaxf(mx[j >> 1], v);
@@ -206,8 +199,8 @@ enc_attn_tc_kernel(const __half* __restrict__ qkv_hi, const __half* __restrict__
         __half* ol = out_lo + (win.row_off + q) * (int64_t)d + h * HD;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-            const float a = __fdiv_rn(fmaf(o_c[i][2 * e], 1.0f / 2048.0f, o_m[i][2 * e]), inv);
-            const float b = __fdiv_rn(fmaf(o_c[i][2 * e + 1], 1.0f / 2048.0f, o_m[i][2 * e + 1]), inv);
+            const float a = __fdiv_rn(hl_join(o_m[i][2 * e], o_c[i][2 * e]), inv);
+            const float b = __fdiv_rn(hl_join(o_m[i][2 * e + 1], o_c[i][2 * e + 1]), inv);
             uint32_t hi, lo;
             split2(a, b, hi, lo);
             *reinterpret_cast<uint32_t*>(oh + i * 8 + 2 * t) = hi;

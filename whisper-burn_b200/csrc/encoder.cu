@@ -1,6 +1,7 @@
 // Encoder-side kernels other than the GEMMs: LayerNorm and non-causal multi-head attention
 // (reference: burn nn::LayerNorm used at src/model/mod.rs:300-301,259; qkv_attention mod.rs:493-533).
 #include <cuda_fp16.h>
+#include "prims.cuh"
 #include "wb_internal.h"
 
 namespace wb {
@@ -51,7 +52,7 @@ layernorm_kernel(const float* __restrict__ x, float* __restrict__ y, const float
     }
 }
 
-// Same LayerNorm, output as fp16 hi / lo planes (x = hi + lo / 2048, gemm_f16.cu) for the tensor-core GEMM that consumes the row;
+// Same LayerNorm, output as fp16 hi / lo planes (x = hi + lo / 2048, prims.cuh) for the tensor-core GEMM that consumes the row;
 // y (fp32 rows) is written as well when non-null (ln_post: the encoder output returned through the ABI).
 __global__ void __launch_bounds__(256)
 layernorm_f16_kernel(const float* __restrict__ x, float* __restrict__ y, __half* __restrict__ y_hi, __half* __restrict__ y_lo,
@@ -89,9 +90,7 @@ layernorm_f16_kernel(const float* __restrict__ x, float* __restrict__ y, __half*
         if (c < d) {
             const float o = __fadd_rn(__fmul_rn(__fdiv_rn(v[i], den), g[c]), b[c]);
             if (y) y[(int64_t)row * d + c] = o;
-            const __half h = __float2half_rn(o);
-            y_hi[(int64_t)row * d + c] = h;
-            y_lo[(int64_t)row * d + c] = __float2half_rn((o - __half2float(h)) * 2048.0f);
+            hl_split(o, y_hi[(int64_t)row * d + c], y_lo[(int64_t)row * d + c]);
         }
     }
 }

@@ -9,6 +9,7 @@
 // transposed in shared memory (k-major) so the inner loop reads two float4 of A and one of B per
 // 32 FMAs.  fp32 CUDA-core FMA keeps the reference's f32 numerics exactly (up to summation order);
 // the tensor-core path (gemm_f16.cu, wgmma over fp16 hi/lo planes) replaces this kernel for the large GEMMs.
+#include "prims.cuh"
 #include "wb_internal.h"
 
 namespace wb {
@@ -19,12 +20,6 @@ constexpr int BM = 128, BN = 64, BK = 16;
 constexpr int GEMM_THREADS = 256;
 constexpr int AS_STRIDE = BM + 4;
 constexpr int BS_STRIDE = BN + 4;
-
-__device__ __forceinline__ float gelu_erf(float x) {
-    // burn activation::gelu (erf form): x * (erf(x / sqrt2) + 1) / 2, evaluated in that order
-    const float t = __fadd_rn(erff(__fdiv_rn(x, 1.41421356237309504880f)), 1.0f);
-    return __fdiv_rn(__fmul_rn(x, t), 2.0f);
-}
 
 struct GemmArgs {
     const float* A;

@@ -3,12 +3,10 @@
 //
 //   C[g][m][n] = epi( sum_k A[g][m][k] * B[n][k] )      same contract and epilogues as gemm.cu
 //
-// Precision: the reference computes in f32 and the parity bar is identical greedy tokens (encoder output within 2e-5 of scale),
-// so a single fp16 / bf16 pass is not acceptable.  Every weight of a released Whisper checkpoint is fp16-representable (they
-// are stored in fp16), so B is EXACT in fp16; the fp32 activations travel between the encoder kernels as a PAIR of fp16 planes
-//     A = A_hi + A_lo / 2048,   A_hi = fp16(A),  A_lo = fp16((A - A_hi) * 2048)        (22 mantissa bits, decoder5.cu's split)
-// written by the producing kernel (LayerNorm, attention, the GELU epilogue below).  Every product A_hi*B, A_lo*B is exact in the
-// fp32 accumulator; the two planes accumulate into TWO register accumulators that the epilogue combines as hi + lo / 2048.
+// Precision: the parity bar is identical greedy tokens (encoder output within 2e-5 of scale), so a single fp16 / bf16 pass is
+// not acceptable.  B (the weights) is exact in fp16; the fp32 activations travel between the encoder kernels as a PAIR of fp16
+// planes A = A_hi + A_lo / 2048 (the hi/lo split of prims.cuh), written by the producing kernel (LayerNorm, attention, the GELU
+// epilogue below).  The two planes accumulate into TWO register accumulators that the epilogue combines as hi + lo / 2048.
 // Against a TF32 hi/lo formulation: half the bytes per k-block through shared memory, the weight tile loaded once instead of
 // twice, and twice the MMA rate.
 //
@@ -28,6 +26,7 @@
 #include <cstring>
 #include <mutex>
 
+#include "prims.cuh"
 #include "wb_internal.h"
 #include "wgmma.cuh"
 
@@ -40,17 +39,6 @@ constexpr int F_BM = 128, F_BK = 64, F_STAGES = 4;   // 4 stages x 48 KB (BN = 1
 constexpr int F_CONSUMERS = 256;                     // two warpgroups
 constexpr int F_THREADS = F_CONSUMERS + 32;          // + the TMA producer warp
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count)); }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory"); }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t done = 0;
-    while (!done)
-        asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}" : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-}
 __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(smem_u32(dst)), "l"(map),
                  "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
@@ -65,15 +53,6 @@ template <int BN>
 __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t desc_a, uint64_t desc_b) {
     if constexpr (BN == 128) wgmma_m64n128k16(d, desc_a, desc_b);
     else wgmma_m64n64k16(d, desc_a, desc_b);
-}
-__device__ __forceinline__ float gelu_erf(float x) {
-    const float t = __fadd_rn(erff(__fdiv_rn(x, 1.41421356237309504880f)), 1.0f);
-    return __fdiv_rn(__fmul_rn(x, t), 2.0f);
-}
-__device__ __forceinline__ void split_pair(float x, float y, __half2& hi, __half2& lo) {
-    hi = __floats2half2_rn(x, y);
-    const float2 f = __half22float2(hi);
-    lo = __floats2half2_rn((x - f.x) * 2048.0f, (y - f.y) * 2048.0f);
 }
 
 struct F16Args {
@@ -118,7 +97,7 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_co
             mbar_init(full + s, 1);
             mbar_init(empty + s, 2);   // one arrival per consumer warpgroup
         }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_fence_init();
     }
     __syncthreads();
 
@@ -179,7 +158,7 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_co
             float v[2];
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-                float t = fmaf(acc_l[4 * j + 2 * hrow + e], 1.0f / 2048.0f, acc_h[4 * j + 2 * hrow + e]);
+                float t = hl_join(acc_h[4 * j + 2 * hrow + e], acc_l[4 * j + 2 * hrow + e]);
                 if (g.bias) t = __fadd_rn(t, __ldg(g.bias + n + e));
                 if (g.act == ACT_GELU) t = gelu_erf(t);
                 if (n + e < g.scale_cols) t = __fmul_rn(t, g.scale);
@@ -196,7 +175,7 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_co
             if (g.C) *reinterpret_cast<float2*>(g.C + crow + n) = make_float2(v[0], v[1]);
             if (g.P_hi) {
                 __half2 h, l;
-                split_pair(v[0], v[1], h, l);
+                hl_split_pair(v[0], v[1], h, l);
                 *reinterpret_cast<__half2*>(g.P_hi + crow + n) = h;
                 *reinterpret_cast<__half2*>(g.P_lo + crow + n) = l;
             }
@@ -206,17 +185,8 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_co
 
 // fp32 -> (hi, lo) fp16 planes
 __global__ void split_f16_kernel(const float4* __restrict__ src, uint2* __restrict__ hi, uint2* __restrict__ lo, int64_t n4) {
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
-        const float4 v = src[i];
-        __half2 h0, l0, h1, l1;
-        split_pair(v.x, v.y, h0, l0);
-        split_pair(v.z, v.w, h1, l1);
-        uint2 uh, ul;
-        uh.x = *reinterpret_cast<uint32_t*>(&h0); uh.y = *reinterpret_cast<uint32_t*>(&h1);
-        ul.x = *reinterpret_cast<uint32_t*>(&l0); ul.y = *reinterpret_cast<uint32_t*>(&l1);
-        hi[i] = uh;
-        lo[i] = ul;
-    }
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x)
+        hl_split4(src[i], hi[i], lo[i]);
 }
 
 // ---- host: tensor maps ----------------------------------------------------------------------------------
