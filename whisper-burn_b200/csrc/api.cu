@@ -284,37 +284,10 @@ int wb_forward_decoder(wb_model* m, const int64_t* tokens, int64_t n_batch, int6
         const wb_dims& D = m->impl.dims;
         WB_REQUIRE(n_batch >= 1 && seq_len >= 1, "forward_decoder: empty input");
         WB_REQUIRE(seq_len <= D.n_text_ctx, "Token sequence length must not exceed n_text_ctx (mod.rs:134-139)");
-        const int V = D.n_vocab;
         std::lock_guard<std::mutex> lock(m->fwd_mu);
         wb::Session& s = m->forward_session(n_batch, std::min<int64_t>(D.n_text_ctx, std::max<int64_t>(seq_len, 2)));
         s.load_encoder_output_host(encoder_output, n_batch, n_enc_ctx);
-        struct FullLogits { wb::Session& s; explicit FullLogits(wb::Session& x) : s(x) { s.full_logits = true; } ~FullLogits() { s.full_logits = false; } } full_guard(s);
-        // position by position through the cached step; logits of every position are kept
-        wb::DevBuf<float> all;
-        all.alloc((size_t)n_batch * seq_len * V);
-        s.R = (int)n_batch;
-        std::vector<int> rw((size_t)n_batch), tk((size_t)n_batch);
-        for (int64_t r = 0; r < n_batch; ++r) rw[(size_t)r] = (int)r;
-        WB_CUDA(cudaMemcpyAsync(s.row_window.p, rw.data(), rw.size() * sizeof(int), cudaMemcpyHostToDevice, s.st));
-        WB_CUDA(cudaMemsetAsync(s.pos.p, 0, sizeof(int), s.st));
-        WB_CUDA(cudaMemsetAsync(s.finished.p, 0, sizeof(int) * s.Rmax, s.st));
-        s.anc_identity = true;
-        s.host_pos = 0;
-        for (int64_t p = 0; p < seq_len; ++p) {
-            for (int64_t r = 0; r < n_batch; ++r) {
-                const int64_t t = tokens[r * seq_len + p];
-                WB_REQUIRE(t >= 0 && t < V, "forward_decoder: token out of range");
-                tk[(size_t)r] = (int)t;
-            }
-            WB_CUDA(cudaMemcpyAsync(s.cur_tok.p, tk.data(), tk.size() * sizeof(int), cudaMemcpyHostToDevice, s.st));
-            WB_CUDA(cudaStreamSynchronize(s.st));
-            s.step_core(true, 0, 1, false, -1);
-            for (int64_t r = 0; r < n_batch; ++r)
-                WB_CUDA(cudaMemcpyAsync(all.p + ((size_t)r * seq_len + p) * V, s.logits.p + (size_t)r * V,
-                                        (size_t)V * sizeof(float), cudaMemcpyDeviceToDevice, s.st));
-        }
-        WB_CUDA(cudaMemcpyAsync(logits_out, all.p, all.n * sizeof(float), cudaMemcpyDeviceToHost, s.st));
-        WB_CUDA(cudaStreamSynchronize(s.st));
+        s.teacher_forced_logits(tokens, n_batch, seq_len, logits_out);
     });
 }
 
@@ -344,8 +317,7 @@ void wb_session_destroy(wb_session* s) { delete s; }
 int wb_session_set_search(wb_session* s, int rule) {
     return guarded([&] {
         WB_REQUIRE(s, "set_search: null pointer");
-        WB_REQUIRE(rule == WB_SEARCH_BEAM || rule == WB_SEARCH_GREEDY_LOOP, "set_search: unknown search rule");
-        s->impl->search = rule;
+        s->impl->set_search(rule);
     });
 }
 
@@ -716,7 +688,7 @@ int wb_session_profile_decode(wb_session* s, const wb_special_ids* ids, int n_st
     return guarded([&] {
         WB_REQUIRE(s && ids && logits_kernel_ms && step_ms, "null pointer");
         const int64_t prompt[4] = {ids->sot, ids->lang, ids->transcribe, ids->notimestamps};
-        s->impl->profile_decode(prompt, 4, n_steps, ids->eot, logits_kernel_ms, step_ms);
+        s->impl->profile_decode(prompt, 4, n_steps, logits_kernel_ms, step_ms);
     });
 }
 

@@ -871,6 +871,12 @@ __device__ __forceinline__ void fold_records(const DecArgs& a, const float* rec,
     for (int k = 0; k < KC; ++k) { a.lg_v[o * KC + k] = best.v[k]; a.lg_i[o * KC + k] = best.i[k]; }
 }
 
+// whether the vocabulary stage at position p masks the special ids (DecArgs::mask_mode): position p produces token p + 1,
+// and the beam search masks them while the sequence has at most 5 tokens (transcribe.rs:271-275).  A macro: the same
+// expression behind a __forceinline__ function compiles to different predicate code in every decoder.
+#define SPECIAL_MASKED(a, p) \
+    ((a).is_special != nullptr && ((a).mask_mode == MASK_ALWAYS || ((a).mask_mode == MASK_SHORT && (p) + 1 <= 5)))
+
 // ---- per-row finish: log-probs (v - max) - lse of the candidates, lse from the NP records of the row (DESIGN.md section 2)
 // greedy bookkeeping of row r at position p (beam.rs:9-37 with beam_size 1): the token and its rounded log-prob lp, the
 // length, EOT

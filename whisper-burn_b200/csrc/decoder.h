@@ -8,6 +8,9 @@
 namespace wb {
 
 constexpr int DEC_KC = 8;   // top candidates a persistent decoder keeps per record (k <= 7)
+// DecArgs::mask_mode: when the vocabulary stage masks the special ids (is_special): never, at every position, or while the
+// sequence has at most 5 tokens (transcribe.rs:271-275; dec_common.cuh SPECIAL_MASKED)
+constexpr int MASK_NONE = 0, MASK_ALWAYS = 1, MASK_SHORT = 2;
 
 // ---- persistent decoders (decoder3.cu .. decoder6.cu) -------------------------------------------------
 struct DecLayer {

@@ -253,7 +253,7 @@ dec3_kernel(const DecArgs a) {
         if (want_logits) {
             // ================= logits = LN(x) tok_emb^T (mod.rs:155-156) + mask + online softmax + candidates.
             // 8 lanes per vocabulary row, 8 rows per warp step; lane (sub, l8) tracks batch row l8.
-            const bool use_mask = a.is_special != nullptr && (a.mask_mode == 1 || (a.mask_mode == 2 && p + 1 <= 5));
+            const bool use_mask = SPECIAL_MASKED(a, p);
             const int eot_cap = a.loop_rules ? a.eot : -1;   // the id whose logit the greedy loop's EOT test reads
             const WT* E = reinterpret_cast<const WT*>(a.E);
             const int sub = lane >> 3, l8 = lane & 7;

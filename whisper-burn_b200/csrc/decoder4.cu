@@ -722,7 +722,7 @@ dec4_kernel(const DecArgs a) {
         WB_TRACE();
         // ================= logits (all CTAs): LN(x) tok_emb^T + mask + online softmax + candidates
         {
-            const bool use_mask = a.is_special != nullptr && (a.mask_mode == 1 || (a.mask_mode == 2 && p + 1 <= 5));
+            const bool use_mask = SPECIAL_MASKED(a, p);
             const int eot_cap = a.loop_rules ? a.eot : -1;   // the id whose logit the greedy loop's EOT test reads
             // the published rows: fp16 hi / lo planes in MMA fragment order (decoder5.cu); rows >= R are never used
             for (int i = tid; i < 2 * (D / 32) * 32; i += NT) cp_async16(pl_hi + i, gpl_hi + i);   // pl_lo follows pl_hi in both spaces

@@ -560,7 +560,7 @@ dec5_kernel(const DecArgs a) {
             // ================= per (row, slice): special-token mask (transcribe.rs:271-275), max, sum-exp, top candidates
             const int NSL = a.lg_slices;
             {
-                const bool use_mask = a.is_special != nullptr && (a.mask_mode == 1 || (a.mask_mode == 2 && p + 1 <= 5));
+                const bool use_mask = SPECIAL_MASKED(a, p);
                 const int per = (V + NSL - 1) / NSL;
                 // k == 1 (greedy): a compact scan -- running (max, sum-exp) and the best (value, lowest index); this code runs
                 // once per step, i.e. from a cold instruction cache, so its size is its cost

@@ -973,7 +973,7 @@ dec6_kernel(const DecArgs a) {
                 bar_consumers();
                 trace();
                 // ================= logits (all CTAs): LN(x) tok_emb^T + mask + online softmax + arg-max (mod.rs:155-156, transcribe.rs:271-276)
-                const bool use_mask = a.is_special != nullptr && (a.mask_mode == 1 || (a.mask_mode == 2 && p + 1 <= 5));
+                const bool use_mask = SPECIAL_MASKED(a, p);
                 const int eot_cap = !BEAM && a.loop_rules ? a.eot : -1;   // the id whose logit the greedy loop's EOT test reads
                 // LayerNorm rows straight into fp16 hi / lo planes in MMA fragment order (decoder5.cu); rows >= R are zero
                 for (int r = warp; r < 8 * NT8; r += NCW) {

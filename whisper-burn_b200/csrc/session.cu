@@ -3,7 +3,6 @@
 //   (mod.rs:228-260) -> cross K/V (mod.rs:484-485, hoisted out of the step loop) -> decoder steps.
 // Windows of one call are batched: encoder rows of all windows are packed back to back.
 #include <algorithm>
-#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -42,7 +41,6 @@ Session::Session(Model* model, int64_t max_w, int64_t max_b, int64_t max_text_le
     Mcap = (int64_t)max_windows * Tcap;
     const int d = D.n_audio_state, H = D.n_text_head, L = D.n_text_layer, V = D.n_vocab;
     WB_REQUIRE(max_beams <= DEC_KC - 1, "session: max_beams must be <= 7 (candidates kept per record by the persistent decoders)");
-    kmax = DEC_KC;
     if (const char* e = getenv("WB200_DECODER"); e && e[0]) {   // run every launch on this decoder (comparisons, tests)
         only_decoder = atoi(e);
         WB_REQUIRE(only_decoder >= 3 && only_decoder <= 6, "session: WB200_DECODER must be 3, 4, 5 or 6");
@@ -81,7 +79,7 @@ Session::Session(Model* model, int64_t max_w, int64_t max_b, int64_t max_text_le
     tokens.alloc((size_t)Rmax * t_max); token_lp.alloc((size_t)Rmax * t_max); lengths.alloc(Rmax); cur_tok.alloc(Rmax); finished.alloc(Rmax);
     row_window.alloc(Rmax); anc0.alloc((size_t)Rmax * t_max); anc1.alloc((size_t)Rmax * t_max); parent.alloc(Rmax);
     pos.alloc(1); n_unfinished.alloc(128);
-    topk_id.alloc((size_t)Rmax * kmax); topk_lp.alloc((size_t)Rmax * kmax);
+    topk_id.alloc((size_t)Rmax * DEC_KC); topk_lp.alloc((size_t)Rmax * DEC_KC);
     eot_logit.alloc(Rmax);
     is_special.alloc(V);
     {
@@ -89,7 +87,7 @@ Session::Session(Model* model, int64_t max_w, int64_t max_b, int64_t max_text_le
         cudaDeviceProp prop;
         WB_CUDA(cudaGetDeviceProperties(&prop, m->device));
         n_sm = prop.multiProcessorCount;
-        n_logit_ctas = 2 * prop.multiProcessorCount;
+        const int n_logit_ctas = 2 * prop.multiProcessorCount;
         // persistent decoder: per-layer pointer table, barrier words, larger split-KV partial buffers
         part_o.alloc((size_t)Rmax * H * 16 * 64); part_m.alloc((size_t)Rmax * H * 16); part_l.alloc((size_t)Rmax * H * 16);
         datt.alloc((size_t)Rmax * d); steps_done.alloc(128); dec_bar.alloc(4);
@@ -115,17 +113,32 @@ Session::Session(Model* model, int64_t max_w, int64_t max_b, int64_t max_text_le
         lg_m.alloc((size_t)n_logit_ctas * Rmax); lg_s.alloc((size_t)n_logit_ctas * Rmax);
         lg_v.alloc((size_t)n_logit_ctas * Rmax * DEC_KC); lg_i.alloc((size_t)n_logit_ctas * Rmax * DEC_KC);
     }
-    WB_CUDA(cudaMallocHost((void**)&h_int, sizeof(int) * (4 * (size_t)Rmax + 16 + (size_t)Rmax * kmax)));
-    WB_CUDA(cudaMallocHost((void**)&h_float, sizeof(float) * (size_t)Rmax * kmax));
+    h_parent = pinned<int>(Rmax); h_window = pinned<int>(Rmax); h_token = pinned<int>(Rmax);
+    h_topk_id = pinned<int>((size_t)Rmax * DEC_KC);
     WB_CUDA(cudaMemsetAsync(is_special.p, 0, V, st));
+
+    DecArgs& a = dec_base;
+    a.Rmax = Rmax; a.d = D.n_text_state; a.H = H; a.L = L; a.V = V; a.t_max = t_max; a.Mcap = Mcap;
+    a.eps_outside = m->ln_eps_outside; a.qk_scale = (float)std::pow((double)D.n_text_state / (double)H, -0.25);
+    a.layers = dec_layers.p; a.tok_emb = m->tok_emb32; a.pos_emb = m->dec_pos;
+    a.E = m->fp16_exact ? (const void*)m->tok_emb16 : (const void*)m->tok_emb32;
+    a.E_tiled = m->tok_emb16_tiled;
+    a.lnf_g = m->dec_ln.g; a.lnf_b = m->dec_ln.b; a.lnf_eps = m->dec_ln.eps;
+    a.x = dx.p; a.q = dq.p; a.att = datt.p; a.hid = dhid.p;
+    a.ypart = ypart.p; a.lgbuf = logits.p; a.att_pl = att_pl.p; a.hid_pl = hid_pl.p;
+    a.kv_half = kv == WB_KV_F16 ? 1 : 0;
+    if (a.kv_half) { a.kc = kc16.p; a.vc = vc16.p; a.ckv = ckv16.p; } else { a.kc = kc.p; a.vc = vc.p; a.ckv = ckv.p; }
+    a.row_window = row_window.p; a.win_row_off = d_win_row_off.p; a.win_T = d_win_T.p;
+    a.part_o = part_o.p; a.part_m = part_m.p; a.part_l = part_l.p;
+    a.tokens = tokens.p; a.token_lp = token_lp.p; a.cur_tok = cur_tok.p; a.lengths = lengths.p; a.finished = finished.p;
+    a.eot_logit = eot_logit.p; a.topk_id = topk_id.p; a.topk_lp = topk_lp.p;
+    a.lg_m = lg_m.p; a.lg_s = lg_s.p; a.lg_v = lg_v.p; a.lg_i = lg_i.p;
+    a.pos = pos.p; a.n_unfinished = n_unfinished.p; a.steps_done = steps_done.p; a.bar = dec_bar.p;
     WB_CUDA(cudaStreamSynchronize(st));
 }
 
 Session::~Session() {
     if (st) cudaStreamSynchronize(st);
-    for (auto& e : prof_ev) cudaEventDestroy(e);
-    if (h_int) cudaFreeHost(h_int);
-    if (h_float) cudaFreeHost(h_float);
     for (auto& e : ev)
         if (e) cudaEventDestroy(e);
     if (st) cudaStreamDestroy(st);
@@ -170,14 +183,12 @@ void Session::encode_from_device_wave(const float* wave_dev, const int64_t* offs
     WB_REQUIRE(n >= 1 && n <= max_windows, "encode: n_windows out of range for this session");
     std::vector<LogMelWindow> lw((size_t)n);
     std::vector<int> Tm((size_t)n);
-    win_F.resize((size_t)n);
     int max_frames = 0;
     for (int64_t w = 0; w < n; ++w) {
         WB_REQUIRE(lens[w] >= N_FFT, "prep_audio: waveform shorter than n_fft (audio.rs:292)");
         WB_REQUIRE(lens[w] < (int64_t)1 << 30, "prep_audio: waveform too long");
         const int F = (int)(lens[w] / HOP);                        // frames after dropping the last one
         const int keep = std::min(F, mel_limit - MEL_PADDING);      // transcribe.rs:173
-        win_F[(size_t)w] = F;
         Tm[(size_t)w] = keep + MEL_PADDING;
         lw[(size_t)w] = LogMelWindow{offsets[w], (int)lens[w], F, keep, (int)w, ((int64_t)w * TmS + 1) * N_MELS};
         max_frames = std::max(max_frames, F);
@@ -376,71 +387,68 @@ void Session::set_special(const uint8_t* sp) {
     }
 }
 
-void Session::begin(const int64_t* prompt, int64_t prompt_len, bool prefill) {
-    if (!encoded) fail(WB_ERR_STATE, "session: begin before encode");
-    WB_REQUIRE(prompt_len >= 1 && prompt_len < t_max, "begin: prompt length out of range");
+void Session::seat_rows(int rows, int per_window, const int64_t* prompt, int64_t prompt_len, int64_t prompt_stride) {
+    if (!encoded) fail(WB_ERR_STATE, "session: decode before encode");
+    WB_REQUIRE(rows <= Rmax && prompt_len >= 1 && prompt_len <= t_max, "decode: rows or prompt length out of range");
     const int V = m->dims.n_vocab;
-    R = n_windows;
-    WB_REQUIRE(R <= Rmax, "begin: too many rows");
-    std::vector<int> tk((size_t)R * t_max, 0), rw((size_t)R), first((size_t)R);
-    for (int r = 0; r < R; ++r) {
+    std::vector<int> tk((size_t)rows * t_max, 0), rw((size_t)rows), len((size_t)rows, (int)prompt_len);
+    for (int r = 0; r < rows; ++r) {
+        rw[(size_t)r] = r / per_window;
         for (int64_t i = 0; i < prompt_len; ++i) {
-            WB_REQUIRE(prompt[i] >= 0 && prompt[i] < V, "begin: prompt token out of range");
-            tk[(size_t)r * t_max + i] = (int)prompt[i];
+            const int64_t t = prompt[r * prompt_stride + i];
+            WB_REQUIRE(t >= 0 && t < V, "decode: prompt token out of range");
+            tk[(size_t)r * t_max + i] = (int)t;
         }
-        rw[(size_t)r] = r;
-        first[(size_t)r] = (int)prompt[0];
     }
     WB_CUDA(cudaMemcpyAsync(tokens.p, tk.data(), tk.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     WB_CUDA(cudaMemcpyAsync(row_window.p, rw.data(), rw.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-    WB_CUDA(cudaMemcpyAsync(cur_tok.p, first.data(), first.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     WB_CUDA(cudaMemsetAsync(finished.p, 0, sizeof(int) * Rmax, st));
     WB_CUDA(cudaMemsetAsync(pos.p, 0, sizeof(int), st));
-    std::vector<int> len((size_t)R, (int)prompt_len);
     WB_CUDA(cudaMemcpyAsync(lengths.p, len.data(), len.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    R = rows;
     anc_identity = true;
     anc_cur = 0;
     host_pos = 0;
-    // feed prompt[0 .. prompt_len-1): no logits needed
-    for (int64_t i = 0; prefill && i + 1 < prompt_len; ++i) {
-        step_core(false, 0, 1, false, -1);
-        std::vector<int> nxt((size_t)R, (int)prompt[i + 1]);
-        WB_CUDA(cudaMemcpyAsync(cur_tok.p, nxt.data(), nxt.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-        WB_CUDA(cudaStreamSynchronize(st));
+}
+
+void Session::feed_positions(int n, float* logits_out) {
+    const size_t V = (size_t)m->dims.n_vocab;
+    const StepLogits out = logits_out ? StepLogits::topk_and_raw : StepLogits::none;
+    for (int p = 0; p < n; ++p, ++host_pos) {
+        // every row's token at p: column p of the token buffer
+        WB_CUDA(cudaMemcpy2DAsync(cur_tok.p, sizeof(int), tokens.p + p, t_max * sizeof(int), sizeof(int), R, cudaMemcpyDeviceToDevice, st));
+        launch_decoder(DecodeLaunch::cached_step(R, host_pos, out, MASK_NONE, 1));
+        if (logits_out)
+            WB_CUDA(cudaMemcpy2DAsync(logits_out + p * V, n * V * sizeof(float), logits.p, V * sizeof(float), V * sizeof(float), R,
+                                      cudaMemcpyDeviceToHost, st));
     }
+}
+
+void Session::begin(const int64_t* prompt, int64_t prompt_len, bool prefill) {
+    WB_REQUIRE(prompt_len >= 1 && prompt_len < t_max, "begin: prompt length out of range");
+    seat_rows(n_windows, 1, prompt, prompt_len, 0);
+    if (prefill) feed_positions((int)prompt_len - 1, nullptr);   // prompt[0 .. prompt_len-1): no logits needed
     WB_CUDA(cudaStreamSynchronize(st));
 }
 
-// The persistent decoder for n_steps positions starting at pos0: the first of decoder4 -> decoder6 -> decoder5 -> decoder3
-// that covers the launch (each launch_decN decides that itself), or only the one WB200_DECODER names.
-bool Session::launch_decoder(int R_, int pos0, int n_steps, int logits_from, bool use_cur_tok, int mask_mode, int k,
-                        bool greedy, int eot, int beam, int max_depth, bool loop_rules) {
-    const wb_dims& D = m->dims;
-    const int d = D.n_text_state, H = D.n_text_head;
-    DecArgs a;
-    a.R = R_; a.Rmax = Rmax; a.d = d; a.H = H; a.L = D.n_text_layer; a.V = D.n_vocab; a.t_max = t_max; a.Mcap = Mcap;
-    a.eps_outside = m->ln_eps_outside; a.qk_scale = (float)std::pow((double)d / (double)H, -0.25);
-    a.layers = dec_layers.p; a.tok_emb = m->tok_emb32; a.pos_emb = m->dec_pos;
-    a.E = m->fp16_exact ? (const void*)m->tok_emb16 : (const void*)m->tok_emb32;
-    a.E_tiled = m->tok_emb16_tiled;
-    a.lnf_g = m->dec_ln.g; a.lnf_b = m->dec_ln.b; a.lnf_eps = m->dec_ln.eps;
-    a.x = dx.p; a.q = dq.p; a.att = datt.p; a.hid = dhid.p;
-    a.ypart = ypart.p; a.lgbuf = logits.p; a.att_pl = att_pl.p; a.hid_pl = hid_pl.p;
-    a.lg_slices = std::max(1, std::min(16, n_sm / std::max(1, R_)));
-    a.kv_half = kv_dtype == WB_KV_F16 ? 1 : 0;
-    if (a.kv_half) { a.kc = kc16.p; a.vc = vc16.p; a.ckv = ckv16.p; } else { a.kc = kc.p; a.vc = vc.p; a.ckv = ckv.p; }
-    a.row_window = row_window.p; a.win_row_off = d_win_row_off.p; a.win_T = d_win_T.p;
+void Session::teacher_forced_logits(const int64_t* toks, int64_t n_rows, int64_t seq_len, float* logits_out) {
+    seat_rows((int)n_rows, 1, toks, seq_len, seq_len);
+    feed_positions((int)seq_len, logits_out);
+    WB_CUDA(cudaStreamSynchronize(st));
+}
+
+// The first of decoder4 -> decoder6 -> decoder5 -> decoder3 that covers the launch (each launch_decN decides that itself),
+// or only the one WB200_DECODER names.
+bool Session::launch_decoder(const DecodeLaunch& l) {
+    DecArgs a = dec_base;
+    a.R = l.rows;
+    a.lg_slices = std::max(1, std::min(16, n_sm / std::max(1, l.rows)));
+    a.n_splits = std::max(1, std::min(16, n_sm / std::max(1, l.rows * a.H)));
     a.anc = anc_identity ? nullptr : (anc_cur == 0 ? anc0.p : anc1.p);
-    a.n_splits = std::max(1, std::min(16, n_sm / std::max(1, R_ * H)));
-    a.part_o = part_o.p; a.part_m = part_m.p; a.part_l = part_l.p;
-    a.tokens = tokens.p; a.token_lp = token_lp.p; a.cur_tok = cur_tok.p; a.use_cur_tok = use_cur_tok ? 1 : 0;
-    a.pos0 = pos0; a.n_steps = n_steps; a.logits_from = logits_from;
-    a.is_special = have_special ? is_special.p : nullptr; a.mask_mode = mask_mode;
-    a.k = k; a.greedy = greedy ? 1 : 0; a.eot = eot; a.lengths = lengths.p; a.finished = finished.p;
-    a.loop_rules = loop_rules ? 1 : 0; a.eot_logit = eot_logit.p;
-    a.topk_id = topk_id.p; a.topk_lp = topk_lp.p; a.logits_out = full_logits ? logits.p : nullptr;
-    a.lg_m = lg_m.p; a.lg_s = lg_s.p; a.lg_v = lg_v.p; a.lg_i = lg_i.p;
-    a.pos = pos.p; a.n_unfinished = n_unfinished.p; a.steps_done = steps_done.p; a.bar = dec_bar.p;
+    a.use_cur_tok = l.use_cur_tok; a.pos0 = l.pos0; a.n_steps = l.n_steps; a.logits_from = l.logits_from;
+    a.is_special = have_special ? is_special.p : nullptr; a.mask_mode = l.mask_mode;
+    a.k = l.k; a.greedy = l.greedy; a.eot = l.eot; a.loop_rules = l.loop_rules;
+    a.logits_out = l.raw_logits ? logits.p : nullptr;
     if (getenv("WB200_TRACE")) {
         dec_trace.ensure(1 << 16);
         WB_CUDA(cudaMemsetAsync(dec_trace.p, 0, sizeof(unsigned long long) * (1 << 16), st));
@@ -452,8 +460,8 @@ bool Session::launch_decoder(int R_, int pos0, int n_steps, int logits_from, boo
     auto allowed = [&](int n) { return only_decoder == 0 || only_decoder == n; };
     int groups = 0;
     last_groups = 1;
-    if (beam > 1) {   // the whole search: only decoder6 has a beam mode
-        a.beam = beam; a.n_win = R_ / beam; a.max_depth = max_depth;
+    if (l.beam > 1) {   // the whole search: only decoder6 has a beam mode
+        a.beam = l.beam; a.n_win = l.rows / l.beam; a.max_depth = l.max_depth;
         a.anc = anc0.p; a.anc_alt = anc1.p; a.slot_live = slot_live.p;
         a.bm_head = bm_head.p; a.bm_seq = bm_seq.p; a.bm_cnt = bm_cnt.p; a.bm_win = bm_win.p; a.bm_out = bm_out.p; a.bm_out_len = bm_out_len.p;
         a.bm_seq_lp = bm_seq_lp.p; a.bm_out_lp = bm_out_lp.p;
@@ -464,8 +472,8 @@ bool Session::launch_decoder(int R_, int pos0, int n_steps, int logits_from, boo
     else if (allowed(5) && (groups = launch_dec5(a, d5, n_sm, h16, st)) > 0) { last_decoder = 5; last_groups = groups; }
     else if (allowed(3)) { launch_dec3(a, n_sm, h16, st); last_decoder = 3; }
     else fail(WB_ERR_UNSUPPORTED, "WB200_DECODER=" + std::to_string(only_decoder) + ": decoder" + std::to_string(only_decoder) + " does not cover this launch");
-    last_rows = R_;
-    last_k = k;
+    last_rows = l.rows;
+    last_k = l.k;
     if (a.trace) {
         std::vector<unsigned long long> h(1 << 16);
         WB_CUDA(cudaStreamSynchronize(st));
@@ -480,30 +488,17 @@ bool Session::launch_decoder(int R_, int pos0, int n_steps, int logits_from, boo
     return true;
 }
 
-void Session::step_core(bool with_logits, int mask_mode, int k, bool greedy, int eot) {
-    WB_REQUIRE(k >= 1 && k <= DEC_KC - 1, "step: k must be in [1, 7]");
-    launch_decoder(R, host_pos, 1, with_logits ? 0 : INT_MAX, true, mask_mode, k, greedy, eot);
-    ++host_pos;
-}
-
-void Session::profile_decode(const int64_t* prompt, int64_t prompt_len, int n_steps, int64_t eot, float* logits_ms,
-                             float* step_ms) {
+void Session::profile_decode(const int64_t* prompt, int64_t prompt_len, int n_steps, float* logits_ms, float* step_ms) {
     WB_REQUIRE(n_steps >= 1 && prompt_len + n_steps <= t_max, "profile: n_steps out of range");
-    while (prof_ev.size() < 2) {
-        cudaEvent_t e;
-        WB_CUDA(cudaEventCreate(&e));
-        prof_ev.push_back(e);
-    }
     // the whole decode is ONE kernel: time the launch (prefill + n_steps greedy steps) and report per position
     begin(prompt, prompt_len, false);
     const int total = (int)prompt_len - 1 + n_steps;
-    WB_CUDA(cudaEventRecord(prof_ev[0], st));
-    launch_decoder(R, 0, total, (int)prompt_len - 1, false, 2, 1, true, -1 /* never stop early */);
-    WB_CUDA(cudaEventRecord(prof_ev[1], st));
+    WB_CUDA(cudaEventRecord(ev[4], st));
+    launch_decoder(DecodeLaunch::greedy_search(R, (int)prompt_len, n_steps, /*eot=*/-1, /*loop_rules=*/false));
+    WB_CUDA(cudaEventRecord(ev[5], st));
     WB_CUDA(cudaStreamSynchronize(st));
     float t = 0.f;
-    WB_CUDA(cudaEventElapsedTime(&t, prof_ev[0], prof_ev[1]));
-    (void)eot;
+    WB_CUDA(cudaEventElapsedTime(&t, ev[4], ev[5]));
     *logits_ms = t / (float)total;
     *step_ms = t / (float)total;
 }
@@ -512,23 +507,20 @@ void Session::step_beams(int64_t n_rows, const int32_t* window_of_row, const int
                          int apply_mask, int k, int64_t* topk_ids_out, float* topk_lp_out) {
     if (!encoded) fail(WB_ERR_STATE, "session: step before encode/begin");
     WB_REQUIRE(n_rows >= 1 && n_rows <= Rmax, "step: n_rows out of range");
-    WB_REQUIRE(k >= 1 && k <= kmax, "step: k out of range");
+    WB_REQUIRE(k >= 1 && k <= DEC_KC - 1, "step: k must be in [1, 7]");
     WB_REQUIRE(host_pos + 1 < t_max, "step: session max_text_len exceeded");
     const int V = m->dims.n_vocab;
-    int* hp = h_int;                  // parent
-    int* hw = h_int + Rmax;           // window
-    int* ht = h_int + 2 * Rmax;       // token
     for (int64_t r = 0; r < n_rows; ++r) {
         WB_REQUIRE(parent_row[r] >= 0 && parent_row[r] < R, "step: parent_row out of range");
         WB_REQUIRE(window_of_row[r] >= 0 && window_of_row[r] < n_windows, "step: window_of_row out of range");
         WB_REQUIRE(token[r] >= 0 && token[r] < V, "step: token out of range");
-        hp[r] = parent_row[r];
-        hw[r] = window_of_row[r];
-        ht[r] = (int)token[r];
+        h_parent[r] = parent_row[r];
+        h_window[r] = window_of_row[r];
+        h_token[r] = (int)token[r];
     }
-    WB_CUDA(cudaMemcpyAsync(parent.p, hp, sizeof(int) * n_rows, cudaMemcpyHostToDevice, st));
-    WB_CUDA(cudaMemcpyAsync(row_window.p, hw, sizeof(int) * n_rows, cudaMemcpyHostToDevice, st));
-    WB_CUDA(cudaMemcpyAsync(cur_tok.p, ht, sizeof(int) * n_rows, cudaMemcpyHostToDevice, st));
+    WB_CUDA(cudaMemcpyAsync(parent.p, h_parent.get(), sizeof(int) * n_rows, cudaMemcpyHostToDevice, st));
+    WB_CUDA(cudaMemcpyAsync(row_window.p, h_window.get(), sizeof(int) * n_rows, cudaMemcpyHostToDevice, st));
+    WB_CUDA(cudaMemcpyAsync(cur_tok.p, h_token.get(), sizeof(int) * n_rows, cudaMemcpyHostToDevice, st));
     if (anc_identity) {   // rows so far (prompt) live in their own cache rows
         launch_dec_anc_identity(anc0.p, Rmax, t_max, st);
         anc_cur = 0;
@@ -541,15 +533,12 @@ void Session::step_beams(int64_t n_rows, const int32_t* window_of_row, const int
         launch_dec_reorder(cur, nxt, parent.p, pos.p, R, t_max, st);
         anc_cur ^= 1;
     }
-    step_core(true, apply_mask ? 1 : 0, k, false, -1);
-    int* hid_ = h_int + 4 * Rmax + 16;
-    WB_CUDA(cudaMemcpyAsync(hid_, topk_id.p, sizeof(int) * n_rows * k, cudaMemcpyDeviceToHost, st));
-    WB_CUDA(cudaMemcpyAsync(h_float, topk_lp.p, sizeof(float) * n_rows * k, cudaMemcpyDeviceToHost, st));
+    launch_decoder(DecodeLaunch::cached_step(R, host_pos, StepLogits::topk, apply_mask ? MASK_ALWAYS : MASK_NONE, k));
+    ++host_pos;
+    WB_CUDA(cudaMemcpyAsync(h_topk_id.get(), topk_id.p, sizeof(int) * n_rows * k, cudaMemcpyDeviceToHost, st));
+    WB_CUDA(cudaMemcpyAsync(topk_lp_out, topk_lp.p, sizeof(float) * n_rows * k, cudaMemcpyDeviceToHost, st));
     WB_CUDA(cudaStreamSynchronize(st));
-    for (int64_t i = 0; i < n_rows * k; ++i) {
-        topk_ids_out[i] = hid_[i];
-        topk_lp_out[i] = h_float[i];
-    }
+    for (int64_t i = 0; i < n_rows * k; ++i) topk_ids_out[i] = h_topk_id[i];
 }
 
 void Session::last_topk(int64_t n_rows, int64_t k, int64_t* ids_out, float* lp_out) {
@@ -566,12 +555,10 @@ void Session::last_topk(int64_t n_rows, int64_t k, int64_t* ids_out, float* lp_o
 void Session::greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_depth, int64_t eot,
                             std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp, bool loop_rules) {
     WB_REQUIRE(prompt_len + max_depth <= t_max, "greedy: prompt + max_depth exceeds the session's max_text_len");
-    // one launch: prompt prefill + every greedy step, early exit inside the kernel.  The beam rule masks the special ids while
-    // a sequence has at most 5 tokens (mask_mode 2); the greedy loop masks nothing, and its context stop, at
+    // one launch: prompt prefill + every greedy step, early exit inside the kernel.  The greedy loop's context stop, at
     // prompt_len + max_depth <= t_max <= n_text_ctx tokens, is the end of the launch.
     begin(prompt, prompt_len, /*prefill=*/false);
-    const int n_steps = (int)prompt_len - 1 + max_depth;
-    if (max_depth > 0) launch_decoder(R, 0, n_steps, (int)prompt_len - 1, false, loop_rules ? 0 : 2, 1, true, (int)eot, 0, 0, loop_rules);
+    if (max_depth > 0) launch_decoder(DecodeLaunch::greedy_search(R, (int)prompt_len, max_depth, (int)eot, loop_rules));
     std::vector<int> tk((size_t)R * t_max), len((size_t)R);
     std::vector<float> lp((size_t)R * t_max);
     int sdv[128] = {0};
@@ -605,23 +592,18 @@ void Session::greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_d
 bool Session::beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_size, int max_depth, int64_t eot,
                           std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp) {
     namespace fx = beamfx;
-    if (!encoded) fail(WB_ERR_STATE, "session: decode before encode");
     WB_REQUIRE(prompt_len >= 1 && prompt_len + max_depth <= t_max, "beam: prompt + max_depth exceeds the session's max_text_len");
-    const int B = beam_size, W = n_windows, Rb = W * B, V = m->dims.n_vocab;
+    const int B = beam_size, W = n_windows, Rb = W * B;
     if (B < 2 || B > fx::MAX_BEAM || max_depth < 1 || Rb > Rmax) return false;
-    for (int64_t i = 0; i < prompt_len; ++i) WB_REQUIRE(prompt[i] >= 0 && prompt[i] < V, "beam: prompt token out of range");
+    // slot i of window w = row w * B + i; until the first search step only slot 0 holds a beam: the prompt, in its own cache row
+    seat_rows(Rb, B, prompt, prompt_len, 0);
     constexpr int MN = fx::MAX_NODES;
     slot_live.ensure((size_t)Rmax);
     bm_head.ensure((size_t)2 * W * MN); bm_seq.ensure((size_t)2 * W * MN * t_max); bm_seq_lp.ensure((size_t)2 * W * MN * t_max);
     bm_cnt.ensure((size_t)2 * W); bm_win.ensure((size_t)2 * W);
     bm_out.ensure((size_t)W * t_max); bm_out_lp.ensure((size_t)W * t_max); bm_out_len.ensure((size_t)W);
-    // slot i of window w = row w * B + i; until the first search step only slot 0 holds a beam: the prompt, in its own cache row
-    std::vector<int> tk((size_t)Rb * t_max, 0), rw((size_t)Rb), live((size_t)Rb);
-    for (int r = 0; r < Rb; ++r) {
-        for (int64_t i = 0; i < prompt_len; ++i) tk[(size_t)r * t_max + i] = (int)prompt[i];
-        rw[(size_t)r] = r / B;
-        live[(size_t)r] = r % B == 0 ? 1 : 0;
-    }
+    std::vector<int> live((size_t)Rb);
+    for (int r = 0; r < Rb; ++r) live[(size_t)r] = r % B == 0 ? 1 : 0;
     std::vector<fx::Head> heads((size_t)W * MN, fx::Head{0.0, 0, 0, 0, 0});
     std::vector<int> seq((size_t)W * MN * t_max, 0), cnt((size_t)2 * W, 0), win((size_t)2 * W, 0);   // depth-0 buffer; window: {buffer, done}
     for (int w = 0; w < W; ++w) {
@@ -629,8 +611,6 @@ bool Session::beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_si
         for (int64_t i = 0; i < prompt_len; ++i) seq[(size_t)w * MN * t_max + i] = (int)prompt[i];
         cnt[(size_t)w] = 1;
     }
-    WB_CUDA(cudaMemcpyAsync(tokens.p, tk.data(), tk.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-    WB_CUDA(cudaMemcpyAsync(row_window.p, rw.data(), rw.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     WB_CUDA(cudaMemcpyAsync(slot_live.p, live.data(), live.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     WB_CUDA(cudaMemcpyAsync(bm_head.p, heads.data(), heads.size() * sizeof(fx::Head), cudaMemcpyHostToDevice, st));
     WB_CUDA(cudaMemcpyAsync(bm_seq.p, seq.data(), seq.size() * sizeof(int), cudaMemcpyHostToDevice, st));
@@ -638,7 +618,7 @@ bool Session::beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_si
     WB_CUDA(cudaMemcpyAsync(bm_cnt.p, cnt.data(), cnt.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     WB_CUDA(cudaMemcpyAsync(bm_win.p, win.data(), win.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     launch_dec_anc_identity(anc0.p, Rb, t_max, st);
-    const bool ran = launch_decoder(Rb, 0, (int)prompt_len - 1 + max_depth, (int)prompt_len - 1, false, 2, B, false, (int)eot, B, max_depth);
+    const bool ran = launch_decoder(DecodeLaunch::beam_search(Rb, B, (int)prompt_len, max_depth, (int)eot));
     std::vector<int> res((size_t)W * t_max), res_len((size_t)W);
     std::vector<float> res_lp((size_t)W * t_max);
     int sd = 0;
@@ -650,8 +630,7 @@ bool Session::beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_si
     }
     WB_CUDA(cudaStreamSynchronize(st));   // the host vectors above are in flight until here
     if (!ran) return false;
-    // session state as the host search leaves it: rows, position, ancestry of the last position
-    R = Rb;
+    // session state as the host search leaves it: position, ancestry of the last position
     last_steps = sd;
     host_pos = (int)prompt_len - 1 + sd;
     anc_identity = false;

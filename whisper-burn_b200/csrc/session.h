@@ -1,5 +1,6 @@
 // Decoding session: all device state between prep_audio and the emitted token ids.  Internal.
 #pragma once
+#include <climits>
 #include <memory>
 #include <vector>
 
@@ -17,22 +18,61 @@ constexpr int MEL_PADDING = 10;   // transcribe.rs:33
 int window_mel_frames(int n_audio_ctx, int window_mode);
 int64_t window_samples(int n_audio_ctx, int window_mode);
 
+// what a cached step computes besides K/V: nothing (prefill), each row's k best candidates, or those and its raw logits
+enum class StepLogits { none, topk, topk_and_raw };
+
+// One persistent-decoder launch (Session::launch_decoder).  The named constructors are its three kinds; each field sets
+// the DecArgs field of the same name (raw_logits: logits_out).
+struct DecodeLaunch {
+    int rows = 0, pos0 = 0, n_steps = 1, logits_from = INT_MAX;   // logits of the positions from logits_from on
+    bool use_cur_tok = false, raw_logits = false;                  // tokens from cur_tok, else from the token buffer
+    int mask_mode = MASK_NONE, k = 1, eot = -1;                    // k candidates per row; eot -1: no early finish
+    bool greedy = false, loop_rules = false;
+    int beam = 0, max_depth = 0;
+
+    // position pos of every row, tokens from cur_tok
+    static DecodeLaunch cached_step(int rows, int pos, StepLogits out, int mask_mode, int k) {
+        DecodeLaunch l;
+        l.rows = rows; l.pos0 = pos; l.use_cur_tok = true; l.mask_mode = mask_mode; l.k = k;
+        l.logits_from = out == StepLogits::none ? INT_MAX : 0; l.raw_logits = out == StepLogits::topk_and_raw;
+        return l;
+    }
+    // the prompt prefill (no logits), then max_depth positions of beam_size 1 of the beam search (special ids masked while
+    // a sequence has <= 5 tokens) or, with loop_rules, of the reference's greedy loop (no mask); tokens from the token buffer
+    static DecodeLaunch greedy_search(int rows, int prompt_len, int max_depth, int eot, bool loop_rules) {
+        DecodeLaunch l;
+        l.rows = rows; l.n_steps = prompt_len - 1 + max_depth; l.logits_from = prompt_len - 1; l.eot = eot;
+        l.greedy = true; l.loop_rules = loop_rules; l.mask_mode = loop_rules ? MASK_NONE : MASK_SHORT;
+        return l;
+    }
+    // the same positions for the whole width-`beam` search of rows / beam windows (decoder6 beam mode)
+    static DecodeLaunch beam_search(int rows, int beam, int prompt_len, int max_depth, int eot) {
+        DecodeLaunch l = greedy_search(rows, prompt_len, max_depth, eot, false);
+        l.greedy = false; l.k = l.beam = beam; l.max_depth = max_depth;
+        return l;
+    }
+};
+
+// pinned host array
+struct PinnedFree { void operator()(void* p) const { cudaFreeHost(p); } };
+template <typename T> using Pinned = std::unique_ptr<T[], PinnedFree>;
+template <typename T> Pinned<T> pinned(size_t n) { void* p = nullptr; WB_CUDA(cudaMallocHost(&p, n * sizeof(T))); return Pinned<T>((T*)p); }
+
 struct Session {
     Model* m = nullptr;
     cudaStream_t st = nullptr;
     int max_windows = 0, max_beams = 0, t_max = 0, kv_dtype = WB_KV_F32;
     int window_mode = WB_WINDOWS_REFERENCE;
-    int search = WB_SEARCH_BEAM;   // wb_session_set_search: the rule transcribe_windows decodes by
+    int search = WB_SEARCH_BEAM;   // set_search: the rule transcribe_windows decodes by
     int mel_limit = 0;   // window_mel_frames(n_audio_ctx, window_mode)
     int Rmax = 0;        // max_windows * max_beams decode rows
     int TmS = 0;         // rows per window in the token-major mel / conv1 buffers (mel_limit + 2 halo rows)
     int Tcap = 0;        // max encoder positions per window: (mel_limit - 1) / 2 + 1
     int64_t Mcap = 0;    // max packed encoder rows
-    int kmax = 8;        // candidates per row the step API can return (k <= 7)
 
     // ---- geometry of the windows currently encoded (host mirrors)
     int n_windows = 0;
-    std::vector<int> win_F, win_Tm, win_T;
+    std::vector<int> win_Tm, win_T;
     std::vector<int64_t> win_row_off;
     int64_t M_tot = 0;
     int max_T = 0, max_Tm = 0;
@@ -52,7 +92,6 @@ struct Session {
     // tensor-core path (fp16-exact weights): every GEMM input travels as a pair of fp16 planes (gemm_f16.cu)
     DevBuf<__half> mel_h, mel_l, h1_h, h1_l, xn_h, xn_l, qkv_h, qkv_l, att_h, att_l, hid_h, hid_l, xa_h, xa_l;
     std::vector<std::unique_ptr<GemmF16Plan>> enc_plans;   // conv1, conv2, per encoder layer qkv / out / mlp1 / mlp2, per decoder layer cross K|V
-    bool conv_tc_ok = true;            // cleared if the driver rejects the overlapping-row tensor maps of the conv stems
     bool use_tc = true;                // fp16-exact weights: tensor-core encoder; else the fp32 CUDA-core GEMM
     void run_encoder_f16();            // tensor-core encoder
     void run_encoder_f32();            // fp32 CUDA-core encoder (weights that are not fp16-exact)
@@ -75,11 +114,10 @@ struct Session {
     bool anc_identity = true;
     int R = 0;             // live rows
     int host_pos = 0;      // host mirror of *pos
-    // pinned host staging
-    int* h_int = nullptr;      // [4 * Rmax + 16]
-    float* h_float = nullptr;  // [Rmax * kmax]
-    // timings of the last transcribe call
-    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    // pinned host staging of step_beams: [Rmax] rows in, [Rmax][DEC_KC] candidate ids out
+    Pinned<int> h_parent, h_window, h_token, h_topk_id;
+    // ev[0..3]: timings of the last transcribe call; ev[4], ev[5]: the launch profile_decode times
+    cudaEvent_t ev[6] = {};
     float last_ms[4] = {0, 0, 0, 0};
     int64_t last_steps = 0;
     int last_groups = 1;         // row groups (launches) of the last decode
@@ -93,19 +131,18 @@ struct Session {
     DevBuf<int> steps_done;
     DevBuf<float> datt;
     DevBuf<unsigned long long> dec_trace;   // debug: WB200_TRACE=1
-    // beam > 1: the whole beam search in one decoder6 launch (beam_decode); returns false when decoder6 does not cover it
-    bool launch_decoder(int R_, int pos0, int n_steps, int logits_from, bool use_cur_tok, int mask_mode, int k, bool greedy,
-                   int eot, int beam = 0, int max_depth = 0, bool loop_rules = false);
+    DecArgs dec_base;   // the DecArgs fields that are fixed once the session exists; launch_decoder sets the rest
+    // the first persistent decoder that covers the launch; false when a beam search launch is not covered (only decoder6
+    // has a beam mode)
+    bool launch_decoder(const DecodeLaunch& l);
     // device beam search state (decoder6.cu beam mode), allocated on first use
     DevBuf<int> slot_live, bm_seq, bm_cnt, bm_win, bm_out, bm_out_len;
     DevBuf<float> bm_seq_lp, bm_out_lp;
     DevBuf<beamfx::Head> bm_head;
-    bool full_logits = false;    // also write raw logits [R][V] (stateless forward_decoder)
-    int n_logit_ctas = 0;
     DevBuf<float> ypart, lg_m, lg_s, lg_v;
     DevBuf<int> lg_i;
-    std::vector<cudaEvent_t> prof_ev;   // wb_session_profile_decode: launch begin / end
-    void profile_decode(const int64_t* prompt, int64_t prompt_len, int n_steps, int64_t eot, float* logits_ms, float* step_ms);
+    // the greedy search launch of n_steps positions after the prompt, with no early stop, timed by events
+    void profile_decode(const int64_t* prompt, int64_t prompt_len, int n_steps, float* logits_ms, float* step_ms);
 
     Session(Model* model, int64_t max_windows, int64_t max_beams, int64_t max_text_len, int kv_dtype,
             int window_mode = WB_WINDOWS_REFERENCE);
@@ -122,10 +159,20 @@ struct Session {
     void run_encoder();      // conv stems .. ln_post .. cross K/V, from mel_rows
     void run_cross_kv();
 
+    void set_search(int rule) {
+        WB_REQUIRE(rule == WB_SEARCH_BEAM || rule == WB_SEARCH_GREEDY_LOOP, "set_search: unknown search rule");
+        search = rule;
+    }
     void set_special(const uint8_t* is_special_host);
+    // Seats `rows` rows for a new decode from position 0: row r decodes window r / per_window from the prompt_len tokens at
+    // prompt + r * prompt_stride (token buffer, lengths); no row is finished and every row reads only its own cache rows
+    void seat_rows(int rows, int per_window, const int64_t* prompt, int64_t prompt_len, int64_t prompt_stride);
+    // teacher forcing right after seat_rows: positions [0, n) of every row from its token buffer, one cached step each;
+    // with logits_out (host), each position's raw logits go to logits_out [R][n][V]
+    void feed_positions(int n, float* logits_out);
     void begin(const int64_t* prompt, int64_t prompt_len, bool prefill = true);
-    // one decoder position for R rows; tokens come from cur_tok
-    void step_core(bool with_logits, int mask_mode, int k, bool greedy, int eot);
+    // the stateless forward_decoder: every position's logits [n_rows][seq_len][V] of tokens [n_rows][seq_len]
+    void teacher_forced_logits(const int64_t* tokens, int64_t n_rows, int64_t seq_len, float* logits_out);
     void step_beams(int64_t n_rows, const int32_t* window_of_row, const int32_t* parent_row, const int64_t* token,
                     int apply_mask, int k, int64_t* topk_ids_out, float* topk_lp_out);
     // the [n_rows][k] candidates the last launch wrote at its last position

@@ -61,34 +61,10 @@ struct BeamSearchToken {   // transcribe.rs:142-146 (+ the cache row that produc
 };
 using Node = beam::BeamNode<BeamSearchToken>;
 
-}  // namespace
-
-void transcribe_windows(Session& s, int beam_size, int max_depth, const wb_special_ids& ids, const uint8_t* is_special,
-                        std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp) {
-    const bool loop = s.search == WB_SEARCH_GREEDY_LOOP;
-    WB_REQUIRE(!loop || beam_size == 1, "transcribe: the greedy loop takes beam_size 1");
-    WB_REQUIRE(beam_size >= 1 && beam_size <= s.max_beams, "transcribe: beam_size exceeds the session's max_beams");
-    WB_REQUIRE(max_depth >= 0, "transcribe: negative max_depth");
-    const int V = s.m->dims.n_vocab;
-    const int64_t prompt[4] = {ids.sot, ids.lang, ids.transcribe, ids.notimestamps};   // transcribe.rs:203
-    for (int64_t t : prompt) WB_REQUIRE(t >= 0 && t < V, "transcribe: special id out of range");
-    WB_REQUIRE(ids.eot >= 0 && ids.eot < V, "transcribe: eot id out of range");
-    WB_REQUIRE(4 + max_depth <= s.t_max, "transcribe: 4 + max_depth exceeds the session's max_text_len");
-    s.set_special(is_special);
+// the beam search on the host, all windows in lock-step, one decoder launch per depth (Session::step_beams)
+void host_beam_search(Session& s, const int64_t (&prompt)[4], int beam_size, int max_depth, int64_t eot,
+                      std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp) {
     const int W = s.n_windows;
-    if (beam_size == 1) {   // greedy: beam_size 1 of the search, or the greedy loop (transcribe.rs:314-380)
-        s.greedy_decode(prompt, 4, max_depth, ids.eot, out, out_lp, loop);
-        WB_CUDA(cudaEventRecord(s.ev[3], s.st));
-        return;
-    }
-    // ---- beam search: on the device in one launch where decoder6 covers it (fp16-exact weights, d = 128 / 384,
-    // n_windows * beam_size <= 24, t_max <= 128), same selection rules and ids as the host search below
-    if (max_depth > 0 && s.beam_decode(prompt, 4, beam_size, max_depth, ids.eot, out, out_lp)) {
-        WB_CUDA(cudaEventRecord(s.ev[3], s.st));
-        return;
-    }
-    // ---- otherwise the host search, all windows in lock-step
-    const int64_t eot = ids.eot;
     auto is_finished = [eot](const std::vector<BeamSearchToken>& seq) { return !seq.empty() && seq.back().token == eot; };
     std::vector<std::vector<Node>> beams((size_t)W);
     std::vector<char> done((size_t)W, 0);
@@ -170,6 +146,28 @@ void transcribe_windows(Session& s, int beam_size, int max_depth, const wb_speci
                 out_lp[(size_t)w].push_back((float)t.log_prob);   // exact: a widened f32 (transcribe.rs:291-299)
             }
     }
+}
+
+}  // namespace
+
+void transcribe_windows(Session& s, int beam_size, int max_depth, const wb_special_ids& ids, const uint8_t* is_special,
+                        std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp) {
+    const bool loop = s.search == WB_SEARCH_GREEDY_LOOP;
+    WB_REQUIRE(!loop || beam_size == 1, "transcribe: the greedy loop takes beam_size 1");
+    WB_REQUIRE(beam_size >= 1 && beam_size <= s.max_beams, "transcribe: beam_size exceeds the session's max_beams");
+    WB_REQUIRE(max_depth >= 0, "transcribe: negative max_depth");
+    const int V = s.m->dims.n_vocab;
+    const int64_t prompt[4] = {ids.sot, ids.lang, ids.transcribe, ids.notimestamps};   // transcribe.rs:203
+    for (int64_t t : prompt) WB_REQUIRE(t >= 0 && t < V, "transcribe: special id out of range");
+    WB_REQUIRE(ids.eot >= 0 && ids.eot < V, "transcribe: eot id out of range");
+    WB_REQUIRE(4 + max_depth <= s.t_max, "transcribe: 4 + max_depth exceeds the session's max_text_len");
+    s.set_special(is_special);
+    if (beam_size == 1)   // greedy: beam_size 1 of the search, or the greedy loop (transcribe.rs:314-380)
+        s.greedy_decode(prompt, 4, max_depth, ids.eot, out, out_lp, loop);
+    // beam search: on the device in one launch where decoder6 covers it (fp16-exact weights, d = 128 / 384,
+    // n_windows * beam_size <= 24, t_max <= 128), same selection rules and ids as the host search
+    else if (max_depth == 0 || !s.beam_decode(prompt, 4, beam_size, max_depth, ids.eot, out, out_lp))
+        host_beam_search(s, prompt, beam_size, max_depth, ids.eot, out, out_lp);
     WB_CUDA(cudaEventRecord(s.ev[3], s.st));
 }
 
