@@ -7,8 +7,9 @@
 //     so every stage reads its input from LOCAL shared memory;
 //   * stages are separated by the hardware cluster barrier (barrier.cluster arrive.release / wait.acquire,
 //     ~0.2 us) instead of the 1.3 us grid barrier through L2 (decoder3.cu: 34 per step);
-//   * the weight rows a warp needs for the NEXT stage are loaded into registers BEFORE the barrier (they do
-//     not depend on activations), so after the barrier a stage is LayerNorm + FMAs on on-chip data;
+//   * weights do not depend on activations: the CTA's rows of the large matrices (Wqkv, W1, W2) are bulk-copied into
+//     shared memory stages ahead, the small ones' rows loaded into registers BEFORE the barrier, so after the barrier
+//     a stage is LayerNorm + FMAs on on-chip data;
 //   * every CTA keeps its own copy of the row's residual stream x and applies the broadcast deltas itself.
 // Only the vocabulary projection is chip-wide: x rows are published, a grid barrier, all 128 CTAs stream the
 // tied-embedding matrix (fused mask / online softmax / top candidates), a grid barrier, one CTA per row
@@ -77,21 +78,30 @@ __device__ __forceinline__ uint64_t ckv_policy() { return D4_L2_CKV_KEEP ? l2_po
 __device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
 __device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 
-template <int NR, int VPL>
-struct RowRegs {
-    uint4 v[NR][VPL];
-    float bias[NR];   // fetched together with the rows, before the barrier
+template <int NR>
+struct RowBias {
+    float bias[NR];   // fetched before the barrier
     float bias_own;   // bias of row (lane >> 1): the row whose sum warp_reduce_owner leaves in this lane
 };
+template <int NR, int VPL>
+struct RowRegs : RowBias<NR> {
+    uint4 v[NR][VPL];
+};
 
+// biases of rows row0, row0 + step, ... -> registers
+template <int NR>
+__device__ __forceinline__ void load_bias(const float* __restrict__ bias, int row0, int step, RowBias<NR>& r) {
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int i = 0; i < NR; ++i) r.bias[i] = __ldg(bias + row0 + i * step);
+    r.bias_own = __ldg(bias + row0 + min(lane >> 1, NR - 1) * step);
+}
 // rows row0, row0 + step, ... of W[.][K] (fp16) -> registers; lane-strided 16-byte vectors
 template <int NR, int VPL>
 __device__ __forceinline__ void load_rows(const __half* __restrict__ W, const float* __restrict__ bias, int K, int row0, int step,
                                           RowRegs<NR, VPL>& r, uint64_t pol) {
     const int lane = threadIdx.x & 31, nv = K / 8;
-#pragma unroll
-    for (int i = 0; i < NR; ++i) r.bias[i] = __ldg(bias + row0 + i * step);
-    r.bias_own = __ldg(bias + row0 + min(lane >> 1, NR - 1) * step);
+    load_bias<NR>(bias, row0, step, r);
 #pragma unroll
     for (int i = 0; i < NR; ++i) {
         const uint4* p = reinterpret_cast<const uint4*>(W + (int64_t)(row0 + i * step) * K);
@@ -141,8 +151,9 @@ __device__ __forceinline__ float warp_reduce_owner(const float (&acc)[NR]) {
     return v;
 }
 
-template <int NR, int VPL, bool REDUCE = true>
-__device__ __forceinline__ void dot_rows1(const RowRegs<NR, VPL>& r, const float* xs, int K, float (&acc)[NR]) {
+// wv(i, j): 16-byte vector j * 32 + lane of the warp's row i
+template <int NR, int VPL, bool REDUCE, typename WV>
+__device__ __forceinline__ void dot_rows(WV&& wv, const float* xs, int K, float (&acc)[NR]) {
     const int lane = threadIdx.x & 31, nv = K / 8;
 #pragma unroll
     for (int i = 0; i < NR; ++i) acc[i] = 0.0f;
@@ -155,7 +166,7 @@ __device__ __forceinline__ void dot_rows1(const RowRegs<NR, VPL>& r, const float
 #pragma unroll
             for (int i = 0; i < NR; ++i) {
                 float w[8];
-                cvt8(r.v[i][j], w);
+                cvt8(wv(i, j), w);
                 float a = acc[i];
                 a = fmaf(w[0], x0.x, a); a = fmaf(w[1], x0.y, a); a = fmaf(w[2], x0.z, a); a = fmaf(w[3], x0.w, a);
                 a = fmaf(w[4], x1.x, a); a = fmaf(w[5], x1.y, a); a = fmaf(w[6], x1.z, a); a = fmaf(w[7], x1.w, a);
@@ -167,6 +178,26 @@ __device__ __forceinline__ void dot_rows1(const RowRegs<NR, VPL>& r, const float
 #pragma unroll
         for (int i = 0; i < NR; ++i) acc[i] = warp_sum(acc[i]);
     }
+}
+// the warp's rows from registers (load_rows)
+template <int NR, int VPL, bool REDUCE = true>
+__device__ __forceinline__ void dot_rows1(const RowRegs<NR, VPL>& r, const float* xs, int K, float (&acc)[NR]) {
+    dot_rows<NR, VPL, REDUCE>([&](int i, int j) { return r.v[i][j]; }, xs, K, acc);
+}
+// the same rows from shared memory: ws is the CTA's slice [NR * NW][K] (bulk_rows), row i of warp w is row w + i * NW
+template <int NR, int VPL, bool REDUCE = true>
+__device__ __forceinline__ void dot_rows1s(const uint8_t* ws, const float* xs, int K, float (&acc)[NR]) {
+    const int lane = threadIdx.x & 31, nv = K / 8;
+    const uint4* w = reinterpret_cast<const uint4*>(ws) + (threadIdx.x >> 5) * nv;
+    dot_rows<NR, VPL, REDUCE>([&](int i, int j) { return w[i * NW * nv + j * 32 + lane]; }, xs, K, acc);
+}
+// rows [row0, row0 + n) of W[.][K] (fp16, one contiguous block) -> shared memory at dst: one bulk copy, completing on bar.
+// Called by one thread; fence_proxy_async() orders the CTA's generic reads of dst (before a barrier) ahead of the copy.
+__device__ __forceinline__ void bulk_rows(uint8_t* dst, const __half* W, int K, int row0, int n, uint64_t* bar) {
+    const uint32_t bytes = (uint32_t)n * K * 2;
+    fence_proxy_async();
+    mbar_expect_tx(bar, bytes);
+    bulk_g2s_l2(dst, W + (int64_t)row0 * K, bytes, bar, l2_policy_evict_last());
 }
 
 // 16 bytes -> shared memory of another CTA of the cluster, completing 16 transaction bytes on that CTA's mbarrier
@@ -311,13 +342,30 @@ dec4_kernel(const DecArgs a) {
     uint64_t* lg_bar = reinterpret_cast<uint64_t*>(ring + (size_t)NW * RINGW);   // [NW][LG_NBUF]
     uint64_t* kv_bar = lg_bar + NW * LG_NBUF;   // [NW][KV_STG] cross-attention K/V ring (aliases the logits ring: different stages)
     uint64_t* xbar = kv_bar + NW * KV_STG;      // [8] stage exchange barriers (D4_ASYNC): transaction bytes sent by the 16 CTAs of the cluster
-    uint4* pl_hi = reinterpret_cast<uint4*>(xbar + 8);   // logits stage: fragment-order fp16 hi plane of the 8 (padded) LayerNorm rows [D/32][32]
+    uint64_t* wt_bar = xbar + 8;                // [3] this CTA's Wqkv / W1 / W2 rows in the ring (each copy completes once per layer)
+    uint4* pl_hi = reinterpret_cast<uint4*>(wt_bar + 4);   // logits stage: fragment-order fp16 hi plane of the 8 (padded) LayerNorm rows [D/32][32]
     uint4* pl_lo = pl_hi + (D / 32) * 32;                           // same, residual * 2^11
+    // The large layer matrices come from shared memory (DESIGN.md section 5): this CTA's rows of Wqkv, W1 and W2 are one
+    // contiguous block each, bulk-copied into the ring while it is otherwise idle.  Timeline of the ring within a layer:
+    //   S1      Wqkv [QKV_OFF, +QKV_B)                  (issued during S7 of the previous layer, or after the vocabulary loop)
+    //   S1-S2   self K/V staging, first 8 KB of each warp's RINGW
+    //   S3-S5   cross K/V ring, first 16 KB of each warp's RINGW
+    //   S5-S7   W1 [W1_OFF, +W1_B)                      (issued when S5's cross attention has released the ring)
+    //   S5-S8   W2 [W2_OFF, +W2_B)                      (same)
+    //   S7-S1   next layer's Wqkv                       (issued when S7 has read W1; W2 is still being read)
+    //   last layer, logits positions: the vocabulary half-tiles take the whole ring once S8 has read W2
+    constexpr int QKV_B = 3 * D / CS * D * 2, W1_B = 4 * D / CS * D * 2, W2_B = D / CS * 4 * D * 2;
+    constexpr int QKV_OFF = 0, W1_OFF = 0, W2_OFF = W1_OFF + W1_B;
+    static_assert(W2_OFF + W2_B <= NW * RINGW, "W1 and W2 must fit the ring");
+    static_assert(QKV_OFF + QKV_B <= W2_OFF, "the next layer's Wqkv arrives while W2 is read: no overlap");
+    static_assert(QKV_B % 16 == 0 && W1_B % 16 == 0 && W2_B % 16 == 0 && W2_OFF % 16 == 0, "bulk copies move 16-byte units");
     if (lane == 0) {
         for (int j = 0; j < KV_STG; ++j) mbar_init(kv_bar + warp * KV_STG + j, 1);
         for (int j = 0; j < LG_NBUF; ++j) mbar_init(lg_bar + warp * LG_NBUF + j, 1);
-        if (warp == 0)
+        if (warp == 0) {
             for (int j = 0; j < 8; ++j) mbar_init(xbar + j, 1);
+            for (int j = 0; j < 3; ++j) mbar_init(wt_bar + j, 1);
+        }
         mbar_fence_init();
     }
     cl.sync();                   // every CTA's stage barriers exist before the first remote store can target them
@@ -328,6 +376,10 @@ dec4_kernel(const DecArgs a) {
     unsigned int lstep = 0;      // vocabulary steps this launch has finished (ticket / flag bookkeeping)
     int tr_n = 0;
     const float scale = a.qk_scale;
+    // this CTA's rows of layer l's Wqkv -> the ring (thread 0: every reader of the region is behind a barrier)
+    auto issue_qkv = [&](int l) {
+        if (tid == 0) bulk_rows(ring + QKV_OFF, reinterpret_cast<const __half*>(a.layers[l].Wqkv), D, rank * (3 * D / CS), 3 * D / CS, wt_bar + 0);
+    };
     // L2 plan (DESIGN.md section 5): the layer weights, LayerNorm parameters and self K/V are re-read at every position and
     // kept (evict_last); the vocabulary half-tiles and is_special are read once per position and go first (evict_first);
     // cross K/V follows D4_L2_CKV_KEEP; biases keep normal priority.
@@ -412,8 +464,9 @@ dec4_kernel(const DecArgs a) {
 #pragma unroll
                 for (int k = 0; k < PF; ++k) reinterpret_cast<float4*>(xb)[lane + 32 * k] = x.v[k];
             }
-            RowRegs<NR_QKV, VPL> w_qkv;
-            load_rows<NR_QKV, VPL>(reinterpret_cast<const __half*>(a.layers[0].Wqkv), a.layers[0].bqkv, D, rank * (3 * D / CS) + warp, NW, w_qkv, l2_policy_evict_last());
+            RowBias<NR_QKV> b_qkv;
+            load_bias<NR_QKV>(a.layers[0].bqkv, rank * (3 * D / CS) + warp, NW, b_qkv);
+            if (step == 0) issue_qkv(0);   // later steps: issued by the previous step (last layer, or after its vocabulary loop)
             if (step == 0) ln_fetch<D, PF>(lnp, a.layers[0].ln1_g, a.layers[0].ln1_b, l2_policy_evict_last());   // later steps: fetched by the previous step's last layer
             __syncthreads();
             for (int l = 0; l < L; ++l) {
@@ -429,16 +482,17 @@ dec4_kernel(const DecArgs a) {
                 ln_fetch<D, PF>(lnp, W.ln2_g, W.ln2_b, l2_policy_evict_last());
                 {
                     float acc[NR_QKV];
-                    dot_rows1<NR_QKV, VPL, false>(w_qkv, xn_s, D, acc);
+                    mbar_wait(wt_bar + 0, lc & 1u);
+                    dot_rows1s<NR_QKV, VPL, false>(ring + QKV_OFF, xn_s, D, acc);
                     float mine = warp_reduce_owner<NR_QKV>(acc);   // lanes 2i, 2i+1: sum of row i
-                    mine = __fadd_rn(mine, w_qkv.bias_own);
+                    mine = __fadd_rn(mine, b_qkv.bias_own);
                     const int j = warp + (lane >> 1) * NW;          // index inside this CTA's slice
                     if (rank * (3 * D / CS) + j < 2 * D) mine = __fmul_rn(mine, scale);
                     if (!(lane & 1) && (lane >> 1) < NR_QKV) stg_s[j] = mine;
                 }
                 RowRegs<NR_D, VPL> w_o;
                 // self attention (next stage): the cached positions j < p of this head are copied (asynchronously, lane-private
-                // slots of this warp's ring, free until the cross K/V prefill of S3) ahead of their use -- they are from earlier
+                // slots of this warp's ring, free from S1's read of Wqkv until the cross K/V prefill of S3) ahead of their use -- they are from earlier
                 // steps; position p itself is taken from the broadcast q|k|v row afterwards.  Key j = warp + NW*(u*8+sub).
                 constexpr int SNV = sizeof(KVT) == 4 ? 4 : 2;   // 16-byte vectors per lane and tensor (16 dims)
                 uint8_t* sring = ring + (size_t)warp * RINGW;
@@ -562,7 +616,9 @@ dec4_kernel(const DecArgs a) {
                 RowRegs<NR_D, VPL> w_cq;
                 auto pre_s4 = [&]() {
                     load_rows<NR_D, VPL>(reinterpret_cast<const __half*>(W.Wcq), W.bcq, D, rank * (D / CS) + warp, NW, w_cq, l2_policy_evict_last());
-                    // first batches of this layer's cross K/V: static data, two barriers ahead of its use
+                    // first batches of this layer's cross K/V: static data, two barriers ahead of its use; the ring held Wqkv and
+                    // the self K/V (generic reads before the barrier)
+                    fence_proxy_async();
                     attn_bulk_prefill<KV_STG, KVT, true>(reinterpret_cast<const KVT*>(a.ckv) + (size_t)l * a.Mcap * 2 * D + xoff, xT, xci * NW + warp,
                                                          xnch * NW, ring + (size_t)warp * RINGW, kv_bar + warp * KV_STG, kv_count, ckv_policy());
                 };
@@ -598,12 +654,6 @@ dec4_kernel(const DecArgs a) {
                     AttnAcc A;
                     attn_warp_bulk<KV_STG, KVT, true>(q2_s + h * 64, kbase, T, ci * NW + warp, nch * NW, 0, ring + (size_t)warp * RINGW,
                                                       kv_bar + warp * KV_STG, kv_count, A, true, ckv_policy());
-                    if (l == L - 1 && want_logits) {   // the ring is free until the next position: first vocabulary half-tiles of this warp
-                        __syncwarp();
-                        fence_proxy_async();   // generic reads of the ring before the bulk copies
-#pragma unroll
-                        for (int j = 0; j < LG_NBUF; ++j) issue(j);
-                    }
                     if (lane < 4) {
 #pragma unroll
                         for (int c = 0; c < 16; ++c) wo[warp * 64 + attn_bulk_dim<KVT>(lane, c)] = A.o[c];
@@ -627,7 +677,13 @@ dec4_kernel(const DecArgs a) {
                     }
                 }
                 auto send_s5 = [&]() { put_slice<68>(cl, stg_s, part_s + rank * 68, xbar + 4); };
-                D4_EXCHANGE(4, CS * 68 * 4, send_s5, pf_none);
+                auto pre_mlp = [&]() {   // the cross K/V ring is drained: this CTA's W1 and W2 rows, two and three stages ahead
+                    if (tid == 0) {
+                        bulk_rows(ring + W1_OFF, reinterpret_cast<const __half*>(W.W1), D, rank * (4 * D / CS), 4 * D / CS, wt_bar + 1);
+                        bulk_rows(ring + W2_OFF, reinterpret_cast<const __half*>(W.W2), 4 * D, rank * (D / CS), D / CS, wt_bar + 2);
+                    }
+                };
+                D4_EXCHANGE(4, CS * 68 * 4, send_s5, pre_mlp);
                 WB_TRACE();
                 // ================= S6: merge the head partials, delta = cross Wco + bco
                 for (int c = tid; c < D; c += NT) {
@@ -652,8 +708,8 @@ dec4_kernel(const DecArgs a) {
                         for (int i = 0; i < NR_D; ++i) stg_s[warp + i * NW] = __fadd_rn(acc[i], w_co.bias[i]);
                     }
                 }
-                RowRegs<NR_H, VPL> w_1;
-                auto pre_s7 = [&]() { load_rows<NR_H, VPL>(reinterpret_cast<const __half*>(W.W1), W.b1, D, rank * (4 * D / CS) + warp, NW, w_1, l2_policy_evict_last()); };
+                RowBias<NR_H> b_1;
+                auto pre_s7 = [&]() { load_bias<NR_H>(W.b1, rank * (4 * D / CS) + warp, NW, b_1); };
                 auto send_s6 = [&]() { put_slice<D / CS>(cl, stg_s, dl_s + rank * (D / CS), xbar + 5); };
                 D4_EXCHANGE(5, D * 4, send_s6, pre_s7);
                 WB_TRACE();
@@ -670,30 +726,42 @@ dec4_kernel(const DecArgs a) {
                 WB_FINE();
                 {
                     float acc[NR_H];
-                    dot_rows1<NR_H, VPL, false>(w_1, xn_s, D, acc);
+                    mbar_wait(wt_bar + 1, lc & 1u);
+                    dot_rows1s<NR_H, VPL, false>(ring + W1_OFF, xn_s, D, acc);
                     // lanes 2i, 2i+1 end up with the sum of row i: ONE erf-GELU per row instead of one per lane and row
                     float mine = warp_reduce_owner<NR_H>(acc);
-                    mine = gelu_erf(__fadd_rn(mine, w_1.bias_own));
+                    mine = gelu_erf(__fadd_rn(mine, b_1.bias_own));
                     WB_FINE();
                     if (!(lane & 1) && (lane >> 1) < NR_H) stg_s[warp + (lane >> 1) * NW] = mine;
                 }
-                RowRegs<NR_D, VPL4> w_2;
-                auto pre_s8 = [&]() { load_rows<NR_D, VPL4>(reinterpret_cast<const __half*>(W.W2), W.b2, 4 * D, rank * (D / CS) + warp, NW, w_2, l2_policy_evict_last()); };
+                RowBias<NR_D> b_2;
+                auto pre_s8 = [&]() {
+                    load_bias<NR_D>(W.b2, rank * (D / CS) + warp, NW, b_2);
+                    // W1 is read: the next layer's Wqkv (or layer 0's for the next position when this one has no vocabulary stage)
+                    if (l + 1 < L) issue_qkv(l + 1);
+                    else if (!want_logits && step + 1 < a.n_steps) issue_qkv(0);
+                };
                 auto send_s7 = [&]() { put_slice<4 * D / CS>(cl, stg_s, hid_s + rank * (4 * D / CS), xbar + 6); };
                 D4_EXCHANGE(6, 4 * D * 4, send_s7, pre_s8);
                 WB_TRACE();
                 // ================= S8: delta = hid W2 + b2
                 {
                     float acc[NR_D];
-                    dot_rows1<NR_D, VPL4>(w_2, hid_s, 4 * D, acc);
+                    mbar_wait(wt_bar + 2, lc & 1u);
+                    dot_rows1s<NR_D, VPL4>(ring + W2_OFF, hid_s, 4 * D, acc);
                     if (lane == 0) {
 #pragma unroll
-                        for (int i = 0; i < NR_D; ++i) stg_s[warp + i * NW] = __fadd_rn(acc[i], w_2.bias[i]);
+                        for (int i = 0; i < NR_D; ++i) stg_s[warp + i * NW] = __fadd_rn(acc[i], b_2.bias[i]);
                     }
                 }
                 auto pre_s1 = [&]() {
-                    if (l + 1 < L)
-                        load_rows<NR_QKV, VPL>(reinterpret_cast<const __half*>(a.layers[l + 1].Wqkv), a.layers[l + 1].bqkv, D, rank * (3 * D / CS) + warp, NW, w_qkv, l2_policy_evict_last());
+                    if (l + 1 < L) {
+                        load_bias<NR_QKV>(a.layers[l + 1].bqkv, rank * (3 * D / CS) + warp, NW, b_qkv);
+                    } else if (want_logits) {   // W2 is read, the ring is free until the next position: first vocabulary half-tiles of this warp
+                        fence_proxy_async();    // generic reads of the ring before the bulk copies
+#pragma unroll
+                        for (int j = 0; j < LG_NBUF; ++j) issue(j);
+                    }
                 };
                 auto send_s8 = [&]() { put_slice<D / CS>(cl, stg_s, dl_s + rank * (D / CS), xbar + 7); };
                 D4_EXCHANGE(7, D * 4, send_s8, pre_s1);
@@ -802,6 +870,7 @@ dec4_kernel(const DecArgs a) {
                 }
             }
             __syncthreads();
+            if (active && step + 1 < a.n_steps) issue_qkv(0);   // every warp has drained its ring: layer 0's Wqkv for the next position
             if (tid < R) fold_records_top1(a, red + tid * 4, NW, 8 * 4, (int64_t)blockIdx.x * R + tid);
         }
         WB_TRACE();
@@ -824,6 +893,7 @@ dec4_kernel(const DecArgs a) {
         __syncthreads();
         WB_TRACE();
         if (rows_open(a) == 0) {
+            if (active && tid == 0 && step + 1 < a.n_steps) mbar_wait(wt_bar + 0, lc & 1u);   // no bulk copy outlives the CTA
             if (blockIdx.x == 0 && tid == 0) decode_done(a, p + 1, 0, step + 1);
             demote();   // every CTA is past the flag: no evict_last load is left
             return;
@@ -836,10 +906,11 @@ dec4_kernel(const DecArgs a) {
 }
 
 template <int D, int RC>
-size_t dec4_smem() {
+constexpr size_t dec4_smem() {
     return sizeof(float) * ((size_t)(2 * NW + 13) * D + (4 * D / CS > 68 ? 4 * D / CS : 68) + CS * 68 + 2 * NW + NW * 64 + 64 + 4 + (size_t)NW * 4 * RC * 6 + 16) +
-           (size_t)NW * std::max(LG_NBUF * LG_RB * D * 2, KV_STG * 8 * 128 * 4) + NW * LG_NBUF * 8 + NW * KV_STG * 8 + 8 * 8 + (size_t)2 * (D / 32) * 32 * 16 + 16;
+           (size_t)NW * std::max(LG_NBUF * LG_RB * D * 2, KV_STG * 8 * 128 * 4) + NW * LG_NBUF * 8 + NW * KV_STG * 8 + 8 * 8 + 4 * 8 + (size_t)2 * (D / 32) * 32 * 16 + 16;
 }
+static_assert(dec4_smem<384, 8>() <= 227 * 1024 && dec4_smem<384, 4>() <= 227 * 1024, "dec4_kernel exceeds the shared memory of an sm_90 CTA");
 
 template <int D, int RC, typename KVT>
 bool launch4_t(const DecArgs& a, cudaStream_t st) {
