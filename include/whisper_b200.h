@@ -13,6 +13,7 @@
  *   Whisper::forward_decoder           src/model/mod.rs:56-62      -> wb_forward_decoder
  *   Whisper::{encoder,decoder}_ctx_size src/model/mod.rs:64-70     -> wb_model_get_dims
  *   beamsearch_next closure            src/transcribe.rs:253-307   -> wb_session_step (KV-cached, top-k only)
+ *   forward_decoder + log_softmax      mod.rs:131-157, transcribe.rs:276 -> wb_session_score_tokens (every position)
  *   beam::beam_search(_step)           src/beam.rs:9-79            -> wb_beam_* (host C++, same tie-breaks)
  *   mels_to_text (token part)          src/transcribe.rs:148-383   -> wb_transcribe_windows
  *   waveform_to_text (token part)      src/transcribe.rs:23-74     -> wb_waveform_to_tokens
@@ -230,6 +231,20 @@ int wb_waveforms_to_tokens(wb_session* s, const float* const* waveforms, const i
  *     repetition cut, context stop);
  *   - wb_waveform(s)_to_tokens: each log-prob travels with its id through the overlap merge (transcribe.rs:56-63). */
 int wb_session_last_logprobs(wb_session* s, int64_t index, float* out, int64_t capacity, int64_t* n_out);
+/* Teacher-forced scoring of n_seqs token sequences against windows this session has encoded:
+ * forward_decoder (mod.rs:131-157) + log_softmax (transcribe.rs:276) at every position, in one pass on the GPU.
+ * Sequence i is tokens[off_i .. off_i + lens[i]) with off_i = lens[0] + .. + lens[i-1], on window window_of_seq[i].
+ * For j >= 1:  lp_out[off_i + j]     = log_softmax(logits of position j-1)[tokens[off_i + j]]   (f32)
+ *              argmax_out[off_i + j] = arg-max id of that row, ties to the lower id               (argmax_out may be NULL)
+ * and lp_out[off_i] = 0, argmax_out[off_i] = -1.
+ * apply_special_mask != 0 adds -inf on is_special ids to the rows whose prefix has <= 5 tokens (j <= 5; the beam rule of
+ * transcribe.rs:271-275), so a masked target scores -inf.  Several sequences may share a window.
+ * WB_ERR_STATE before an encode call; WB_ERR_INVALID_ARG for lens[i] outside [1, n_text_ctx], a token outside [0, n_vocab),
+ * a window outside the encoded ones, or apply_special_mask without is_special; WB_ERR_UNSUPPORTED when the weights are not
+ * fp16-exact.  Leaves the session's decode state and every wb_session_last_* result as they were. */
+int wb_session_score_tokens(wb_session* s, int64_t n_seqs, const int32_t* window_of_seq, const int64_t* tokens,
+                            const int64_t* lens, int apply_special_mask, const uint8_t* is_special,
+                            float* lp_out, int64_t* argmax_out);
 /* transcribe.rs:114-138: number of windows and their [start, end) bounds */
 int64_t wb_window_count(int64_t n_samples, int64_t sample_rate, int64_t window_len);
 int wb_window_bounds(int64_t n_samples, int64_t sample_rate, int64_t window_len, int64_t* starts, int64_t* ends);

@@ -58,6 +58,9 @@ pub mod ffi {
         pub fn wb_waveform_to_tokens(s: *mut c_void, waveform: *const f32, n_samples: i64, sample_rate: i64, beam_size: c_int, max_depth: c_int,
                                      ids: *const wb_special_ids, is_special: *const u8, tokens_out: *mut i64, capacity: i64, n_tokens_out: *mut i64) -> c_int;
         pub fn wb_session_last_logprobs(s: *mut c_void, index: i64, out: *mut f32, capacity: i64, n_out: *mut i64) -> c_int;
+        pub fn wb_session_encode_waveforms(s: *mut c_void, waves: *const *const f32, lens: *const i64, n_windows: i64) -> c_int;
+        pub fn wb_session_score_tokens(s: *mut c_void, n_seqs: i64, window_of_seq: *const i32, tokens: *const i64, lens: *const i64,
+                                       apply_special_mask: c_int, is_special: *const u8, lp_out: *mut f32, argmax_out: *mut i64) -> c_int;
     }
 }
 
@@ -283,6 +286,26 @@ pub mod transcribe {
         })?;
         assert_eq!(n, n_lp, "one log-prob per token");
         Ok((0..n as usize).map(|i| BeamSearchToken { token: out[i] as usize, log_prob: lps[i] as f64 }).collect())
+    }
+
+    /// How well given token sequences fit one audio window: `forward_decoder` (mod.rs:131-157) and `log_softmax`
+    /// (transcribe.rs:276) at every position, without the special-token mask.  The window (at most
+    /// max_waveform_samples(n_audio_ctx - 10) samples) is encoded in the cached session, then every sequence is scored in one
+    /// pass on the GPU (wb_session_score_tokens): entry j of a sequence's result is the log-prob of its token j given tokens
+    /// 0 .. j-1, entry 0 is 0.0.
+    pub fn score_tokens(whisper: &model::Whisper, waveform_window: &[f32], sequences: &[Vec<usize>]) -> Result<Vec<Vec<f64>>, Error> {
+        let lens: Vec<i64> = sequences.iter().map(|q| q.len() as i64).collect();
+        let tokens: Vec<i64> = sequences.iter().flatten().map(|&t| t as i64).collect();
+        let windows = vec![0i32; sequences.len()];
+        let mut lp = vec![0f32; tokens.len().max(1)];
+        whisper.with_session(1, 1, 2, |s| {
+            let (wave, n) = (waveform_window.as_ptr(), waveform_window.len() as i64);
+            check(unsafe { ffi::wb_session_encode_waveforms(s, &wave, &n, 1) })?;
+            check(unsafe { ffi::wb_session_score_tokens(s, sequences.len() as i64, windows.as_ptr(), tokens.as_ptr(), lens.as_ptr(), 0,
+                                                        std::ptr::null(), lp.as_mut_ptr(), std::ptr::null_mut()) })
+        })?;
+        let mut off = 0;
+        Ok(sequences.iter().map(|q| { let r = lp[off..off + q.len()].iter().map(|&x| x as f64).collect(); off += q.len(); r }).collect())
     }
 
     /// The greedy loop the reference leaves commented out in `mels_to_text` (src/transcribe.rs:314-380), with waveform_to_text's

@@ -532,6 +532,14 @@ int wb_session_last_logprobs(wb_session* s, int64_t index, float* out, int64_t c
     });
 }
 
+int wb_session_score_tokens(wb_session* s, int64_t n_seqs, const int32_t* window_of_seq, const int64_t* tokens, const int64_t* lens,
+                            int apply_special_mask, const uint8_t* is_special, float* lp_out, int64_t* argmax_out) {
+    return guarded([&] {
+        WB_REQUIRE(s && window_of_seq && tokens && lens && lp_out, "score_tokens: null pointer");
+        s->impl->score_tokens(n_seqs, window_of_seq, tokens, lens, apply_special_mask != 0, is_special, lp_out, argmax_out);
+    });
+}
+
 int wb_find_chunk_overlap(const int64_t* prev, int64_t n_prev, const int64_t* curr, int64_t n_curr, int64_t max_n_offsets,
                           int64_t min_n_overlaps, int64_t* prev_index, int64_t* curr_index) {
     int64_t pi = 0, ci = 0;

@@ -20,11 +20,18 @@
 //               warpgroups' MMAs that read it have completed
 // The conv stems use the same kernel: their A rows are overlapping windows of a token-major buffer, expressed as a tensor map
 // whose row stride is smaller than the row length.
+//
+// Token scoring (score.cu) runs the same main loop over the tied token embedding (logits = x E^T, mod.rs:154-156) with a
+// statistics epilogue (LogitArgs) instead of writing the P x V logits: per (row, column tile) the tile max, the sum of
+// exp(x - tile max), the tile arg-max (lowest id on ties) and, in the tile that holds it, the row's target logit.  Columns
+// past V (zero-filled by TMA) and special ids of masked rows are excluded.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
+#include <climits>
 #include <cstring>
 #include <mutex>
+#include <type_traits>
 
 #include "prims.cuh"
 #include "wb_internal.h"
@@ -69,11 +76,68 @@ struct F16Args {
     float scale;
     int scale_cols;
 };
+struct LogitArgs : F16Args {
+    const int* target;          // [rows] id whose logit is gathered
+    const uint8_t* row_mask;    // [rows] 1: the row excludes special ids (null: no row does)
+    const uint8_t* is_special;  // [V]
+    int V, n_tiles;             // n_tiles = gridDim.x: the stride of the per-row tile statistics
+    float *tile_m, *tile_s, *tgt_logit;
+    int* tile_i;
+};
 
+// Statistics epilogue of the logits GEMM: the 4 lanes of a quad hold one row's BN / 4 columns per accumulator half
 template <int BN>
+__device__ __forceinline__ void logit_stats_epilogue(const float (&acc_h)[BN / 2], const float (&acc_l)[BN / 2], const LogitArgs& g, int rows,
+                                                     int m_base, int n0, int lane) {
+#pragma unroll
+    for (int hrow = 0; hrow < 2; ++hrow) {
+        const int m = m_base + 8 * hrow;
+        const bool live = m < rows;   // quad-uniform; every lane stays for the shuffles
+        const int mr = live ? m : 0;
+        const bool masked = g.row_mask != nullptr && g.row_mask[mr] != 0;
+        const int tgt = g.target[mr];
+        float mx = -INFINITY;
+        int ai = INT_MAX;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int n = n0 + 8 * j + 2 * (lane & 3) + e;
+                const float x = hl_join(acc_h[4 * j + 2 * hrow + e], acc_l[4 * j + 2 * hrow + e]);
+                if (live && n == tgt) g.tgt_logit[m] = x;
+                const bool ok = n < g.V && !(masked && __ldg(g.is_special + n));
+                if (ok && x > mx) { mx = x; ai = n; }   // ascending n: the lowest id of a tie stays
+            }
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1) {
+            const float om = __shfl_xor_sync(0xffffffffu, mx, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, ai, o);
+            if (om > mx || (om == mx && oi < ai)) { mx = om; ai = oi; }
+        }
+        float s = 0.0f;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int n = n0 + 8 * j + 2 * (lane & 3) + e;
+                const float x = hl_join(acc_h[4 * j + 2 * hrow + e], acc_l[4 * j + 2 * hrow + e]);
+                if (n < g.V && !(masked && __ldg(g.is_special + n))) s += expf(x - mx);
+            }
+        s += __shfl_xor_sync(0xffffffffu, s, 1);
+        s += __shfl_xor_sync(0xffffffffu, s, 2);
+        if (live && (lane & 3) == 0) {
+            const int64_t o = (int64_t)m * g.n_tiles + blockIdx.x;
+            g.tile_m[o] = mx;
+            g.tile_s[o] = s;
+            g.tile_i[o] = ai;
+        }
+    }
+}
+
+template <int BN, typename Args>
 __global__ void __launch_bounds__(F_THREADS, 1)
 gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-                   const __grid_constant__ CUtensorMap map_b, const F16Args g) {
+                   const __grid_constant__ CUtensorMap map_b, const Args g) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     constexpr int A_BYTES = F_BM * F_BK * 2;   // 16 KB per plane
     constexpr int B_BYTES = BN * F_BK * 2;
@@ -145,39 +209,43 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_co
     wgmma_fence_regs(acc_h);
     wgmma_fence_regs(acc_l);
 
-    // ===== epilogue.  Accumulator fragment of a m64nBN wgmma: register 4j + e of thread (warp w, lane) holds row
-    // 16 w + lane / 4 (+ 8 for e >= 2), column 8 j + 2 (lane % 4) + (e & 1).
+    if constexpr (std::is_same<Args, LogitArgs>::value) {
+        logit_stats_epilogue<BN>(acc_h, acc_l, g, grp.rows, m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), n0, lane);
+    } else {
+        // ===== epilogue.  Accumulator fragment of a m64nBN wgmma: register 4j + e of thread (warp w, lane) holds row
+        // 16 w + lane / 4 (+ 8 for e >= 2), column 8 j + 2 (lane % 4) + (e & 1).
 #pragma unroll
-    for (int hrow = 0; hrow < 2; ++hrow) {
-        const int m = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * hrow;
-        if (m >= grp.rows) continue;
-        const int64_t crow = grp.c_off + (int64_t)m * g.ldc;
+        for (int hrow = 0; hrow < 2; ++hrow) {
+            const int m = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * hrow;
+            if (m >= grp.rows) continue;
+            const int64_t crow = grp.c_off + (int64_t)m * g.ldc;
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-            const int n = n0 + 8 * j + 2 * (lane & 3);
-            float v[2];
+            for (int j = 0; j < BN / 8; ++j) {
+                const int n = n0 + 8 * j + 2 * (lane & 3);
+                float v[2];
 #pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                float t = hl_join(acc_h[4 * j + 2 * hrow + e], acc_l[4 * j + 2 * hrow + e]);
-                if (g.bias) t = __fadd_rn(t, __ldg(g.bias + n + e));
-                if (g.act == ACT_GELU) t = gelu_erf(t);
-                if (n + e < g.scale_cols) t = __fmul_rn(t, g.scale);
-                v[e] = t;
-            }
-            if (g.pos) {
-                const float2 p2 = __ldg(reinterpret_cast<const float2*>(g.pos + (int64_t)m * g.N + n));
-                v[0] = __fadd_rn(v[0], p2.x); v[1] = __fadd_rn(v[1], p2.y);
-            }
-            if (g.residual) {
-                const float2 r2 = *reinterpret_cast<const float2*>(g.residual + crow + n);
-                v[0] = __fadd_rn(r2.x, v[0]); v[1] = __fadd_rn(r2.y, v[1]);
-            }
-            if (g.C) *reinterpret_cast<float2*>(g.C + crow + n) = make_float2(v[0], v[1]);
-            if (g.P_hi) {
-                __half2 h, l;
-                hl_split_pair(v[0], v[1], h, l);
-                *reinterpret_cast<__half2*>(g.P_hi + crow + n) = h;
-                *reinterpret_cast<__half2*>(g.P_lo + crow + n) = l;
+                for (int e = 0; e < 2; ++e) {
+                    float t = hl_join(acc_h[4 * j + 2 * hrow + e], acc_l[4 * j + 2 * hrow + e]);
+                    if (g.bias) t = __fadd_rn(t, __ldg(g.bias + n + e));
+                    if (g.act == ACT_GELU) t = gelu_erf(t);
+                    if (n + e < g.scale_cols) t = __fmul_rn(t, g.scale);
+                    v[e] = t;
+                }
+                if (g.pos) {
+                    const float2 p2 = __ldg(reinterpret_cast<const float2*>(g.pos + (int64_t)m * g.N + n));
+                    v[0] = __fadd_rn(v[0], p2.x); v[1] = __fadd_rn(v[1], p2.y);
+                }
+                if (g.residual) {
+                    const float2 r2 = *reinterpret_cast<const float2*>(g.residual + crow + n);
+                    v[0] = __fadd_rn(r2.x, v[0]); v[1] = __fadd_rn(r2.y, v[1]);
+                }
+                if (g.C) *reinterpret_cast<float2*>(g.C + crow + n) = make_float2(v[0], v[1]);
+                if (g.P_hi) {
+                    __half2 h, l;
+                    hl_split_pair(v[0], v[1], h, l);
+                    *reinterpret_cast<__half2*>(g.P_hi + crow + n) = h;
+                    *reinterpret_cast<__half2*>(g.P_lo + crow + n) = l;
+                }
             }
         }
     }
@@ -220,8 +288,8 @@ CUtensorMap make_map(const __half* base, uint64_t dim0, uint64_t dim1, uint64_t 
     return m;
 }
 
-template <int BN>
-void launch_f16_t(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b, const F16Args& a, dim3 grid, cudaStream_t st) {
+template <int BN, typename Args>
+void launch_f16_t(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b, const Args& a, dim3 grid, cudaStream_t st) {
     constexpr size_t smem = 1024 + (size_t)F_STAGES * (2 * F_BM * F_BK * 2 + BN * F_BK * 2) + 2 * F_STAGES * sizeof(uint64_t);
     static std::mutex mu;
     static bool configured[16] = {};   // per device ordinal
@@ -230,11 +298,11 @@ void launch_f16_t(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMa
     {
         std::lock_guard<std::mutex> lock(mu);
         if (dev >= 0 && dev < 16 && !configured[dev]) {
-            WB_CUDA(cudaFuncSetAttribute(gemm_f16_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            WB_CUDA(cudaFuncSetAttribute(gemm_f16_tc_kernel<BN, Args>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             configured[dev] = true;
         }
     }
-    gemm_f16_tc_kernel<BN><<<grid, F_THREADS, smem, st>>>(ah, al, b, a);
+    gemm_f16_tc_kernel<BN, Args><<<grid, F_THREADS, smem, st>>>(ah, al, b, a);
     WB_LAUNCH_CHECK();
 }
 
@@ -285,6 +353,23 @@ void GemmF16Plan::launch(cudaStream_t st) const {
     if (!impl || impl->args.single.rows <= 0 || impl->grid.y == 0) return;
     if (impl->BN == 128) launch_f16_t<128>(impl->ah, impl->al, impl->b, impl->args, impl->grid, st);
     else launch_f16_t<64>(impl->ah, impl->al, impl->b, impl->args, impl->grid, st);
+}
+
+int logit_stats_tiles(int V) { return (V + 127) / 128; }
+
+void launch_logit_stats(const LogitStatsParams& p, cudaStream_t st) {
+    WB_REQUIRE(p.rows >= 1 && p.K % 8 == 0 && p.V >= 1, "logit_stats: unsupported shape");
+    constexpr int BN = 128;
+    const CUtensorMap ah = make_map(p.A_hi, (uint64_t)p.K, (uint64_t)p.rows, 1, (uint64_t)p.K, (uint64_t)p.K * p.rows, F_BK, F_BM, 3);
+    const CUtensorMap al = make_map(p.A_lo, (uint64_t)p.K, (uint64_t)p.rows, 1, (uint64_t)p.K, (uint64_t)p.K * p.rows, F_BK, F_BM, 3);
+    const CUtensorMap b = make_map(p.E, (uint64_t)p.K, (uint64_t)p.V, 1, (uint64_t)p.K, (uint64_t)p.K * p.V, F_BK, BN, 2);   // rows past V read 0
+    LogitArgs a{};
+    a.single = GemmGroup{0, 0, p.rows};
+    a.K = p.K;
+    a.target = p.target; a.row_mask = p.row_mask; a.is_special = p.is_special;
+    a.V = p.V; a.n_tiles = logit_stats_tiles(p.V);
+    a.tile_m = p.tile_m; a.tile_s = p.tile_s; a.tile_i = p.tile_i; a.tgt_logit = p.tgt_logit;
+    launch_f16_t<BN>(ah, al, b, a, dim3(a.n_tiles, (p.rows + F_BM - 1) / F_BM, 1), st);
 }
 
 }  // namespace wb

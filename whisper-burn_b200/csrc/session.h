@@ -53,6 +53,16 @@ struct DecodeLaunch {
     }
 };
 
+// workspace of token scoring (score.cu), grown on demand
+struct ScoreWs {
+    DevBuf<int> tok, pos, target, seq_win, tile_i, am;   // per row: input token, position, target id; per sequence: window
+    DevBuf<uint8_t> row_mask, special;
+    DevBuf<AttnWindow> seqs;                              // rows of each sequence
+    DevBuf<float> x, tile_m, tile_s, tgt_logit, lp;
+    DevBuf<__half> xn_h, xn_l, qkv_h, qkv_l, att_h, att_l, hid_h, hid_l;
+    std::vector<std::unique_ptr<GemmF16Plan>> plans;      // per decoder layer: qkv, out, cross query, cross out, mlp1, mlp2
+};
+
 // pinned host array
 struct PinnedFree { void operator()(void* p) const { cudaFreeHost(p); } };
 template <typename T> using Pinned = std::unique_ptr<T[], PinnedFree>;
@@ -186,6 +196,11 @@ struct Session {
     // decoded) when no decoder covers it, and the caller runs the host search
     bool beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_size, int max_depth, int64_t eot,
                      std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp);
+    // teacher-forced scoring of n_seqs packed token sequences (wb_session_score_tokens): per position j >= 1 the log-prob of
+    // token j given tokens 0 .. j-1 and the arg-max id; reads the cross K/V of the encoded windows, writes no decode state
+    void score_tokens(int64_t n_seqs, const int32_t* window_of_seq, const int64_t* tokens, const int64_t* lens, bool apply_mask,
+                      const uint8_t* is_special_host, float* lp_out, int64_t* argmax_out);
+    ScoreWs score_ws;
 };
 
 // host pipeline (transcribe.cu): per window the ids and the log-prob each was chosen with (BeamSearchToken.log_prob)

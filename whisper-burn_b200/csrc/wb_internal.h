@@ -306,6 +306,20 @@ private:
     int key_rows = -1, key_groups = -1;
 };
 void launch_split_f16(const float* src, __half* hi, __half* lo, int64_t n, cudaStream_t st);
+// Logits GEMM of token scoring (gemm_f16.cu, LogitArgs): rows x E^T over E = the fp16 token embedding [V][K], reduced per
+// (row, 128-column tile) to the tile max, sum of exp(x - max) and arg-max, plus each row's target logit; no logits are stored.
+struct LogitStatsParams {
+    const __half *A_hi = nullptr, *A_lo = nullptr;   // [rows][K] planes of the final LayerNorm
+    const __half* E = nullptr;                       // [V][K]
+    int rows = 0, K = 0, V = 0;
+    const int* target = nullptr;                     // [rows]
+    const uint8_t* row_mask = nullptr;               // [rows] or null
+    const uint8_t* is_special = nullptr;             // [V]
+    float *tile_m = nullptr, *tile_s = nullptr, *tgt_logit = nullptr;   // [rows][logit_stats_tiles(V)], [rows]
+    int* tile_i = nullptr;
+};
+int logit_stats_tiles(int V);
+void launch_logit_stats(const LogitStatsParams& p, cudaStream_t st);
 
 // ---- frontend (logmel.cu) ---------------------------------------------------------------------
 struct LogMelWindow {
@@ -338,6 +352,14 @@ void launch_encoder_attention(const float* qkv, float* out, const AttnWindow* wi
 // tensor-core version on fp16 hi/lo planes (enc_attn_tc.cu): q | k | v planes [rows][3d] -> output planes [rows][d]
 void launch_encoder_attention_tc(const __half* qkv_hi, const __half* qkv_lo, __half* out_hi, __half* out_lo, const AttnWindow* win_dev,
                                  int n_windows, int max_T, int d, int n_head, cudaStream_t st);
+// token scoring (enc_attn_tc.cu): causal self attention over the packed rows of each sequence (q | k | v planes [rows][3d];
+// kv_f16: K and V enter as their fp16 rounding), and cross attention of each sequence's cross-query planes [rows][d] over its
+// window's head-major cross K/V of one layer (Session::ckv / ckv16)
+void launch_causal_attention_tc(const __half* qkv_hi, const __half* qkv_lo, __half* out_hi, __half* out_lo, const AttnWindow* seq_dev,
+                                int n_seqs, int max_T, int d, int n_head, bool kv_f16, cudaStream_t st);
+void launch_cross_attention_tc(const __half* q_hi, const __half* q_lo, const void* ckv_layer, bool kv_f16, __half* out_hi, __half* out_lo,
+                               const AttnWindow* seq_dev, const int* seq_win_dev, const int64_t* win_row_off_dev, const int* win_T_dev,
+                               int n_seqs, int max_T, int d, int n_head, cudaStream_t st);
 // LayerNorm whose output leaves as fp16 hi/lo planes (and optionally as fp32 rows too: y may be null)
 void launch_layernorm_f16(const float* x, float* y, __half* y_hi, __half* y_lo, const LayerNormW& ln, int rows, int d, int eps_outside,
                           cudaStream_t st);

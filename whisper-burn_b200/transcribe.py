@@ -177,6 +177,26 @@ class Session:
         ffi.check(ffi.lib().wb_session_last_logprobs(self._h, index, ffi.fptr(out), n.value, C.byref(n)))
         return out
 
+    def score_tokens(self, seqs: Sequence[Sequence[int]], windows: Sequence[int], apply_special_mask: bool = False,
+                     is_special: Optional[np.ndarray] = None):
+        """Teacher-forced scoring of token sequences against the encoded windows (wb_session_score_tokens): sequence i on
+        window windows[i].  Returns per sequence (lp float32[len], argmax int64[len]): lp[j] is the log-softmax of position
+        j - 1's logits at seqs[i][j] and argmax[j] that row's arg-max id, for j >= 1; lp[0] = 0, argmax[0] = -1.
+        apply_special_mask: special ids get -inf in the rows whose prefix has <= 5 tokens (the beam search's rule)."""
+        lens = np.asarray([len(s) for s in seqs], dtype=np.int64)
+        toks = np.ascontiguousarray(np.concatenate([np.asarray(s, dtype=np.int64) for s in seqs]) if len(seqs)
+                                    else np.zeros(0, dtype=np.int64), dtype=np.int64)
+        win = np.ascontiguousarray(windows, dtype=np.int32)
+        if len(win) != len(lens):
+            raise ValueError(f"score_tokens: {len(lens)} sequences but {len(win)} windows")
+        lp = np.empty(max(len(toks), 1), dtype=np.float32)
+        am = np.empty(max(len(toks), 1), dtype=np.int64)
+        ffi.check(ffi.lib().wb_session_score_tokens(self._h, len(lens), ffi.i32ptr(win), ffi.i64ptr(toks), ffi.i64ptr(lens),
+                                                   1 if apply_special_mask else 0, _special(is_special), ffi.fptr(lp),
+                                                   ffi.i64ptr(am)))
+        offs = np.concatenate([[0], np.cumsum(lens)])
+        return [(lp[offs[i]:offs[i + 1]].copy(), am[offs[i]:offs[i + 1]].copy()) for i in range(len(lens))]
+
     def last_decoder(self) -> int:
         return int(ffi.lib().wb_session_last_decoder(self._h))
 
