@@ -2,8 +2,10 @@
 (oracle/ on float64 weights, oracle.model.as_dtype), step by step on continuous values.
 
 The token-id tests elsewhere pass unless an error moves an argmax; the synthetic models decode one or two distinct tokens per
-window, so a dropped key, a lost bias or a misplaced LayerNorm eps can hide there.  Here each persistent decoder instance is
-compared on the log-probs it selects, and the encoder on its output, at the shapes where the instance's tiling has edges:
+window, so a dropped key or a lost bias can hide there.  Here each persistent decoder instance is compared on the log-probs it
+selects, and the encoder on its output, at the shapes where the instance's tiling has edges (these models give every LayerNorm
+eps = 1e-5 in the default placement, so a wrong eps or placement is invisible here: test_layernorm_eps_gpu.py checks those on
+the same models with a distinct eps per LayerNorm, in both placements, and test_layernorm_eps_cpu.py shows that it can fail):
 
   * models of real width with few layers (1 audio layer, 2 text layers): the kernels are instantiated on d, heads, rows, k
     and the K/V type, not on the layer count, so the float64 reference stays cheap;

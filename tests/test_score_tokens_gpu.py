@@ -39,10 +39,10 @@ def random_seqs(V, seed, lengths=LENGTHS):
     return [[int(t) for t in rng.integers(0, V, size=n)] for n in lengths]
 
 
-def f64_rows(w64, dims, xa, seq, kv):
+def f64_rows(w64, dims, xa, seq, kv, ln_eps_mode="outside"):
     """float64 log-softmax rows of every position of seq: [len, V]"""
     logits = o_model.forward_decoder(w64, dims, torch.tensor([seq], dtype=torch.int64), xa,
-                                     opts=o_model.OracleOptions(kv_dtype=kv))
+                                     opts=o_model.OracleOptions(ln_eps_mode=ln_eps_mode, kv_dtype=kv))
     return o_model.log_softmax_last(logits)[0].numpy()
 
 

@@ -55,19 +55,19 @@ def rows_of(sess, ids, rule_eots=None):
     return out
 
 
-def teacher_forced(w, dims, sp, xa, ids, kv, unmask=False):
+def teacher_forced(w, dims, sp, xa, ids, kv, unmask=False, ln_eps_mode="outside"):
     """The log-prob of ids[j], j >= 4, given ids[:j]: one greedy_path_log_probs pass over the path (mask of the beam rule, or
     none for the greedy loop)."""
     rows = o_tr.greedy_path_log_probs(w, dims, olp.unmasked(sp) if unmask else sp, xa, ids,
-                                      opts=o_model.OracleOptions(kv_dtype=kv))
+                                      opts=o_model.OracleOptions(ln_eps_mode=ln_eps_mode, kv_dtype=kv))
     return np.array([float(rows[j - 4][ids[j]]) for j in range(4, len(ids))])
 
 
-def check_against_f64(sess, w64, dims, sp, ids, lps, kv, unmask=False, skip_nan=False):
+def check_against_f64(sess, w64, dims, sp, ids, lps, kv, unmask=False, skip_nan=False, ln_eps_mode="outside"):
     worst = 0.0
     for r, t in enumerate(ids):
         xa = torch.from_numpy(sess.get_encoder_output(r)).double()[None]
-        ref = teacher_forced(w64, dims, sp, xa, t, kv, unmask)
+        ref = teacher_forced(w64, dims, sp, xa, t, kv, unmask, ln_eps_mode)
         got = lps[r][4:].astype(np.float64)
         ok = ~np.isnan(got) if skip_nan else np.ones(len(got), bool)
         err = np.abs(got[ok] - ref[ok]).max(initial=0.0)
