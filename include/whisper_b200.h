@@ -167,6 +167,14 @@ int wb_session_create_windows(wb_model* m, int64_t max_windows, int64_t max_beam
 void wb_session_destroy(wb_session* s);
 /* Sets the search rule (WB_SEARCH_*) of the session's decode calls; WB_ERR_INVALID_ARG on an unknown rule. */
 int wb_session_set_search(wb_session* s, int rule);
+/* The previous-text prompt of wb_waveform(s)_to_tokens (the prompt transcribe.rs:43-54, 195-199 builds and line 201
+ * shadows).  startofprev = -1 (the default) keeps the 4-id prompt.  An id in [0, n_vocab), the tokenizer's
+ * <|startofprev|>, prompts window i of a waveform with [startofprev] + prev + [sot, lang, transcribe, notimestamps], prev =
+ * the last (at most) 5 ids of that waveform's merged ids so far with is_special 0, in order (window 0: the 4 ids alone).
+ * A waveform's windows are then decoded in order: round i decodes window i of every waveform that has one, so the rule is
+ * slower than the default.  is_special must be given, and the rule does not combine with WB_SEARCH_GREEDY_LOOP
+ * (WB_ERR_INVALID_ARG from the waveform call); WB_ERR_INVALID_ARG here for any other id. */
+int wb_session_set_prev_prompt(wb_session* s, int64_t startofprev);
 /* prep_audio + mel padding of mels_to_text (transcribe.rs:161-177) + forward_encoder + cross
  * K/V for n_windows waveforms; waves[i] has lens[i] samples (ragged; each >= 400). */
 int wb_session_encode_waveforms(wb_session* s, const float* const* waves, const int64_t* lens,
@@ -205,6 +213,20 @@ int wb_transcribe_windows(wb_session* s, const float* const* waves, const int64_
 int wb_transcribe_windows_dev(wb_session* s, const float* wave_dev, const int64_t* offsets, const int64_t* lens,
                               int64_t n_windows, int beam_size, int max_depth, const wb_special_ids* ids,
                               const uint8_t* is_special, int64_t* tokens_out, int64_t capacity, int64_t* lens_out);
+/* wb_transcribe_windows with mels_to_text's prev_nonspecial_tokens given per window (transcribe.rs:195-203 without the
+ * shadowing at :201).  Window w's previous ids are prev_tokens[off_w .. off_w + prev_lens[w]), off_w = prev_lens[0] + .. +
+ * prev_lens[w-1] (packed as wb_session_score_tokens packs its sequences; prev_tokens may be NULL when every prev_lens is 0).
+ * Its prompt is [startofprev] + those ids + [sot, lang, transcribe, notimestamps], or the 4 ids when prev_lens[w] = 0.
+ * Windows with prompts of different lengths share one decoder launch.  The search rules apply per window at absolute
+ * positions: the special ids are masked while a sequence has at most 5 tokens (never for a prompt of 6 or more), and
+ * max_depth counts steps after the window's own prompt.  Rows are written as wb_transcribe_windows writes them, prompt
+ * included, and wb_session_last_logprobs gives 0.0 for every prompt id.  WB_ERR_INVALID_ARG for startofprev or a previous
+ * id outside [0, n_vocab), a negative prev_lens entry, Lp + max_depth > max_text_len or capacity < Lp + max_depth + 1 (Lp:
+ * the longest prompt), and for any previous ids under WB_SEARCH_GREEDY_LOOP (the greedy loop builds its own prompt). */
+int wb_transcribe_windows_prev(wb_session* s, const float* const* waves, const int64_t* lens, int64_t n_windows,
+                               const int64_t* prev_tokens, const int64_t* prev_lens, int64_t startofprev, int beam_size,
+                               int max_depth, const wb_special_ids* ids, const uint8_t* is_special, int64_t* tokens_out,
+                               int64_t capacity, int64_t* lens_out);
 /* waveform_to_text without detokenisation: windowing (transcribe.rs:114-138), per-window
  * decoding, overlap merge (transcribe.rs:56-63).  Writes the merged ids.
  * sample_rate must be 16000 (WB_ERR_INVALID_ARG otherwise): the log-mel tables are the 16 kHz ones the reference's binary
@@ -222,7 +244,7 @@ int wb_waveforms_to_tokens(wb_session* s, const float* const* waveforms, const i
  * call on this session, aligned with the ids that call wrote: n_out = that row's id count.  WB_ERR_STATE before the first such
  * call, WB_ERR_INVALID_ARG for an index out of range or capacity < n_out.  out == NULL only sets n_out.
  * The values (float32; the reference's BeamSearchToken.log_prob, transcribe.rs:142-146, holds the same f32 widened to f64):
- *   - the 4 prompt ids: 0.0 (transcribe.rs:205-208);
+ *   - the prompt ids (4, or those of a previous-text prompt): 0.0 (transcribe.rs:205-208);
  *   - WB_SEARCH_BEAM, beam_size >= 2: the f32 log_softmax value the search scored the id with, special-id mask included
  *     while sequences have <= 5 tokens (transcribe.rs:291-299).  The left-to-right f64 sum of a row is the cumulative
  *     log-prob the search chose the row by;

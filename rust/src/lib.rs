@@ -61,6 +61,10 @@ pub mod ffi {
         pub fn wb_session_encode_waveforms(s: *mut c_void, waves: *const *const f32, lens: *const i64, n_windows: i64) -> c_int;
         pub fn wb_session_score_tokens(s: *mut c_void, n_seqs: i64, window_of_seq: *const i32, tokens: *const i64, lens: *const i64,
                                        apply_special_mask: c_int, is_special: *const u8, lp_out: *mut f32, argmax_out: *mut i64) -> c_int;
+        pub fn wb_session_set_prev_prompt(s: *mut c_void, startofprev: i64) -> c_int;
+        pub fn wb_transcribe_windows_prev(s: *mut c_void, waves: *const *const f32, lens: *const i64, n_windows: i64, prev_tokens: *const i64,
+                                          prev_lens: *const i64, startofprev: i64, beam_size: c_int, max_depth: c_int, ids: *const wb_special_ids,
+                                          is_special: *const u8, tokens_out: *mut i64, capacity: i64, lens_out: *mut i64) -> c_int;
     }
 }
 
@@ -286,6 +290,30 @@ pub mod transcribe {
         })?;
         assert_eq!(n, n_lp, "one log-prob per token");
         Ok((0..n as usize).map(|i| BeamSearchToken { token: out[i] as usize, log_prob: lps[i] as f64 }).collect())
+    }
+
+    /// waveform_to_text with the previous-text prompt the reference builds and then shadows (transcribe.rs:43-54, 195-201): window
+    /// i is decoded from [<|startofprev|>] + the last (at most) 5 non-special ids merged so far + [sot, lang, transcribe,
+    /// notimestamps] (window 0 from the 4 ids alone).  The windows of the waveform are decoded in order, one launch each.
+    pub fn waveform_to_text_with_prev_prompt(whisper: &model::Whisper, bpe: &Gpt2Tokenizer, lang: Language, waveform: Vec<f32>,
+                                             sample_rate: usize) -> token::Result<(String, Vec<usize>)> {
+        let sp = SpecialTokens::from_tokenizer(bpe, lang);
+        let startofprev = bpe.special_token(SpecialToken::StartofPrev).unwrap() as i64;              // transcribe.rs:181
+        let window = audio::max_waveform_samples(whisper.encoder_ctx_size() - 10);            // transcribe.rs:32-34
+        let shift = window.saturating_sub(sample_rate * 3).max(1);                             // transcribe.rs:120-123
+        let n_windows = waveform.len().saturating_sub(1) / shift + 1;
+        let cap = n_windows * (10 + MAX_DEPTH + 1) + 16;
+        let mut out = vec![0i64; cap];
+        let mut n = 0i64;
+        whisper.with_session(1, BEAM_SIZE, 10 + MAX_DEPTH + 1, |s| {
+            check(unsafe { ffi::wb_session_set_prev_prompt(s, startofprev) })?;
+            let r = check(unsafe { ffi::wb_waveform_to_tokens(s, waveform.as_ptr(), waveform.len() as i64, sample_rate as i64, BEAM_SIZE as c_int,
+                                                              MAX_DEPTH as c_int, &sp.ids, sp.is_special.as_ptr(), out.as_mut_ptr(), cap as i64, &mut n) });
+            check(unsafe { ffi::wb_session_set_prev_prompt(s, -1) })?;   // the cached session's other callers use the 4-id prompt
+            r
+        })?;
+        let tokens: Vec<usize> = out[..n as usize].iter().map(|&t| t as usize).collect();
+        Ok((bpe.decode(&tokens[..], true)?, tokens))
     }
 
     /// How well given token sequences fit one audio window: `forward_decoder` (mod.rs:131-157) and `log_softmax`

@@ -1,5 +1,6 @@
 // extern "C" boundary (include/whisper_b200.h).  No exceptions cross it: every entry point maps
 // wb::Error / std::exception to a status code and a thread-local message.
+#include <algorithm>
 #include <cstring>
 #include <map>
 #include <memory>
@@ -321,6 +322,13 @@ int wb_session_set_search(wb_session* s, int rule) {
     });
 }
 
+int wb_session_set_prev_prompt(wb_session* s, int64_t startofprev) {
+    return guarded([&] {
+        WB_REQUIRE(s, "set_prev_prompt: null pointer");
+        s->impl->set_prev_prompt(startofprev);
+    });
+}
+
 int wb_session_encode_waveforms(wb_session* s, const float* const* waves, const int64_t* lens, int64_t n_windows) {
     return guarded([&] {
         WB_REQUIRE(s && waves && lens, "encode: null pointer");
@@ -380,7 +388,8 @@ int wb_session_get_encoder_output(wb_session* s, int64_t window, float* out, int
 int wb_session_begin(wb_session* s, const int64_t* prompt, int64_t prompt_len) {
     return guarded([&] {
         WB_REQUIRE(s && prompt, "begin: null pointer");
-        s->impl->begin(prompt, prompt_len);
+        WB_REQUIRE(prompt_len >= 1, "begin: prompt length out of range");
+        s->impl->begin(std::vector<std::vector<int64_t>>((size_t)s->impl->n_windows, std::vector<int64_t>(prompt, prompt + prompt_len)));
     });
 }
 
@@ -406,6 +415,42 @@ int wb_transcribe_windows(wb_session* s, const float* const* waves, const int64_
         wb::transcribe_windows(*s->impl, beam_size, max_depth, *ids, is_special, toks, s->logprobs);
         copy_tokens_out(toks, tokens_out, capacity, lens_out);
         collect_timings(*s->impl);
+        s->have_logprobs = true;
+    });
+}
+
+int wb_transcribe_windows_prev(wb_session* s, const float* const* waves, const int64_t* lens, int64_t n_windows,
+                               const int64_t* prev_tokens, const int64_t* prev_lens, int64_t startofprev, int beam_size,
+                               int max_depth, const wb_special_ids* ids, const uint8_t* is_special, int64_t* tokens_out,
+                               int64_t capacity, int64_t* lens_out) {
+    return guarded([&] {
+        WB_REQUIRE(s && waves && lens && prev_lens && ids && special_given(s, is_special) && tokens_out && lens_out,
+                   "transcribe_windows_prev: null pointer");
+        wb::Session& S = *s->impl;
+        WB_REQUIRE(n_windows >= 1 && n_windows <= S.max_windows, "transcribe_windows_prev: n_windows out of range");
+        WB_REQUIRE(startofprev >= 0 && startofprev < S.m->dims.n_vocab, "transcribe_windows_prev: startofprev id out of range");
+        WB_REQUIRE(max_depth >= 0, "transcribe_windows_prev: negative max_depth");
+        std::vector<std::vector<int64_t>> prev((size_t)n_windows);
+        int64_t off = 0, max_lp = 4;
+        for (int64_t w = 0; w < n_windows; ++w) {
+            WB_REQUIRE(prev_lens[w] >= 0, "transcribe_windows_prev: negative prev_lens entry");
+            WB_REQUIRE(prev_lens[w] == 0 || prev_tokens, "transcribe_windows_prev: null prev_tokens");
+            WB_REQUIRE(prev_lens[w] == 0 || S.search != WB_SEARCH_GREEDY_LOOP,
+                       "transcribe_windows_prev: the greedy loop builds its own prompt; no previous ids with it");
+            prev[(size_t)w].assign(prev_tokens + off, prev_tokens + off + prev_lens[w]);
+            for (int64_t t : prev[(size_t)w])
+                WB_REQUIRE(t >= 0 && t < S.m->dims.n_vocab, "transcribe_windows_prev: previous id out of range");
+            off += prev_lens[w];
+            max_lp = std::max(max_lp, prev_lens[w] > 0 ? prev_lens[w] + 5 : 4);
+        }
+        WB_REQUIRE(max_lp + max_depth <= S.t_max, "transcribe_windows_prev: prompt + max_depth exceeds the session's max_text_len");
+        WB_REQUIRE(capacity >= max_lp + max_depth + 1, "transcribe_windows_prev: capacity below prompt + max_depth + 1");
+        s->have_logprobs = false;
+        S.encode_waveforms_host(waves, lens, n_windows);
+        std::vector<std::vector<int64_t>> toks;
+        wb::transcribe_windows(S, beam_size, max_depth, *ids, is_special, toks, s->logprobs, prev, startofprev);
+        copy_tokens_out(toks, tokens_out, capacity, lens_out);
+        collect_timings(S);
         s->have_logprobs = true;
     });
 }
@@ -437,9 +482,35 @@ int wb_window_bounds(int64_t n_samples, int64_t sample_rate, int64_t window_len,
     });
 }
 
+// the overlap merge of one window's ids and log-probs into its waveform's (transcribe.rs:56-63)
+static void merge_window(std::vector<int64_t>& tokens, std::vector<float>& tlp, const std::vector<int64_t>& nt,
+                         const std::vector<float>& nl) {
+    int64_t pi = 0, ci = 0;
+    if (wb::find_chunk_overlap(tokens.data(), (int64_t)tokens.size(), nt.data(), (int64_t)nt.size(), 40, 3, &pi, &ci)) {
+        tokens.resize((size_t)pi);                                    // transcribe.rs:59-60
+        tokens.insert(tokens.end(), nt.begin() + ci, nt.end());
+        tlp.resize((size_t)pi);
+        tlp.insert(tlp.end(), nl.begin() + ci, nl.end());
+    } else {
+        tokens.insert(tokens.end(), nt.begin(), nt.end());
+        tlp.insert(tlp.end(), nl.begin(), nl.end());
+    }
+}
+
+// transcribe.rs:43-50: the last (at most) 5 ids of the merged tokens that are not special, in order
+static std::vector<int64_t> prev_nonspecial(const std::vector<int64_t>& tokens, const uint8_t* is_special) {
+    std::vector<int64_t> prev;
+    for (size_t i = tokens.size(); i-- > 0 && prev.size() < 5;)
+        if (!is_special[tokens[i]]) prev.push_back(tokens[i]);
+    std::reverse(prev.begin(), prev.end());
+    return prev;
+}
+
 // windows of ALL waveforms are decoded together in batches of the session's capacity (they are independent,
 // SURVEY.md F9), then each waveform's windows are merged in order exactly like the reference's sequential
-// loop (transcribe.rs:42-71); each id's log-prob travels with it through the merge into out_lp
+// loop (transcribe.rs:42-71); each id's log-prob travels with it through the merge into out_lp.
+// With the previous-text prompt (Session::startofprev >= 0) window i of a waveform needs the merged ids of windows
+// 0 .. i-1: round i decodes window i of every waveform that has one, in batches of the session's capacity.
 static void waveforms_to_tokens(wb::Session& S, const float* const* waveforms, const int64_t* n_samples, int64_t n_waveforms,
                                 int64_t sample_rate, int beam_size, int max_depth, const wb_special_ids& ids,
                                 const uint8_t* is_special, std::vector<std::vector<int64_t>>& out,
@@ -459,27 +530,41 @@ static void waveforms_to_tokens(wb::Session& S, const float* const* waveforms, c
         }
     out.assign((size_t)n_waveforms, {});
     out_lp.assign((size_t)n_waveforms, {});
-    for (size_t b0 = 0; b0 < ptrs.size(); b0 += (size_t)S.max_windows) {
-        const size_t nb = std::min(ptrs.size() - b0, (size_t)S.max_windows);
-        S.encode_waveforms_host(ptrs.data() + b0, lens.data() + b0, (int64_t)nb);
-        std::vector<std::vector<int64_t>> toks;
-        std::vector<std::vector<float>> lps;
-        wb::transcribe_windows(S, beam_size, max_depth, ids, is_special, toks, lps);
-        for (size_t i = 0; i < nb; ++i) {
-            std::vector<int64_t>& tokens = out[(size_t)owner[b0 + i]];
-            std::vector<float>& tlp = out_lp[(size_t)owner[b0 + i]];
-            const auto& nt = toks[i];
-            const auto& nl = lps[i];
-            int64_t pi = 0, ci = 0;
-            if (wb::find_chunk_overlap(tokens.data(), (int64_t)tokens.size(), nt.data(), (int64_t)nt.size(), 40, 3, &pi, &ci)) {
-                tokens.resize((size_t)pi);                                    // transcribe.rs:59-60
-                tokens.insert(tokens.end(), nt.begin() + ci, nt.end());
-                tlp.resize((size_t)pi);
-                tlp.insert(tlp.end(), nl.begin() + ci, nl.end());
-            } else {
-                tokens.insert(tokens.end(), nt.begin(), nt.end());
-                tlp.insert(tlp.end(), nl.begin(), nl.end());
+    const bool prev_prompt = S.startofprev >= 0;
+    if (prev_prompt) {
+        WB_REQUIRE(S.search != WB_SEARCH_GREEDY_LOOP, "waveform_to_tokens: the greedy loop builds its own prompt; no previous-text prompt with it");
+        WB_REQUIRE(is_special != nullptr, "waveform_to_tokens: the previous-text prompt needs is_special");
+    }
+    // batches: window-major order (all windows at once) or, with the previous-text prompt, rounds of window index i
+    std::vector<std::vector<size_t>> rounds(1);
+    if (prev_prompt) {
+        std::vector<int> idx((size_t)n_waveforms, 0);
+        for (size_t j = 0; j < ptrs.size(); ++j) {
+            const size_t i = (size_t)idx[(size_t)owner[j]]++;
+            if (rounds.size() <= i) rounds.resize(i + 1);
+            rounds[i].push_back(j);
+        }
+    } else {
+        for (size_t j = 0; j < ptrs.size(); ++j) rounds[0].push_back(j);
+    }
+    for (const std::vector<size_t>& round : rounds) {
+        for (size_t b0 = 0; b0 < round.size(); b0 += (size_t)S.max_windows) {
+            const size_t nb = std::min(round.size() - b0, (size_t)S.max_windows);
+            std::vector<const float*> bp(nb);
+            std::vector<int64_t> bl(nb);
+            std::vector<std::vector<int64_t>> prev(prev_prompt ? nb : 0);
+            for (size_t i = 0; i < nb; ++i) {
+                const size_t j = round[b0 + i];
+                bp[i] = ptrs[j];
+                bl[i] = lens[j];
+                if (prev_prompt) prev[i] = prev_nonspecial(out[(size_t)owner[j]], is_special);
             }
+            S.encode_waveforms_host(bp.data(), bl.data(), (int64_t)nb);
+            std::vector<std::vector<int64_t>> toks;
+            std::vector<std::vector<float>> lps;
+            wb::transcribe_windows(S, beam_size, max_depth, ids, is_special, toks, lps, prev, S.startofprev);
+            for (size_t i = 0; i < nb; ++i)
+                merge_window(out[(size_t)owner[round[b0 + i]]], out_lp[(size_t)owner[round[b0 + i]]], toks[i], lps[i]);
         }
     }
     collect_timings(S);

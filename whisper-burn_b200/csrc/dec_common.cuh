@@ -879,14 +879,19 @@ __device__ __forceinline__ void fold_records(const DecArgs& a, const float* rec,
 
 // ---- per-row finish: log-probs (v - max) - lse of the candidates, lse from the NP records of the row (DESIGN.md section 2)
 // greedy bookkeeping of row r at position p (beam.rs:9-37 with beam_size 1): the token and its rounded log-prob lp, the
-// length, EOT
+// length, EOT.  A row whose position p + 1 is still inside its prompt commits nothing (its token is in the buffer, its
+// log-prob 0); a row is finished by EOT or once it holds prompt_len + max_depth ids.
+// the most ids row r may hold, its prompt length + max_depth (DecArgs::lengths): a greedy row is finished when it holds them;
+// a beam window's search starts at position id_limit(slot 0) - max_depth - 1
+__device__ __forceinline__ int id_limit(const DecArgs& a, int r) { return __ldg(a.lengths + a.Rmax + r); }
 __device__ __forceinline__ void greedy_commit(const DecArgs& a, int r, int p, int id, float lp) {
-    if (a.greedy && !__ldcg(a.finished + r)) {
-        a.tokens[(int64_t)r * a.t_max + p + 1] = id;
-        a.token_lp[(int64_t)r * a.t_max + p + 1] = lp;
-        a.lengths[r] = p + 2;
-        if (id == a.eot) a.finished[r] = 1;
-    }
+    // lengths[r] holds the prompt length until the first commit, then p + 2 < p' + 2: the test passes from then on.  The
+    // limit is read at its use (an L1 hit) rather than held: the finishers run at the decoders' register limit
+    if (!a.greedy || __ldcg(a.finished + r) || p + 1 < __ldcg(a.lengths + r)) return;
+    a.tokens[(int64_t)r * a.t_max + p + 1] = id;
+    a.token_lp[(int64_t)r * a.t_max + p + 1] = lp;
+    a.lengths[r] = p + 2;
+    if (id == a.eot || p + 2 >= id_limit(a, r)) a.finished[r] = 1;
 }
 // The greedy loop's rules (DecArgs::loop_rules, host/loop_rules.hpp) for row r after greedy_commit put `id` at p + 1: the EOT
 // test on the raw logits of `id` (`top`) and of EOT, then the repetition cut over tokens[0, p + 2), lane l taking windows

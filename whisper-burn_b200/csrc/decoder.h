@@ -75,6 +75,10 @@ struct DecArgs {
     const uint8_t* is_special = nullptr;
     int mask_mode = 0;
     int k = 1, greedy = 0, eot = -1;
+    // lengths [R] ids of each row (the prompt length until its first commit); behind them, lengths[Rmax + r], the most ids
+    // the row may hold, its prompt length + max_depth (Session::seat_rows, dec_common.cuh id_limit): kept in the same buffer
+    // so that DecArgs, which decoder6's register allocation is sensitive to, does not grow, and decoder5's row groups offset
+    // both with one pointer
     int *lengths = nullptr, *finished = nullptr;
     // greedy loop (WB_SEARCH_GREEDY_LOOP, host/loop_rules.hpp): the row finish also applies the EOT test and the repetition
     // cut (dec_common.cuh loop_finish); the vocabulary stage stores each row's raw EOT logit in eot_logit [R].  The context
@@ -94,6 +98,7 @@ struct DecArgs {
     int trace_cap = 0;
     // decoder6.cu beam mode (beam > 1): prefill + the whole width-B search of n_win windows in one launch.  Row w * B + i is
     // slot i of window w; anc (read at even depths) / anc_alt (odd depths) are the double-buffered ancestry tables.
+    // max_depth: search steps after each row's own prompt (greedy and beam mode).
     int beam = 0, n_win = 0, max_depth = 0;
     int* anc_alt = nullptr;
     int* slot_live = nullptr;             // [R] the slot holds a live beam at the current position

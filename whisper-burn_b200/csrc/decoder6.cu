@@ -482,8 +482,10 @@ constexpr int BM_NX = 3 * BM_LIVE + 3 * NCW * beamfx::MAX_NODES;     // finish_b
 //       records -> topk_id / topk_lp [row][B];
 //   (b) one warp per unfinished window: beamfx::beam_step on the carried nodes (lane 0), the new nodes' sequences and the
 //       log-probs their tokens were scored with (bm_seq / bm_seq_lp, the warp); the next position's live slots w * B + i in
-//       carried order, each with its parent's cache row and its token;
-//   (c) the search ends when every window is done (its best carried node is finished) or at max_depth: then the best
+//       carried order, each with its parent's cache row and its token.  A window whose search has not started (p + 1 is
+//       inside its prompt: dec_common.cuh id_limit) keeps slot 0 live in its own row with its next prompt token;
+//   (c) a window is done when its best carried node is finished or at max_depth steps after its own prompt; the search
+//       ends when every window is done: then the best
 //       sequence of every window goes to bm_out / bm_out_lp and bar[3] is set; otherwise the next position's slots, tokens and ancestry
 //       table (anc_new[r][j] = anc_old[parent[r]][j] for j <= p, anc_new[r][p + 1] = r) are written.
 // Called by the 256 consumer threads; ends with a barrier of the consumers.
@@ -552,6 +554,14 @@ __device__ __noinline__ void finish_beam(const DecArgs& a, int p, int depth, con
             if (lane < B) nx_live[w * B + lane] = 0;
             continue;
         }
+        if (p + 2 + a.max_depth <= id_limit(a, w * B)) {   // the window's search starts at its last prompt position
+            if (lane < B) nx_live[w * B + lane] = lane == 0 ? 1 : 0;
+            if (lane == 0) {
+                nx_par[w * B] = w * B;
+                nx_tok[w * B] = __ldcg(a.tokens + (int64_t)w * B * t_max + p + 1);
+            }
+            continue;
+        }
         const int nb = buf ^ 1;
         int n_out = 0;
         if (lane == 0) {
@@ -597,7 +607,7 @@ __device__ __noinline__ void finish_beam(const DecArgs& a, int p, int depth, con
             for (; nl < B; ++nl) nx_live[w * B + nl] = 0;
             a.bm_cnt[nb * NW + w] = n_out;
             a.bm_win[2 * w] = nb;
-            a.bm_win[2 * w + 1] = fx::search_done(in, n_out) ? 1 : 0;
+            a.bm_win[2 * w + 1] = (fx::search_done(in, n_out) || p + 2 >= id_limit(a, w * B)) ? 1 : 0;
         }
         n_out = __shfl_sync(0xffffffffu, n_out, 0);
         __syncwarp();
@@ -622,7 +632,7 @@ __device__ __noinline__ void finish_beam(const DecArgs& a, int p, int depth, con
     if (tid == 0) {
         int open = 0;
         for (int w = 0; w < NW; ++w) open += __ldcg(a.bm_win + 2 * w + 1) ? 0 : 1;
-        ctl[2] = (depth + 1 >= a.max_depth || open == 0) ? 1 : 0;
+        ctl[2] = open == 0 ? 1 : 0;
         ctl[3] = open;
     }
     bar_consumers();

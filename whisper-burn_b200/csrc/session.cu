@@ -76,7 +76,7 @@ Session::Session(Model* model, int64_t max_w, int64_t max_b, int64_t max_text_le
     WB_CUDA(cudaMemsetAsync(hid_pl.p, 0, 8 * dec5_plane_uint4(d) * sizeof(uint4), st));
     dq.alloc((size_t)Rmax * d); dhid.alloc((size_t)Rmax * 4 * d);
     logits.alloc((size_t)Rmax * V);
-    tokens.alloc((size_t)Rmax * t_max); token_lp.alloc((size_t)Rmax * t_max); lengths.alloc(Rmax); cur_tok.alloc(Rmax); finished.alloc(Rmax);
+    tokens.alloc((size_t)Rmax * t_max); token_lp.alloc((size_t)Rmax * t_max); lengths.alloc((size_t)2 * Rmax); cur_tok.alloc(Rmax); finished.alloc(Rmax);
     row_window.alloc(Rmax); anc0.alloc((size_t)Rmax * t_max); anc1.alloc((size_t)Rmax * t_max); parent.alloc(Rmax);
     pos.alloc(1); n_unfinished.alloc(128);
     topk_id.alloc((size_t)Rmax * DEC_KC); topk_lp.alloc((size_t)Rmax * DEC_KC);
@@ -387,17 +387,20 @@ void Session::set_special(const uint8_t* sp) {
     }
 }
 
-void Session::seat_rows(int rows, int per_window, const int64_t* prompt, int64_t prompt_len, int64_t prompt_stride) {
+void Session::seat_rows(int rows, int per_window, const std::vector<std::vector<int64_t>>& prompts, int max_depth) {
     if (!encoded) fail(WB_ERR_STATE, "session: decode before encode");
-    WB_REQUIRE(rows <= Rmax && prompt_len >= 1 && prompt_len <= t_max, "decode: rows or prompt length out of range");
+    WB_REQUIRE(rows <= Rmax && (int64_t)prompts.size() * per_window >= rows, "decode: rows out of range");
     const int V = m->dims.n_vocab;
-    std::vector<int> tk((size_t)rows * t_max, 0), rw((size_t)rows), len((size_t)rows, (int)prompt_len);
+    std::vector<int> tk((size_t)rows * t_max, 0), rw((size_t)rows), len((size_t)rows), lim((size_t)rows);
     for (int r = 0; r < rows; ++r) {
+        const std::vector<int64_t>& pr = prompts[(size_t)(r / per_window)];
+        WB_REQUIRE(!pr.empty() && (int64_t)pr.size() <= t_max, "decode: prompt length out of range");
         rw[(size_t)r] = r / per_window;
-        for (int64_t i = 0; i < prompt_len; ++i) {
-            const int64_t t = prompt[r * prompt_stride + i];
-            WB_REQUIRE(t >= 0 && t < V, "decode: prompt token out of range");
-            tk[(size_t)r * t_max + i] = (int)t;
+        len[(size_t)r] = (int)pr.size();
+        lim[(size_t)r] = (int)pr.size() + max_depth;
+        for (size_t i = 0; i < pr.size(); ++i) {
+            WB_REQUIRE(pr[i] >= 0 && pr[i] < V, "decode: prompt token out of range");
+            tk[(size_t)r * t_max + i] = (int)pr[i];
         }
     }
     WB_CUDA(cudaMemcpyAsync(tokens.p, tk.data(), tk.size() * sizeof(int), cudaMemcpyHostToDevice, st));
@@ -405,6 +408,7 @@ void Session::seat_rows(int rows, int per_window, const int64_t* prompt, int64_t
     WB_CUDA(cudaMemsetAsync(finished.p, 0, sizeof(int) * Rmax, st));
     WB_CUDA(cudaMemsetAsync(pos.p, 0, sizeof(int), st));
     WB_CUDA(cudaMemcpyAsync(lengths.p, len.data(), len.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    WB_CUDA(cudaMemcpyAsync(lengths.p + Rmax, lim.data(), lim.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     R = rows;
     anc_identity = true;
     anc_cur = 0;
@@ -424,15 +428,26 @@ void Session::feed_positions(int n, float* logits_out) {
     }
 }
 
-void Session::begin(const int64_t* prompt, int64_t prompt_len, bool prefill) {
-    WB_REQUIRE(prompt_len >= 1 && prompt_len < t_max, "begin: prompt length out of range");
-    seat_rows(n_windows, 1, prompt, prompt_len, 0);
-    if (prefill) feed_positions((int)prompt_len - 1, nullptr);   // prompt[0 .. prompt_len-1): no logits needed
+// the shortest and longest of n prompts
+static std::pair<int, int> prompt_range(const std::vector<std::vector<int64_t>>& prompts) {
+    int lo = INT_MAX, hi = 0;
+    for (const auto& pr : prompts) { lo = std::min(lo, (int)pr.size()); hi = std::max(hi, (int)pr.size()); }
+    return {lo, hi};
+}
+
+void Session::begin(const std::vector<std::vector<int64_t>>& prompts, bool prefill, int max_depth) {
+    WB_REQUIRE((int64_t)prompts.size() == n_windows, "begin: one prompt per encoded window");
+    for (const auto& pr : prompts) WB_REQUIRE(!pr.empty() && (int64_t)pr.size() < t_max, "begin: prompt length out of range");
+    seat_rows(n_windows, 1, prompts, max_depth);
+    if (prefill) feed_positions(prompt_range(prompts).first - 1, nullptr);   // before every prompt's last token: no logits needed
     WB_CUDA(cudaStreamSynchronize(st));
 }
 
 void Session::teacher_forced_logits(const int64_t* toks, int64_t n_rows, int64_t seq_len, float* logits_out) {
-    seat_rows((int)n_rows, 1, toks, seq_len, seq_len);
+    WB_REQUIRE(n_rows >= 1 && seq_len >= 1, "forward_decoder: empty input");
+    std::vector<std::vector<int64_t>> rows((size_t)n_rows);
+    for (int64_t r = 0; r < n_rows; ++r) rows[(size_t)r].assign(toks + r * seq_len, toks + (r + 1) * seq_len);
+    seat_rows((int)n_rows, 1, rows);
     feed_positions((int)seq_len, logits_out);
     WB_CUDA(cudaStreamSynchronize(st));
 }
@@ -447,7 +462,7 @@ bool Session::launch_decoder(const DecodeLaunch& l) {
     a.anc = anc_identity ? nullptr : (anc_cur == 0 ? anc0.p : anc1.p);
     a.use_cur_tok = l.use_cur_tok; a.pos0 = l.pos0; a.n_steps = l.n_steps; a.logits_from = l.logits_from;
     a.is_special = have_special ? is_special.p : nullptr; a.mask_mode = l.mask_mode;
-    a.k = l.k; a.greedy = l.greedy; a.eot = l.eot; a.loop_rules = l.loop_rules;
+    a.k = l.k; a.greedy = l.greedy; a.eot = l.eot; a.loop_rules = l.loop_rules; a.max_depth = l.max_depth;
     a.logits_out = l.raw_logits ? logits.p : nullptr;
     if (getenv("WB200_TRACE")) {
         dec_trace.ensure(1 << 16);
@@ -461,7 +476,7 @@ bool Session::launch_decoder(const DecodeLaunch& l) {
     int groups = 0;
     last_groups = 1;
     if (l.beam > 1) {   // the whole search: only decoder6 has a beam mode
-        a.beam = l.beam; a.n_win = l.rows / l.beam; a.max_depth = l.max_depth;
+        a.beam = l.beam; a.n_win = l.rows / l.beam;
         a.anc = anc0.p; a.anc_alt = anc1.p; a.slot_live = slot_live.p;
         a.bm_head = bm_head.p; a.bm_seq = bm_seq.p; a.bm_cnt = bm_cnt.p; a.bm_win = bm_win.p; a.bm_out = bm_out.p; a.bm_out_len = bm_out_len.p;
         a.bm_seq_lp = bm_seq_lp.p; a.bm_out_lp = bm_out_lp.p;
@@ -491,10 +506,10 @@ bool Session::launch_decoder(const DecodeLaunch& l) {
 void Session::profile_decode(const int64_t* prompt, int64_t prompt_len, int n_steps, float* logits_ms, float* step_ms) {
     WB_REQUIRE(n_steps >= 1 && prompt_len + n_steps <= t_max, "profile: n_steps out of range");
     // the whole decode is ONE kernel: time the launch (prefill + n_steps greedy steps) and report per position
-    begin(prompt, prompt_len, false);
+    begin(std::vector<std::vector<int64_t>>((size_t)n_windows, std::vector<int64_t>(prompt, prompt + prompt_len)), false, n_steps);
     const int total = (int)prompt_len - 1 + n_steps;
     WB_CUDA(cudaEventRecord(ev[4], st));
-    launch_decoder(DecodeLaunch::greedy_search(R, (int)prompt_len, n_steps, /*eot=*/-1, /*loop_rules=*/false));
+    launch_decoder(DecodeLaunch::greedy_search(R, (int)prompt_len, (int)prompt_len, n_steps, /*eot=*/-1, /*loop_rules=*/false));
     WB_CUDA(cudaEventRecord(ev[5], st));
     WB_CUDA(cudaStreamSynchronize(st));
     float t = 0.f;
@@ -552,13 +567,14 @@ void Session::last_topk(int64_t n_rows, int64_t k, int64_t* ids_out, float* lp_o
     for (size_t i = 0; i < ids.size(); ++i) ids_out[i] = ids[i];
 }
 
-void Session::greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_depth, int64_t eot,
+void Session::greedy_decode(const std::vector<std::vector<int64_t>>& prompts, int max_depth, int64_t eot,
                             std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp, bool loop_rules) {
-    WB_REQUIRE(prompt_len + max_depth <= t_max, "greedy: prompt + max_depth exceeds the session's max_text_len");
-    // one launch: prompt prefill + every greedy step, early exit inside the kernel.  The greedy loop's context stop, at
-    // prompt_len + max_depth <= t_max <= n_text_ctx tokens, is the end of the launch.
-    begin(prompt, prompt_len, /*prefill=*/false);
-    if (max_depth > 0) launch_decoder(DecodeLaunch::greedy_search(R, (int)prompt_len, max_depth, (int)eot, loop_rules));
+    const auto [min_lp, max_lp] = prompt_range(prompts);
+    WB_REQUIRE(max_lp + max_depth <= t_max, "greedy: prompt + max_depth exceeds the session's max_text_len");
+    // one launch: prompt prefill + every greedy step, early exit inside the kernel.  A row stops at EOT or at its own
+    // prompt_len + max_depth ids; the greedy loop's context stop (prompt_len + max_depth <= t_max <= n_text_ctx) is the latter.
+    begin(prompts, /*prefill=*/false, max_depth);
+    if (max_depth > 0) launch_decoder(DecodeLaunch::greedy_search(R, min_lp, max_lp, max_depth, (int)eot, loop_rules));
     std::vector<int> tk((size_t)R * t_max), len((size_t)R);
     std::vector<float> lp((size_t)R * t_max);
     int sdv[128] = {0};
@@ -569,11 +585,12 @@ void Session::greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_d
     WB_CUDA(cudaStreamSynchronize(st));
     int sd = 0;
     for (int g = 0; g < std::min(last_groups, 128); ++g) sd = std::max(sd, sdv[g]);   // row groups stop on their own
-    last_steps = max_depth > 0 ? sd - ((int)prompt_len - 1) : 0;
-    host_pos = (int)prompt_len - 1 + (int)last_steps;
+    last_steps = max_depth > 0 ? sd - (min_lp - 1) : 0;
+    host_pos = min_lp - 1 + (int)last_steps;
     out.assign((size_t)R, {});
     out_lp.assign((size_t)R, {});
     for (int r = 0; r < R; ++r) {
+        const int64_t prompt_len = (int64_t)prompts[(size_t)r].size();
         for (int i = 0; i < len[(size_t)r]; ++i) {
             out[(size_t)r].push_back(tk[(size_t)r * t_max + i]);
             out_lp[(size_t)r].push_back(i < prompt_len ? 0.0f : lp[(size_t)r * t_max + i]);   // transcribe.rs:205-208
@@ -589,14 +606,16 @@ void Session::greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_d
     }
 }
 
-bool Session::beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_size, int max_depth, int64_t eot,
+bool Session::beam_decode(const std::vector<std::vector<int64_t>>& prompts, int beam_size, int max_depth, int64_t eot,
                           std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp) {
     namespace fx = beamfx;
-    WB_REQUIRE(prompt_len >= 1 && prompt_len + max_depth <= t_max, "beam: prompt + max_depth exceeds the session's max_text_len");
+    const auto [min_lp, max_lp] = prompt_range(prompts);
+    WB_REQUIRE(min_lp >= 1 && max_lp + max_depth <= t_max, "beam: prompt + max_depth exceeds the session's max_text_len");
     const int B = beam_size, W = n_windows, Rb = W * B;
     if (B < 2 || B > fx::MAX_BEAM || max_depth < 1 || Rb > Rmax) return false;
-    // slot i of window w = row w * B + i; until the first search step only slot 0 holds a beam: the prompt, in its own cache row
-    seat_rows(Rb, B, prompt, prompt_len, 0);
+    // slot i of window w = row w * B + i; until the window's first search step only slot 0 holds a beam: the prompt, in its
+    // own cache row
+    seat_rows(Rb, B, prompts, max_depth);
     constexpr int MN = fx::MAX_NODES;
     slot_live.ensure((size_t)Rmax);
     bm_head.ensure((size_t)2 * W * MN); bm_seq.ensure((size_t)2 * W * MN * t_max); bm_seq_lp.ensure((size_t)2 * W * MN * t_max);
@@ -607,8 +626,9 @@ bool Session::beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_si
     std::vector<fx::Head> heads((size_t)W * MN, fx::Head{0.0, 0, 0, 0, 0});
     std::vector<int> seq((size_t)W * MN * t_max, 0), cnt((size_t)2 * W, 0), win((size_t)2 * W, 0);   // depth-0 buffer; window: {buffer, done}
     for (int w = 0; w < W; ++w) {
-        heads[(size_t)w * MN] = fx::Head{0.0, prompt[prompt_len - 1] == eot ? 1 : 0, w * B, (int)prompt_len, 0};
-        for (int64_t i = 0; i < prompt_len; ++i) seq[(size_t)w * MN * t_max + i] = (int)prompt[i];
+        const std::vector<int64_t>& pr = prompts[(size_t)w];
+        heads[(size_t)w * MN] = fx::Head{0.0, pr.back() == eot ? 1 : 0, w * B, (int)pr.size(), 0};
+        for (size_t i = 0; i < pr.size(); ++i) seq[(size_t)w * MN * t_max + i] = (int)pr[i];
         cnt[(size_t)w] = 1;
     }
     WB_CUDA(cudaMemcpyAsync(slot_live.p, live.data(), live.size() * sizeof(int), cudaMemcpyHostToDevice, st));
@@ -618,7 +638,7 @@ bool Session::beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_si
     WB_CUDA(cudaMemcpyAsync(bm_cnt.p, cnt.data(), cnt.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     WB_CUDA(cudaMemcpyAsync(bm_win.p, win.data(), win.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     launch_dec_anc_identity(anc0.p, Rb, t_max, st);
-    const bool ran = launch_decoder(DecodeLaunch::beam_search(Rb, B, (int)prompt_len, max_depth, (int)eot));
+    const bool ran = launch_decoder(DecodeLaunch::beam_search(Rb, B, min_lp, max_lp, max_depth, (int)eot));
     std::vector<int> res((size_t)W * t_max), res_len((size_t)W);
     std::vector<float> res_lp((size_t)W * t_max);
     int sd = 0;
@@ -632,7 +652,7 @@ bool Session::beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_si
     if (!ran) return false;
     // session state as the host search leaves it: position, ancestry of the last position
     last_steps = sd;
-    host_pos = (int)prompt_len - 1 + sd;
+    host_pos = min_lp - 1 + sd;
     anc_identity = false;
     anc_cur = (sd - 1) & 1;
     out.assign((size_t)W, {});

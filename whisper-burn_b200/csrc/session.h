@@ -38,17 +38,19 @@ struct DecodeLaunch {
         return l;
     }
     // the prompt prefill (no logits), then max_depth positions of beam_size 1 of the beam search (special ids masked while
-    // a sequence has <= 5 tokens) or, with loop_rules, of the reference's greedy loop (no mask); tokens from the token buffer
-    static DecodeLaunch greedy_search(int rows, int prompt_len, int max_depth, int eot, bool loop_rules) {
+    // a sequence has <= 5 tokens) or, with loop_rules, of the reference's greedy loop (no mask); tokens from the token buffer.
+    // Rows' prompts hold min_lp .. max_lp tokens (DecArgs::lengths): logits from the shortest prompt's last position on,
+    // until the longest prompt's row has had max_depth steps
+    static DecodeLaunch greedy_search(int rows, int min_lp, int max_lp, int max_depth, int eot, bool loop_rules) {
         DecodeLaunch l;
-        l.rows = rows; l.n_steps = prompt_len - 1 + max_depth; l.logits_from = prompt_len - 1; l.eot = eot;
+        l.rows = rows; l.n_steps = max_lp - 1 + max_depth; l.logits_from = min_lp - 1; l.eot = eot; l.max_depth = max_depth;
         l.greedy = true; l.loop_rules = loop_rules; l.mask_mode = loop_rules ? MASK_NONE : MASK_SHORT;
         return l;
     }
     // the same positions for the whole width-`beam` search of rows / beam windows (decoder6 beam mode)
-    static DecodeLaunch beam_search(int rows, int beam, int prompt_len, int max_depth, int eot) {
-        DecodeLaunch l = greedy_search(rows, prompt_len, max_depth, eot, false);
-        l.greedy = false; l.k = l.beam = beam; l.max_depth = max_depth;
+    static DecodeLaunch beam_search(int rows, int beam, int min_lp, int max_lp, int max_depth, int eot) {
+        DecodeLaunch l = greedy_search(rows, min_lp, max_lp, max_depth, eot, false);
+        l.greedy = false; l.k = l.beam = beam;
         return l;
     }
 };
@@ -74,6 +76,7 @@ struct Session {
     int max_windows = 0, max_beams = 0, t_max = 0, kv_dtype = WB_KV_F32;
     int window_mode = WB_WINDOWS_REFERENCE;
     int search = WB_SEARCH_BEAM;   // set_search: the rule transcribe_windows decodes by
+    int64_t startofprev = -1;      // set_prev_prompt: >= 0 prompts each waveform window with the text before it
     int mel_limit = 0;   // window_mel_frames(n_audio_ctx, window_mode)
     int Rmax = 0;        // max_windows * max_beams decode rows
     int TmS = 0;         // rows per window in the token-major mel / conv1 buffers (mel_limit + 2 halo rows)
@@ -114,6 +117,7 @@ struct Session {
     Dec5Tables d5;                  // decoder5.cu stage descriptors
     DevBuf<uint4> att_pl, hid_pl;   // decoder5.cu activation planes
     DevBuf<float> part_o, part_m, part_l;
+    // lengths: [2][Rmax] each row's id count, then each seated row's id limit (DecArgs::lengths)
     DevBuf<int> tokens, lengths, cur_tok, finished, row_window, anc0, anc1, parent, pos, n_unfinished, topk_id;
     DevBuf<float> topk_lp;
     DevBuf<float> token_lp;    // [Rmax][t_max] log-prob of each token the greedy decoders commit (DecArgs::token_lp)
@@ -173,28 +177,35 @@ struct Session {
         WB_REQUIRE(rule == WB_SEARCH_BEAM || rule == WB_SEARCH_GREEDY_LOOP, "set_search: unknown search rule");
         search = rule;
     }
+    void set_prev_prompt(int64_t id) {
+        WB_REQUIRE(id == -1 || (id >= 0 && id < m->dims.n_vocab), "set_prev_prompt: startofprev must be -1 or an id in [0, n_vocab)");
+        startofprev = id;
+    }
     void set_special(const uint8_t* is_special_host);
-    // Seats `rows` rows for a new decode from position 0: row r decodes window r / per_window from the prompt_len tokens at
-    // prompt + r * prompt_stride (token buffer, lengths); no row is finished and every row reads only its own cache rows
-    void seat_rows(int rows, int per_window, const int64_t* prompt, int64_t prompt_len, int64_t prompt_stride);
+    // Seats `rows` rows for a new decode from position 0: row r decodes window r / per_window from the tokens of
+    // prompts[r / per_window] (token buffer, lengths, id limits prompt length + max_depth); no row is finished and every row
+    // reads only its own cache rows
+    void seat_rows(int rows, int per_window, const std::vector<std::vector<int64_t>>& prompts, int max_depth = 0);
     // teacher forcing right after seat_rows: positions [0, n) of every row from its token buffer, one cached step each;
     // with logits_out (host), each position's raw logits go to logits_out [R][n][V]
     void feed_positions(int n, float* logits_out);
-    void begin(const int64_t* prompt, int64_t prompt_len, bool prefill = true);
+    // seats window w with prompts[w] (max_depth: the greedy search's steps after each prompt); the prefill feeds the
+    // positions before the shortest prompt's last token
+    void begin(const std::vector<std::vector<int64_t>>& prompts, bool prefill = true, int max_depth = 0);
     // the stateless forward_decoder: every position's logits [n_rows][seq_len][V] of tokens [n_rows][seq_len]
     void teacher_forced_logits(const int64_t* tokens, int64_t n_rows, int64_t seq_len, float* logits_out);
     void step_beams(int64_t n_rows, const int32_t* window_of_row, const int32_t* parent_row, const int64_t* token,
                     int apply_mask, int k, int64_t* topk_ids_out, float* topk_lp_out);
     // the [n_rows][k] candidates the last launch wrote at its last position
     void last_topk(int64_t n_rows, int64_t k, int64_t* ids_out, float* lp_out);
-    // greedy search on the device in one launch; returns per-window token lists and the log-prob of each token (0 for the
-    // prompt, NaN for an EOT a rule appended).  loop_rules: the reference's greedy loop (WB_SEARCH_GREEDY_LOOP) instead of
-    // beam_size 1
-    void greedy_decode(const int64_t* prompt, int64_t prompt_len, int max_depth, int64_t eot,
+    // greedy search of window w from prompts[w] on the device in one launch; returns per-window token lists and the log-prob
+    // of each token (0 for the prompt, NaN for an EOT a rule appended).  loop_rules: the reference's greedy loop
+    // (WB_SEARCH_GREEDY_LOOP) instead of beam_size 1
+    void greedy_decode(const std::vector<std::vector<int64_t>>& prompts, int max_depth, int64_t eot,
                        std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp, bool loop_rules = false);
-    // the whole beam search (prefill + up to max_depth steps) of every encoded window in ONE decoder launch; false (nothing
-    // decoded) when no decoder covers it, and the caller runs the host search
-    bool beam_decode(const int64_t* prompt, int64_t prompt_len, int beam_size, int max_depth, int64_t eot,
+    // the whole beam search (prefill + up to max_depth steps after each window's prompt) of every encoded window in ONE
+    // decoder launch; false (nothing decoded) when no decoder covers it, and the caller runs the host search
+    bool beam_decode(const std::vector<std::vector<int64_t>>& prompts, int beam_size, int max_depth, int64_t eot,
                      std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp);
     // teacher-forced scoring of n_seqs packed token sequences (wb_session_score_tokens): per position j >= 1 the log-prob of
     // token j given tokens 0 .. j-1 and the arg-max id; reads the cross K/V of the encoded windows, writes no decode state
@@ -203,10 +214,12 @@ struct Session {
     ScoreWs score_ws;
 };
 
-// host pipeline (transcribe.cu): per window the ids and the log-prob each was chosen with (BeamSearchToken.log_prob)
+// host pipeline (transcribe.cu): per window the ids and the log-prob each was chosen with (BeamSearchToken.log_prob).
+// prev: per encoded window the previous ids of its prompt (mels_to_text's prev_nonspecial_tokens), or empty for none
 void transcribe_windows(Session& s, int beam_size, int max_depth, const wb_special_ids& ids,
                         const uint8_t* is_special, std::vector<std::vector<int64_t>>& out,
-                        std::vector<std::vector<float>>& out_lp);
+                        std::vector<std::vector<float>>& out_lp,
+                        const std::vector<std::vector<int64_t>>& prev = {}, int64_t startofprev = -1);
 std::vector<std::pair<int64_t, int64_t>> window_bounds(int64_t n_samples, int64_t sample_rate, int64_t window_len);
 bool find_chunk_overlap(const int64_t* prev, int64_t n_prev, const int64_t* curr, int64_t n_curr, int64_t max_n_offsets,
                         int64_t min_n_overlaps, int64_t* prev_index, int64_t* curr_index);

@@ -64,6 +64,7 @@ SYMBOLS = {
     "wb_session_create_windows": (C.c_int, [_P, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_int, C.POINTER(_P)]),
     "wb_session_destroy": (None, [_P]),
     "wb_session_set_search": (C.c_int, [_P, C.c_int]),
+    "wb_session_set_prev_prompt": (C.c_int, [_P, C.c_int64]),
     "wb_session_encode_waveforms": (C.c_int, [_P, C.POINTER(_F), _I64, C.c_int64]),
     "wb_session_encode_waveforms_dev": (C.c_int, [_P, _P, _I64, _I64, C.c_int64]),
     "wb_session_encode_mels": (C.c_int, [_P, _F, C.c_int64, C.c_int64, C.c_int64]),
@@ -75,6 +76,8 @@ SYMBOLS = {
                                         C.POINTER(SpecialIds), _U8, _I64, C.c_int64, _I64]),
     "wb_transcribe_windows_dev": (C.c_int, [_P, _P, _I64, _I64, C.c_int64, C.c_int, C.c_int,
                                             C.POINTER(SpecialIds), _U8, _I64, C.c_int64, _I64]),
+    "wb_transcribe_windows_prev": (C.c_int, [_P, C.POINTER(_F), _I64, C.c_int64, _I64, _I64, C.c_int64, C.c_int, C.c_int,
+                                             C.POINTER(SpecialIds), _U8, _I64, C.c_int64, _I64]),
     "wb_waveform_to_tokens": (C.c_int, [_P, _F, C.c_int64, C.c_int64, C.c_int, C.c_int,
                                         C.POINTER(SpecialIds), _U8, _I64, C.c_int64, _I64]),
     "wb_waveforms_to_tokens": (C.c_int, [_P, C.POINTER(C.c_void_p), _I64, C.c_int64, C.c_int64, C.c_int, C.c_int,

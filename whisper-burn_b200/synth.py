@@ -12,7 +12,7 @@ across numpy versions and machines):
                logits are trivially self-predicting and parity checks would be vacuous.
                Every value is rounded to an fp16-representable f32, as OpenAI's released
                checkpoints are (they are stored in fp16; python/dump.py writes them out as f32).
-  * tokenizer stand-in: 5 special ids >= eot and ``is_special(id) <=> id >= eot``.
+  * tokenizer stand-in: 6 special ids >= eot (startofprev = eot + 5) and ``is_special(id) <=> id >= eot``.
 """
 from __future__ import annotations
 
@@ -51,6 +51,7 @@ class SpecialTokens:
     eot: int
     first_special: int   # is_special(id) <=> id >= first_special (stand-in for src/token.rs:41-47)
     n_vocab: int
+    startofprev: int = -1   # <|startofprev|> (token.rs:280-294), the first id of a previous-text prompt; -1: unknown
 
     def is_special(self, tok: int) -> bool:
         return tok >= self.first_special
@@ -115,7 +116,7 @@ def special_tokens(dims: WhisperDims) -> SpecialTokens:
     v = dims.n_vocab
     eot = 50256 if v == 51864 else (50257 if v == 51865 else v - 16)
     return SpecialTokens(sot=eot + 1, lang=eot + 2, transcribe=eot + 3, notimestamps=eot + 4,
-                         eot=eot, first_special=eot, n_vocab=v)
+                         eot=eot, first_special=eot, n_vocab=v, startofprev=eot + 5)
 
 
 def _fp16_exact(a: np.ndarray) -> np.ndarray:

@@ -51,7 +51,8 @@ def is_special_bitmap(path, n_vocab: int = 0) -> np.ndarray:
 
 
 def special_tokens(path, language: str = "en", n_vocab: int = 0) -> SpecialTokens:
-    """The ids mels_to_text looks up (transcribe.rs:179-185): prompt = [sot, <|lang|>, transcribe, notimestamps]."""
+    """The ids mels_to_text looks up (transcribe.rs:179-185): prompt = [sot, <|lang|>, transcribe, notimestamps], and
+    <|startofprev|>, which begins a previous-text prompt (transcribe.rs:195-199)."""
     vocab, special = _tables(path)
 
     def tid(s: str) -> int:
@@ -62,4 +63,4 @@ def special_tokens(path, language: str = "en", n_vocab: int = 0) -> SpecialToken
     v = n_vocab or len(set(vocab.values()))
     return SpecialTokens(sot=tid("<|startoftranscript|>"), lang=tid(f"<|{language}|>"), transcribe=tid("<|transcribe|>"),
                          notimestamps=tid("<|notimestamps|>"), eot=tid("<|endoftext|>"),
-                         first_special=min(special) if special else v, n_vocab=v)
+                         first_special=min(special) if special else v, n_vocab=v, startofprev=vocab.get("<|startofprev|>", -1))

@@ -66,6 +66,12 @@ class Session:
             pass
 
     # ---- encode
+    def set_prev_prompt(self, startofprev: int) -> None:
+        """The previous-text prompt of waveform(s)_to_tokens (wb_session_set_prev_prompt): -1 (the default) decodes every window
+        from [sot, lang, transcribe, notimestamps]; the <|startofprev|> id prompts window i of a waveform with
+        [startofprev] + the last (at most) 5 non-special merged ids so far + those 4 ids, the windows of a waveform in order."""
+        ffi.check(ffi.lib().wb_session_set_prev_prompt(self._h, startofprev))
+
     def encode_waveforms(self, waves: Sequence[np.ndarray]) -> None:
         ws = [np.ascontiguousarray(w, dtype=np.float32) for w in waves]
         ptrs = (ffi._F * len(ws))(*[ffi.fptr(w) for w in ws])
@@ -125,6 +131,29 @@ class Session:
                                                  C.byref(ids), sp, ffi.i64ptr(out), cap, ffi.i64ptr(out_len)))
         return [[int(t) for t in out[i, :out_len[i]]] for i in range(len(ws))]
 
+    def transcribe_windows_prev(self, waves: Sequence[np.ndarray], prev: Sequence[Sequence[int]], special,
+                                is_special: Optional[np.ndarray], beam_size: int = 5, max_depth: int = 100,
+                                startofprev: Optional[int] = None) -> List[List[int]]:
+        """mels_to_text with its prev_nonspecial_tokens given per window (wb_transcribe_windows_prev): window i is decoded
+        from [startofprev] + prev[i] + [sot, lang, transcribe, notimestamps], or the 4 ids when prev[i] is empty; rows hold
+        the prompt first.  startofprev defaults to special.startofprev."""
+        ws = [np.ascontiguousarray(w, dtype=np.float32) for w in waves]
+        if len(prev) != len(ws):
+            raise ValueError(f"transcribe_windows_prev: {len(ws)} windows but {len(prev)} previous-id lists")
+        ptrs = (ffi._F * len(ws))(*[ffi.fptr(w) for w in ws])
+        lens = np.asarray([w.shape[0] for w in ws], dtype=np.int64)
+        prev_lens = np.asarray([len(p) for p in prev], dtype=np.int64)
+        prev_toks = np.ascontiguousarray(np.concatenate([np.asarray(p, dtype=np.int64) for p in prev] + [np.zeros(1, np.int64)]))
+        cap = max([4] + [len(p) + 5 for p in prev if len(p)]) + max_depth + 1
+        out = np.zeros((len(ws), cap), dtype=np.int64)
+        out_len = np.zeros(len(ws), dtype=np.int64)
+        ids = ffi.SpecialIds(special.sot, special.lang, special.transcribe, special.notimestamps, special.eot)
+        sop = special.startofprev if startofprev is None else startofprev
+        ffi.check(ffi.lib().wb_transcribe_windows_prev(self._h, ptrs, ffi.i64ptr(lens), len(ws), ffi.i64ptr(prev_toks),
+                                                      ffi.i64ptr(prev_lens), sop, beam_size, max_depth, C.byref(ids),
+                                                      _special(is_special), ffi.i64ptr(out), cap, ffi.i64ptr(out_len)))
+        return [[int(t) for t in out[i, :out_len[i]]] for i in range(len(ws))]
+
     def transcribe_windows_dev(self, wave_dev_ptr: int, offsets, lens, special, is_special: np.ndarray,
                                beam_size: int = 5, max_depth: int = 100) -> List[List[int]]:
         """Same, windows already resident in HBM (device pointer + element offsets)."""
@@ -143,7 +172,7 @@ class Session:
     def waveform_to_tokens(self, waveform: np.ndarray, special, is_special: np.ndarray, sample_rate: int = 16000,
                            beam_size: int = 5, max_depth: int = 100) -> List[int]:
         w = np.ascontiguousarray(waveform, dtype=np.float32)
-        cap = (len(w) // 1000 + 2) * (4 + max_depth + 1) + 16
+        cap = (len(w) // 1000 + 2) * (10 + max_depth + 1) + 16
         out = np.zeros(cap, dtype=np.int64)
         n = C.c_int64(0)
         ids = ffi.SpecialIds(special.sot, special.lang, special.transcribe, special.notimestamps, special.eot)
@@ -156,7 +185,7 @@ class Session:
                             beam_size: int = 5, max_depth: int = 100) -> List[List[int]]:
         """Batched waveform_to_tokens: all windows of all waveforms decoded together (wb_waveforms_to_tokens)."""
         ws = [np.ascontiguousarray(w, dtype=np.float32) for w in waveforms]
-        cap = (max(len(w) for w in ws) // 1000 + 2) * (4 + max_depth + 1) + 16
+        cap = (max(len(w) for w in ws) // 1000 + 2) * (10 + max_depth + 1) + 16
         out = np.zeros((len(ws), cap), dtype=np.int64)
         n = np.zeros(len(ws), dtype=np.int64)
         ptrs = (C.c_void_p * len(ws))(*[w.ctypes.data for w in ws])
