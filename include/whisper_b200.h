@@ -240,9 +240,12 @@ int wb_waveform_to_tokens(wb_session* s, const float* waveform, int64_t n_sample
 int wb_waveforms_to_tokens(wb_session* s, const float* const* waveforms, const int64_t* n_samples, int64_t n_waveforms,
                            int64_t sample_rate, int beam_size, int max_depth, const wb_special_ids* ids,
                            const uint8_t* is_special, int64_t* tokens_out, int64_t capacity, int64_t* n_tokens_out);
-/* Per-token log-probs of the last wb_transcribe_windows[_dev] (index = window) or wb_waveform(s)_to_tokens (index = waveform)
- * call on this session, aligned with the ids that call wrote: n_out = that row's id count.  WB_ERR_STATE before the first such
- * call, WB_ERR_INVALID_ARG for an index out of range or capacity < n_out.  out == NULL only sets n_out.
+/* Per-token log-probs of the last wb_transcribe_windows[_dev/_prev] (index = window) or wb_waveform(s)_to_tokens (index =
+ * waveform) call on this session, aligned with the ids that call wrote: n_out = that row's id count.  WB_ERR_STATE before the
+ * first such call, WB_ERR_INVALID_ARG for an index out of range or capacity < n_out.  out == NULL only sets n_out.
+ * Those calls check every argument that does not depend on decoded ids before they encode (the waveform calls: each batch's
+ * before that batch's encode); a call rejected there leaves the encoded windows, these log-probs, wb_session_last_timings
+ * and wb_session_last_steps as they were.  A call that fails later (a row beyond capacity, say) leaves no log-probs.
  * The values (float32; the reference's BeamSearchToken.log_prob, transcribe.rs:142-146, holds the same f32 widened to f64):
  *   - the prompt ids (4, or those of a previous-text prompt): 0.0 (transcribe.rs:205-208);
  *   - WB_SEARCH_BEAM, beam_size >= 2: the f32 log_softmax value the search scored the id with, special-id mask included
@@ -318,7 +321,8 @@ int wb_session_last_topk(wb_session* s, int64_t n_rows, int64_t k, int64_t* ids_
 int64_t wb_kernel_launch_count(void);
 void wb_kernel_launch_count_reset(void);
 /* device-side duration (CUDA events on the session stream) of the phases of the last
- * wb_transcribe_windows* call, in milliseconds: [0]=log-mel, [1]=encoder+cross-KV, [2]=decode, [3]=total */
+ * wb_transcribe_windows* call, in milliseconds: [0]=log-mel, [1]=encoder+cross-KV, [2]=decode, [3]=total; a call rejected
+ * before it encodes leaves them as they were (wb_session_last_logprobs) */
 int wb_session_last_timings(wb_session* s, float* ms_out4);
 int wb_session_last_steps(wb_session* s, int64_t* n_steps_out);
 /* roofline aid: re-runs n_steps greedy decoder steps on the currently encoded windows with CUDA

@@ -29,11 +29,6 @@ struct wb_model {
 };
 struct wb_session {
     std::unique_ptr<wb::Session> impl;
-    wb_model* model;
-    // per output row of the last transcribe / waveform(s)_to_tokens call, the log-prob of each id (wb_session_last_logprobs);
-    // empty with have_logprobs == false until a call succeeds
-    std::vector<std::vector<float>> logprobs;
-    bool have_logprobs = false;
 };
 
 namespace {
@@ -66,26 +61,12 @@ void require_device(int device) {
     WB_CUDA(cudaSetDevice(device));
 }
 
-void copy_tokens_out(const std::vector<std::vector<int64_t>>& toks, int64_t* tokens_out, int64_t capacity,
-                     int64_t* lens_out) {
+// row w of the ids to tokens_out[w * capacity ..], its length to lens_out[w] (the pipeline has checked that rows fit)
+void copy_tokens_out(const std::vector<std::vector<int64_t>>& toks, int64_t* tokens_out, int64_t capacity, int64_t* lens_out) {
     for (size_t w = 0; w < toks.size(); ++w) {
-        WB_REQUIRE((int64_t)toks[w].size() <= capacity, "tokens_out capacity too small");
-        for (size_t i = 0; i < toks[w].size(); ++i) tokens_out[(int64_t)w * capacity + (int64_t)i] = toks[w][i];
+        std::copy(toks[w].begin(), toks[w].end(), tokens_out + (int64_t)w * capacity);
         lens_out[w] = (int64_t)toks[w].size();
     }
-}
-
-// the decode calls need the is_special bitmap, except under the greedy loop, which masks nothing
-bool special_given(const wb_session* s, const uint8_t* is_special) {
-    return is_special != nullptr || (s && s->impl->search == WB_SEARCH_GREEDY_LOOP);
-}
-
-void collect_timings(wb::Session& s) {
-    WB_CUDA(cudaStreamSynchronize(s.st));
-    cudaEventElapsedTime(&s.last_ms[0], s.ev[0], s.ev[1]);
-    cudaEventElapsedTime(&s.last_ms[1], s.ev[1], s.ev[2]);
-    cudaEventElapsedTime(&s.last_ms[2], s.ev[2], s.ev[3]);
-    cudaEventElapsedTime(&s.last_ms[3], s.ev[0], s.ev[3]);
 }
 
 // prep_audio on the device; `wave` and `mel_out` are device pointers
@@ -302,7 +283,6 @@ int wb_session_create_windows(wb_model* m, int64_t max_windows, int64_t max_beam
     return guarded([&] {
         WB_REQUIRE(m && out, "session_create: null pointer");
         std::unique_ptr<wb_session> s(new wb_session());
-        s->model = m;
         s->impl.reset(new wb::Session(&m->impl, max_windows, max_beams, max_text_len, kv_dtype, window_mode));
         *out = s.release();
     });
@@ -408,14 +388,12 @@ int wb_transcribe_windows(wb_session* s, const float* const* waves, const int64_
                           int beam_size, int max_depth, const wb_special_ids* ids, const uint8_t* is_special,
                           int64_t* tokens_out, int64_t capacity, int64_t* lens_out) {
     return guarded([&] {
-        WB_REQUIRE(s && waves && lens && ids && special_given(s, is_special) && tokens_out && lens_out, "transcribe: null pointer");
-        s->have_logprobs = false;
-        s->impl->encode_waveforms_host(waves, lens, n_windows);
-        std::vector<std::vector<int64_t>> toks;
-        wb::transcribe_windows(*s->impl, beam_size, max_depth, *ids, is_special, toks, s->logprobs);
-        copy_tokens_out(toks, tokens_out, capacity, lens_out);
-        collect_timings(*s->impl);
-        s->have_logprobs = true;
+        WB_REQUIRE(s && waves && lens && ids && tokens_out && lens_out, "transcribe: null pointer");
+        wb::Session& S = *s->impl;
+        const auto prompts = wb::window_prompts(S, n_windows, beam_size, max_depth, *ids, is_special);
+        copy_tokens_out(wb::transcribe_windows(S, prompts, beam_size, max_depth, ids->eot, is_special, capacity,
+                                               [&] { S.encode_waveforms_host(waves, lens, n_windows); }),
+                        tokens_out, capacity, lens_out);
     });
 }
 
@@ -424,34 +402,24 @@ int wb_transcribe_windows_prev(wb_session* s, const float* const* waves, const i
                                int max_depth, const wb_special_ids* ids, const uint8_t* is_special, int64_t* tokens_out,
                                int64_t capacity, int64_t* lens_out) {
     return guarded([&] {
-        WB_REQUIRE(s && waves && lens && prev_lens && ids && special_given(s, is_special) && tokens_out && lens_out,
-                   "transcribe_windows_prev: null pointer");
+        WB_REQUIRE(s && waves && lens && prev_lens && ids && tokens_out && lens_out, "transcribe_windows_prev: null pointer");
         wb::Session& S = *s->impl;
         WB_REQUIRE(n_windows >= 1 && n_windows <= S.max_windows, "transcribe_windows_prev: n_windows out of range");
-        WB_REQUIRE(startofprev >= 0 && startofprev < S.m->dims.n_vocab, "transcribe_windows_prev: startofprev id out of range");
-        WB_REQUIRE(max_depth >= 0, "transcribe_windows_prev: negative max_depth");
         std::vector<std::vector<int64_t>> prev((size_t)n_windows);
-        int64_t off = 0, max_lp = 4;
+        int64_t off = 0;
         for (int64_t w = 0; w < n_windows; ++w) {
             WB_REQUIRE(prev_lens[w] >= 0, "transcribe_windows_prev: negative prev_lens entry");
             WB_REQUIRE(prev_lens[w] == 0 || prev_tokens, "transcribe_windows_prev: null prev_tokens");
-            WB_REQUIRE(prev_lens[w] == 0 || S.search != WB_SEARCH_GREEDY_LOOP,
-                       "transcribe_windows_prev: the greedy loop builds its own prompt; no previous ids with it");
             prev[(size_t)w].assign(prev_tokens + off, prev_tokens + off + prev_lens[w]);
-            for (int64_t t : prev[(size_t)w])
-                WB_REQUIRE(t >= 0 && t < S.m->dims.n_vocab, "transcribe_windows_prev: previous id out of range");
             off += prev_lens[w];
-            max_lp = std::max(max_lp, prev_lens[w] > 0 ? prev_lens[w] + 5 : 4);
         }
-        WB_REQUIRE(max_lp + max_depth <= S.t_max, "transcribe_windows_prev: prompt + max_depth exceeds the session's max_text_len");
-        WB_REQUIRE(capacity >= max_lp + max_depth + 1, "transcribe_windows_prev: capacity below prompt + max_depth + 1");
-        s->have_logprobs = false;
-        S.encode_waveforms_host(waves, lens, n_windows);
-        std::vector<std::vector<int64_t>> toks;
-        wb::transcribe_windows(S, beam_size, max_depth, *ids, is_special, toks, s->logprobs, prev, startofprev);
-        copy_tokens_out(toks, tokens_out, capacity, lens_out);
-        collect_timings(S);
-        s->have_logprobs = true;
+        const auto prompts = wb::window_prompts(S, n_windows, beam_size, max_depth, *ids, is_special, prev, startofprev);
+        size_t max_lp = 0;
+        for (const auto& pr : prompts) max_lp = std::max(max_lp, pr.size());
+        WB_REQUIRE(capacity >= (int64_t)max_lp + max_depth + 1, "transcribe_windows_prev: capacity below prompt + max_depth + 1");
+        copy_tokens_out(wb::transcribe_windows(S, prompts, beam_size, max_depth, ids->eot, is_special, capacity,
+                                               [&] { S.encode_waveforms_host(waves, lens, n_windows); }),
+                        tokens_out, capacity, lens_out);
     });
 }
 
@@ -459,14 +427,12 @@ int wb_transcribe_windows_dev(wb_session* s, const float* wave_dev, const int64_
                               int64_t n_windows, int beam_size, int max_depth, const wb_special_ids* ids,
                               const uint8_t* is_special, int64_t* tokens_out, int64_t capacity, int64_t* lens_out) {
     return guarded([&] {
-        WB_REQUIRE(s && wave_dev && offsets && lens && ids && special_given(s, is_special) && tokens_out && lens_out, "transcribe: null pointer");
-        s->have_logprobs = false;
-        s->impl->encode_from_device_wave(wave_dev, offsets, lens, n_windows);
-        std::vector<std::vector<int64_t>> toks;
-        wb::transcribe_windows(*s->impl, beam_size, max_depth, *ids, is_special, toks, s->logprobs);
-        copy_tokens_out(toks, tokens_out, capacity, lens_out);
-        collect_timings(*s->impl);
-        s->have_logprobs = true;
+        WB_REQUIRE(s && wave_dev && offsets && lens && ids && tokens_out && lens_out, "transcribe: null pointer");
+        wb::Session& S = *s->impl;
+        const auto prompts = wb::window_prompts(S, n_windows, beam_size, max_depth, *ids, is_special);
+        copy_tokens_out(wb::transcribe_windows(S, prompts, beam_size, max_depth, ids->eot, is_special, capacity,
+                                               [&] { S.encode_from_device_wave(wave_dev, offsets, lens, n_windows); }),
+                        tokens_out, capacity, lens_out);
     });
 }
 
@@ -482,134 +448,32 @@ int wb_window_bounds(int64_t n_samples, int64_t sample_rate, int64_t window_len,
     });
 }
 
-// the overlap merge of one window's ids and log-probs into its waveform's (transcribe.rs:56-63)
-static void merge_window(std::vector<int64_t>& tokens, std::vector<float>& tlp, const std::vector<int64_t>& nt,
-                         const std::vector<float>& nl) {
-    int64_t pi = 0, ci = 0;
-    if (wb::find_chunk_overlap(tokens.data(), (int64_t)tokens.size(), nt.data(), (int64_t)nt.size(), 40, 3, &pi, &ci)) {
-        tokens.resize((size_t)pi);                                    // transcribe.rs:59-60
-        tokens.insert(tokens.end(), nt.begin() + ci, nt.end());
-        tlp.resize((size_t)pi);
-        tlp.insert(tlp.end(), nl.begin() + ci, nl.end());
-    } else {
-        tokens.insert(tokens.end(), nt.begin(), nt.end());
-        tlp.insert(tlp.end(), nl.begin(), nl.end());
-    }
-}
-
-// transcribe.rs:43-50: the last (at most) 5 ids of the merged tokens that are not special, in order
-static std::vector<int64_t> prev_nonspecial(const std::vector<int64_t>& tokens, const uint8_t* is_special) {
-    std::vector<int64_t> prev;
-    for (size_t i = tokens.size(); i-- > 0 && prev.size() < 5;)
-        if (!is_special[tokens[i]]) prev.push_back(tokens[i]);
-    std::reverse(prev.begin(), prev.end());
-    return prev;
-}
-
-// windows of ALL waveforms are decoded together in batches of the session's capacity (they are independent,
-// SURVEY.md F9), then each waveform's windows are merged in order exactly like the reference's sequential
-// loop (transcribe.rs:42-71); each id's log-prob travels with it through the merge into out_lp.
-// With the previous-text prompt (Session::startofprev >= 0) window i of a waveform needs the merged ids of windows
-// 0 .. i-1: round i decodes window i of every waveform that has one, in batches of the session's capacity.
-static void waveforms_to_tokens(wb::Session& S, const float* const* waveforms, const int64_t* n_samples, int64_t n_waveforms,
-                                int64_t sample_rate, int beam_size, int max_depth, const wb_special_ids& ids,
-                                const uint8_t* is_special, std::vector<std::vector<int64_t>>& out,
-                                std::vector<std::vector<float>>& out_lp) {
-    // the frontend tables (mel filterbank, DFT bins) are the 16 kHz ones: the reference builds them from the caller's rate
-    // (audio.rs:44, 67-143) but its binary only ever passes 16 kHz (src/bin/transcribe/main.rs:38-41 asserts it)
-    WB_REQUIRE(sample_rate == 16000, "waveform_to_tokens: only 16 kHz input is supported (frontend tables are built for 16 kHz)");
-    const int64_t window_len = wb::window_samples(S.m->dims.n_audio_ctx, S.window_mode);   // transcribe.rs:32-34
-    std::vector<const float*> ptrs;
-    std::vector<int64_t> lens;
-    std::vector<int> owner;
-    for (int64_t w = 0; w < n_waveforms; ++w)
-        for (const auto& b : wb::window_bounds(n_samples[w], sample_rate, window_len)) {
-            ptrs.push_back(waveforms[w] + b.first);
-            lens.push_back(b.second - b.first);
-            owner.push_back((int)w);
-        }
-    out.assign((size_t)n_waveforms, {});
-    out_lp.assign((size_t)n_waveforms, {});
-    const bool prev_prompt = S.startofprev >= 0;
-    if (prev_prompt) {
-        WB_REQUIRE(S.search != WB_SEARCH_GREEDY_LOOP, "waveform_to_tokens: the greedy loop builds its own prompt; no previous-text prompt with it");
-        WB_REQUIRE(is_special != nullptr, "waveform_to_tokens: the previous-text prompt needs is_special");
-    }
-    // batches: window-major order (all windows at once) or, with the previous-text prompt, rounds of window index i
-    std::vector<std::vector<size_t>> rounds(1);
-    if (prev_prompt) {
-        std::vector<int> idx((size_t)n_waveforms, 0);
-        for (size_t j = 0; j < ptrs.size(); ++j) {
-            const size_t i = (size_t)idx[(size_t)owner[j]]++;
-            if (rounds.size() <= i) rounds.resize(i + 1);
-            rounds[i].push_back(j);
-        }
-    } else {
-        for (size_t j = 0; j < ptrs.size(); ++j) rounds[0].push_back(j);
-    }
-    for (const std::vector<size_t>& round : rounds) {
-        for (size_t b0 = 0; b0 < round.size(); b0 += (size_t)S.max_windows) {
-            const size_t nb = std::min(round.size() - b0, (size_t)S.max_windows);
-            std::vector<const float*> bp(nb);
-            std::vector<int64_t> bl(nb);
-            std::vector<std::vector<int64_t>> prev(prev_prompt ? nb : 0);
-            for (size_t i = 0; i < nb; ++i) {
-                const size_t j = round[b0 + i];
-                bp[i] = ptrs[j];
-                bl[i] = lens[j];
-                if (prev_prompt) prev[i] = prev_nonspecial(out[(size_t)owner[j]], is_special);
-            }
-            S.encode_waveforms_host(bp.data(), bl.data(), (int64_t)nb);
-            std::vector<std::vector<int64_t>> toks;
-            std::vector<std::vector<float>> lps;
-            wb::transcribe_windows(S, beam_size, max_depth, ids, is_special, toks, lps, prev, S.startofprev);
-            for (size_t i = 0; i < nb; ++i)
-                merge_window(out[(size_t)owner[round[b0 + i]]], out_lp[(size_t)owner[round[b0 + i]]], toks[i], lps[i]);
-        }
-    }
-    collect_timings(S);
-}
-
 int wb_waveform_to_tokens(wb_session* s, const float* waveform, int64_t n_samples, int64_t sample_rate, int beam_size,
                           int max_depth, const wb_special_ids* ids, const uint8_t* is_special, int64_t* tokens_out,
                           int64_t capacity, int64_t* n_tokens_out) {
-    return guarded([&] {
-        WB_REQUIRE(s && waveform && ids && special_given(s, is_special) && tokens_out && n_tokens_out, "waveform_to_tokens: null pointer");
-        s->have_logprobs = false;
-        std::vector<std::vector<int64_t>> out;
-        waveforms_to_tokens(*s->impl, &waveform, &n_samples, 1, sample_rate, beam_size, max_depth, *ids, is_special, out, s->logprobs);
-        WB_REQUIRE((int64_t)out[0].size() <= capacity, "tokens_out capacity too small");
-        std::memcpy(tokens_out, out[0].data(), out[0].size() * sizeof(int64_t));
-        *n_tokens_out = (int64_t)out[0].size();
-        s->have_logprobs = true;
-    });
+    if (!waveform) return guarded([] { wb::fail(WB_ERR_INVALID_ARG, "waveform_to_tokens: null pointer"); });
+    return wb_waveforms_to_tokens(s, &waveform, &n_samples, 1, sample_rate, beam_size, max_depth, ids, is_special, tokens_out,
+                                  capacity, n_tokens_out);
 }
 
 int wb_waveforms_to_tokens(wb_session* s, const float* const* waveforms, const int64_t* n_samples, int64_t n_waveforms,
                            int64_t sample_rate, int beam_size, int max_depth, const wb_special_ids* ids,
                            const uint8_t* is_special, int64_t* tokens_out, int64_t capacity, int64_t* n_tokens_out) {
     return guarded([&] {
-        WB_REQUIRE(s && waveforms && n_samples && ids && special_given(s, is_special) && tokens_out && n_tokens_out, "waveforms_to_tokens: null pointer");
-        WB_REQUIRE(n_waveforms >= 1, "waveforms_to_tokens: n_waveforms must be >= 1");
-        s->have_logprobs = false;
-        std::vector<std::vector<int64_t>> out;
-        waveforms_to_tokens(*s->impl, waveforms, n_samples, n_waveforms, sample_rate, beam_size, max_depth, *ids, is_special, out,
-                            s->logprobs);
-        for (int64_t w = 0; w < n_waveforms; ++w) {
-            WB_REQUIRE((int64_t)out[(size_t)w].size() <= capacity, "tokens_out capacity (per waveform) too small");
-            std::memcpy(tokens_out + w * capacity, out[(size_t)w].data(), out[(size_t)w].size() * sizeof(int64_t));
-            n_tokens_out[w] = (int64_t)out[(size_t)w].size();
-        }
-        s->have_logprobs = true;
+        WB_REQUIRE(s && waveforms && n_samples && ids && tokens_out && n_tokens_out, "waveforms_to_tokens: null pointer");
+        copy_tokens_out(wb::waveforms_to_tokens(*s->impl, waveforms, n_samples, n_waveforms, sample_rate, beam_size, max_depth,
+                                                *ids, is_special, capacity),
+                        tokens_out, capacity, n_tokens_out);
     });
 }
 
 int wb_session_last_logprobs(wb_session* s, int64_t index, float* out, int64_t capacity, int64_t* n_out) {
     return guarded([&] {
         WB_REQUIRE(s && n_out, "last_logprobs: null pointer");
-        if (!s->have_logprobs) wb::fail(WB_ERR_STATE, "last_logprobs: no transcribe or waveform(s)_to_tokens call yet");
-        WB_REQUIRE(index >= 0 && index < (int64_t)s->logprobs.size(), "last_logprobs: index out of range");
-        const std::vector<float>& v = s->logprobs[(size_t)index];
+        const wb::Session& S = *s->impl;
+        if (!S.have_logprobs) wb::fail(WB_ERR_STATE, "last_logprobs: no transcribe or waveform(s)_to_tokens call yet");
+        WB_REQUIRE(index >= 0 && index < (int64_t)S.last_logprobs.size(), "last_logprobs: index out of range");
+        const std::vector<float>& v = S.last_logprobs[(size_t)index];
         *n_out = (int64_t)v.size();
         if (!out) return;   // size query
         WB_REQUIRE(capacity >= (int64_t)v.size(), "last_logprobs: capacity too small");

@@ -1,6 +1,7 @@
 // Decoding session: all device state between prep_audio and the emitted token ids.  Internal.
 #pragma once
 #include <climits>
+#include <functional>
 #include <memory>
 #include <vector>
 
@@ -132,8 +133,12 @@ struct Session {
     Pinned<int> h_parent, h_window, h_token, h_topk_id;
     // ev[0..3]: timings of the last transcribe call; ev[4], ev[5]: the launch profile_decode times
     cudaEvent_t ev[6] = {};
+    // results of the last transcribe / waveform(s)_to_tokens call: timings, search steps, per output row the log-prob of each
+    // id (have_logprobs: that call succeeded).  A call rejected before it encodes leaves them as they were.
     float last_ms[4] = {0, 0, 0, 0};
     int64_t last_steps = 0;
+    std::vector<std::vector<float>> last_logprobs;
+    bool have_logprobs = false;
     int last_groups = 1;         // row groups (launches) of the last decode
     int last_decoder = 0;        // which persistent decoder the last launch used (6, 5, 4 or 3); 0 = none yet
     int last_rows = 0, last_k = 0;   // rows and candidates per row of the last launch (its topk_id / topk_lp)
@@ -214,12 +219,20 @@ struct Session {
     ScoreWs score_ws;
 };
 
-// host pipeline (transcribe.cu): per window the ids and the log-prob each was chosen with (BeamSearchToken.log_prob).
-// prev: per encoded window the previous ids of its prompt (mels_to_text's prev_nonspecial_tokens), or empty for none
-void transcribe_windows(Session& s, int beam_size, int max_depth, const wb_special_ids& ids,
-                        const uint8_t* is_special, std::vector<std::vector<int64_t>>& out,
-                        std::vector<std::vector<float>>& out_lp,
-                        const std::vector<std::vector<int64_t>>& prev = {}, int64_t startofprev = -1);
+// host pipeline (transcribe.cu).  window_prompts checks every argument of a decode call and builds each window's prompt
+// (transcribe.rs:195-203 without the shadowing at :201): [startofprev] + prev[w] + [sot, lang, transcribe, notimestamps],
+// or the four ids where prev[w] (mels_to_text's prev_nonspecial_tokens) is empty or prev is.
+std::vector<std::vector<int64_t>> window_prompts(const Session& s, int64_t n_windows, int beam_size, int max_depth,
+                                                 const wb_special_ids& ids, const uint8_t* is_special,
+                                                 const std::vector<std::vector<int64_t>>& prev = {}, int64_t startofprev = -1);
+// transcribe_windows runs `encode` (prompts.size() windows), then decodes each window from its prompt.  Both it and
+// waveforms_to_tokens return at most capacity ids per row and leave the ids' log-probs and the timings in s.
+std::vector<std::vector<int64_t>> transcribe_windows(Session& s, const std::vector<std::vector<int64_t>>& prompts, int beam_size,
+                                                     int max_depth, int64_t eot, const uint8_t* is_special, int64_t capacity,
+                                                     const std::function<void()>& encode);
+std::vector<std::vector<int64_t>> waveforms_to_tokens(Session& s, const float* const* waveforms, const int64_t* n_samples,
+                                                      int64_t n_waveforms, int64_t sample_rate, int beam_size, int max_depth,
+                                                      const wb_special_ids& ids, const uint8_t* is_special, int64_t capacity);
 std::vector<std::pair<int64_t, int64_t>> window_bounds(int64_t n_samples, int64_t sample_rate, int64_t window_len);
 bool find_chunk_overlap(const int64_t* prev, int64_t n_prev, const int64_t* curr, int64_t n_curr, int64_t max_n_offsets,
                         int64_t min_n_overlaps, int64_t* prev_index, int64_t* curr_index);

@@ -1,12 +1,14 @@
-// Host pipeline above the kernels: the token side of src/transcribe.rs.
+// Host pipeline above the kernels: the token side of src/transcribe.rs, behind every decode entry point of the C ABI.
+//   waveforms_to_tokens  waveform_to_text        transcribe.rs:23-74 (previous ids :43-54, merge :56-63)
 //   window_bounds        waveform_to_mel_tensor  transcribe.rs:114-138
-//   transcribe_windows   mels_to_text            transcribe.rs:148-383 (prompt :195-203, search :232-309)
+//   transcribe_windows   mels_to_text            transcribe.rs:148-383 (prompt: window_prompts :195-203, search :232-309)
 //   find_chunk_overlap                           transcribe.rs:76-110
 // All windows of a call advance in lock-step: one batched device step per search depth evaluates
 // the live beams of every unfinished window (the reference evaluates one window at a time and
 // re-runs the whole decoder per step; results per window are identical because windows are
 // independent, SURVEY.md F9).
 #include <algorithm>
+#include <functional>
 
 #include "../host/beam.hpp"
 #include "session.h"
@@ -162,28 +164,75 @@ void host_beam_search(Session& s, const std::vector<std::vector<int64_t>>& promp
     }
 }
 
+// per window the ids and the log-prob each was chosen with (BeamSearchToken.log_prob), decoded from prompts[w] on the
+// encoded windows
+void decode_windows(Session& s, const std::vector<std::vector<int64_t>>& prompts, int beam_size, int max_depth, int64_t eot,
+                    const uint8_t* is_special, std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp) {
+    s.set_special(is_special);
+    if (beam_size == 1)   // greedy: beam_size 1 of the search, or the greedy loop (transcribe.rs:314-380)
+        s.greedy_decode(prompts, max_depth, eot, out, out_lp, s.search == WB_SEARCH_GREEDY_LOOP);
+    // beam search: on the device in one launch where decoder6 covers it (fp16-exact weights, d = 128 / 384,
+    // n_windows * beam_size <= 24, t_max <= 128), same selection rules and ids as the host search
+    else if (max_depth == 0 || !s.beam_decode(prompts, beam_size, max_depth, eot, out, out_lp))
+        host_beam_search(s, prompts, beam_size, max_depth, eot, out, out_lp);
+    WB_CUDA(cudaEventRecord(s.ev[3], s.st));
+}
+
+// the phases the encode and decode_windows recorded: log-mel, encoder + cross K/V, decode, total
+void collect_timings(Session& s) {
+    WB_CUDA(cudaStreamSynchronize(s.st));
+    cudaEventElapsedTime(&s.last_ms[0], s.ev[0], s.ev[1]);
+    cudaEventElapsedTime(&s.last_ms[1], s.ev[1], s.ev[2]);
+    cudaEventElapsedTime(&s.last_ms[2], s.ev[2], s.ev[3]);
+    cudaEventElapsedTime(&s.last_ms[3], s.ev[0], s.ev[3]);
+}
+
+// the overlap merge of one window's ids and log-probs into its waveform's (transcribe.rs:56-63)
+void merge_window(std::vector<int64_t>& tokens, std::vector<float>& tlp, const std::vector<int64_t>& nt,
+                  const std::vector<float>& nl) {
+    int64_t pi = 0, ci = 0;
+    if (find_chunk_overlap(tokens.data(), (int64_t)tokens.size(), nt.data(), (int64_t)nt.size(), 40, 3, &pi, &ci)) {
+        tokens.resize((size_t)pi);                                    // transcribe.rs:59-60
+        tokens.insert(tokens.end(), nt.begin() + ci, nt.end());
+        tlp.resize((size_t)pi);
+        tlp.insert(tlp.end(), nl.begin() + ci, nl.end());
+    } else {
+        tokens.insert(tokens.end(), nt.begin(), nt.end());
+        tlp.insert(tlp.end(), nl.begin(), nl.end());
+    }
+}
+
+// transcribe.rs:43-50: the last (at most) 5 ids of the merged tokens that are not special, in order
+std::vector<int64_t> prev_nonspecial(const std::vector<int64_t>& tokens, const uint8_t* is_special) {
+    std::vector<int64_t> prev;
+    for (size_t i = tokens.size(); i-- > 0 && prev.size() < 5;)
+        if (!is_special[tokens[i]]) prev.push_back(tokens[i]);
+    std::reverse(prev.begin(), prev.end());
+    return prev;
+}
+
 }  // namespace
 
-void transcribe_windows(Session& s, int beam_size, int max_depth, const wb_special_ids& ids, const uint8_t* is_special,
-                        std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp,
-                        const std::vector<std::vector<int64_t>>& prev, int64_t startofprev) {
+std::vector<std::vector<int64_t>> window_prompts(const Session& s, int64_t n_windows, int beam_size, int max_depth,
+                                                 const wb_special_ids& ids, const uint8_t* is_special,
+                                                 const std::vector<std::vector<int64_t>>& prev, int64_t startofprev) {
     const bool loop = s.search == WB_SEARCH_GREEDY_LOOP;
+    WB_REQUIRE(n_windows >= 1 && n_windows <= s.max_windows, "transcribe: n_windows out of range for this session");
+    WB_REQUIRE(is_special || loop, "transcribe: is_special is needed outside the greedy loop");
     WB_REQUIRE(!loop || beam_size == 1, "transcribe: the greedy loop takes beam_size 1");
     WB_REQUIRE(beam_size >= 1 && beam_size <= s.max_beams, "transcribe: beam_size exceeds the session's max_beams");
     WB_REQUIRE(max_depth >= 0, "transcribe: negative max_depth");
-    WB_REQUIRE(prev.empty() || (int64_t)prev.size() == s.n_windows, "transcribe: one previous-id list per window");
+    WB_REQUIRE(prev.empty() || (int64_t)prev.size() == n_windows, "transcribe: one previous-id list per window");
     const int V = s.m->dims.n_vocab;
+    WB_REQUIRE(prev.empty() || (startofprev >= 0 && startofprev < V), "transcribe: startofprev id out of range");
     const int64_t head[4] = {ids.sot, ids.lang, ids.transcribe, ids.notimestamps};   // transcribe.rs:203
     for (int64_t t : head) WB_REQUIRE(t >= 0 && t < V, "transcribe: special id out of range");
     WB_REQUIRE(ids.eot >= 0 && ids.eot < V, "transcribe: eot id out of range");
-    // window w's prompt: [startofprev] + prev[w] + the four ids when prev[w] is not empty (transcribe.rs:195-203 without the
-    // shadowing at :201), else the four ids
-    std::vector<std::vector<int64_t>> prompts((size_t)s.n_windows);
+    std::vector<std::vector<int64_t>> prompts((size_t)n_windows);
     for (size_t w = 0; w < prompts.size(); ++w) {
         std::vector<int64_t>& pr = prompts[w];
         if (!prev.empty() && !prev[w].empty()) {
             WB_REQUIRE(!loop, "transcribe: the greedy loop builds its own prompt; no previous ids with it");
-            WB_REQUIRE(startofprev >= 0 && startofprev < V, "transcribe: startofprev id out of range");
             pr.push_back(startofprev);
             for (int64_t t : prev[w]) {
                 WB_REQUIRE(t >= 0 && t < V, "transcribe: previous id out of range");
@@ -193,14 +242,84 @@ void transcribe_windows(Session& s, int beam_size, int max_depth, const wb_speci
         pr.insert(pr.end(), head, head + 4);
         WB_REQUIRE((int64_t)pr.size() + max_depth <= s.t_max, "transcribe: prompt + max_depth exceeds the session's max_text_len");
     }
-    s.set_special(is_special);
-    if (beam_size == 1)   // greedy: beam_size 1 of the search, or the greedy loop (transcribe.rs:314-380)
-        s.greedy_decode(prompts, max_depth, ids.eot, out, out_lp, loop);
-    // beam search: on the device in one launch where decoder6 covers it (fp16-exact weights, d = 128 / 384,
-    // n_windows * beam_size <= 24, t_max <= 128), same selection rules and ids as the host search
-    else if (max_depth == 0 || !s.beam_decode(prompts, beam_size, max_depth, ids.eot, out, out_lp))
-        host_beam_search(s, prompts, beam_size, max_depth, ids.eot, out, out_lp);
-    WB_CUDA(cudaEventRecord(s.ev[3], s.st));
+    return prompts;
+}
+
+std::vector<std::vector<int64_t>> transcribe_windows(Session& s, const std::vector<std::vector<int64_t>>& prompts, int beam_size,
+                                                     int max_depth, int64_t eot, const uint8_t* is_special, int64_t capacity,
+                                                     const std::function<void()>& encode) {
+    s.have_logprobs = false;
+    encode();
+    std::vector<std::vector<int64_t>> out;
+    decode_windows(s, prompts, beam_size, max_depth, eot, is_special, out, s.last_logprobs);
+    for (const auto& row : out) WB_REQUIRE((int64_t)row.size() <= capacity, "tokens_out capacity too small");
+    collect_timings(s);
+    s.have_logprobs = true;
+    return out;
+}
+
+// windows of ALL waveforms are decoded together in batches of the session's capacity (they are independent,
+// SURVEY.md F9), then each waveform's windows are merged in order exactly like the reference's sequential
+// loop (transcribe.rs:42-71); each id's log-prob travels with it through the merge.
+// With the previous-text prompt (Session::startofprev >= 0) window i of a waveform needs the merged ids of windows
+// 0 .. i-1: round i decodes window i of every waveform that has one, in batches of the session's capacity.
+std::vector<std::vector<int64_t>> waveforms_to_tokens(Session& s, const float* const* waveforms, const int64_t* n_samples,
+                                                      int64_t n_waveforms, int64_t sample_rate, int beam_size, int max_depth,
+                                                      const wb_special_ids& ids, const uint8_t* is_special, int64_t capacity) {
+    WB_REQUIRE(n_waveforms >= 1, "waveforms_to_tokens: n_waveforms must be >= 1");
+    // the frontend tables (mel filterbank, DFT bins) are the 16 kHz ones: the reference builds them from the caller's rate
+    // (audio.rs:44, 67-143) but its binary only ever passes 16 kHz (src/bin/transcribe/main.rs:38-41 asserts it)
+    WB_REQUIRE(sample_rate == 16000, "waveform_to_tokens: only 16 kHz input is supported (frontend tables are built for 16 kHz)");
+    const bool prev_prompt = s.startofprev >= 0;
+    WB_REQUIRE(!prev_prompt || s.search != WB_SEARCH_GREEDY_LOOP,
+               "waveform_to_tokens: the previous-text prompt (set_prev_prompt) does not combine with the greedy loop");
+    const int64_t window_len = window_samples(s.m->dims.n_audio_ctx, s.window_mode);   // transcribe.rs:32-34
+    std::vector<const float*> ptrs;
+    std::vector<int64_t> lens;
+    std::vector<int> owner;
+    for (int64_t w = 0; w < n_waveforms; ++w)
+        for (const auto& b : window_bounds(n_samples[w], sample_rate, window_len)) {
+            ptrs.push_back(waveforms[w] + b.first);
+            lens.push_back(b.second - b.first);
+            owner.push_back((int)w);
+        }
+    std::vector<std::vector<int64_t>> out((size_t)n_waveforms);
+    std::vector<std::vector<float>> out_lp((size_t)n_waveforms);
+    // batches: window-major order (all windows at once) or, with the previous-text prompt, rounds of window index i
+    std::vector<std::vector<size_t>> rounds(1);
+    std::vector<size_t> idx((size_t)n_waveforms, 0);   // per waveform, the index of its next window
+    for (size_t j = 0; j < ptrs.size(); ++j) {
+        const size_t i = prev_prompt ? idx[(size_t)owner[j]]++ : 0;
+        if (rounds.size() <= i) rounds.resize(i + 1);
+        rounds[i].push_back(j);
+    }
+    for (const std::vector<size_t>& round : rounds) {
+        for (size_t b0 = 0; b0 < round.size(); b0 += (size_t)s.max_windows) {
+            const size_t nb = std::min(round.size() - b0, (size_t)s.max_windows);
+            std::vector<const float*> bp(nb);
+            std::vector<int64_t> bl(nb);
+            std::vector<std::vector<int64_t>> prev(prev_prompt ? nb : 0);
+            for (size_t i = 0; i < nb; ++i) {
+                const size_t j = round[b0 + i];
+                bp[i] = ptrs[j];
+                bl[i] = lens[j];
+                if (prev_prompt) prev[i] = prev_nonspecial(out[(size_t)owner[j]], is_special);
+            }
+            const auto prompts = window_prompts(s, (int64_t)nb, beam_size, max_depth, ids, is_special, prev, s.startofprev);
+            s.have_logprobs = false;
+            s.encode_waveforms_host(bp.data(), bl.data(), (int64_t)nb);
+            std::vector<std::vector<int64_t>> toks;
+            std::vector<std::vector<float>> lps;
+            decode_windows(s, prompts, beam_size, max_depth, ids.eot, is_special, toks, lps);
+            for (size_t i = 0; i < nb; ++i)
+                merge_window(out[(size_t)owner[round[b0 + i]]], out_lp[(size_t)owner[round[b0 + i]]], toks[i], lps[i]);
+        }
+    }
+    collect_timings(s);
+    for (const auto& row : out) WB_REQUIRE((int64_t)row.size() <= capacity, "tokens_out capacity (per waveform) too small");
+    s.last_logprobs = std::move(out_lp);
+    s.have_logprobs = true;
+    return out;
 }
 
 }  // namespace wb

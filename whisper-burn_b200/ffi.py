@@ -80,7 +80,7 @@ SYMBOLS = {
                                              C.POINTER(SpecialIds), _U8, _I64, C.c_int64, _I64]),
     "wb_waveform_to_tokens": (C.c_int, [_P, _F, C.c_int64, C.c_int64, C.c_int, C.c_int,
                                         C.POINTER(SpecialIds), _U8, _I64, C.c_int64, _I64]),
-    "wb_waveforms_to_tokens": (C.c_int, [_P, C.POINTER(C.c_void_p), _I64, C.c_int64, C.c_int64, C.c_int, C.c_int,
+    "wb_waveforms_to_tokens": (C.c_int, [_P, C.POINTER(_F), _I64, C.c_int64, C.c_int64, C.c_int, C.c_int,
                                          C.POINTER(SpecialIds), _U8, _I64, C.c_int64, _I64]),
     "wb_session_last_logprobs": (C.c_int, [_P, C.c_int64, _F, C.c_int64, _I64]),
     "wb_session_score_tokens": (C.c_int, [_P, C.c_int64, _I32, _I64, _I64, C.c_int, _U8, _F, _I64]),

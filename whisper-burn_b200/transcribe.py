@@ -29,6 +29,17 @@ def _special(is_special: Optional[np.ndarray]):
     return None if is_special is None else ffi.u8ptr(np.ascontiguousarray(is_special, dtype=np.uint8))
 
 
+def _special_ids(special) -> ffi.SpecialIds:
+    """The five ids the decode calls take (wb_special_ids) from a tokenizer's special tokens."""
+    return ffi.SpecialIds(special.sot, special.lang, special.transcribe, special.notimestamps, special.eot)
+
+
+def _host_waves(waves: Sequence[np.ndarray]):
+    """(float32 arrays, which must outlive the call, their pointers, int64 sample counts) for calls taking host waveforms."""
+    ws = [np.ascontiguousarray(w, dtype=np.float32) for w in waves]
+    return ws, (ffi._F * len(ws))(*[ffi.fptr(w) for w in ws]), np.asarray([len(w) for w in ws], dtype=np.int64)
+
+
 class Session:
     """KV-cached decoding session (wb_session): encoder output, cross/self K/V, workspaces.
     windows="reference" (default) gives the encoder at most n_audio_ctx mel frames per window, as the reference does;
@@ -73,9 +84,7 @@ class Session:
         ffi.check(ffi.lib().wb_session_set_prev_prompt(self._h, startofprev))
 
     def encode_waveforms(self, waves: Sequence[np.ndarray]) -> None:
-        ws = [np.ascontiguousarray(w, dtype=np.float32) for w in waves]
-        ptrs = (ffi._F * len(ws))(*[ffi.fptr(w) for w in ws])
-        lens = np.asarray([w.shape[0] for w in ws], dtype=np.int64)
+        ws, ptrs, lens = _host_waves(waves)
         ffi.check(ffi.lib().wb_session_encode_waveforms(self._h, ptrs, ffi.i64ptr(lens), len(ws)))
 
     def encode_mels(self, mels: np.ndarray) -> None:
@@ -110,25 +119,22 @@ class Session:
         n = len(w)
         ids = np.empty((n, k), dtype=np.int64)
         lps = np.empty((n, k), dtype=np.float32)
-        sp = ffi.u8ptr(np.ascontiguousarray(is_special, dtype=np.uint8)) if is_special is not None else None
         ffi.check(ffi.lib().wb_session_step(self._h, n, ffi.i32ptr(w), ffi.i32ptr(pr), ffi.i64ptr(tk),
-                                           1 if apply_special_mask else 0, sp, k, ffi.i64ptr(ids), ffi.fptr(lps)))
+                                           1 if apply_special_mask else 0, _special(is_special), k, ffi.i64ptr(ids),
+                                           ffi.fptr(lps)))
         return ids, lps
 
     # ---- pipelines
     def transcribe_windows(self, waves: Sequence[np.ndarray], special, is_special: np.ndarray, beam_size: int = 5,
                            max_depth: int = 100) -> List[List[int]]:
         """mels_to_text for a batch of windows (transcribe.rs:148-383), ids only."""
-        ws = [np.ascontiguousarray(w, dtype=np.float32) for w in waves]
-        ptrs = (ffi._F * len(ws))(*[ffi.fptr(w) for w in ws])
-        lens = np.asarray([w.shape[0] for w in ws], dtype=np.int64)
+        ws, ptrs, lens = _host_waves(waves)
         cap = 4 + max_depth + 1
         out = np.zeros((len(ws), cap), dtype=np.int64)
         out_len = np.zeros(len(ws), dtype=np.int64)
-        ids = ffi.SpecialIds(special.sot, special.lang, special.transcribe, special.notimestamps, special.eot)
-        sp = _special(is_special)
         ffi.check(ffi.lib().wb_transcribe_windows(self._h, ptrs, ffi.i64ptr(lens), len(ws), beam_size, max_depth,
-                                                 C.byref(ids), sp, ffi.i64ptr(out), cap, ffi.i64ptr(out_len)))
+                                                 C.byref(_special_ids(special)), _special(is_special), ffi.i64ptr(out), cap,
+                                                 ffi.i64ptr(out_len)))
         return [[int(t) for t in out[i, :out_len[i]]] for i in range(len(ws))]
 
     def transcribe_windows_prev(self, waves: Sequence[np.ndarray], prev: Sequence[Sequence[int]], special,
@@ -137,20 +143,18 @@ class Session:
         """mels_to_text with its prev_nonspecial_tokens given per window (wb_transcribe_windows_prev): window i is decoded
         from [startofprev] + prev[i] + [sot, lang, transcribe, notimestamps], or the 4 ids when prev[i] is empty; rows hold
         the prompt first.  startofprev defaults to special.startofprev."""
-        ws = [np.ascontiguousarray(w, dtype=np.float32) for w in waves]
+        ws, ptrs, lens = _host_waves(waves)
         if len(prev) != len(ws):
             raise ValueError(f"transcribe_windows_prev: {len(ws)} windows but {len(prev)} previous-id lists")
-        ptrs = (ffi._F * len(ws))(*[ffi.fptr(w) for w in ws])
-        lens = np.asarray([w.shape[0] for w in ws], dtype=np.int64)
         prev_lens = np.asarray([len(p) for p in prev], dtype=np.int64)
         prev_toks = np.ascontiguousarray(np.concatenate([np.asarray(p, dtype=np.int64) for p in prev] + [np.zeros(1, np.int64)]))
         cap = max([4] + [len(p) + 5 for p in prev if len(p)]) + max_depth + 1
         out = np.zeros((len(ws), cap), dtype=np.int64)
         out_len = np.zeros(len(ws), dtype=np.int64)
-        ids = ffi.SpecialIds(special.sot, special.lang, special.transcribe, special.notimestamps, special.eot)
         sop = special.startofprev if startofprev is None else startofprev
         ffi.check(ffi.lib().wb_transcribe_windows_prev(self._h, ptrs, ffi.i64ptr(lens), len(ws), ffi.i64ptr(prev_toks),
-                                                      ffi.i64ptr(prev_lens), sop, beam_size, max_depth, C.byref(ids),
+                                                      ffi.i64ptr(prev_lens), sop, beam_size, max_depth,
+                                                      C.byref(_special_ids(special)),
                                                       _special(is_special), ffi.i64ptr(out), cap, ffi.i64ptr(out_len)))
         return [[int(t) for t in out[i, :out_len[i]]] for i in range(len(ws))]
 
@@ -162,11 +166,9 @@ class Session:
         cap = 4 + max_depth + 1
         out = np.zeros((len(ln), cap), dtype=np.int64)
         out_len = np.zeros(len(ln), dtype=np.int64)
-        ids = ffi.SpecialIds(special.sot, special.lang, special.transcribe, special.notimestamps, special.eot)
-        sp = _special(is_special)
         ffi.check(ffi.lib().wb_transcribe_windows_dev(self._h, C.c_void_p(wave_dev_ptr), ffi.i64ptr(offs), ffi.i64ptr(ln),
-                                                     len(ln), beam_size, max_depth, C.byref(ids), sp,
-                                                     ffi.i64ptr(out), cap, ffi.i64ptr(out_len)))
+                                                     len(ln), beam_size, max_depth, C.byref(_special_ids(special)),
+                                                     _special(is_special), ffi.i64ptr(out), cap, ffi.i64ptr(out_len)))
         return [[int(t) for t in out[i, :out_len[i]]] for i in range(len(ln))]
 
     def waveform_to_tokens(self, waveform: np.ndarray, special, is_special: np.ndarray, sample_rate: int = 16000,
@@ -175,25 +177,21 @@ class Session:
         cap = (len(w) // 1000 + 2) * (10 + max_depth + 1) + 16
         out = np.zeros(cap, dtype=np.int64)
         n = C.c_int64(0)
-        ids = ffi.SpecialIds(special.sot, special.lang, special.transcribe, special.notimestamps, special.eot)
-        sp = _special(is_special)
         ffi.check(ffi.lib().wb_waveform_to_tokens(self._h, ffi.fptr(w), len(w), sample_rate, beam_size, max_depth,
-                                                 C.byref(ids), sp, ffi.i64ptr(out), cap, C.byref(n)))
+                                                 C.byref(_special_ids(special)), _special(is_special), ffi.i64ptr(out), cap,
+                                                 C.byref(n)))
         return [int(t) for t in out[:n.value]]
 
     def waveforms_to_tokens(self, waveforms: Sequence[np.ndarray], special, is_special: np.ndarray, sample_rate: int = 16000,
                             beam_size: int = 5, max_depth: int = 100) -> List[List[int]]:
         """Batched waveform_to_tokens: all windows of all waveforms decoded together (wb_waveforms_to_tokens)."""
-        ws = [np.ascontiguousarray(w, dtype=np.float32) for w in waveforms]
+        ws, ptrs, lens = _host_waves(waveforms)
         cap = (max(len(w) for w in ws) // 1000 + 2) * (10 + max_depth + 1) + 16
         out = np.zeros((len(ws), cap), dtype=np.int64)
         n = np.zeros(len(ws), dtype=np.int64)
-        ptrs = (C.c_void_p * len(ws))(*[w.ctypes.data for w in ws])
-        lens = np.array([len(w) for w in ws], dtype=np.int64)
-        ids = ffi.SpecialIds(special.sot, special.lang, special.transcribe, special.notimestamps, special.eot)
-        sp = _special(is_special)
         ffi.check(ffi.lib().wb_waveforms_to_tokens(self._h, ptrs, ffi.i64ptr(lens), len(ws), sample_rate, beam_size, max_depth,
-                                                  C.byref(ids), sp, ffi.i64ptr(out), cap, ffi.i64ptr(n)))
+                                                  C.byref(_special_ids(special)), _special(is_special), ffi.i64ptr(out), cap,
+                                                  ffi.i64ptr(n)))
         return [[int(t) for t in out[i, :n[i]]] for i in range(len(ws))]
 
     def last_logprobs(self, index: int) -> np.ndarray:
@@ -243,9 +241,8 @@ class Session:
 
     def profile_decode(self, special, n_steps: int = 50):
         """(average logits-GEMV ms, average whole-step ms) over n_steps re-run greedy steps."""
-        ids = ffi.SpecialIds(special.sot, special.lang, special.transcribe, special.notimestamps, special.eot)
         a, b = C.c_float(0), C.c_float(0)
-        ffi.check(ffi.lib().wb_session_profile_decode(self._h, C.byref(ids), n_steps, C.byref(a), C.byref(b)))
+        ffi.check(ffi.lib().wb_session_profile_decode(self._h, C.byref(_special_ids(special)), n_steps, C.byref(a), C.byref(b)))
         return float(a.value), float(b.value)
 
     def last_steps(self) -> int:
