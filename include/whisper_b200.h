@@ -15,6 +15,7 @@
  *   beamsearch_next closure            src/transcribe.rs:253-307   -> wb_session_step (KV-cached, top-k only)
  *   forward_decoder + log_softmax      mod.rs:131-157, transcribe.rs:276 -> wb_session_score_tokens (every position)
  *   beam::beam_search(_step)           src/beam.rs:9-79            -> wb_beam_* (host C++, same tie-breaks)
+ *   beam_search's final carried list   src/beam.rs:33-36           -> wb_session_last_nbest (the n-best the search drops)
  *   mels_to_text (token part)          src/transcribe.rs:148-383   -> wb_transcribe_windows
  *   waveform_to_text (token part)      src/transcribe.rs:23-74     -> wb_waveform_to_tokens
  *   find_chunk_overlap                 src/transcribe.rs:76-110    -> wb_find_chunk_overlap
@@ -256,6 +257,26 @@ int wb_waveforms_to_tokens(wb_session* s, const float* const* waveforms, const i
  *     repetition cut, context stop);
  *   - wb_waveform(s)_to_tokens: each log-prob travels with its id through the overlap merge (transcribe.rs:56-63). */
 int wb_session_last_logprobs(wb_session* s, int64_t index, float* out, int64_t capacity, int64_t* n_out);
+/* The n-best list of one window of the last wb_transcribe_windows[_dev/_prev] call (index = window) or wb_waveform(s)_to_tokens
+ * call (index = window in waveform-major order: waveform 0's windows as wb_window_bounds lists them, then waveform 1's, ...).
+ * ids_out / lp_out are [max_hyps][capacity], lens_out / scores_out / finished_out [max_hyps]; hypotheses best first.
+ * ids_out == NULL only sets *n_hyps_out (and lens_out when given).  lp_out / finished_out may be NULL.
+ * Under WB_SEARCH_BEAM the list is the search's carried list when beam::beam_search returns (`beams` at beam.rs:33): the
+ * search stopped because its best node was finished (beam.rs:22-27), or it ran max_depth steps past the window's own prompt.
+ * It holds at most 2 * beam_size hypotheses (up to beam_size live ones, then up to beam_size finished ones, beam.rs:71-78),
+ * ranked by applying max_by_last repeatedly to what remains: descending score, exact ties with the LATER carried node first.
+ * Rank 0 is therefore always the row the decode call wrote.  Each hypothesis has
+ *   - ids:      the window's prompt (any previous-text prompt included) + the generated ids, laid out as a transcribe row;
+ *   - lp:       0 for each prompt id, else the f32 log-prob the search scored the id with (as wb_session_last_logprobs);
+ *   - score:    the node's cumulative f64 log-prob as the search carried it, bit-equal to the left-to-right f64 sum of lp;
+ *   - finished: 1 when the last id is EOT.
+ * beam_size 1 gives one hypothesis, the row itself; max_depth 0 one hypothesis, the prompt, with score 0.
+ * WB_ERR_STATE before the first decode call and after a WB_SEARCH_GREEDY_LOOP call (the greedy loop carries no list);
+ * WB_ERR_INVALID_ARG for an index out of range, max_hyps below the list's size or capacity below its longest hypothesis.
+ * A decode call rejected before it encodes leaves the previous n-best as it was, a call that fails later leaves none, and
+ * wb_session_score_tokens / wb_session_step leave it as it was. */
+int wb_session_last_nbest(wb_session* s, int64_t index, int64_t max_hyps, int64_t capacity, int64_t* ids_out,
+                          float* lp_out, int64_t* lens_out, double* scores_out, int32_t* finished_out, int64_t* n_hyps_out);
 /* Teacher-forced scoring of n_seqs token sequences against windows this session has encoded:
  * forward_decoder (mod.rs:131-157) + log_softmax (transcribe.rs:276) at every position, in one pass on the GPU.
  * Sequence i is tokens[off_i .. off_i + lens[i]) with off_i = lens[0] + .. + lens[i-1], on window window_of_seq[i].
@@ -300,6 +321,13 @@ int64_t wb_beam_search_table(const double* table, int64_t n_ctx, int64_t n_vocab
  * each live beam contributes its beam_size best table entries.  beam_size <= 7.  Same return values; for tests. */
 int64_t wb_beam_search_table_fixed(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token, int64_t eot,
                                    int64_t beam_size, int64_t max_depth, int64_t* seq_out, int64_t capacity);
+/* The ranked final carried list (the n-best of wb_session_last_nbest) of the same table-driven search, stepped as
+ * wb_beam_search_table (fixed = 0) or wb_beam_search_table_fixed (fixed != 0, beam_size <= 7).  ids_out is
+ * [max_hyps][capacity], lens_out / scores_out / finished_out [max_hyps] (finished_out may be NULL); hypotheses best first.
+ * Returns the hypothesis count, or -1 on bad arguments, a list longer than max_hyps or a sequence longer than capacity. */
+int64_t wb_beam_nbest_table(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token, int64_t eot, int64_t beam_size,
+                            int64_t max_depth, int fixed, int64_t max_hyps, int64_t capacity, int64_t* ids_out, int64_t* lens_out,
+                            double* scores_out, int32_t* finished_out);
 
 /* ---- transcribe binary helpers (host) ---------------------------------------------------------- */
 /* load_audio_waveform (src/bin/transcribe/main.rs:31-55): PCM int samples / (2^(bits-1) - 1), float samples as they

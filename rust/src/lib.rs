@@ -65,6 +65,8 @@ pub mod ffi {
         pub fn wb_transcribe_windows_prev(s: *mut c_void, waves: *const *const f32, lens: *const i64, n_windows: i64, prev_tokens: *const i64,
                                           prev_lens: *const i64, startofprev: i64, beam_size: c_int, max_depth: c_int, ids: *const wb_special_ids,
                                           is_special: *const u8, tokens_out: *mut i64, capacity: i64, lens_out: *mut i64) -> c_int;
+        pub fn wb_session_last_nbest(s: *mut c_void, index: i64, max_hyps: i64, capacity: i64, ids_out: *mut i64, lp_out: *mut f32,
+                                     lens_out: *mut i64, scores_out: *mut f64, finished_out: *mut i32, n_hyps_out: *mut i64) -> c_int;
     }
 }
 
@@ -179,6 +181,30 @@ pub mod beam {
     /// beam.rs:9-37
     pub fn beam_search<T, F, G>(initial_beams: Vec<BeamNode<T>>, next: F, is_finished: G, beam_size: usize, max_depth: usize) -> Vec<T>
     where T: Clone, F: Fn(&[BeamNode<T>]) -> Vec<Vec<(T, f64)>> + Clone, G: Fn(&[T]) -> bool + Clone {
+        let beams = beam_search_final(initial_beams, next, is_finished, beam_size, max_depth);
+        last_max(&beams).map(|b| b.seq.clone()).unwrap_or_default()
+    }
+
+    /// beam_search's n-best list: the carried beams when the search stops (`beams` at beam.rs:33), ranked by applying
+    /// beam.rs:33-36's max_by again to what remains after each pick (descending log_prob, exact ties with the LATER carried beam
+    /// first).  Element 0 is what beam_search returns; at most 2 * beam_size beams.
+    pub fn beam_search_nbest<T, F, G>(initial_beams: Vec<BeamNode<T>>, next: F, is_finished: G, beam_size: usize, max_depth: usize)
+            -> Vec<BeamNode<T>>
+    where T: Clone, F: Fn(&[BeamNode<T>]) -> Vec<Vec<(T, f64)>> + Clone, G: Fn(&[T]) -> bool + Clone {
+        let mut rest = beam_search_final(initial_beams, next, is_finished, beam_size, max_depth);
+        let mut ranked = Vec::with_capacity(rest.len());
+        while !rest.is_empty() {
+            let mut best = 0;
+            for i in 1..rest.len() { if !(rest[i].log_prob < rest[best].log_prob) { best = i; } }
+            ranked.push(rest.remove(best));
+        }
+        ranked
+    }
+
+    /// beam.rs:9-32: the carried beams when the search stops, in carried order
+    fn beam_search_final<T, F, G>(initial_beams: Vec<BeamNode<T>>, next: F, is_finished: G, beam_size: usize, max_depth: usize)
+            -> Vec<BeamNode<T>>
+    where T: Clone, F: Fn(&[BeamNode<T>]) -> Vec<Vec<(T, f64)>> + Clone, G: Fn(&[T]) -> bool + Clone {
         let mut beams = initial_beams;
         for _ in 0..max_depth {
             if let Some(best) = last_max(&beams) {
@@ -186,7 +212,7 @@ pub mod beam {
             }
             beams = beam_search_step(beams, next.clone(), is_finished.clone(), beam_size);
         }
-        last_max(&beams).map(|b| b.seq.clone()).unwrap_or_default()
+        beams
     }
 
     /// beam.rs:39-79: `next` sees every beam (finished ones included, their continuations are dropped); up to 2 * beam_size
@@ -314,6 +340,43 @@ pub mod transcribe {
         })?;
         let tokens: Vec<usize> = out[..n as usize].iter().map(|&t| t as usize).collect();
         Ok((bpe.decode(&tokens[..], true)?, tokens))
+    }
+
+    /// One hypothesis of a window's n-best list: its tokens (prompt included, 0.0 log-probs there), the cumulative log-prob the
+    /// search carried it with (the f64 sum of the tokens' log-probs), and whether it ends in EOT.
+    #[derive(Clone, Debug, PartialEq)]
+    pub struct Hypothesis { pub tokens: Vec<BeamSearchToken>, pub log_prob: f64, pub finished: bool }
+
+    /// waveform_to_text's windowing, beam width and depth, returning per window (in waveform order) the n-best list the beam
+    /// search ranks and drops at beam.rs:33-36 (wb_session_last_nbest): at most 2 * 5 hypotheses, best first, the first being
+    /// the window's transcribed row before the overlap merge.
+    pub fn waveform_to_tokens_nbest(whisper: &model::Whisper, bpe: &Gpt2Tokenizer, lang: Language, waveform: Vec<f32>,
+                                    sample_rate: usize) -> token::Result<Vec<Vec<Hypothesis>>> {
+        let sp = SpecialTokens::from_tokenizer(bpe, lang);
+        let window = audio::max_waveform_samples(whisper.encoder_ctx_size() - 10);            // transcribe.rs:32-34
+        let shift = window.saturating_sub(sample_rate * 3).max(1);                             // transcribe.rs:120-123
+        let n_windows = waveform.len().saturating_sub(1) / shift + 1;
+        let cap = n_windows * (4 + MAX_DEPTH + 1) + 16;
+        let (max_hyps, row_cap) = (2 * BEAM_SIZE, 4 + MAX_DEPTH + 1);
+        let mut out = vec![0i64; cap];
+        let mut n = 0i64;
+        whisper.with_session(n_windows.min(64), BEAM_SIZE, 4 + MAX_DEPTH + 1, |s| {
+            check(unsafe { ffi::wb_waveform_to_tokens(s, waveform.as_ptr(), waveform.len() as i64, sample_rate as i64, BEAM_SIZE as c_int,
+                                                      MAX_DEPTH as c_int, &sp.ids, sp.is_special.as_ptr(), out.as_mut_ptr(), cap as i64, &mut n) })?;
+            let mut windows = Vec::with_capacity(n_windows);
+            for w in 0..n_windows {
+                let (mut ids, mut lps) = (vec![0i64; max_hyps * row_cap], vec![0f32; max_hyps * row_cap]);
+                let (mut lens, mut scores, mut fin) = (vec![0i64; max_hyps], vec![0f64; max_hyps], vec![0i32; max_hyps]);
+                let mut n_hyps = 0i64;
+                check(unsafe { ffi::wb_session_last_nbest(s, w as i64, max_hyps as i64, row_cap as i64, ids.as_mut_ptr(), lps.as_mut_ptr(),
+                                                          lens.as_mut_ptr(), scores.as_mut_ptr(), fin.as_mut_ptr(), &mut n_hyps) })?;
+                windows.push((0..n_hyps as usize).map(|r| Hypothesis {
+                    tokens: (0..lens[r] as usize).map(|j| BeamSearchToken { token: ids[r * row_cap + j] as usize,
+                                                                           log_prob: lps[r * row_cap + j] as f64 }).collect(),
+                    log_prob: scores[r], finished: fin[r] != 0 }).collect());
+            }
+            Ok(windows)
+        })
     }
 
     /// How well given token sequences fit one audio window: `forward_decoder` (mod.rs:131-157) and `log_softmax`

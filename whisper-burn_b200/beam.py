@@ -31,3 +31,21 @@ def beam_search_table(table, first_token: int, eot: int, beam_size: int, max_dep
     if n < 0:
         raise ffi.WbError(ffi.WB_ERR_INVALID_ARG, "beam_search_table: bad arguments")
     return [int(v) for v in out[:n]]
+
+
+def nbest_table(table, first_token: int, eot: int, beam_size: int, max_depth: int, fixed: bool = False):
+    """The ranked final carried list of beam_search_table's search (wb_beam_nbest_table): (ids, f64 score, finished) per
+    hypothesis, best first; element 0's ids are what beam_search_table returns."""
+    import ctypes as C
+    t = np.ascontiguousarray(table, dtype=np.float64)
+    max_hyps, cap = 2 * max(beam_size, 1), max_depth + 1
+    ids = np.zeros((max_hyps, cap), dtype=np.int64)
+    lens = np.zeros(max_hyps, dtype=np.int64)
+    scores = np.zeros(max_hyps, dtype=np.float64)
+    fin = np.zeros(max_hyps, dtype=np.int32)
+    n = ffi.lib().wb_beam_nbest_table(t.ctypes.data_as(C.POINTER(C.c_double)), t.shape[0], t.shape[1], first_token, eot,
+                                      beam_size, max_depth, 1 if fixed else 0, max_hyps, cap, ffi.i64ptr(ids), ffi.i64ptr(lens),
+                                      scores.ctypes.data_as(C.POINTER(C.c_double)), ffi.i32ptr(fin))
+    if n < 0:
+        raise ffi.WbError(ffi.WB_ERR_INVALID_ARG, "nbest_table: bad arguments")
+    return [([int(v) for v in ids[r, :lens[r]]], float(scores[r]), bool(fin[r])) for r in range(n)]

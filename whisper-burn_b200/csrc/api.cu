@@ -127,6 +127,89 @@ FrontendOnly& frontend_for(int device) {
     return *slot;
 }
 
+// beam::beam_search (src/beam.rs:9-37) over a TABLE-driven `next`: the continuation log-prob of token v after a beam whose last
+// token is t and whose length is n is table[((t * 131 + n) % n_ctx) * n_vocab + v] (added to the beam's cumulative f64 log-prob);
+// a beam is finished when its last token is eot.  Host only: lets the CPU tests drive the complete C++ search (host/beam.hpp:
+// step, carry of finished beams, both tie-break rules) against the oracle without a GPU.  Returns the carried list when the
+// search stops (beam.rs:33), in carried order.
+// fixed: the same search stepped by the fixed-capacity selection that decoder6.cu runs on the device (host/beam_fixed.hpp).
+// Each live beam contributes its beam_size best table entries (get_top_elements over the whole row, as the device contributes
+// its top-k), and the step re-ranks them exactly as the reference does.
+std::vector<wb::beam::BeamNode<int64_t>> table_search_final(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token,
+                                                            int64_t eot, int64_t beam_size, int64_t max_depth, bool fixed) {
+    using Node = wb::beam::BeamNode<int64_t>;
+    std::vector<Node> init(1);
+    init[0].seq = {first_token};
+    init[0].log_prob = 0.0;
+    if (!fixed) {
+        auto next = [&](const std::vector<Node>& beams) {
+            std::vector<std::vector<std::pair<int64_t, double>>> out(beams.size());
+            for (size_t b = 0; b < beams.size(); ++b) {
+                const int64_t t = beams[b].seq.back(), n = (int64_t)beams[b].seq.size();
+                const double* row = table + ((t * 131 + n) % n_ctx) * n_vocab;
+                out[b].reserve((size_t)n_vocab);
+                for (int64_t v = 0; v < n_vocab; ++v) out[b].emplace_back(v, beams[b].log_prob + row[v]);
+            }
+            return out;
+        };
+        auto fin = [&](const std::vector<int64_t>& seq) { return !seq.empty() && seq.back() == eot; };
+        return wb::beam::beam_search_final(init, next, fin, (size_t)beam_size, (size_t)max_depth);
+    }
+    namespace fx = wb::beamfx;
+    const int B = (int)beam_size;
+    std::vector<fx::Head> heads(1);
+    std::vector<std::vector<int64_t>> seqs(1, std::vector<int64_t>{first_token});
+    heads[0] = fx::Head{0.0, first_token == eot ? 1 : 0, 0, 1, 0};
+    std::vector<double> scores((size_t)n_vocab);
+    for (int64_t depth = 0; depth < max_depth; ++depth) {
+        const int n = (int)heads.size();
+        if (fx::search_done(heads.data(), n)) break;
+        int step_row[fx::MAX_NODES], cand_id[fx::MAX_NODES * fx::MAX_BEAM];
+        double cand_lp[fx::MAX_NODES * fx::MAX_BEAM];
+        for (int b = 0; b < n; ++b) {
+            step_row[b] = b;
+            for (int i = 0; i < B; ++i) cand_id[b * B + i] = -1;
+            if (heads[(size_t)b].finished) continue;
+            const int64_t t = seqs[(size_t)b].back(), len = (int64_t)seqs[(size_t)b].size();
+            const double* row = table + ((t * 131 + len) % n_ctx) * n_vocab;
+            for (int64_t v = 0; v < n_vocab; ++v) scores[(size_t)v] = heads[(size_t)b].log_prob + row[v];
+            int top[fx::MAX_BEAM + 1];
+            const int nt = fx::top_elements(scores.data(), (int)n_vocab, B, top);
+            for (int i = 0; i < nt; ++i) {
+                cand_id[b * B + i] = top[i];
+                cand_lp[b * B + i] = row[top[i]];
+            }
+        }
+        fx::Pick out[fx::MAX_NODES];
+        const int n_out = fx::beam_step(heads.data(), n, step_row, cand_id, cand_lp, B, (int)eot, out);
+        std::vector<fx::Head> nh((size_t)n_out);
+        std::vector<std::vector<int64_t>> ns((size_t)n_out);
+        for (int i = 0; i < n_out; ++i) {
+            nh[(size_t)i] = out[i].head;
+            ns[(size_t)i] = seqs[(size_t)out[i].src];
+            if (out[i].token >= 0) ns[(size_t)i].push_back(out[i].token);
+        }
+        heads.swap(nh);
+        seqs.swap(ns);
+    }
+    std::vector<Node> beams(heads.size());
+    for (size_t i = 0; i < heads.size(); ++i) {
+        beams[i].seq = std::move(seqs[i]);
+        beams[i].log_prob = heads[i].log_prob;
+    }
+    return beams;
+}
+
+// the best sequence of a final carried list (beam.rs:33-36) to seq_out: its length, or -1 when it exceeds capacity
+int64_t copy_best(const std::vector<wb::beam::BeamNode<int64_t>>& beams, int64_t* seq_out, int64_t capacity) {
+    const int best = wb::beam::max_by_last(beams);
+    if (best < 0) return 0;
+    const std::vector<int64_t>& s = beams[(size_t)best].seq;
+    if ((int64_t)s.size() > capacity) return -1;
+    std::copy(s.begin(), s.end(), seq_out);
+    return (int64_t)s.size();
+}
+
 }  // namespace
 
 extern "C" {
@@ -481,6 +564,35 @@ int wb_session_last_logprobs(wb_session* s, int64_t index, float* out, int64_t c
     });
 }
 
+int wb_session_last_nbest(wb_session* s, int64_t index, int64_t max_hyps, int64_t capacity, int64_t* ids_out, float* lp_out,
+                          int64_t* lens_out, double* scores_out, int32_t* finished_out, int64_t* n_hyps_out) {
+    return guarded([&] {
+        WB_REQUIRE(s && n_hyps_out, "last_nbest: null pointer");
+        const wb::Session& S = *s->impl;
+        if (!S.have_nbest)
+            wb::fail(WB_ERR_STATE, "last_nbest: no beam-search transcribe or waveform(s)_to_tokens call yet (the greedy loop keeps none)");
+        WB_REQUIRE(index >= 0 && index < (int64_t)S.last_nbest.size(), "last_nbest: index out of range");
+        const wb::NBest& nb = S.last_nbest[(size_t)index];
+        *n_hyps_out = (int64_t)nb.size();
+        if (!ids_out) {   // size query
+            if (lens_out)
+                for (size_t r = 0; r < nb.size() && (int64_t)r < max_hyps; ++r) lens_out[r] = (int64_t)nb[r].ids.size();
+            return;
+        }
+        WB_REQUIRE(lens_out && scores_out, "last_nbest: null pointer");
+        WB_REQUIRE(max_hyps >= (int64_t)nb.size(), "last_nbest: max_hyps below the list's hypothesis count");
+        for (const wb::Hypothesis& h : nb) WB_REQUIRE(capacity >= (int64_t)h.ids.size(), "last_nbest: capacity below the longest hypothesis");
+        for (size_t r = 0; r < nb.size(); ++r) {
+            const wb::Hypothesis& h = nb[r];
+            std::copy(h.ids.begin(), h.ids.end(), ids_out + (int64_t)r * capacity);
+            if (lp_out) std::copy(h.lps.begin(), h.lps.end(), lp_out + (int64_t)r * capacity);
+            lens_out[r] = (int64_t)h.ids.size();
+            scores_out[r] = h.score;
+            if (finished_out) finished_out[r] = h.finished ? 1 : 0;
+        }
+    });
+}
+
 int wb_session_score_tokens(wb_session* s, int64_t n_seqs, const int32_t* window_of_seq, const int64_t* tokens, const int64_t* lens,
                             int apply_special_mask, const uint8_t* is_special, float* lp_out, int64_t* argmax_out) {
     return guarded([&] {
@@ -551,83 +663,38 @@ int wb_session_last_topk(wb_session* s, int64_t n_rows, int64_t k, int64_t* ids_
     });
 }
 
-// beam::beam_search (src/beam.rs:9-37) over a TABLE-driven `next`: the continuation log-prob of token v after a beam whose last
-// token is t and whose length is n is table[((t * 131 + n) % n_ctx) * n_vocab + v] (added to the beam's cumulative f64 log-prob);
-// a beam is finished when its last token is eot.  Host only: lets the CPU tests drive the complete C++ search (host/beam.hpp:
-// step, carry of finished beams, both tie-break rules) against the oracle without a GPU.
 int64_t wb_beam_search_table(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token, int64_t eot, int64_t beam_size,
                              int64_t max_depth, int64_t* seq_out, int64_t capacity) {
     if (!table || !seq_out || n_ctx < 1 || n_vocab < 1 || beam_size < 1 || max_depth < 0) return -1;
-    using Node = wb::beam::BeamNode<int64_t>;
-    auto next = [&](const std::vector<Node>& beams) {
-        std::vector<std::vector<std::pair<int64_t, double>>> out(beams.size());
-        for (size_t b = 0; b < beams.size(); ++b) {
-            const int64_t t = beams[b].seq.back(), n = (int64_t)beams[b].seq.size();
-            const double* row = table + ((t * 131 + n) % n_ctx) * n_vocab;
-            out[b].reserve((size_t)n_vocab);
-            for (int64_t v = 0; v < n_vocab; ++v) out[b].emplace_back(v, beams[b].log_prob + row[v]);
-        }
-        return out;
-    };
-    auto fin = [&](const std::vector<int64_t>& seq) { return !seq.empty() && seq.back() == eot; };
-    std::vector<Node> init(1);
-    init[0].seq = {first_token};
-    init[0].log_prob = 0.0;
-    const std::vector<int64_t> best = wb::beam::beam_search(init, next, fin, (size_t)beam_size, (size_t)max_depth);
-    if ((int64_t)best.size() > capacity) return -1;
-    for (size_t i = 0; i < best.size(); ++i) seq_out[i] = best[i];
-    return (int64_t)best.size();
+    const auto beams = table_search_final(table, n_ctx, n_vocab, first_token, eot, beam_size, max_depth, false);
+    return copy_best(beams, seq_out, capacity);
 }
 
-// The same search as wb_beam_search_table, stepped by the fixed-capacity selection that decoder6.cu runs on the device
-// (host/beam_fixed.hpp).  Each live beam contributes its beam_size best table entries (get_top_elements over the whole
-// row, as the device contributes its top-k), and the step re-ranks them exactly as the reference does.
 int64_t wb_beam_search_table_fixed(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token, int64_t eot,
                                    int64_t beam_size, int64_t max_depth, int64_t* seq_out, int64_t capacity) {
-    namespace fx = wb::beamfx;
-    if (!table || !seq_out || n_ctx < 1 || n_vocab < 1 || beam_size < 1 || beam_size > fx::MAX_BEAM || max_depth < 0) return -1;
-    const int B = (int)beam_size;
-    std::vector<fx::Head> heads(1);
-    std::vector<std::vector<int64_t>> seqs(1, std::vector<int64_t>{first_token});
-    heads[0] = fx::Head{0.0, first_token == eot ? 1 : 0, 0, 1, 0};
-    std::vector<double> scores((size_t)n_vocab);
-    for (int64_t depth = 0; depth < max_depth; ++depth) {
-        const int n = (int)heads.size();
-        if (fx::search_done(heads.data(), n)) break;
-        int step_row[fx::MAX_NODES], cand_id[fx::MAX_NODES * fx::MAX_BEAM];
-        double cand_lp[fx::MAX_NODES * fx::MAX_BEAM];
-        for (int b = 0; b < n; ++b) {
-            step_row[b] = b;
-            for (int i = 0; i < B; ++i) cand_id[b * B + i] = -1;
-            if (heads[(size_t)b].finished) continue;
-            const int64_t t = seqs[(size_t)b].back(), len = (int64_t)seqs[(size_t)b].size();
-            const double* row = table + ((t * 131 + len) % n_ctx) * n_vocab;
-            for (int64_t v = 0; v < n_vocab; ++v) scores[(size_t)v] = heads[(size_t)b].log_prob + row[v];
-            int top[fx::MAX_BEAM + 1];
-            const int nt = fx::top_elements(scores.data(), (int)n_vocab, B, top);
-            for (int i = 0; i < nt; ++i) {
-                cand_id[b * B + i] = top[i];
-                cand_lp[b * B + i] = row[top[i]];
-            }
-        }
-        fx::Pick out[fx::MAX_NODES];
-        const int n_out = fx::beam_step(heads.data(), n, step_row, cand_id, cand_lp, B, (int)eot, out);
-        std::vector<fx::Head> nh((size_t)n_out);
-        std::vector<std::vector<int64_t>> ns((size_t)n_out);
-        for (int i = 0; i < n_out; ++i) {
-            nh[(size_t)i] = out[i].head;
-            ns[(size_t)i] = seqs[(size_t)out[i].src];
-            if (out[i].token >= 0) ns[(size_t)i].push_back(out[i].token);
-        }
-        heads.swap(nh);
-        seqs.swap(ns);
+    if (!table || !seq_out || n_ctx < 1 || n_vocab < 1 || beam_size < 1 || beam_size > wb::beamfx::MAX_BEAM || max_depth < 0) return -1;
+    const auto beams = table_search_final(table, n_ctx, n_vocab, first_token, eot, beam_size, max_depth, true);
+    return copy_best(beams, seq_out, capacity);
+}
+
+int64_t wb_beam_nbest_table(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token, int64_t eot, int64_t beam_size,
+                            int64_t max_depth, int fixed, int64_t max_hyps, int64_t capacity, int64_t* ids_out, int64_t* lens_out,
+                            double* scores_out, int32_t* finished_out) {
+    if (!table || !ids_out || !lens_out || !scores_out || n_ctx < 1 || n_vocab < 1 || beam_size < 1 ||
+        (fixed && beam_size > wb::beamfx::MAX_BEAM) || max_depth < 0 || max_hyps < 0 || capacity < 0) return -1;
+    const auto beams = table_search_final(table, n_ctx, n_vocab, first_token, eot, beam_size, max_depth, fixed != 0);
+    if ((int64_t)beams.size() > max_hyps) return -1;
+    int64_t r = 0;
+    for (int i : wb::beam::rank_final(beams)) {
+        const auto& n = beams[(size_t)i];
+        if ((int64_t)n.seq.size() > capacity) return -1;
+        std::copy(n.seq.begin(), n.seq.end(), ids_out + r * capacity);
+        lens_out[r] = (int64_t)n.seq.size();
+        scores_out[r] = n.log_prob;
+        if (finished_out) finished_out[r] = !n.seq.empty() && n.seq.back() == eot ? 1 : 0;
+        ++r;
     }
-    const int best = fx::max_by_last(heads.data(), (int)heads.size());
-    if (best < 0) return 0;
-    const std::vector<int64_t>& s = seqs[(size_t)best];
-    if ((int64_t)s.size() > capacity) return -1;
-    for (size_t i = 0; i < s.size(); ++i) seq_out[i] = s[i];
-    return (int64_t)s.size();
+    return r;
 }
 
 int64_t wb_kernel_launch_count(void) { return wb::g_launch_count; }

@@ -607,7 +607,8 @@ void Session::greedy_decode(const std::vector<std::vector<int64_t>>& prompts, in
 }
 
 bool Session::beam_decode(const std::vector<std::vector<int64_t>>& prompts, int beam_size, int max_depth, int64_t eot,
-                          std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp) {
+                          std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp,
+                          std::vector<NBest>& nbest) {
     namespace fx = beamfx;
     const auto [min_lp, max_lp] = prompt_range(prompts);
     WB_REQUIRE(min_lp >= 1 && max_lp + max_depth <= t_max, "beam: prompt + max_depth exceeds the session's max_text_len");
@@ -641,12 +642,25 @@ bool Session::beam_decode(const std::vector<std::vector<int64_t>>& prompts, int 
     const bool ran = launch_decoder(DecodeLaunch::beam_search(Rb, B, min_lp, max_lp, max_depth, (int)eot));
     std::vector<int> res((size_t)W * t_max), res_len((size_t)W);
     std::vector<float> res_lp((size_t)W * t_max);
+    // the final carried lists: a window that finished early keeps its buffer (stage (b) skips done windows), so bm_win
+    // picks each window's list out of both buffers.  Only the first max_lp + max_depth ids of a sequence can be set.
+    const int used = max_lp + max_depth;
+    std::vector<fx::Head> fin_head((size_t)2 * W * MN);
+    std::vector<int> fin_cnt((size_t)2 * W), fin_win((size_t)2 * W), fin_seq((size_t)2 * W * MN * used);
+    std::vector<float> fin_lp(fin_seq.size());
     int sd = 0;
     if (ran) {
         WB_CUDA(cudaMemcpyAsync(res.data(), bm_out.p, res.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
         WB_CUDA(cudaMemcpyAsync(res_lp.data(), bm_out_lp.p, res_lp.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
         WB_CUDA(cudaMemcpyAsync(res_len.data(), bm_out_len.p, res_len.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
         WB_CUDA(cudaMemcpyAsync(&sd, steps_done.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+        WB_CUDA(cudaMemcpyAsync(fin_head.data(), bm_head.p, fin_head.size() * sizeof(fx::Head), cudaMemcpyDeviceToHost, st));
+        WB_CUDA(cudaMemcpyAsync(fin_cnt.data(), bm_cnt.p, fin_cnt.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+        WB_CUDA(cudaMemcpyAsync(fin_win.data(), bm_win.p, fin_win.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+        WB_CUDA(cudaMemcpy2DAsync(fin_seq.data(), used * sizeof(int), bm_seq.p, t_max * sizeof(int), used * sizeof(int),
+                                  (size_t)2 * W * MN, cudaMemcpyDeviceToHost, st));
+        WB_CUDA(cudaMemcpy2DAsync(fin_lp.data(), used * sizeof(float), bm_seq_lp.p, t_max * sizeof(float), used * sizeof(float),
+                                  (size_t)2 * W * MN, cudaMemcpyDeviceToHost, st));
     }
     WB_CUDA(cudaStreamSynchronize(st));   // the host vectors above are in flight until here
     if (!ran) return false;
@@ -662,6 +676,25 @@ bool Session::beam_decode(const std::vector<std::vector<int64_t>>& prompts, int 
             out[(size_t)w].push_back(res[(size_t)w * t_max + i]);
             out_lp[(size_t)w].push_back(res_lp[(size_t)w * t_max + i]);
         }
+    nbest.assign((size_t)W, {});
+    for (int w = 0; w < W; ++w) {
+        const size_t node0 = ((size_t)fin_win[(size_t)2 * w] * W + w) * MN;   // the window's current buffer
+        const int n = fin_cnt[(size_t)fin_win[(size_t)2 * w] * W + w];
+        double lp[MN];
+        int order[MN];
+        for (int i = 0; i < n; ++i) lp[i] = fin_head[node0 + i].log_prob;
+        fx::rank_final(lp, n, order);
+        for (int r = 0; r < n; ++r) {
+            const fx::Head& h = fin_head[node0 + order[r]];
+            const size_t o = (node0 + order[r]) * used;
+            Hypothesis hy;
+            hy.ids.assign(fin_seq.begin() + o, fin_seq.begin() + o + h.len);
+            hy.lps.assign(fin_lp.begin() + o, fin_lp.begin() + o + h.len);
+            hy.score = h.log_prob;
+            hy.finished = h.finished != 0;
+            nbest[(size_t)w].push_back(std::move(hy));
+        }
+    }
     return true;
 }
 

@@ -66,6 +66,15 @@ struct ScoreWs {
     std::vector<std::unique_ptr<GemmF16Plan>> plans;      // per decoder layer: qkv, out, cross query, cross out, mlp1, mlp2
 };
 
+// one hypothesis of a window's n-best list (wb_session_last_nbest): a node of the beam search's final carried list
+struct Hypothesis {
+    std::vector<int64_t> ids;   // prompt + generated ids
+    std::vector<float> lps;     // 0 for each prompt id, else the log-prob the search scored the id with
+    double score = 0.0;         // the node's cumulative log-prob as the search carried it
+    bool finished = false;      // last id is eot
+};
+using NBest = std::vector<Hypothesis>;   // best first (beamfx::rank_final)
+
 // pinned host array
 struct PinnedFree { void operator()(void* p) const { cudaFreeHost(p); } };
 template <typename T> using Pinned = std::unique_ptr<T[], PinnedFree>;
@@ -139,6 +148,10 @@ struct Session {
     int64_t last_steps = 0;
     std::vector<std::vector<float>> last_logprobs;
     bool have_logprobs = false;
+    // per window of that call (waveform calls: waveform-major) its n-best list; have_nbest: that call succeeded under
+    // WB_SEARCH_BEAM (the greedy loop carries no list)
+    std::vector<NBest> last_nbest;
+    bool have_nbest = false;
     int last_groups = 1;         // row groups (launches) of the last decode
     int last_decoder = 0;        // which persistent decoder the last launch used (6, 5, 4 or 3); 0 = none yet
     int last_rows = 0, last_k = 0;   // rows and candidates per row of the last launch (its topk_id / topk_lp)
@@ -209,9 +222,10 @@ struct Session {
     void greedy_decode(const std::vector<std::vector<int64_t>>& prompts, int max_depth, int64_t eot,
                        std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp, bool loop_rules = false);
     // the whole beam search (prefill + up to max_depth steps after each window's prompt) of every encoded window in ONE
-    // decoder launch; false (nothing decoded) when no decoder covers it, and the caller runs the host search
+    // decoder launch; false (nothing decoded) when no decoder covers it, and the caller runs the host search.  nbest: each
+    // window's final carried list, ranked
     bool beam_decode(const std::vector<std::vector<int64_t>>& prompts, int beam_size, int max_depth, int64_t eot,
-                     std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp);
+                     std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp, std::vector<NBest>& nbest);
     // teacher-forced scoring of n_seqs packed token sequences (wb_session_score_tokens): per position j >= 1 the log-prob of
     // token j given tokens 0 .. j-1 and the arg-max id; reads the cross K/V of the encoded windows, writes no decode state
     void score_tokens(int64_t n_seqs, const int32_t* window_of_seq, const int64_t* tokens, const int64_t* lens, bool apply_mask,

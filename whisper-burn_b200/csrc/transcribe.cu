@@ -67,7 +67,7 @@ using Node = beam::BeamNode<BeamSearchToken>;
 // (Session::step_beams).  Window w's search starts at p = prompts[w].size() - 1; until then its prompt node rides along in
 // one row (its own row as parent, its next prompt token) and its candidates are discarded.
 void host_beam_search(Session& s, const std::vector<std::vector<int64_t>>& prompts, int beam_size, int max_depth, int64_t eot,
-                      std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp) {
+                      std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp, std::vector<NBest>& nbest) {
     const int W = s.n_windows;
     auto is_finished = [eot](const std::vector<BeamSearchToken>& seq) { return !seq.empty() && seq.back().token == eot; };
     std::vector<std::vector<Node>> beams((size_t)W);
@@ -152,29 +152,57 @@ void host_beam_search(Session& s, const std::vector<std::vector<int64_t>>& promp
         }
     }
     s.last_steps = steps;
+    // each window's final carried list, ranked; the best row is its rank 0 (max_by_last)
     out.assign((size_t)W, {});
     out_lp.assign((size_t)W, {});
+    nbest.assign((size_t)W, {});
     for (int w = 0; w < W; ++w) {
-        const int best = beam::max_by_last(beams[(size_t)w]);
-        if (best >= 0)
-            for (const auto& t : beams[(size_t)w][(size_t)best].seq) {
-                out[(size_t)w].push_back(t.token);
-                out_lp[(size_t)w].push_back((float)t.log_prob);   // exact: a widened f32 (transcribe.rs:291-299)
+        for (int i : beam::rank_final(beams[(size_t)w])) {
+            const Node& n = beams[(size_t)w][(size_t)i];
+            Hypothesis h;
+            for (const auto& t : n.seq) {
+                h.ids.push_back(t.token);
+                h.lps.push_back((float)t.log_prob);   // exact: a widened f32 (transcribe.rs:291-299)
             }
+            h.score = n.log_prob;
+            h.finished = is_finished(n.seq);
+            nbest[(size_t)w].push_back(std::move(h));
+        }
+        if (!nbest[(size_t)w].empty()) {
+            out[(size_t)w] = nbest[(size_t)w][0].ids;
+            out_lp[(size_t)w] = nbest[(size_t)w][0].lps;
+        }
     }
 }
 
+// the one-hypothesis list of a beam_size 1 row: the carried list of a width-1 search holds one node, the row itself, whose
+// cumulative log-prob is the left-to-right f64 sum of its ids' log-probs
+NBest row_nbest(const std::vector<int64_t>& ids, const std::vector<float>& lps, int64_t eot) {
+    Hypothesis h;
+    h.ids = ids;
+    h.lps = lps;
+    for (float l : lps) h.score += (double)l;
+    h.finished = !ids.empty() && ids.back() == eot;
+    return NBest{std::move(h)};
+}
+
 // per window the ids and the log-prob each was chosen with (BeamSearchToken.log_prob), decoded from prompts[w] on the
-// encoded windows
+// encoded windows, and the window's n-best list (none under the greedy loop)
 void decode_windows(Session& s, const std::vector<std::vector<int64_t>>& prompts, int beam_size, int max_depth, int64_t eot,
-                    const uint8_t* is_special, std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp) {
+                    const uint8_t* is_special, std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp,
+                    std::vector<NBest>& nbest) {
     s.set_special(is_special);
-    if (beam_size == 1)   // greedy: beam_size 1 of the search, or the greedy loop (transcribe.rs:314-380)
-        s.greedy_decode(prompts, max_depth, eot, out, out_lp, s.search == WB_SEARCH_GREEDY_LOOP);
+    nbest.clear();
+    if (beam_size == 1) {   // greedy: beam_size 1 of the search, or the greedy loop (transcribe.rs:314-380)
+        const bool loop = s.search == WB_SEARCH_GREEDY_LOOP;
+        s.greedy_decode(prompts, max_depth, eot, out, out_lp, loop);
+        if (!loop)
+            for (size_t w = 0; w < out.size(); ++w) nbest.push_back(row_nbest(out[w], out_lp[w], eot));
+    }
     // beam search: on the device in one launch where decoder6 covers it (fp16-exact weights, d = 128 / 384,
     // n_windows * beam_size <= 24, t_max <= 128), same selection rules and ids as the host search
-    else if (max_depth == 0 || !s.beam_decode(prompts, beam_size, max_depth, eot, out, out_lp))
-        host_beam_search(s, prompts, beam_size, max_depth, eot, out, out_lp);
+    else if (max_depth == 0 || !s.beam_decode(prompts, beam_size, max_depth, eot, out, out_lp, nbest))
+        host_beam_search(s, prompts, beam_size, max_depth, eot, out, out_lp, nbest);
     WB_CUDA(cudaEventRecord(s.ev[3], s.st));
 }
 
@@ -249,12 +277,14 @@ std::vector<std::vector<int64_t>> transcribe_windows(Session& s, const std::vect
                                                      int max_depth, int64_t eot, const uint8_t* is_special, int64_t capacity,
                                                      const std::function<void()>& encode) {
     s.have_logprobs = false;
+    s.have_nbest = false;
     encode();
     std::vector<std::vector<int64_t>> out;
-    decode_windows(s, prompts, beam_size, max_depth, eot, is_special, out, s.last_logprobs);
+    decode_windows(s, prompts, beam_size, max_depth, eot, is_special, out, s.last_logprobs, s.last_nbest);
     for (const auto& row : out) WB_REQUIRE((int64_t)row.size() <= capacity, "tokens_out capacity too small");
     collect_timings(s);
     s.have_logprobs = true;
+    s.have_nbest = s.search == WB_SEARCH_BEAM;
     return out;
 }
 
@@ -285,6 +315,7 @@ std::vector<std::vector<int64_t>> waveforms_to_tokens(Session& s, const float* c
         }
     std::vector<std::vector<int64_t>> out((size_t)n_waveforms);
     std::vector<std::vector<float>> out_lp((size_t)n_waveforms);
+    std::vector<NBest> nbest(ptrs.size());   // per window, waveform-major
     // batches: window-major order (all windows at once) or, with the previous-text prompt, rounds of window index i
     std::vector<std::vector<size_t>> rounds(1);
     std::vector<size_t> idx((size_t)n_waveforms, 0);   // per waveform, the index of its next window
@@ -307,18 +338,24 @@ std::vector<std::vector<int64_t>> waveforms_to_tokens(Session& s, const float* c
             }
             const auto prompts = window_prompts(s, (int64_t)nb, beam_size, max_depth, ids, is_special, prev, s.startofprev);
             s.have_logprobs = false;
+            s.have_nbest = false;
             s.encode_waveforms_host(bp.data(), bl.data(), (int64_t)nb);
             std::vector<std::vector<int64_t>> toks;
             std::vector<std::vector<float>> lps;
-            decode_windows(s, prompts, beam_size, max_depth, ids.eot, is_special, toks, lps);
-            for (size_t i = 0; i < nb; ++i)
+            std::vector<NBest> nbs;
+            decode_windows(s, prompts, beam_size, max_depth, ids.eot, is_special, toks, lps, nbs);
+            for (size_t i = 0; i < nb; ++i) {
                 merge_window(out[(size_t)owner[round[b0 + i]]], out_lp[(size_t)owner[round[b0 + i]]], toks[i], lps[i]);
+                if (!nbs.empty()) nbest[round[b0 + i]] = std::move(nbs[i]);
+            }
         }
     }
     collect_timings(s);
     for (const auto& row : out) WB_REQUIRE((int64_t)row.size() <= capacity, "tokens_out capacity (per waveform) too small");
     s.last_logprobs = std::move(out_lp);
     s.have_logprobs = true;
+    s.last_nbest = std::move(nbest);
+    s.have_nbest = s.search == WB_SEARCH_BEAM;
     return out;
 }
 

@@ -6,7 +6,8 @@
 //   * get_top_elements (beam.rs:81-110): ascending insertion list, a candidate equal to the minimum
 //     of a full list is inserted in front and evicted at once  ->  on exact ties the EARLIER
 //     element wins; k = 1 is a first-index arg-max.  Output order: ascending score.
-//   * beam_search (beam.rs:9-37): Rust Iterator::max_by returns the LAST maximum.
+//   * beam_search (beam.rs:9-37): Rust Iterator::max_by returns the LAST maximum.  beam_search_final returns the carried list
+//     it picks from (the n-best list, ranked by rank_final / beamfx::rank_final).
 //   * beam_search_step (beam.rs:39-79): `next` sees every beam, finished ones included; up to
 //     2*beam_size beams are carried (k live + k finished).
 #pragma once
@@ -15,6 +16,8 @@
 #include <functional>
 #include <utility>
 #include <vector>
+
+#include "beam_fixed.hpp"
 
 namespace wb {
 namespace beam {
@@ -88,17 +91,35 @@ std::vector<BeamNode<T>> beam_search_step(const std::vector<BeamNode<T>>& beams,
     return out;
 }
 
-// beam.rs:9-37
+// beam.rs:9-32: the carried list when the search stops (`beams` at beam.rs:33), in carried order
 template <typename T, typename NextFn, typename FinFn>
-std::vector<T> beam_search(std::vector<BeamNode<T>> beams, NextFn&& next, FinFn&& is_finished, size_t beam_size,
-                           size_t max_depth) {
+std::vector<BeamNode<T>> beam_search_final(std::vector<BeamNode<T>> beams, NextFn&& next, FinFn&& is_finished, size_t beam_size,
+                                           size_t max_depth) {
     for (size_t i = 0; i < max_depth; ++i) {
         const int best = max_by_last(beams);
         if (best >= 0 && is_finished(beams[(size_t)best].seq)) break;
         beams = beam_search_step(beams, next, is_finished, beam_size);
     }
+    return beams;
+}
+
+// beam.rs:9-37
+template <typename T, typename NextFn, typename FinFn>
+std::vector<T> beam_search(std::vector<BeamNode<T>> beams, NextFn&& next, FinFn&& is_finished, size_t beam_size,
+                           size_t max_depth) {
+    beams = beam_search_final(std::move(beams), next, is_finished, beam_size, max_depth);
     const int best = max_by_last(beams);
     return best >= 0 ? beams[(size_t)best].seq : std::vector<T>();
+}
+
+// the n-best order of a final carried list (beamfx::rank_final): indices into `beams`, best first
+template <typename T>
+std::vector<int> rank_final(const std::vector<BeamNode<T>>& beams) {
+    std::vector<double> lp(beams.size());
+    for (size_t i = 0; i < beams.size(); ++i) lp[i] = beams[i].log_prob;
+    std::vector<int> order(beams.size());
+    beamfx::rank_final(lp.data(), (int)lp.size(), order.data());
+    return order;
 }
 
 }  // namespace beam

@@ -69,6 +69,18 @@ WB_HD inline int max_by_last(const Head* h, int n) {
     return best;
 }
 
+// The n-best ranking of a final carried list (beam.rs:33-36 applied again to what remains after each pick): max_by_last
+// repeatedly, i.e. descending log-prob with exact ties ordered by LATER carried position first.  Writes the carried indices
+// best first to order[0..n); order[0] is max_by_last.  Every n-best list (host search, device search, table helpers) is
+// ranked here.  (An insertion that places node i before the first kept node it is not below gives the same order.)
+WB_HD inline void rank_final(const double* log_prob, int n, int* order) {
+    for (int i = 0; i < n; ++i) {
+        int k = i;
+        for (; k > 0 && !(log_prob[order[k - 1]] > log_prob[i]); --k) order[k] = order[k - 1];
+        order[k] = i;
+    }
+}
+
 // beam_search (beam.rs:22-27): the search stops when its best carried node is finished
 WB_HD inline bool search_done(const Head* h, int n) {
     const int best = max_by_last(h, n);

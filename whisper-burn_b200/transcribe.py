@@ -204,6 +204,26 @@ class Session:
         ffi.check(ffi.lib().wb_session_last_logprobs(self._h, index, ffi.fptr(out), n.value, C.byref(n)))
         return out
 
+    def last_nbest(self, index: int):
+        """The n-best list of window `index` of the last transcribe_windows[_dev/_prev] call, or of window `index` in
+        waveform-major order of the last waveform(s)_to_tokens call (wb_session_last_nbest): the beam search's final carried
+        list, best first, as (ids, float32 log-probs (0 for the prompt), f64 score = their left-to-right sum, finished).
+        Rank 0 is the row the call returned.  WbError (WB_ERR_STATE) after a greedy-loop call."""
+        n = C.c_int64(0)
+        ffi.check(ffi.lib().wb_session_last_nbest(self._h, index, 0, 0, None, None, None, None, None, C.byref(n)))
+        lens = np.zeros(max(n.value, 1), dtype=np.int64)
+        ffi.check(ffi.lib().wb_session_last_nbest(self._h, index, n.value, 0, None, None, ffi.i64ptr(lens), None, None,
+                                                  C.byref(n)))
+        cap = max(int(lens[:n.value].max(initial=0)), 1)
+        ids = np.zeros((max(n.value, 1), cap), dtype=np.int64)
+        lps = np.zeros((max(n.value, 1), cap), dtype=np.float32)
+        scores = np.zeros(max(n.value, 1), dtype=np.float64)
+        fin = np.zeros(max(n.value, 1), dtype=np.int32)
+        ffi.check(ffi.lib().wb_session_last_nbest(self._h, index, n.value, cap, ffi.i64ptr(ids), ffi.fptr(lps), ffi.i64ptr(lens),
+                                                  scores.ctypes.data_as(C.POINTER(C.c_double)), ffi.i32ptr(fin), C.byref(n)))
+        return [([int(t) for t in ids[r, :lens[r]]], lps[r, :lens[r]].copy(), float(scores[r]), bool(fin[r]))
+                for r in range(n.value)]
+
     def score_tokens(self, seqs: Sequence[Sequence[int]], windows: Sequence[int], apply_special_mask: bool = False,
                      is_special: Optional[np.ndarray] = None):
         """Teacher-forced scoring of token sequences against the encoded windows (wb_session_score_tokens): sequence i on
