@@ -152,12 +152,15 @@ def default_decoder(d, rows, t_max):
 
 
 # ---------------------------------------------------------------- a. greedy, per step, top-1 against float64
-def check_greedy(dims, wh, kv, n_rows, decoder, seed, steps=SHALLOW_STEPS, max_text_len=None, full_depth=False):
+def check_greedy(dims, wh, kv, n_rows, decoder, seed, steps=SHALLOW_STEPS, max_text_len=None, full_depth=False, tol=None,
+                 ref_rows=None):
     """Greedy-decodes n_rows windows once to the deepest step of `steps` and once to each step s of `steps`, and checks the
     top-1 (id, log-prob) of every row at every step s against float64 on the GPU's own path.  max_text_len defaults to the
     deepest step plus the prompt and one.  full_depth: EOT is declared to be a special id past the named ones that no row
     emits (the largest one not emitted by an earlier full-depth launch that a row stopped in), and every row must reach the
-    deepest step.  Returns the worst |log-prob error|."""
+    deepest step.  tol defaults to GREEDY_LP_TOL[kv].  ref_rows(sp, xa, paths, kv, steps) -> per row {s: float64 log-prob
+    row} computes the reference in this process (xa: the rows' float64 encoder outputs [1, T, d], steps: per row); by
+    default worker processes rebuild the model with _weights.  Returns the worst |log-prob error|."""
     depth = max(steps)
     sp = synth.special_tokens(dims)
     bitmap = sp.is_special_bitmap()
@@ -174,9 +177,10 @@ def check_greedy(dims, wh, kv, n_rows, decoder, seed, steps=SHALLOW_STEPS, max_t
     if full_depth:
         assert sess.last_steps() == depth and [len(t) for t in full] == [4 + depth] * n_rows
     xa = encoder_outputs64(sess, Ts)
-    key = (dims.n_text_state, dims.n_text_head, dims.n_vocab, dims.n_text_layer, wh.weights_fp16_exact)
-    refs = [_ref_pool().submit(_greedy_ref_rows, key, sp, xa[r][0].numpy(), full[r], kv,
-                               [s for s in steps if 4 + s <= len(full[r])]) for r in range(n_rows)]
+    row_steps = [[s for s in steps if 4 + s <= len(full[r])] for r in range(n_rows)]
+    if ref_rows is None:
+        key = (dims.n_text_state, dims.n_text_head, dims.n_vocab, dims.n_text_layer, wh.weights_fp16_exact)
+        refs = [_ref_pool().submit(_greedy_ref_rows, key, sp, xa[r][0].numpy(), full[r], kv, row_steps[r]) for r in range(n_rows)]
     got = [dict() for _ in range(n_rows)]      # step -> (id, log-prob) of every row that produced a token at that step
     for s in steps:
         toks = sess.transcribe_windows(waves, sp, bitmap, beam_size=1, max_depth=s)
@@ -187,10 +191,11 @@ def check_greedy(dims, wh, kv, n_rows, decoder, seed, steps=SHALLOW_STEPS, max_t
             if len(toks[r]) == 4 + s:
                 assert int(ids[r, 0]) == toks[r][-1]
                 got[r][s] = float(lps[r, 0])
-    tol = GREEDY_LP_TOL[kv]
+    tol = tol or GREEDY_LP_TOL[kv]
     worst = 0.0
+    local = ref_rows(sp, xa, full, kv, row_steps) if ref_rows is not None else None
     for r in range(n_rows):
-        ref = refs[r].result()
+        ref = local[r] if local is not None else refs[r].result()
         assert sorted(got[r]) == sorted(ref)
         for s, lp in got[r].items():
             tok = full[r][4 + s - 1]
@@ -362,11 +367,20 @@ def test_session_step_k7_beams_vs_float64(decoder, d, exact, kv, monkeypatch):
     against float64 oracle.model.CachedDecoder rows reordered the same way."""
     dims, wh, w64 = make_model(d, d // 64, 51864 if d == 384 else 2051, exact=exact)
     use_decoder(monkeypatch, 3 if decoder == 3 else 0)
+    worst = check_step_k7(dims, wh, w64, decoder, kv)
+    report(f"step k=7 decoder{decoder} d={d} {'fp16' if exact else 'fp32'} weights kv={kv}", worst, STEP_LP_TOL[kv])
+
+
+def check_step_k7(dims, wh, w64, decoder, kv, sess=None, tol=None, out=None):
+    """The steps of test_session_step_k7_beams_vs_float64 on `sess` (default: a fresh session of 2 windows, 5 beams,
+    max_text_len 16), each checked against float64 within tol (default STEP_LP_TOL[kv]).  out, a list, receives every
+    step's (ids, log-probs).  Returns the worst |log-prob error|."""
     sp = synth.special_tokens(dims)
     bitmap = sp.is_special_bitmap()
     K = 7
     Ts, waves = windows(2, seed=700, order=(65, 6))
-    sess = transcribe.Session(wh, max_windows=2, max_beams=5, max_text_len=16, kv_dtype=kv_code(kv))
+    if sess is None:
+        sess = transcribe.Session(wh, max_windows=2, max_beams=5, max_text_len=16, kv_dtype=kv_code(kv))
     sess.encode_waveforms(waves)
     xa = encoder_outputs64(sess, Ts)
     opts = o_model.OracleOptions(kv_dtype=kv)
@@ -378,7 +392,7 @@ def test_session_step_k7_beams_vs_float64(decoder, d, exact, kv, monkeypatch):
             dec.step(torch.tensor([t], dtype=torch.int64))
     rows = [(0, 0), (1, 0)]          # GPU row -> (window, row of that window's float64 decoder)
     maskout = torch.from_numpy(sp.maskout())
-    tol = STEP_LP_TOL[kv]
+    tol = tol or STEP_LP_TOL[kv]
     worst = 0.0
 
     def step(parents, tokens, masked):
@@ -386,6 +400,8 @@ def test_session_step_k7_beams_vs_float64(decoder, d, exact, kv, monkeypatch):
         win = [rows[p][0] for p in parents]
         ids, lps = sess.step(win, parents, tokens, masked, bitmap, K)
         assert sess.last_decoder() == decoder
+        if out is not None:
+            out.append((ids, lps))
         new_rows = []
         for w in range(2):
             mine = [i for i in range(len(parents)) if win[i] == w]
@@ -413,7 +429,7 @@ def test_session_step_k7_beams_vs_float64(decoder, d, exact, kv, monkeypatch):
     ids = step([2, 0, 1, 5, 3], [int(ids[2, 1]), int(ids[0, 0]), int(ids[1, 6]), int(ids[5, 0]), int(ids[3, 2])], False)
     ids = step([4, 0, 2], [int(ids[4, 3]), int(ids[0, 0]), int(ids[2, 5])], False)   # back to 3 rows from other parents
     step([1, 0, 2, 2, 1], [int(ids[1, 0]), int(ids[0, 1]), int(ids[2, 0]), int(ids[2, 4]), int(ids[1, 2])], False)
-    report(f"step k=7 decoder{decoder} d={d} {'fp16' if exact else 'fp32'} weights kv={kv}", worst, tol)
+    return worst
 
 
 # ---------------------------------------------------------------- c. full logits at the maximum text length
@@ -423,14 +439,20 @@ def test_forward_decoder_448_positions_vs_float64(decoder, d, monkeypatch):
     self-attention over up to 448 keys.  Forcing the decoder makes any other choice an error."""
     use_decoder(monkeypatch, decoder)
     dims, wh, w64 = make_model(d, d // 64, 2051)
+    worst = forward_decoder_448_error(dims, wh, w64)
+    report(f"forward_decoder 448 positions decoder{decoder} d={d}", worst, LOGITS_REL_TOL)
+    assert worst < LOGITS_REL_TOL
+
+
+def forward_decoder_448_error(dims, wh, w64):
+    """The worst relative-to-scale error of forward_decoder's logits at every one of n_text_ctx positions."""
+    d = dims.n_text_state
     rng = np.random.default_rng(d)
     xa = rng.standard_normal((1, 65, d)).astype(np.float32)
     toks = rng.integers(0, dims.n_vocab, size=(1, dims.n_text_ctx)).astype(np.int64)
     got = wh.forward_decoder(toks, xa)
     want = o_model.forward_decoder(w64, dims, torch.from_numpy(toks), torch.from_numpy(xa).double()).numpy()
-    worst = max(rel_to_scale(got[0, p], want[0, p]) for p in range(dims.n_text_ctx))
-    report(f"forward_decoder 448 positions decoder{decoder} d={d}", worst, LOGITS_REL_TOL)
-    assert worst < LOGITS_REL_TOL
+    return max(rel_to_scale(got[0, p], want[0, p]) for p in range(dims.n_text_ctx))
 
 
 # ---------------------------------------------------------------- d. encoder at real widths, ragged windows
