@@ -309,24 +309,20 @@ int wb_find_repeated_tokens_index(const int64_t* tokens, int64_t n, int64_t wind
                                   int64_t* first_repeat_index, int64_t* end);
 
 /* ---- beam.rs (host) ------------------------------------------------------------------------ */
-/* get_top_elements (beam.rs:81-110) on f64 scores: writes the indices of the kept elements in
- * the reference's output order (ascending score); returns how many were kept. */
+/* get_top_elements (beam.rs:81-110) on f64 scores, num 0 .. 7: writes the indices of the kept elements in
+ * the reference's output order (ascending score); returns how many were kept, or -1 on bad arguments. */
 int64_t wb_beam_get_top_elements(const double* scores, int64_t n, int64_t num, int64_t* idx_out);
 
-/* beam::beam_search (beam.rs:9-37) with a table-driven `next` (see csrc/api.cu): the complete host search, for tests.  Returns the
- * length of the best sequence written to seq_out, or -1 on bad arguments. */
+/* beam::beam_search (beam.rs:9-37) with a table-driven `next` (see csrc/api.cu): the library's beam search (host/beam.hpp) on
+ * the CPU, for tests.  Each live beam contributes its beam_size best table entries, as the device contributes its top-k
+ * candidates.  beam_size 1 .. 7.  Returns the length of the best sequence written to seq_out, or -1 on bad arguments. */
 int64_t wb_beam_search_table(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token, int64_t eot,
                              int64_t beam_size, int64_t max_depth, int64_t* seq_out, int64_t capacity);
-/* The same search stepped by the fixed-capacity selection the on-device beam search runs (host/beam_fixed.hpp), on the CPU:
- * each live beam contributes its beam_size best table entries.  beam_size <= 7.  Same return values; for tests. */
-int64_t wb_beam_search_table_fixed(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token, int64_t eot,
-                                   int64_t beam_size, int64_t max_depth, int64_t* seq_out, int64_t capacity);
-/* The ranked final carried list (the n-best of wb_session_last_nbest) of the same table-driven search, stepped as
- * wb_beam_search_table (fixed = 0) or wb_beam_search_table_fixed (fixed != 0, beam_size <= 7).  ids_out is
+/* The ranked final carried list (the n-best of wb_session_last_nbest) of the same table-driven search.  ids_out is
  * [max_hyps][capacity], lens_out / scores_out / finished_out [max_hyps] (finished_out may be NULL); hypotheses best first.
  * Returns the hypothesis count, or -1 on bad arguments, a list longer than max_hyps or a sequence longer than capacity. */
 int64_t wb_beam_nbest_table(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token, int64_t eot, int64_t beam_size,
-                            int64_t max_depth, int fixed, int64_t max_hyps, int64_t capacity, int64_t* ids_out, int64_t* lens_out,
+                            int64_t max_depth, int64_t max_hyps, int64_t capacity, int64_t* ids_out, int64_t* lens_out,
                             double* scores_out, int32_t* finished_out);
 
 /* ---- transcribe binary helpers (host) ---------------------------------------------------------- */

@@ -1,6 +1,6 @@
-"""CPU tests of the fixed-capacity beam-search step that the on-device search runs (host/beam_fixed.hpp): driven by a
-table-defined `next`, it must pick the same sequences as the library's host search (host/beam.hpp) and as the oracle, with
-exact score ties common, EOT reached early, late or never, and max_depth 0, 1 and 30."""
+"""CPU tests of the library's beam search (host/beam.hpp): the fixed-capacity step that the on-device search runs, driven
+by the host window loop over a table-defined `next`, must pick the same sequences as the oracle, with exact score ties common,
+EOT reached early, late or never, and max_depth 0, 1 and 30."""
 import numpy as np
 import pytest
 
@@ -43,16 +43,15 @@ def test_fixed_step_matches_host_search_and_oracle(beam_size, quant, eot_boost):
         table = make_table(rng, quant, eot_boost)
         for max_depth in (0, 1, 30):
             want = oracle_search(table, beam_size, max_depth)
-            host = beam.beam_search_table(table, FIRST, EOT, beam_size, max_depth)
-            fixed = beam.beam_search_table(table, FIRST, EOT, beam_size, max_depth, fixed=True)
-            assert fixed == host == want, (trial, max_depth)
+            got = beam.beam_search_table(table, FIRST, EOT, beam_size, max_depth)
+            assert got == want, (trial, max_depth)
             if eot_boost == -30.0:
-                assert EOT not in fixed and len(fixed) == 1 + max_depth
+                assert EOT not in got and len(got) == 1 + max_depth
 
 
 def test_fixed_step_eot_early_and_late():
-    """A table where EOT wins at the first step, and one where it only wins after many steps: both searches stop in the same
-    place and keep carrying the finished beams."""
+    """A table where EOT wins at the first step, and one where it only wins after many steps: the search stops where the
+    oracle's does and keeps carrying the finished beams."""
     rng = np.random.default_rng(7)
     seen = set()
     for boost in (6.0, 1.0, 0.5, 0.2):
@@ -60,7 +59,7 @@ def test_fixed_step_eot_early_and_late():
             table = make_table(rng, 2, boost)
             for b in (2, 5, 7):
                 want = oracle_search(table, b, 30)
-                assert beam.beam_search_table(table, FIRST, EOT, b, 30, fixed=True) == want
+                assert beam.beam_search_table(table, FIRST, EOT, b, 30) == want
                 if want[-1] == EOT:
                     seen.add("early" if len(want) <= 4 else "late")
     assert seen == {"early", "late"}
@@ -70,4 +69,4 @@ def test_fixed_step_rejects_bad_arguments():
     table = np.zeros((N_CTX, V))
     for b in (0, 8):
         with pytest.raises(ffi.WbError):
-            beam.beam_search_table(table, FIRST, EOT, b, 3, fixed=True)
+            beam.beam_search_table(table, FIRST, EOT, b, 3)

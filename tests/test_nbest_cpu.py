@@ -1,6 +1,6 @@
 """CPU tests of the n-best ranking (wb_session_last_nbest): the final carried list of the table-driven search (wb_beam_nbest_table),
-stepped by the host search (host/beam.hpp) and by the fixed-capacity step the on-device search runs (host/beam_fixed.hpp),
-ranked by beamfx::rank_final, must be the oracle's list (tests/oracle_nbest.py) exactly: ids, order, finished flags and f64
+stepped by the host window loop and the fixed-capacity step the on-device search runs (host/beam.hpp), ranked by
+beamfx::rank_final, must be the oracle's list (tests/oracle_nbest.py) exactly: ids, order, finished flags and f64
 scores.  Rank 0 is the sequence wb_beam_search_table returns, and exact ties put the later carried node first."""
 import json
 from pathlib import Path
@@ -39,13 +39,11 @@ def oracle_nbest(table, first, eot, beam_size, max_depth):
     return [(list(b.seq), b.log_prob, b.seq[-1] == eot) for b in onb.rank_final(oracle_final(table, first, eot, beam_size, max_depth))]
 
 
-def check(table, first, eot, beam_size, max_depth, fixed_too=True):
+def check(table, first, eot, beam_size, max_depth):
     want = oracle_nbest(table, first, eot, beam_size, max_depth)
-    best = beam.beam_search_table(table, first, eot, beam_size, max_depth)
-    for fixed in ((False, True) if fixed_too else (False,)):
-        got = beam.nbest_table(table, first, eot, beam_size, max_depth, fixed=fixed)
-        assert got == want, (fixed, beam_size, max_depth)   # ids, order, finished, f64 scores bit-equal
-        assert got[0][0] == best
+    got = beam.nbest_table(table, first, eot, beam_size, max_depth)
+    assert got == want, (beam_size, max_depth)   # ids, order, finished, f64 scores bit-equal
+    assert got[0][0] == beam.beam_search_table(table, first, eot, beam_size, max_depth)
     return want
 
 
@@ -71,17 +69,6 @@ def test_nbest_table_matches_oracle(beam_size, quant, eot_boost):
                 assert want == [([FIRST], 0.0, False)]
             if beam_size == 1:
                 assert len(want) == 1
-
-
-def test_nbest_table_host_stepping_wide_beam():
-    """the host stepping takes any beam_size; the fixed one at most 7"""
-    rng = np.random.default_rng(11)
-    table = make_table(rng, 1, 1.0)
-    for b in (8, 11):
-        want = check(table, FIRST, EOT, b, 12, fixed_too=False)
-        assert len(want) > 7
-    with pytest.raises(ffi.WbError):
-        beam.nbest_table(table, FIRST, EOT, 8, 3, fixed=True)
 
 
 def test_nbest_table_holds_live_and_finished():
@@ -124,8 +111,7 @@ def test_nbest_exact_ties_put_the_later_node_first():
         final = oracle_final(table, 1, 7, b, 3)
         assert len(final) == b and len({f.log_prob for f in final}) == 1
         want = [(list(f.seq), 0.0, False) for f in reversed(final)]
-        for fixed in (False, True):
-            assert beam.nbest_table(table, 1, 7, b, 3, fixed=fixed) == want
+        assert beam.nbest_table(table, 1, 7, b, 3) == want
         assert beam.beam_search_table(table, 1, 7, b, 3) == list(final[-1].seq)
 
 
@@ -136,9 +122,10 @@ def test_rank_final_restatement():
 
 
 def test_nbest_table_rejects_bad_arguments():
+    """beam_size must be 1 .. 7 (beamfx::MAX_BEAM, the sessions' limit)"""
     table = np.zeros((N_CTX, V))
-    for b in (0, 8):
+    for b in (0, 8, 11):
         with pytest.raises(ffi.WbError):
-            beam.nbest_table(table, FIRST, EOT, b, 3, fixed=True)
-    with pytest.raises(ffi.WbError):
-        beam.nbest_table(table, FIRST, EOT, 0, 3)
+            beam.nbest_table(table, FIRST, EOT, b, 3)
+        with pytest.raises(ffi.WbError):
+            beam.beam_search_table(table, FIRST, EOT, b, 3)

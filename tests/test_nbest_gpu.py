@@ -1,5 +1,5 @@
 """GPU tests (-m gpu) of wb_session_last_nbest: each window's n-best list, the beam search's final carried list ranked by
-max_by_last applied repeatedly (host/beam_fixed.hpp beamfx::rank_final), from the on-device search (decoder6 beam mode) and
+max_by_last applied repeatedly (host/beam.hpp beamfx::rank_final), from the on-device search (decoder6 beam mode) and
 from the host search.  Lists are checked against the oracle's (tests/golden/nbest_beam.json, make_golden_nbest.py): ids,
 lengths, finished flags and order; log-probs against float64 teacher forcing; rank 0 against the returned row."""
 import ctypes as C

@@ -8,7 +8,6 @@
 #include <new>
 
 #include "../host/beam.hpp"
-#include "../host/beam_fixed.hpp"
 #include "../host/repeat.hpp"
 #include "session.h"
 
@@ -127,87 +126,35 @@ FrontendOnly& frontend_for(int device) {
     return *slot;
 }
 
-// beam::beam_search (src/beam.rs:9-37) over a TABLE-driven `next`: the continuation log-prob of token v after a beam whose last
-// token is t and whose length is n is table[((t * 131 + n) % n_ctx) * n_vocab + v] (added to the beam's cumulative f64 log-prob);
-// a beam is finished when its last token is eot.  Host only: lets the CPU tests drive the complete C++ search (host/beam.hpp:
-// step, carry of finished beams, both tie-break rules) against the oracle without a GPU.  Returns the carried list when the
-// search stops (beam.rs:33), in carried order.
-// fixed: the same search stepped by the fixed-capacity selection that decoder6.cu runs on the device (host/beam_fixed.hpp).
-// Each live beam contributes its beam_size best table entries (get_top_elements over the whole row, as the device contributes
-// its top-k), and the step re-ranks them exactly as the reference does.
-std::vector<wb::beam::BeamNode<int64_t>> table_search_final(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token,
-                                                            int64_t eot, int64_t beam_size, int64_t max_depth, bool fixed) {
-    using Node = wb::beam::BeamNode<int64_t>;
-    std::vector<Node> init(1);
-    init[0].seq = {first_token};
-    init[0].log_prob = 0.0;
-    if (!fixed) {
-        auto next = [&](const std::vector<Node>& beams) {
-            std::vector<std::vector<std::pair<int64_t, double>>> out(beams.size());
-            for (size_t b = 0; b < beams.size(); ++b) {
-                const int64_t t = beams[b].seq.back(), n = (int64_t)beams[b].seq.size();
-                const double* row = table + ((t * 131 + n) % n_ctx) * n_vocab;
-                out[b].reserve((size_t)n_vocab);
-                for (int64_t v = 0; v < n_vocab; ++v) out[b].emplace_back(v, beams[b].log_prob + row[v]);
-            }
-            return out;
-        };
-        auto fin = [&](const std::vector<int64_t>& seq) { return !seq.empty() && seq.back() == eot; };
-        return wb::beam::beam_search_final(init, next, fin, (size_t)beam_size, (size_t)max_depth);
-    }
+// The ranked final carried list of the search of wb_beam_search_table / wb_beam_nbest_table: beam_search_windows over one
+// window with prompt {first_token} from position 0, stepped by a table.  The candidates of a row fed token t at position p (a
+// sequence of p + 1 ids) are the beam_size best entries of table row (t * 131 + p + 1) % n_ctx, as the device contributes
+// its top-k per-token log-probs; a beam is finished when its last token is eot.  Host only: lets the CPU tests drive the
+// library's search against the oracle without a GPU.
+wb::NBest table_nbest(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token, int64_t eot, int beam_size,
+                      int max_depth) {
     namespace fx = wb::beamfx;
-    const int B = (int)beam_size;
-    std::vector<fx::Head> heads(1);
-    std::vector<std::vector<int64_t>> seqs(1, std::vector<int64_t>{first_token});
-    heads[0] = fx::Head{0.0, first_token == eot ? 1 : 0, 0, 1, 0};
-    std::vector<double> scores((size_t)n_vocab);
-    for (int64_t depth = 0; depth < max_depth; ++depth) {
-        const int n = (int)heads.size();
-        if (fx::search_done(heads.data(), n)) break;
-        int step_row[fx::MAX_NODES], cand_id[fx::MAX_NODES * fx::MAX_BEAM];
-        double cand_lp[fx::MAX_NODES * fx::MAX_BEAM];
-        for (int b = 0; b < n; ++b) {
-            step_row[b] = b;
-            for (int i = 0; i < B; ++i) cand_id[b * B + i] = -1;
-            if (heads[(size_t)b].finished) continue;
-            const int64_t t = seqs[(size_t)b].back(), len = (int64_t)seqs[(size_t)b].size();
-            const double* row = table + ((t * 131 + len) % n_ctx) * n_vocab;
-            for (int64_t v = 0; v < n_vocab; ++v) scores[(size_t)v] = heads[(size_t)b].log_prob + row[v];
+    auto step = [&](int p, int64_t n_rows, const int32_t*, const int32_t*, const int64_t* token, int, int k, int64_t* ids_out,
+                    double* lps_out) {
+        for (int64_t r = 0; r < n_rows; ++r) {
+            const double* row = table + ((token[r] * 131 + p + 1) % n_ctx) * n_vocab;
             int top[fx::MAX_BEAM + 1];
-            const int nt = fx::top_elements(scores.data(), (int)n_vocab, B, top);
-            for (int i = 0; i < nt; ++i) {
-                cand_id[b * B + i] = top[i];
-                cand_lp[b * B + i] = row[top[i]];
+            const int nt = fx::top_elements(row, (int)n_vocab, k, top);
+            for (int i = 0; i < k; ++i) {
+                ids_out[r * k + i] = i < nt ? top[i] : -1;
+                lps_out[r * k + i] = i < nt ? row[top[i]] : 0.0;
             }
         }
-        fx::Pick out[fx::MAX_NODES];
-        const int n_out = fx::beam_step(heads.data(), n, step_row, cand_id, cand_lp, B, (int)eot, out);
-        std::vector<fx::Head> nh((size_t)n_out);
-        std::vector<std::vector<int64_t>> ns((size_t)n_out);
-        for (int i = 0; i < n_out; ++i) {
-            nh[(size_t)i] = out[i].head;
-            ns[(size_t)i] = seqs[(size_t)out[i].src];
-            if (out[i].token >= 0) ns[(size_t)i].push_back(out[i].token);
-        }
-        heads.swap(nh);
-        seqs.swap(ns);
-    }
-    std::vector<Node> beams(heads.size());
-    for (size_t i = 0; i < heads.size(); ++i) {
-        beams[i].seq = std::move(seqs[i]);
-        beams[i].log_prob = heads[i].log_prob;
-    }
-    return beams;
+    };
+    const std::vector<std::vector<int64_t>> prompt{{first_token}};
+    int64_t steps = 0;
+    return wb::ranked_nbest(wb::beam_search_windows(prompt, 0, beam_size, max_depth, eot, step, &steps)[0]);
 }
 
-// the best sequence of a final carried list (beam.rs:33-36) to seq_out: its length, or -1 when it exceeds capacity
-int64_t copy_best(const std::vector<wb::beam::BeamNode<int64_t>>& beams, int64_t* seq_out, int64_t capacity) {
-    const int best = wb::beam::max_by_last(beams);
-    if (best < 0) return 0;
-    const std::vector<int64_t>& s = beams[(size_t)best].seq;
-    if ((int64_t)s.size() > capacity) return -1;
-    std::copy(s.begin(), s.end(), seq_out);
-    return (int64_t)s.size();
+// the table entry points' arguments: beam_size 1 .. beamfx::MAX_BEAM
+bool table_args_ok(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t beam_size, int64_t max_depth) {
+    return table && n_ctx >= 1 && n_vocab >= 1 && n_vocab <= INT32_MAX && beam_size >= 1 && beam_size <= wb::beamfx::MAX_BEAM &&
+           max_depth >= 0 && max_depth <= INT32_MAX;
 }
 
 }  // namespace
@@ -629,11 +576,11 @@ int wb_find_repeated_tokens_index(const int64_t* tokens, int64_t n, int64_t wind
 }
 
 int64_t wb_beam_get_top_elements(const double* scores, int64_t n, int64_t num, int64_t* idx_out) {
-    if (!scores || !idx_out || n < 0 || num < 0) return -1;
-    std::vector<double> v(scores, scores + n);
-    const auto top = wb::beam::get_top_elements(v, [](double s) { return s; }, (size_t)num);
-    for (size_t i = 0; i < top.size(); ++i) idx_out[i] = (int64_t)top[i];
-    return (int64_t)top.size();
+    if (!scores || !idx_out || n < 0 || n > INT32_MAX || num < 0 || num > wb::beamfx::MAX_BEAM) return -1;
+    int top[wb::beamfx::MAX_BEAM + 1];
+    const int nt = wb::beamfx::top_elements(scores, (int)n, (int)num, top);
+    std::copy(top, top + nt, idx_out);
+    return nt;
 }
 
 int wb_load_wav(const char* path, int strict_16k_mono, float* out, int64_t capacity, int64_t* n_samples_out, int64_t* sample_rate_out,
@@ -665,36 +612,29 @@ int wb_session_last_topk(wb_session* s, int64_t n_rows, int64_t k, int64_t* ids_
 
 int64_t wb_beam_search_table(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token, int64_t eot, int64_t beam_size,
                              int64_t max_depth, int64_t* seq_out, int64_t capacity) {
-    if (!table || !seq_out || n_ctx < 1 || n_vocab < 1 || beam_size < 1 || max_depth < 0) return -1;
-    const auto beams = table_search_final(table, n_ctx, n_vocab, first_token, eot, beam_size, max_depth, false);
-    return copy_best(beams, seq_out, capacity);
-}
-
-int64_t wb_beam_search_table_fixed(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token, int64_t eot,
-                                   int64_t beam_size, int64_t max_depth, int64_t* seq_out, int64_t capacity) {
-    if (!table || !seq_out || n_ctx < 1 || n_vocab < 1 || beam_size < 1 || beam_size > wb::beamfx::MAX_BEAM || max_depth < 0) return -1;
-    const auto beams = table_search_final(table, n_ctx, n_vocab, first_token, eot, beam_size, max_depth, true);
-    return copy_best(beams, seq_out, capacity);
+    if (!seq_out || !table_args_ok(table, n_ctx, n_vocab, beam_size, max_depth)) return -1;
+    const std::vector<int64_t> best = table_nbest(table, n_ctx, n_vocab, first_token, eot, (int)beam_size, (int)max_depth)[0].ids;
+    if ((int64_t)best.size() > capacity) return -1;
+    std::copy(best.begin(), best.end(), seq_out);
+    return (int64_t)best.size();
 }
 
 int64_t wb_beam_nbest_table(const double* table, int64_t n_ctx, int64_t n_vocab, int64_t first_token, int64_t eot, int64_t beam_size,
-                            int64_t max_depth, int fixed, int64_t max_hyps, int64_t capacity, int64_t* ids_out, int64_t* lens_out,
+                            int64_t max_depth, int64_t max_hyps, int64_t capacity, int64_t* ids_out, int64_t* lens_out,
                             double* scores_out, int32_t* finished_out) {
-    if (!table || !ids_out || !lens_out || !scores_out || n_ctx < 1 || n_vocab < 1 || beam_size < 1 ||
-        (fixed && beam_size > wb::beamfx::MAX_BEAM) || max_depth < 0 || max_hyps < 0 || capacity < 0) return -1;
-    const auto beams = table_search_final(table, n_ctx, n_vocab, first_token, eot, beam_size, max_depth, fixed != 0);
-    if ((int64_t)beams.size() > max_hyps) return -1;
-    int64_t r = 0;
-    for (int i : wb::beam::rank_final(beams)) {
-        const auto& n = beams[(size_t)i];
-        if ((int64_t)n.seq.size() > capacity) return -1;
-        std::copy(n.seq.begin(), n.seq.end(), ids_out + r * capacity);
-        lens_out[r] = (int64_t)n.seq.size();
-        scores_out[r] = n.log_prob;
-        if (finished_out) finished_out[r] = !n.seq.empty() && n.seq.back() == eot ? 1 : 0;
-        ++r;
+    if (!ids_out || !lens_out || !scores_out || !table_args_ok(table, n_ctx, n_vocab, beam_size, max_depth) || max_hyps < 0 ||
+        capacity < 0) return -1;
+    const wb::NBest nb = table_nbest(table, n_ctx, n_vocab, first_token, eot, (int)beam_size, (int)max_depth);
+    if ((int64_t)nb.size() > max_hyps) return -1;
+    for (size_t r = 0; r < nb.size(); ++r) {
+        const wb::Hypothesis& h = nb[r];
+        if ((int64_t)h.ids.size() > capacity) return -1;
+        std::copy(h.ids.begin(), h.ids.end(), ids_out + (int64_t)r * capacity);
+        lens_out[r] = (int64_t)h.ids.size();
+        scores_out[r] = h.score;
+        if (finished_out) finished_out[r] = h.finished ? 1 : 0;
     }
-    return r;
+    return (int64_t)nb.size();
 }
 
 int64_t wb_kernel_launch_count(void) { return wb::g_launch_count; }

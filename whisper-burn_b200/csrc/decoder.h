@@ -2,7 +2,7 @@
 #pragma once
 #include <stdint.h>
 
-#include "../host/beam_fixed.hpp"
+#include "../host/beam.hpp"
 #include "wb_internal.h"
 
 namespace wb {

@@ -35,7 +35,7 @@
 //
 // Beam mode (dec6_kernel<..., BEAM = true>, a.beam = B in 2..7): the same kernel runs the prefill and the whole width-B search of
 // R / B windows: row w * B + i is slot i of window w, self attention goes through the ancestry table, the vocabulary records
-// keep DEC_KC candidates, and the finisher selects the next beams on the device (finish_beam, host/beam_fixed.hpp).
+// keep DEC_KC candidates, and the finisher selects the next beams on the device (finish_beam, host/beam.hpp).
 //
 // Requirements: fp16-exact weights, d in {128, 384}, R <= 24 rows, t_max <= 128; greedy (k = 1) with identity ancestry, or
 // the beam mode.  Everything else is handled by decoder5.cu / decoder3.cu.

@@ -680,20 +680,13 @@ bool Session::beam_decode(const std::vector<std::vector<int64_t>>& prompts, int 
     for (int w = 0; w < W; ++w) {
         const size_t node0 = ((size_t)fin_win[(size_t)2 * w] * W + w) * MN;   // the window's current buffer
         const int n = fin_cnt[(size_t)fin_win[(size_t)2 * w] * W + w];
-        double lp[MN];
-        int order[MN];
-        for (int i = 0; i < n; ++i) lp[i] = fin_head[node0 + i].log_prob;
-        fx::rank_final(lp, n, order);
-        for (int r = 0; r < n; ++r) {
-            const fx::Head& h = fin_head[node0 + order[r]];
-            const size_t o = (node0 + order[r]) * used;
-            Hypothesis hy;
-            hy.ids.assign(fin_seq.begin() + o, fin_seq.begin() + o + h.len);
-            hy.lps.assign(fin_lp.begin() + o, fin_lp.begin() + o + h.len);
-            hy.score = h.log_prob;
-            hy.finished = h.finished != 0;
-            nbest[(size_t)w].push_back(std::move(hy));
+        Carried c;
+        for (size_t i = node0; i < node0 + n; ++i) {
+            c.heads.push_back(fin_head[i]);
+            c.ids.emplace_back(fin_seq.begin() + i * used, fin_seq.begin() + i * used + fin_head[i].len);
+            c.lps.emplace_back(fin_lp.begin() + i * used, fin_lp.begin() + i * used + fin_head[i].len);
         }
+        nbest[(size_t)w] = ranked_nbest(c);
     }
     return true;
 }

@@ -66,15 +66,6 @@ struct ScoreWs {
     std::vector<std::unique_ptr<GemmF16Plan>> plans;      // per decoder layer: qkv, out, cross query, cross out, mlp1, mlp2
 };
 
-// one hypothesis of a window's n-best list (wb_session_last_nbest): a node of the beam search's final carried list
-struct Hypothesis {
-    std::vector<int64_t> ids;   // prompt + generated ids
-    std::vector<float> lps;     // 0 for each prompt id, else the log-prob the search scored the id with
-    double score = 0.0;         // the node's cumulative log-prob as the search carried it
-    bool finished = false;      // last id is eot
-};
-using NBest = std::vector<Hypothesis>;   // best first (beamfx::rank_final)
-
 // pinned host array
 struct PinnedFree { void operator()(void* p) const { cudaFreeHost(p); } };
 template <typename T> using Pinned = std::unique_ptr<T[], PinnedFree>;

@@ -56,122 +56,29 @@ bool find_chunk_overlap(const int64_t* prev, int64_t n_prev, const int64_t* curr
 
 namespace {
 
-struct BeamSearchToken {   // transcribe.rs:142-146 (+ the cache row that produced it)
-    int64_t token;
-    double log_prob;
-    int32_t row;           // device row whose K/V ancestry this token extends
-};
-using Node = beam::BeamNode<BeamSearchToken>;
-
-// the beam search on the host, all windows in lock-step at one position p, one decoder launch per position
-// (Session::step_beams).  Window w's search starts at p = prompts[w].size() - 1; until then its prompt node rides along in
-// one row (its own row as parent, its next prompt token) and its candidates are discarded.
+// the host beam search (beam_search_windows) of every encoded window, one decoder launch per position (Session::step_beams)
 void host_beam_search(Session& s, const std::vector<std::vector<int64_t>>& prompts, int beam_size, int max_depth, int64_t eot,
                       std::vector<std::vector<int64_t>>& out, std::vector<std::vector<float>>& out_lp, std::vector<NBest>& nbest) {
-    const int W = s.n_windows;
-    auto is_finished = [eot](const std::vector<BeamSearchToken>& seq) { return !seq.empty() && seq.back().token == eot; };
-    std::vector<std::vector<Node>> beams((size_t)W);
-    std::vector<char> done((size_t)W, 0);
-    for (int w = 0; w < W; ++w) {
-        Node n;
-        for (int64_t t : prompts[(size_t)w]) n.seq.push_back(BeamSearchToken{t, 0.0, w});
-        n.log_prob = 0.0;
-        beams[(size_t)w].push_back(std::move(n));
-    }
     s.begin(prompts);
-    std::vector<int32_t> win_of_row, parent;
-    std::vector<int64_t> tok, top_id;
-    std::vector<float> top_lp;
+    std::vector<float> lp32;
+    auto step = [&](int, int64_t n_rows, const int32_t* window_of_row, const int32_t* parent_row, const int64_t* token,
+                    int apply_mask, int k, int64_t* ids_out, double* lps_out) {
+        lp32.resize((size_t)n_rows * k);
+        s.step_beams(n_rows, window_of_row, parent_row, token, apply_mask, k, ids_out, lp32.data());
+        std::copy(lp32.begin(), lp32.end(), lps_out);
+    };
     int64_t steps = 0;
-    for (;;) {
-        const int p = s.host_pos;
-        auto searching = [&](int w) { return p + 1 >= (int)prompts[(size_t)w].size(); };
-        // beam.rs:22-27: stop a search when its best beam is finished, or after max_depth steps past its prompt
-        bool any = false;
-        for (int w = 0; w < W; ++w) {
-            if (done[(size_t)w]) continue;
-            const int best = beam::max_by_last(beams[(size_t)w]);
-            if (searching(w) && ((best >= 0 && is_finished(beams[(size_t)w][(size_t)best].seq)) ||
-                                 p + 1 - (int)prompts[(size_t)w].size() >= max_depth))
-                done[(size_t)w] = 1;
-            else any = true;
-        }
-        if (!any) break;
-        // rows = live beams of unfinished windows, window-major
-        win_of_row.clear(); parent.clear(); tok.clear();
-        std::vector<std::vector<int>> row_of_beam((size_t)W);
-        size_t max_seq_len = 0;   // over searching windows: every one's longest beam has p + 1 tokens
-        for (int w = 0; w < W; ++w) {
-            if (done[(size_t)w]) continue;
-            if (!searching(w)) {   // the prompt node: the token at p, its row extended by one position
-                BeamSearchToken& last = beams[(size_t)w][0].seq.back();
-                parent.push_back(last.row);
-                last.row = (int32_t)win_of_row.size();
-                win_of_row.push_back(w);
-                tok.push_back(prompts[(size_t)w][(size_t)p]);
-                continue;
-            }
-            row_of_beam[(size_t)w].assign(beams[(size_t)w].size(), -1);
-            for (size_t b = 0; b < beams[(size_t)w].size(); ++b) {
-                const Node& n = beams[(size_t)w][b];
-                max_seq_len = std::max(max_seq_len, n.seq.size());
-                if (is_finished(n.seq)) continue;   // continuations of finished beams are discarded (beam.rs:56-57)
-                row_of_beam[(size_t)w][b] = (int)win_of_row.size();
-                win_of_row.push_back(w);
-                parent.push_back(n.seq.back().row);
-                tok.push_back(n.seq.back().token);
-            }
-        }
-        const int64_t n_rows = (int64_t)win_of_row.size();
-        if (n_rows == 0) break;
-        const int k = beam_size;
-        top_id.resize((size_t)n_rows * k);
-        top_lp.resize((size_t)n_rows * k);
-        const int apply_mask = max_seq_len > 5 ? 0 : 1;   // transcribe.rs:271-275
-        s.step_beams(n_rows, win_of_row.data(), parent.data(), tok.data(), apply_mask, k, top_id.data(), top_lp.data());
-        ++steps;
-        for (int w = 0; w < W; ++w) {
-            if (done[(size_t)w] || !searching(w)) continue;
-            auto next = [&](const std::vector<Node>& bs) {
-                std::vector<std::vector<std::pair<BeamSearchToken, double>>> conts(bs.size());
-                for (size_t b = 0; b < bs.size(); ++b) {
-                    const int row = row_of_beam[(size_t)w][b];
-                    if (row < 0) continue;
-                    // candidates in ascending token order, as the reference enumerates the vocabulary
-                    std::vector<std::pair<int64_t, float>> c;
-                    for (int i = 0; i < k; ++i)
-                        if (top_id[(size_t)row * k + i] >= 0) c.emplace_back(top_id[(size_t)row * k + i], top_lp[(size_t)row * k + i]);
-                    std::sort(c.begin(), c.end(), [](const auto& a, const auto& b2) { return a.first < b2.first; });
-                    for (const auto& e : c)
-                        conts[b].emplace_back(BeamSearchToken{e.first, (double)e.second, row},
-                                              bs[b].log_prob + (double)e.second);   // transcribe.rs:291-299
-                }
-                return conts;
-            };
-            beams[(size_t)w] = beam::beam_search_step(beams[(size_t)w], next, is_finished, (size_t)beam_size);
-        }
-    }
+    const std::vector<Carried> carried = beam_search_windows(prompts, s.host_pos, beam_size, max_depth, eot, step, &steps);
     s.last_steps = steps;
     // each window's final carried list, ranked; the best row is its rank 0 (max_by_last)
-    out.assign((size_t)W, {});
-    out_lp.assign((size_t)W, {});
-    nbest.assign((size_t)W, {});
-    for (int w = 0; w < W; ++w) {
-        for (int i : beam::rank_final(beams[(size_t)w])) {
-            const Node& n = beams[(size_t)w][(size_t)i];
-            Hypothesis h;
-            for (const auto& t : n.seq) {
-                h.ids.push_back(t.token);
-                h.lps.push_back((float)t.log_prob);   // exact: a widened f32 (transcribe.rs:291-299)
-            }
-            h.score = n.log_prob;
-            h.finished = is_finished(n.seq);
-            nbest[(size_t)w].push_back(std::move(h));
-        }
-        if (!nbest[(size_t)w].empty()) {
-            out[(size_t)w] = nbest[(size_t)w][0].ids;
-            out_lp[(size_t)w] = nbest[(size_t)w][0].lps;
-        }
+    out.assign(carried.size(), {});
+    out_lp.assign(carried.size(), {});
+    nbest.assign(carried.size(), {});
+    for (size_t w = 0; w < carried.size(); ++w) {
+        nbest[w] = ranked_nbest(carried[w]);
+        if (nbest[w].empty()) continue;
+        out[w] = nbest[w][0].ids;
+        out_lp[w] = nbest[w][0].lps;
     }
 }
 

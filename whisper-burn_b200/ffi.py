@@ -88,9 +88,8 @@ SYMBOLS = {
     "wb_session_last_decoder": (C.c_int, [_P]),
     "wb_session_last_topk": (C.c_int, [_P, C.c_int64, C.c_int64, _I64, _F]),
     "wb_beam_search_table": (C.c_int64, [C.POINTER(C.c_double), C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _I64, C.c_int64]),
-    "wb_beam_search_table_fixed": (C.c_int64, [C.POINTER(C.c_double), C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _I64, C.c_int64]),
     "wb_beam_nbest_table": (C.c_int64, [C.POINTER(C.c_double), C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
-                                        C.c_int, C.c_int64, C.c_int64, _I64, _I64, C.POINTER(C.c_double), _I32]),
+                                        C.c_int64, C.c_int64, _I64, _I64, C.POINTER(C.c_double), _I32]),
     "wb_load_wav": (C.c_int, [C.c_char_p, C.c_int, _F, C.c_int64, _I64, _I64, C.POINTER(C.c_int)]),
     "wb_window_count": (C.c_int64, [C.c_int64, C.c_int64, C.c_int64]),
     "wb_window_bounds": (C.c_int, [C.c_int64, C.c_int64, C.c_int64, _I64, _I64]),
