@@ -2,7 +2,7 @@
 
 synth.make_weights_np gives every LayerNorm eps = 1e-5, so a kernel that reads another LayerNorm's eps, hard-codes 1e-5 or
 falls back to a default computes the same bits as a correct one.  These are the real-width models of the float64 tests
-(test_f64_reference_gpu._weights) with every LayerNorm given its own eps, a power of two (the same number in float32 and
+(harness.shallow_weights) with every LayerNorm given its own eps, a power of two (the same number in float32 and
 float64), in the order of the sorted /eps keys:
 
   * decoder: 2^-11, 2^-4, 2^-9, 2^-8, 2^-3, 2^-6, 2^-5 (block_0/attn_ln, block_0/cross_attn_ln, block_0/mlp_ln,
@@ -17,7 +17,7 @@ import functools
 import numpy as np
 import torch
 
-import test_f64_reference_gpu as f64
+import harness as h
 
 MODES = ("outside", "inside")
 DEC_EPS = tuple(2.0 ** e for e in (-11, -4, -9, -8, -3, -6, -5))
@@ -50,6 +50,12 @@ def with_eps(w_np, w64, eps):
 
 @functools.lru_cache(maxsize=4)
 def weights(d, H, V, n_text_layer=2, exact=True):
-    """(dims, float32 weights, float64 weights) of f64._weights with the per-LayerNorm eps of this module"""
-    dims, w_np, w64 = f64._weights(d, H, V, n_text_layer, exact)
+    """(dims, float32 weights, float64 weights) of harness.shallow_weights with the per-LayerNorm eps of this module"""
+    dims, w_np, _, w64 = h.shallow_weights(d, H, V, n_text_layer, exact)
     return (dims, *with_eps(w_np, w64, scheme(w_np)))
+
+
+def make_model(d, H, V, mode, exact=True, n_text_layer=2):
+    """(dims, float32 weights, GPU model in placement `mode`, float64 weights) of weights()"""
+    dims, w_np, w64 = weights(d, H, V, n_text_layer, exact)
+    return dims, w_np, h.whisper(dims, w_np, exact, ln_eps_outside=mode == "outside"), w64

@@ -9,18 +9,17 @@ tolerance it is compared with:
   * two layers' LayerNorm parameters (weight and bias) swapped, for every pair of layers and every LayerNorm of a block.
 
 The quantities: the teacher-forced log-probs of the oracle's own DEPTH-step greedy path on one fixed encoder output against
-the fp32 K/V GREEDY_LP_TOL, and the encoder output (relative to its scale) against ENC_REL_TOL.  Against the fp16 K/V
-tolerance (50 times larger) nothing is claimed: a left-out MLP bias moves the log-probs by less."""
+the fp32 K/V harness.DEEP_GREEDY_LP_TOL, and the encoder output (relative to its scale) against harness.DEEP_ENC_REL_TOL.
+Against the fp16 K/V tolerance (50 times larger) nothing is claimed: a left-out MLP bias moves the log-probs by less."""
 import itertools
 
 import numpy as np
 import pytest
 import torch
 
-import test_depth_f64_gpu as dg
-import test_f64_reference_gpu as f64
+import harness as h
+from harness import check_moves, greedy_path, window_mel
 from oracle import model as o_model, synth
-from test_layernorm_eps_cpu import MARGIN, greedy_path, window_mel
 
 V = 2051
 QKV = ("query/weight", "query/bias", "key/weight", "value/weight", "value/bias")
@@ -57,35 +56,32 @@ def changes(w, prefix, L, lns):
 
 
 def check(moved, tol, what):
-    short = {k: v for k, v in moved.items() if v < MARGIN * tol}
-    least = min(moved, key=moved.get)
-    print(f"\n[depth] {what}: smallest move {moved[least]:.2e} ({least}), {moved[least] / tol:.0f}x the tolerance {tol:.0e}")
-    assert not short, f"{what}: moved less than {MARGIN}x {tol:.0e}: {short}"
+    check_moves(moved, tol, what, "depth")
 
 
 def path_log_probs(w64, dims, sp, xa, toks):
-    rows = dg.path_rows(w64, dims, sp, [xa], [toks], "f32", [range(1, len(toks) - 3)])[0]
+    rows = h.forward_rows(w64, dims, [xa], [toks], sp=sp, steps=[range(1, len(toks) - 3)])[0]
     return np.array([rows[s][toks[3 + s]] for s in rows])
 
 
 @pytest.mark.parametrize("d,L", [(384, 3), (384, 4), (512, 6)])
 def test_decoder_log_probs_move(d, L):
-    dims, _, w64 = dg._weights(d, d // 64, V, 1, L)
+    dims, _, _, w64 = h.deep_weights(d, V, 1, L)
     sp = synth.special_tokens(dims)
     xa = o_model.forward_encoder(w64, dims, window_mel(dims))
     toks = greedy_path(w64, dims, sp, xa, o_model.DEFAULT_OPTS)
-    assert len(toks) == 4 + f64.DEPTH, toks
+    assert len(toks) == 4 + h.DEPTH, toks
     base = path_log_probs(w64, dims, sp, xa, toks)
     moved = {what: float(np.abs(path_log_probs(w, dims, sp, xa, toks) - base).max())
              for what, w in changes(w64, "decoder", L, ("attn_ln", "cross_attn_ln", "mlp_ln"))}
-    check(moved, dg.GREEDY_LP_TOL["f32"], f"greedy path d={d} L={L}")
+    check(moved, h.DEEP_GREEDY_LP_TOL["f32"], f"greedy path d={d} L={L}")
 
 
 @pytest.mark.parametrize("d,L", [(384, 4), (512, 6)])
 def test_encoder_output_moves(d, L):
-    dims, _, w64 = dg._weights(d, d // 64, V, L, 1)
+    dims, _, _, w64 = h.deep_weights(d, V, L, 1)
     mel = window_mel(dims)
     base = o_model.forward_encoder(w64, dims, mel)[0].numpy()
-    moved = {what: f64.rel_to_scale(o_model.forward_encoder(w, dims, mel)[0].numpy(), base)
+    moved = {what: h.rel_to_scale(o_model.forward_encoder(w, dims, mel)[0].numpy(), base)
              for what, w in changes(w64, "encoder", L, ("attn_ln", "mlp_ln"))}
-    check(moved, dg.ENC_REL_TOL, f"encoder d={d} L={L}")
+    check(moved, h.DEEP_ENC_REL_TOL, f"encoder d={d} L={L}")

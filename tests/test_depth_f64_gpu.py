@@ -9,8 +9,8 @@ decoder5 chains its stage table into the next layer and folds a layer's MLP2 par
 encoder caches its tensor-map plans per GEMM site (2 + 4 l + ...) and the scorer keeps 6 plans per layer.  Here the same
 checks run on models of 3, 4, 6, 12, 24 and 32 layers (L = 3 breaks the even parity every real depth shares):
 
-  * deep decoder models have 1 audio layer, deep encoder models 1 text layer; one float64 model is held at a time (_weights);
-  * greedy decoders, per step, top-1 against float64 (test_f64_reference_gpu.check_greedy), at the rows that pick each
+  * deep decoder models have 1 audio layer, deep encoder models 1 text layer; one float64 model is held at a time (harness.deep_weights);
+  * greedy decoders, per step, top-1 against float64 (harness.check_greedy), at the rows that pick each
     instance's tile (decoder4 RC = 4 / 8, decoder6 NT8 = 1 / 3, decoder5 row groups) and, for one deep case per decoder, at
     every self-attention key-count edge up to max_text_len;
   * wb_session_step (k = 7, beams) and the stateless forward_decoder at 448 positions;
@@ -20,43 +20,26 @@ checks run on models of 3, 4, 6, 12, 24 and 32 layers (L = 3 breaks the even par
   * one long-lived Session per decoder family taking a sequence of calls whose rows, decoder, search and kind change from
     call to call, each checked against float64 and bit for bit against the same call on a fresh Session.
 
-The float64 reference of a greedy or beam path is one teacher-forced oracle.model.forward_decoder over the whole path (rows
-on windows of one length batched): the same arithmetic as the cached decoder, with the weights read once per path rather than
-once per step, which is what makes 24 and 32 float64 layers affordable in this process.  The error grows with depth, so the
-constants below replace test_f64_reference_gpu.py's, each with the worst error measured on one H100 and its margin.
+The float64 reference of a greedy or beam path is one teacher-forced oracle.model.forward_decoder over the whole path
+(harness.forward_rows, rows on windows of one length batched): the same arithmetic as the cached decoder, with the weights
+read once per path rather than once per step, which is what makes 24 and 32 float64 layers affordable in this process.  The
+error grows with depth, so harness.py's DEEP_* constants replace the float64 suite's here, each with the worst error
+measured on one H100 and its margin.
 test_depth_f64_cpu.py shows that a layer-indexing mistake moves what is compared here by far more than these tolerances."""
 import dataclasses
-import gc
 import resource
 import time
 
 import numpy as np
 import pytest
-import torch
 
-import test_f64_reference_gpu as f64
+import harness as h
 import wb200  # noqa: F401
-from oracle import model as o_model, synth, transcribe as o_tr
-from test_score_tokens_gpu import check_rows, is_special_of, random_seqs
-from whisper_burn_b200 import ffi, model, transcribe
-from whisper_burn_b200.synth import WhisperDims
+from oracle import synth
+from whisper_burn_b200 import ffi, transcribe
 
 pytestmark = pytest.mark.gpu
 
-# Worst errors measured on one H100 80GB HBM3 (700 W power limit) at 3 to 32 layers; each constant keeps a 3x margin or
-# more.  The error grows with depth and width: none of these fit test_f64_reference_gpu.py's constants with that margin.
-# greedy top-1 log-prob (and the log-probs of decoded greedy and beam paths).  Worst: f32 9.8e-6 (decoder5, d = 1280,
-# L = 32, 9 rows), 3.0x; f16 4.5e-4 (the same case), 3.3x
-GREEDY_LP_TOL = {"f32": 3e-5, "f16": 1.5e-3}
-# wb_session_step, all 7 candidates.  Worst: f32 2.1e-6 (decoder3, d = 384, L = 4), 4.7x (test_f64_reference_gpu's
-# constant); f16 2.9e-4 (decoder5, d = 512, L = 6), 3.4x
-STEP_LP_TOL = {"f32": f64.STEP_LP_TOL["f32"], "f16": 1e-3}
-# score_tokens.  Worst: f32 1.8e-5 (d = 1280, L = 32), 3.4x; f16 7.0e-4 (d = 1024, L = 24), 3.6x
-SCORE_LP_TOL = {"f32": 6e-5, "f16": 2.5e-3}
-# forward_decoder logits at 448 positions, relative to scale.  Worst 1.35e-5 (decoder5, d = 512, L = 6), 3.7x
-LOGITS_REL_TOL = 5e-5
-# encoder output, relative to scale.  Worst 2.0e-5 (tensor-core, d = 1280, L = 32), 3.5x
-ENC_REL_TOL = 7e-5
 SCORE_GROUP_ROWS = 4096     # score.cu: rows of one scoring pass
 
 
@@ -68,59 +51,8 @@ def _peak_memory():
     print(f"\n[f64] depth file: {time.time() - t0:.0f} s, peak host memory {peak:.1f} GB")
 
 
-_held = {}
-
-
-def _weights(d, H, V, n_audio_layer, n_text_layer, exact=True):
-    """(dims, float32 weights, float64 weights), one model at a time: a float64 d = 1280, 32-layer decoder is ~7 GB, so the
-    previous model is dropped before the next is made (an lru_cache would make the new one first)."""
-    key = (d, H, V, n_audio_layer, n_text_layer, exact)
-    if key not in _held:
-        _held.clear()
-        gc.collect()
-        dims = WhisperDims(80, 1500, d, H, n_audio_layer, V, 448, d, H, n_text_layer)
-        _, w_np, _ = synth.make_weights(dims, seed=d + V + 100 * n_audio_layer + n_text_layer)
-        if not exact:
-            w_np = {k: (v * np.float32(1.0001) if v.ndim else v) for k, v in w_np.items()}
-        _held[key] = (dims, w_np, o_model.as_dtype(synth.to_torch(w_np)))
-    return _held[key]
-
-
-def make_model(d, V, n_audio_layer=1, n_text_layer=1, exact=True):
-    """(dims, GPU model, float64 weights): a deep decoder (n_audio_layer = 1) or a deep encoder (n_text_layer = 1)"""
-    dims, w_np, w64 = _weights(d, d // 64, V, n_audio_layer, n_text_layer, exact)
-    wh = model.Whisper(dims, w_np)
-    assert wh.weights_fp16_exact == exact
-    return dims, wh, w64
-
-
-def path_rows(w64, dims, sp, xa, paths, kv, row_steps):
-    """float64 log-prob rows along given paths, the special-token mask of greedy_path_log_probs included: per path
-    {s: row that picked paths[r][3 + s]} for the steps row_steps[r].  xa: per path its window's [1, T, d]; paths on windows of
-    one length run as one batch (padded at the end, which the causal mask keeps from earlier positions)."""
-    opts = o_model.OracleOptions(kv_dtype=kv)
-    maskout = torch.from_numpy(sp.maskout()).double()
-    by_T = {}
-    for r, x in enumerate(xa):
-        by_T.setdefault(x.shape[1], []).append(r)
-    out = [None] * len(paths)
-    for rs in by_T.values():
-        n = max(len(paths[r]) for r in rs) - 1
-        toks = torch.tensor([paths[r][:-1] + [0] * (n + 1 - len(paths[r])) for r in rs], dtype=torch.int64)
-        logits = o_model.forward_decoder(w64, dims, toks, torch.cat([xa[r] for r in rs]), opts)
-        for i, r in enumerate(rs):
-            rows = {}
-            for s in row_steps[r]:
-                row = logits[i, s + 2]
-                if o_tr.masks_specials(s + 3):
-                    row = row + maskout
-                rows[s] = o_model.log_softmax_last(row).numpy()
-            out[r] = rows
-    return out
-
-
 def ref_rows_of(w64, dims):
-    return lambda sp, xa, paths, kv, row_steps: path_rows(w64, dims, sp, xa, paths, kv, row_steps)
+    return lambda sp, xa, paths, kv, row_steps: h.forward_rows(w64, dims, xa, paths, kv, sp=sp, steps=row_steps)
 
 
 # ---------------------------------------------------------------- a. greedy decoders, per step, top-1 against float64
@@ -151,20 +83,20 @@ def test_greedy_steps_vs_float64(case, monkeypatch):
     """decoder4 (RC = 4, 8), decoder6 (NT8 = 1, 3), decoder5 (1, 9 and 33 rows: one row group and 32 + 1) and decoder3
     (fp16 and fp32 weights), each forced with WB200_DECODER, at 3 to 32 layers."""
     dec, d, L, V, rows, kv, deep, exact = case
-    dims, wh, w64 = make_model(d, V, n_text_layer=L, exact=exact)
-    f64.use_decoder(monkeypatch, dec)
-    args = dict(tol=GREEDY_LP_TOL[kv], ref_rows=ref_rows_of(w64, dims))
+    dims, wh, w64 = h.make_deep_model(d, V, n_text_layer=L, exact=exact)
+    h.use_decoder(monkeypatch, dec)
+    args = dict(tol=h.DEEP_GREEDY_LP_TOL[kv], ref_rows=ref_rows_of(w64, dims))
     if deep:
         edges, t_max = DEEP_EDGES[dec]
-        args.update(steps=f64.edge_steps(edges, t_max), max_text_len=t_max, full_depth=True)
+        args.update(steps=h.edge_steps(edges, t_max), max_text_len=t_max, full_depth=True)
     try:
-        worst = f64.check_greedy(dims, wh, kv, rows, dec, 3000 + 10 * L + rows, **args)
+        worst = h.check_greedy(dims, wh, kv, rows, dec, 3000 + 10 * L + rows, **args)
     except ffi.WbError as e:
         # decoder4 runs one 16-CTA cluster per row and needs all of them co-resident (test_f64_reference_gpu.check_decoder4)
         if dec != 4 or e.code != ffi.WB_ERR_UNSUPPORTED or rows <= 4:
             raise
         pytest.skip(f"decoder4 does not cover {rows} rows: fewer than {rows} co-resident 16-CTA clusters fit on this GPU")
-    f64.report(case_id(case), worst, GREEDY_LP_TOL[kv])
+    h.report(case_id(case), worst, h.DEEP_GREEDY_LP_TOL[kv])
 
 
 # ---------------------------------------------------------------- b. wb_session_step and forward_decoder
@@ -173,35 +105,23 @@ def test_greedy_steps_vs_float64(case, monkeypatch):
 def test_session_step_k7_beams_vs_float64(decoder, d, L, V, kv, monkeypatch):
     """test_f64_reference_gpu.test_session_step_k7_beams_vs_float64 (rows fanned out and continued from other parents) on
     decoder3 at 384 / 4 layers and decoder5 at 512 / 6."""
-    dims, wh, w64 = make_model(d, V, n_text_layer=L)
-    f64.use_decoder(monkeypatch, decoder)
-    worst = f64.check_step_k7(dims, wh, w64, decoder, kv, tol=STEP_LP_TOL[kv])
-    f64.report(f"step k=7 decoder{decoder} d={d} L={L} kv={kv}", worst, STEP_LP_TOL[kv])
+    dims, wh, w64 = h.make_deep_model(d, V, n_text_layer=L)
+    h.use_decoder(monkeypatch, decoder)
+    worst = h.check_step_k7(dims, wh, w64, decoder, kv, tol=h.DEEP_STEP_LP_TOL[kv])
+    h.report(f"step k=7 decoder{decoder} d={d} L={L} kv={kv}", worst, h.DEEP_STEP_LP_TOL[kv])
 
 
 @pytest.mark.parametrize("decoder,d,L", [(3, 384, 4), (5, 512, 6)])
 def test_forward_decoder_448_positions_vs_float64(decoder, d, L, monkeypatch):
-    f64.use_decoder(monkeypatch, decoder)
-    dims, wh, w64 = make_model(d, 2051, n_text_layer=L)
-    worst = f64.forward_decoder_448_error(dims, wh, w64)
-    f64.report(f"forward_decoder 448 positions decoder{decoder} d={d} L={L}", worst, LOGITS_REL_TOL)
-    assert worst < LOGITS_REL_TOL
+    h.use_decoder(monkeypatch, decoder)
+    dims, wh, w64 = h.make_deep_model(d, 2051, n_text_layer=L)
+    worst = h.forward_decoder_448_error(dims, wh, w64)
+    h.report(f"forward_decoder 448 positions decoder{decoder} d={d} L={L}", worst, h.DEEP_LOGITS_REL_TOL)
+    assert worst < h.DEEP_LOGITS_REL_TOL
 
 
 # ---------------------------------------------------------------- c. encoder
 ENC_DEPTHS = ((384, 4), (512, 6), (768, 12), (1024, 24), (1280, 32))
-
-
-def encoder_error(sess, w64, dims, Ts):
-    worst = 0.0
-    for w, T in enumerate(Ts):
-        got = sess.get_encoder_output(w)
-        assert got.shape == (T, dims.n_audio_state)
-        mel = torch.from_numpy(sess.get_mel(w)).double()[None]
-        e = f64.rel_to_scale(got, o_model.forward_encoder(w64, dims, mel)[0].numpy())
-        worst = max(worst, e)
-        assert e < ENC_REL_TOL, f"window {w} (T = {T}): {e}"
-    return worst
 
 
 @pytest.mark.parametrize("d,L,exact", [(d, L, exact) for d, L in ENC_DEPTHS for exact in (True, False) if exact or L <= 12],
@@ -209,42 +129,25 @@ def encoder_error(sess, w64, dims, Ts):
 def test_deep_encoder_vs_float64(d, L, exact):
     """Windows of T = 6, 64, 65, 750 in one batch (and at 384 / 4 one native T = 1500 window) through L encoder layers:
     wgmma GEMMs and enc_attn_tc.cu on fp16-exact weights, gemm.cu and the fp32 attention otherwise."""
-    dims, wh, w64 = make_model(d, 2051, n_audio_layer=L, exact=exact)
-    Ts, waves = f64.windows(4, seed=900 + L, order=(6, 64, 65, 750))
+    dims, wh, w64 = h.make_deep_model(d, 2051, n_audio_layer=L, exact=exact)
+    Ts, waves = h.windows(4, seed=900 + L, order=(6, 64, 65, 750))
     sess = transcribe.Session(wh, max_windows=4, max_beams=1, max_text_len=8)
     sess.encode_waveforms(waves)
-    worst = encoder_error(sess, w64, dims, Ts)
-    f64.report(f"encoder d={d} L={L} {'tensor-core' if exact else 'fp32'}", worst, ENC_REL_TOL)
+    worst = h.encoder_error(sess, w64, dims, Ts, h.DEEP_ENC_REL_TOL)
+    h.report(f"encoder d={d} L={L} {'tensor-core' if exact else 'fp32'}", worst, h.DEEP_ENC_REL_TOL)
     if d == 384:
         sess = transcribe.Session(wh, max_windows=1, max_beams=1, max_text_len=8, windows="native")
         sess.encode_waveforms([synth.waveform(480000, seed=901)])
-        worst = encoder_error(sess, w64, dataclasses.replace(dims, n_audio_ctx=2 * dims.n_audio_ctx), [1500])
-        f64.report(f"encoder native T=1500 d={d} L={L} {'tensor-core' if exact else 'fp32'}", worst, ENC_REL_TOL)
+        worst = h.encoder_error(sess, w64, dataclasses.replace(dims, n_audio_ctx=2 * dims.n_audio_ctx), [1500], h.DEEP_ENC_REL_TOL)
+        h.report(f"encoder native T=1500 d={d} L={L} {'tensor-core' if exact else 'fp32'}", worst, h.DEEP_ENC_REL_TOL)
 
 
 # ---------------------------------------------------------------- d. scorer
-def scored_rows(w64, dims, xa, seq, kv):
-    logits = o_model.forward_decoder(w64, dims, torch.tensor([seq], dtype=torch.int64), xa, o_model.OracleOptions(kv_dtype=kv))
-    return o_model.log_softmax_last(logits)[0].numpy()
-
-
-def masked_seqs(sp, seed):
-    """prompt + ids with special ids at j = 4, 5 (masked: -inf), 6 and 9 (not masked)"""
-    rng = np.random.default_rng(seed)
-    specials = list(range(sp.first_special, sp.n_vocab))
-    seqs = []
-    for r in range(4):
-        body = [int(t) for t in rng.integers(0, sp.first_special, size=20 + 7 * r)]
-        body[0], body[1], body[2], body[5] = specials[r], specials[r + 1], specials[r + 2], specials[r + 3]
-        seqs.append(list(sp.prompt()) + body)
-    return seqs
-
-
 def check_masked(sess, w64, dims, sp, xa, kv, tol):
-    seqs = masked_seqs(sp, 9)
+    seqs = h.masked_seqs(sp, 9)
     wins = [r % len(xa) for r in range(len(seqs))]
-    out = sess.score_tokens(seqs, wins, apply_special_mask=True, is_special=is_special_of(sp))
-    rows = path_rows(w64, dims, sp, [xa[w] for w in wins], seqs, kv, [range(1, len(s) - 3) for s in seqs])
+    out = sess.score_tokens(seqs, wins, apply_special_mask=True, is_special=h.is_special_of(sp))
+    rows = h.forward_rows(w64, dims, [xa[w] for w in wins], seqs, kv, sp=sp, steps=[range(1, len(s) - 3) for s in seqs])
     worst = 0.0
     for seq, (lp, _), ref in zip(seqs, out, rows):
         assert np.isneginf(lp[4]) and np.isneginf(lp[5]) and np.all(np.isfinite(lp[6:]))
@@ -258,24 +161,24 @@ def check_masked(sess, w64, dims, sp, xa, kv, tol):
 @pytest.mark.parametrize("kv", KVS)
 @pytest.mark.parametrize("d,L,V", [(768, 12, 2051), (1024, 24, 51864), (1280, 32, 51865)])
 def test_score_deep_vs_float64(d, L, V, kv):
-    """The LENGTHS sequences of test_score_tokens_gpu.py (around the 64-row tiles up to n_text_ctx) on windows of T = 6, 64,
+    """The harness.LENGTHS sequences (around the 64-row tiles up to n_text_ctx) on windows of T = 6, 64,
     65, 750, and the masked rows of the beam rule, through 12, 24 and 32 layers."""
-    dims, wh, w64 = make_model(d, V, n_text_layer=L)
+    dims, wh, w64 = h.make_deep_model(d, V, n_text_layer=L)
     sp = synth.special_tokens(dims)
-    Ts, waves = f64.windows(4, seed=11 * L)
-    sess = transcribe.Session(wh, max_windows=4, max_beams=1, max_text_len=8, kv_dtype=f64.kv_code(kv))
+    Ts, waves = h.windows(4, seed=11 * L)
+    sess = transcribe.Session(wh, max_windows=4, max_beams=1, max_text_len=8, kv_dtype=h.kv_code(kv))
     sess.encode_waveforms(waves)
-    xa = f64.encoder_outputs64(sess, Ts)
-    seqs = random_seqs(V, L)
+    xa = h.encoder_outputs64(sess, Ts)
+    seqs = h.random_seqs(V, L)
     wins = [i % 4 for i in range(len(seqs))]
     out = sess.score_tokens(seqs, wins)
-    tol = SCORE_LP_TOL[kv]
+    tol = h.DEEP_SCORE_LP_TOL[kv]
     worst = 0.0
     for (lp, am), seq, w in zip(out, seqs, wins):
-        ref = scored_rows(w64, dims, xa[w], seq, kv) if len(seq) > 1 else None
-        worst = max(worst, check_rows(lp, am, ref, seq, kv, f"d={d} L={L} kv={kv} T={Ts[w]} len={len(seq)}", tol=tol))
+        ref = h.forward_rows(w64, dims, [xa[w]], [seq], kv)[0] if len(seq) > 1 else None
+        worst = max(worst, h.check_rows(lp, am, ref, seq, kv, f"d={d} L={L} kv={kv} T={Ts[w]} len={len(seq)}", tol=tol))
     worst = max(worst, check_masked(sess, w64, dims, sp, xa, kv, tol))
-    f64.report(f"score_tokens d={d} L={L} kv={kv}", worst, tol)
+    h.report(f"score_tokens d={d} L={L} kv={kv}", worst, tol)
 
 
 @pytest.mark.parametrize("kv", KVS)
@@ -283,27 +186,27 @@ def test_score_groups_vs_float64(kv):
     """One call of more than SCORE_GROUP_ROWS rows at 384 / 4 layers: ten length-448 sequences among short ones (length 1
     included) run as two groups; each sequence against float64 and bit for bit against itself scored alone; and a call of
     length-1 sequences only (a group without rows)."""
-    dims, wh, w64 = make_model(384, 2051, n_text_layer=4)
-    Ts, waves = f64.windows(4, seed=13)
-    sess = transcribe.Session(wh, max_windows=4, max_beams=1, max_text_len=8, kv_dtype=f64.kv_code(kv))
+    dims, wh, w64 = h.make_deep_model(384, 2051, n_text_layer=4)
+    Ts, waves = h.windows(4, seed=13)
+    sess = transcribe.Session(wh, max_windows=4, max_beams=1, max_text_len=8, kv_dtype=h.kv_code(kv))
     sess.encode_waveforms(waves)
-    xa = f64.encoder_outputs64(sess, Ts)
-    long = random_seqs(dims.n_vocab, 17, lengths=(448,) * 10)
-    short = random_seqs(dims.n_vocab, 18, lengths=(1, 2, 65, 1, 130, 1, 7, 64, 1, 300, 1))
+    xa = h.encoder_outputs64(sess, Ts)
+    long = h.random_seqs(dims.n_vocab, 17, lengths=(448,) * 10)
+    short = h.random_seqs(dims.n_vocab, 18, lengths=(1, 2, 65, 1, 130, 1, 7, 64, 1, 300, 1))
     seqs = [s for pair in zip(long, short) for s in pair] + short[10:]
     wins = [(3 * i) % 4 for i in range(len(seqs))]
     assert sum(len(s) - 1 for s in seqs) > SCORE_GROUP_ROWS
     out = sess.score_tokens(seqs, wins)
-    tol = SCORE_LP_TOL[kv]
+    tol = h.DEEP_SCORE_LP_TOL[kv]
     worst = 0.0
     for i, ((lp, am), seq, w) in enumerate(zip(out, seqs, wins)):
-        ref = scored_rows(w64, dims, xa[w], seq, kv) if len(seq) > 1 else None
-        worst = max(worst, check_rows(lp, am, ref, seq, kv, f"sequence {i} len={len(seq)} T={Ts[w]}", tol=tol))
+        ref = h.forward_rows(w64, dims, [xa[w]], [seq], kv)[0] if len(seq) > 1 else None
+        worst = max(worst, h.check_rows(lp, am, ref, seq, kv, f"sequence {i} len={len(seq)} T={Ts[w]}", tol=tol))
         alone = sess.score_tokens([seq], [w])[0]
         assert np.array_equal(alone[0], lp) and np.array_equal(alone[1], am), f"sequence {i}: not the bits it scores alone"
     ones = sess.score_tokens([[5], [7], [2050]], [0, 3, 1])
     assert all(np.array_equal(lp, [0.0]) and np.array_equal(am, [-1]) for lp, am in ones)
-    f64.report(f"score_tokens {len(seqs)} sequences, {sum(len(s) - 1 for s in seqs)} rows d=384 L=4 kv={kv}", worst, tol)
+    h.report(f"score_tokens {len(seqs)} sequences, {sum(len(s) - 1 for s in seqs)} rows d=384 L=4 kv={kv}", worst, tol)
 
 
 # ---------------------------------------------------------------- e. one long-lived Session, calls that change
@@ -327,28 +230,28 @@ def run_call(sess, call, decoder, dims, wh, w64, kv):
     """Runs one call on sess and checks it against float64; returns (its outputs, compared bit for bit across sessions,
     the worst |log-prob error|)."""
     sp = synth.special_tokens(dims)
-    tol = GREEDY_LP_TOL[kv]
+    tol = h.DEEP_GREEDY_LP_TOL[kv]
     if call[0] == "step":
         out = []
-        worst = f64.check_step_k7(dims, wh, w64, decoder, kv, sess=sess, tol=STEP_LP_TOL[kv], out=out)
+        worst = h.check_step_k7(dims, wh, w64, decoder, kv, sess=sess, tol=h.DEEP_STEP_LP_TOL[kv], out=out)
         return out, worst
     if call[0] == "score":
-        Ts, waves = f64.windows(3, seed=call[1])
+        Ts, waves = h.windows(3, seed=call[1])
         sess.encode_waveforms(waves)
-        xa = f64.encoder_outputs64(sess, Ts)
-        seqs = random_seqs(dims.n_vocab, call[1], lengths=(2, 65, 448, 1, 130))
+        xa = h.encoder_outputs64(sess, Ts)
+        seqs = h.random_seqs(dims.n_vocab, call[1], lengths=(2, 65, 448, 1, 130))
         wins = [i % 3 for i in range(len(seqs))]
         out = sess.score_tokens(seqs, wins)
-        worst = max(check_rows(lp, am, scored_rows(w64, dims, xa[w], seq, kv) if len(seq) > 1 else None, seq, kv, f"{call}",
-                               tol=SCORE_LP_TOL[kv]) for (lp, am), seq, w in zip(out, seqs, wins))
+        worst = max(h.check_rows(lp, am, h.forward_rows(w64, dims, [xa[w]], [seq], kv)[0] if len(seq) > 1 else None, seq, kv, f"{call}",
+                               tol=h.DEEP_SCORE_LP_TOL[kv]) for (lp, am), seq, w in zip(out, seqs, wins))
         return out, worst
     _, rows, beam, seed = call
-    Ts, waves = f64.windows(rows, seed)
-    toks = sess.transcribe_windows(waves, sp, sp.is_special_bitmap(), beam_size=beam, max_depth=f64.DEPTH)
+    Ts, waves = h.windows(rows, seed)
+    toks = sess.transcribe_windows(waves, sp, sp.is_special_bitmap(), beam_size=beam, max_depth=h.DEPTH)
     assert sess.last_decoder() == decoder, (call, sess.last_decoder())
     lps = [sess.last_logprobs(r) for r in range(rows)]
-    xa = f64.encoder_outputs64(sess, Ts)
-    refs = path_rows(w64, dims, sp, xa, toks, kv, [range(1, len(t) - 3) for t in toks])
+    xa = h.encoder_outputs64(sess, Ts)
+    refs = h.forward_rows(w64, dims, xa, toks, kv, sp=sp, steps=[range(1, len(t) - 3) for t in toks])
     worst = 0.0
     for r, (t, lp, ref) in enumerate(zip(toks, lps, refs)):
         for s in range(1, len(t) - 3):
@@ -376,10 +279,10 @@ def test_long_lived_session_vs_fresh(family, kv):
     result is itself taken twice: a call that two fresh sessions do not repeat bit for bit is reported and left to the
     float64 check."""
     d, L, V, n_win, n_beam, t_max, calls = HISTORY[family]
-    dims, wh, w64 = make_model(d, V, n_text_layer=L)
+    dims, wh, w64 = h.make_deep_model(d, V, n_text_layer=L)
 
     def session():
-        return transcribe.Session(wh, max_windows=n_win, max_beams=n_beam, max_text_len=t_max, kv_dtype=f64.kv_code(kv))
+        return transcribe.Session(wh, max_windows=n_win, max_beams=n_beam, max_text_len=t_max, kv_dtype=h.kv_code(kv))
 
     long_lived = session()
     unrepeatable = []
@@ -394,4 +297,4 @@ def test_long_lived_session_vs_fresh(family, kv):
         assert same_bits(got, fresh[0]), f"call {i} {call}: the long-lived session's result differs from a fresh session's"
     if unrepeatable:
         print(f"\n[f64] {family} kv={kv}: not bit-repeatable on fresh sessions (checked against float64 only): {unrepeatable}")
-    f64.report(f"long-lived session {family} kv={kv}, {len(calls)} calls", worst, SCORE_LP_TOL[kv])
+    h.report(f"long-lived session {family} kv={kv}, {len(calls)} calls", worst, h.DEEP_SCORE_LP_TOL[kv])

@@ -1,47 +1,31 @@
 """GPU tests (-m gpu) of the on-device beam search: with fp16-exact weights, d = 128 / 384 and n_windows * beam_size <= 24,
 transcribe_windows runs prefill and the whole width-B search in one decoder6 launch.  It must give the oracle's ids
 (tests/golden/tokens_beam.json, make_golden_beam.py), and the same ids as the host search driven through decoder3."""
-import json
-from pathlib import Path
-
-import numpy as np
 import pytest
 import torch
 
+import harness as h
 import wb200  # noqa: F401
+from harness import is_special_of, kv_code, pool_waves
 from oracle import audio as o_audio, model as o_model, synth, transcribe as o_tr
-from whisper_burn_b200 import ffi, model, transcribe
+from whisper_burn_b200 import ffi, transcribe
 
 pytestmark = pytest.mark.gpu
-G = Path(__file__).resolve().parent / "golden"
-KV = {"f32": ffi.WB_KV_F32, "f16": ffi.WB_KV_F16}
-
-
-def is_special_of(sp):
-    return (np.arange(sp.n_vocab) >= sp.first_special).astype(np.uint8)
 
 
 @pytest.fixture(scope="module")
 def gold():
-    return json.loads((G / "tokens_beam.json").read_text())
+    return h.golden("tokens_beam")
 
 
 @pytest.fixture(scope="module")
 def small():
-    dims, w_np, w_t = synth.make_weights("test-a", seed=0)
-    return dims, w_t, synth.special_tokens(dims), model.Whisper(dims, w_np)
+    return h.named_model("test-a")
 
 
 @pytest.fixture(scope="module")
 def tiny():
-    dims, w_np, w_t = synth.make_weights("tiny.en", seed=0)
-    return dims, w_t, synth.special_tokens(dims), model.Whisper(dims, w_np)
-
-
-def pool_waves(gold, n):
-    """n windows cycling through the pool of T = 750, 6, 314, 65, 750, 314 encoder positions"""
-    chunk = synth.chunk_waveform(0)
-    return [chunk[off:off + m] for off, m in (gold["pool"][i % len(gold["pool"])] for i in range(n))]
+    return h.named_model("tiny.en")
 
 
 def decode(wh, waves, sp, b, depth, kv, host=False, monkeypatch=None, max_text_len=None):
@@ -49,7 +33,7 @@ def decode(wh, waves, sp, b, depth, kv, host=False, monkeypatch=None, max_text_l
         monkeypatch.setenv("WB200_DECODER", "3")   # the host search on the FMA decoder: a second reference
     try:
         sess = transcribe.Session(wh, max_windows=len(waves), max_beams=7, max_text_len=max_text_len or 4 + depth + 1,
-                                  kv_dtype=KV[kv])
+                                  kv_dtype=kv_code(kv))
     finally:
         if host:
             monkeypatch.delenv("WB200_DECODER", raising=False)
@@ -61,7 +45,7 @@ def decode(wh, waves, sp, b, depth, kv, host=False, monkeypatch=None, max_text_l
 @pytest.mark.parametrize("b", [2, 3, 4, 5, 6, 7])
 def test_device_beam_test_a_vs_oracle_and_host(small, gold, monkeypatch, b, kv):
     """test-a (d = 128): 1 .. 24 // B windows of mixed lengths in one launch each"""
-    _, _, sp, wh = small
+    _, sp, wh, *_ = small
     depth = gold["depth_test_a"]
     want = gold["test_a"][kv][str(b)]
     n_max = 24 // b
@@ -79,8 +63,8 @@ def test_device_beam_test_a_vs_oracle_and_host(small, gold, monkeypatch, b, kv):
 @pytest.mark.parametrize("kv", ["f32", "f16"])
 def test_device_beam_tiny_en_vs_oracle_and_host(tiny, gold, monkeypatch, kv):
     """tiny.en (d = 384): the three reference windows of chunk 0, beam 5, depth 30"""
-    _, _, sp, wh = tiny
-    te = json.loads((G / "tokens_tiny_en.json").read_text())
+    _, sp, wh, *_ = tiny
+    te = h.golden("tokens_tiny_en")
     chunk = synth.chunk_waveform(0)
     waves = [chunk[s:e] for s, e in te["bounds"]]
     got, sess = decode(wh, waves, sp, 5, gold["depth_tiny_en"], kv)
@@ -100,7 +84,7 @@ def test_device_beam_test_a_deep_vs_oracle_and_host(small, gold, monkeypatch, b,
     through the ancestry tables, beam sequences copied to 128 ids.  EOT is declared to be the last vocabulary id, which
     these searches never emit, so every window runs all 124 steps.  The same ids as the live oracle and as the host search
     on decoder3, and the same number of steps."""
-    dims, w_t, sp, wh = small
+    dims, sp, wh, _, w_t, _ = small
     sp2 = o_tr.SpecialTokens(sp.sot, sp.lang, sp.transcribe, sp.notimestamps, sp.n_vocab - 1, sp.first_special, sp.n_vocab)
     waves = pool_waves(gold, min(len(gold["pool"]), 24 // b))
     got, sess = decode(wh, waves, sp2, b, DEEP, kv, max_text_len=4 + DEEP)
@@ -117,7 +101,7 @@ def test_device_beam_test_a_deep_vs_oracle_and_host(small, gold, monkeypatch, b,
 
 def test_device_beam_live_oracle(small):
     """one case against the oracle computed here (the golden file is the oracle's output too)"""
-    dims, w_t, sp, wh = small
+    dims, sp, wh, _, w_t, _ = small
     wave = synth.chunk_waveform(0)[120000:120000 + 98882]
     got, sess = decode(wh, [wave], sp, 4, 8, "f16")
     want = o_tr.mels_to_tokens(w_t, dims, sp, o_audio.prep_audio(torch.from_numpy(wave)[None]), beam_size=4, max_depth=8,
@@ -128,8 +112,8 @@ def test_device_beam_live_oracle(small):
 def test_device_beam_early_stop(small, gold, monkeypatch):
     """EOT declared to be a token the search emits: one window's search ends early (its sequence ends in EOT) while the other
     continues; the launch stops when both are done, after as many steps as the host search takes."""
-    dims, _, sp, wh = small
-    ta = json.loads((G / "tokens_test_a.json").read_text())
+    dims, sp, wh, *_ = small
+    ta = h.golden("tokens_test_a")
     eot = gold["eot"]
     sp2 = o_tr.SpecialTokens(sp.sot, sp.lang, sp.transcribe, sp.notimestamps, eot, sp.first_special, sp.n_vocab)
     chunk = synth.chunk_waveform(0)
@@ -146,7 +130,7 @@ def test_device_beam_early_stop(small, gold, monkeypatch):
 def test_device_beam_is_one_launch(small, gold, monkeypatch):
     """The whole search is one launch: the library launches as many kernels at depth 30 as at depth 5; the host search
     launches more per depth."""
-    _, _, sp, wh = small
+    _, sp, wh, *_ = small
     waves = pool_waves(gold, 2)
 
     def launches(sess, depth):
@@ -168,7 +152,7 @@ def test_device_beam_is_one_launch(small, gold, monkeypatch):
 def test_device_beam_coverage_edge(small, gold):
     """24 rows (4 windows x B = 6) are one decoder6 launch; 25 rows (5 windows x B = 5) fall back to the host search, with
     the same ids"""
-    _, _, sp, wh = small
+    _, sp, wh, *_ = small
     depth = gold["depth_test_a"]
     got, sess = decode(wh, pool_waves(gold, 4), sp, 6, depth, "f32")
     assert sess.last_decoder() == 6

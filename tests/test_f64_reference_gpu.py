@@ -28,118 +28,17 @@ n = E - 1, E, E + 1 and the last step the session allows (n = max_text_len - 1):
   * the default selection on both sides of decoder6's t_max <= 128 (d = 384, 9 rows: decoder6 at 128, decoder3 at 129).
 
 The deep cases use V = 2051 (the vocabulary tails are covered at depth 10) and declare EOT to be an id the windows never emit,
-so every row runs to the last checked step; check_greedy asserts that it does.
-
-Tolerances are absolute on log-probs (|log-prob| ~ 7.6 for V = 2051, ~10.9 for V = 51864) and separate for the fp32 and the
-fp16 K/V cache: at an fp16 rounding boundary a float64 value can round to the neighbour of the one the GPU's float32 value
-rounds to.  Each constant states the worst error measured on one H100 80GB HBM3 and the margin over it."""
-import functools
-import multiprocessing
-import os
-from concurrent.futures import ProcessPoolExecutor
-
-import numpy as np
+so every row runs to the last checked step; harness.check_greedy asserts that it does.  The tolerances are
+harness.py's GREEDY_LP_TOL, STEP_LP_TOL, LOGITS_REL_TOL and ENC_REL_TOL."""
 import pytest
-import torch
 
+from harness import ENC_REL_TOL, GREEDY_LP_TOL, LOGITS_REL_TOL, SHALLOW_STEPS, STEP_LP_TOL, check_greedy, check_step_k7, \
+    edge_steps, encoder_error, forward_decoder_448_error, make_model, report, use_decoder, windows
 import wb200  # noqa: F401
-from oracle import model as o_model, synth, transcribe as o_tr
-from whisper_burn_b200 import ffi, model, transcribe
-from whisper_burn_b200.synth import WhisperDims
+from oracle import synth
+from whisper_burn_b200 import ffi, transcribe
 
 pytestmark = pytest.mark.gpu
-
-# greedy top-1 log-prob vs float64 on the GPU's own path (all greedy decoders).  Worst measured: f32 5.0e-6 (decoder5,
-# d = 1280), 4x margin; f16 1.7e-4 (decoder6, d = 384, 8 rows), 3x margin.  Dropping the 8 tail ids of V = 51864 from the
-# softmax moves a log-prob by ~1.5e-4, 7x the f32 tolerance.
-GREEDY_LP_TOL = {"f32": 2e-5, "f16": 5e-4}
-# wb_session_step, all 7 candidates.  Worst measured: f32 1.2e-6 (decoder3, d = 384), 8x margin; f16 7.8e-5 (decoder3,
-# d = 384), 4x margin
-STEP_LP_TOL = {"f32": 1e-5, "f16": 3e-4}
-# full logits of the stateless forward_decoder at 448 positions, each position relative to its logits' scale (the suite's
-# decoder bar).  Worst measured 6.7e-6 (decoder5, d = 256), 3x margin
-LOGITS_REL_TOL = 2e-5
-# encoder output, relative to its scale (the suite's encoder bar).  Worst measured 6.7e-6 (tensor-core, d = 1280), 3x margin
-ENC_REL_TOL = 2e-5
-
-DEPTH = 10                                       # greedy steps per window: 2 with the special-token mask, 8 without
-SHALLOW_STEPS = tuple(range(1, DEPTH + 1))
-N_OF_T = {6: 400, 64: 18720, 65: 19040, 750: 480000}   # waveform samples giving each encoder length
-T_ORDER = (750, 6, 65, 64)
-
-
-def rel_to_scale(a, b):
-    return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30))
-
-
-def kv_code(kv):
-    return ffi.WB_KV_F16 if kv == "f16" else ffi.WB_KV_F32
-
-
-def report(what, worst, tol):
-    print(f"\n[f64] {what}: worst {worst:.3e} (tolerance {tol:.0e})")
-
-
-@functools.lru_cache(maxsize=2)
-def _weights(d, H, V, n_text_layer, exact):
-    dims = WhisperDims(80, 1500, d, H, 1, V, 448, d, H, n_text_layer)
-    _, w_np, _ = synth.make_weights(dims, seed=d + V)
-    if not exact:   # no longer fp16-representable: the fp32 encoder (gemm.cu) and decoder3<float>
-        w_np = {k: (v * np.float32(1.0001) if v.ndim else v) for k, v in w_np.items()}
-    return dims, w_np, o_model.as_dtype(synth.to_torch(w_np))
-
-
-def _greedy_ref_rows(model_key, sp, xa, tokens, kv, steps):
-    """In a worker process: the float64 log-prob rows of the greedy steps `steps` along `tokens` (greedy_path_log_probs on
-    the weights _weights(*model_key) and the window's encoder output xa [T, d])."""
-    dims, _, w64 = _weights(*model_key)
-    ref = o_tr.greedy_path_log_probs(w64, dims, sp, torch.from_numpy(xa)[None], tokens, opts=o_model.OracleOptions(kv_dtype=kv))
-    return {s: ref[s - 1].numpy() for s in steps}
-
-
-@functools.lru_cache(maxsize=1)
-def _ref_pool():
-    """Worker processes for the float64 reference: scoring one row is a few hundred small sequential float64 steps, so rows
-    run side by side, one torch thread each."""
-    return ProcessPoolExecutor(max(1, min(8, (os.cpu_count() or 2) - 1)), mp_context=multiprocessing.get_context("spawn"),
-                               initializer=torch.set_num_threads, initargs=(1,))
-
-
-def make_model(d, H, V, exact=True, n_text_layer=2):
-    """(dims, GPU model, float64 weights).  A fresh model.Whisper per call: its stateless forward session reads
-    WB200_DECODER when it is created."""
-    dims, w_np, w64 = _weights(d, H, V, n_text_layer, exact)
-    wh = model.Whisper(dims, w_np)
-    assert wh.weights_fp16_exact == exact
-    return dims, wh, w64
-
-
-def windows(n, seed, order=T_ORDER):
-    Ts = [order[i % len(order)] for i in range(n)]
-    return Ts, [synth.waveform(N_OF_T[T], seed=seed + i) for i, T in enumerate(Ts)]
-
-
-def encoder_outputs64(sess, Ts):
-    out = []
-    for r, T in enumerate(Ts):
-        xa = sess.get_encoder_output(r)
-        assert xa.shape[0] == T
-        out.append(torch.from_numpy(xa).double()[None])
-    return out
-
-
-def use_decoder(monkeypatch, n):
-    if n:
-        monkeypatch.setenv("WB200_DECODER", str(n))
-    else:
-        monkeypatch.delenv("WB200_DECODER", raising=False)
-
-
-def edge_steps(edges, max_text_len):
-    """The greedy steps whose self attention runs over E - 1, E and E + 1 keys for every edge E, and the last step a session
-    of max_text_len allows (step s attends over n = s + 3 keys: the 4-id prompt and s - 1 generated ids)."""
-    last = max_text_len - 4
-    return tuple(sorted({s for e in edges for s in (e - 4, e - 3, e - 2) if s <= last} | {last}))
 
 
 def default_decoder(d, rows, t_max):
@@ -152,61 +51,6 @@ def default_decoder(d, rows, t_max):
 
 
 # ---------------------------------------------------------------- a. greedy, per step, top-1 against float64
-def check_greedy(dims, wh, kv, n_rows, decoder, seed, steps=SHALLOW_STEPS, max_text_len=None, full_depth=False, tol=None,
-                 ref_rows=None):
-    """Greedy-decodes n_rows windows once to the deepest step of `steps` and once to each step s of `steps`, and checks the
-    top-1 (id, log-prob) of every row at every step s against float64 on the GPU's own path.  max_text_len defaults to the
-    deepest step plus the prompt and one.  full_depth: EOT is declared to be a special id past the named ones that no row
-    emits (the largest one not emitted by an earlier full-depth launch that a row stopped in), and every row must reach the
-    deepest step.  tol defaults to GREEDY_LP_TOL[kv].  ref_rows(sp, xa, paths, kv, steps) -> per row {s: float64 log-prob
-    row} computes the reference in this process (xa: the rows' float64 encoder outputs [1, T, d], steps: per row); by
-    default worker processes rebuild the model with _weights.  Returns the worst |log-prob error|."""
-    depth = max(steps)
-    sp = synth.special_tokens(dims)
-    bitmap = sp.is_special_bitmap()
-    Ts, waves = windows(n_rows, seed)
-    sess = transcribe.Session(wh, max_windows=n_rows, max_beams=1, max_text_len=max_text_len or 4 + depth + 1,
-                              kv_dtype=kv_code(kv))
-    full = sess.transcribe_windows(waves, sp, bitmap, beam_size=1, max_depth=depth) if not full_depth else None
-    eot = sp.n_vocab
-    while full is None or (full_depth and any(len(t) < 4 + depth for t in full)):
-        eot = max(set(range(sp.first_special, eot)) - {i for t in full or [] for i in t})
-        sp = o_tr.SpecialTokens(sp.sot, sp.lang, sp.transcribe, sp.notimestamps, eot, sp.first_special, sp.n_vocab)
-        full = sess.transcribe_windows(waves, sp, bitmap, beam_size=1, max_depth=depth)
-    assert sess.last_decoder() == decoder
-    if full_depth:
-        assert sess.last_steps() == depth and [len(t) for t in full] == [4 + depth] * n_rows
-    xa = encoder_outputs64(sess, Ts)
-    row_steps = [[s for s in steps if 4 + s <= len(full[r])] for r in range(n_rows)]
-    if ref_rows is None:
-        key = (dims.n_text_state, dims.n_text_head, dims.n_vocab, dims.n_text_layer, wh.weights_fp16_exact)
-        refs = [_ref_pool().submit(_greedy_ref_rows, key, sp, xa[r][0].numpy(), full[r], kv, row_steps[r]) for r in range(n_rows)]
-    got = [dict() for _ in range(n_rows)]      # step -> (id, log-prob) of every row that produced a token at that step
-    for s in steps:
-        toks = sess.transcribe_windows(waves, sp, bitmap, beam_size=1, max_depth=s)
-        assert sess.last_decoder() == decoder
-        ids, lps = sess.last_topk(n_rows, 1)
-        for r in range(n_rows):
-            assert toks[r] == full[r][:len(toks[r])], f"row {r}: the depth-{s} launch is not a prefix of the depth-{depth} one"
-            if len(toks[r]) == 4 + s:
-                assert int(ids[r, 0]) == toks[r][-1]
-                got[r][s] = float(lps[r, 0])
-    tol = tol or GREEDY_LP_TOL[kv]
-    worst = 0.0
-    local = ref_rows(sp, xa, full, kv, row_steps) if ref_rows is not None else None
-    for r in range(n_rows):
-        ref = local[r] if local is not None else refs[r].result()
-        assert sorted(got[r]) == sorted(ref)
-        for s, lp in got[r].items():
-            tok = full[r][4 + s - 1]
-            err = abs(lp - ref[s][tok])
-            worst = max(worst, err)
-            assert err < tol, f"row {r} (T = {Ts[r]}) step {s}: log-prob {lp} vs float64 {ref[s][tok]}"
-            gap = ref[s].max() - ref[s][tok]       # the GPU id is the float64 argmax up to a near-tie
-            assert gap < tol, f"row {r} step {s}: id {tok} is {gap} below the float64 argmax {int(ref[s].argmax())}"
-    return worst
-
-
 def test_last_topk_argument_checks(monkeypatch):
     """wb_session_last_topk reads what the last launch wrote: it refuses a k or a row count that launch did not have."""
     use_decoder(monkeypatch, 0)
@@ -371,67 +215,6 @@ def test_session_step_k7_beams_vs_float64(decoder, d, exact, kv, monkeypatch):
     report(f"step k=7 decoder{decoder} d={d} {'fp16' if exact else 'fp32'} weights kv={kv}", worst, STEP_LP_TOL[kv])
 
 
-def check_step_k7(dims, wh, w64, decoder, kv, sess=None, tol=None, out=None):
-    """The steps of test_session_step_k7_beams_vs_float64 on `sess` (default: a fresh session of 2 windows, 5 beams,
-    max_text_len 16), each checked against float64 within tol (default STEP_LP_TOL[kv]).  out, a list, receives every
-    step's (ids, log-probs).  Returns the worst |log-prob error|."""
-    sp = synth.special_tokens(dims)
-    bitmap = sp.is_special_bitmap()
-    K = 7
-    Ts, waves = windows(2, seed=700, order=(65, 6))
-    if sess is None:
-        sess = transcribe.Session(wh, max_windows=2, max_beams=5, max_text_len=16, kv_dtype=kv_code(kv))
-    sess.encode_waveforms(waves)
-    xa = encoder_outputs64(sess, Ts)
-    opts = o_model.OracleOptions(kv_dtype=kv)
-    prompt = sp.prompt()
-    sess.begin(prompt)
-    ref = [o_model.CachedDecoder(w64, dims, xa[w], opts) for w in range(2)]
-    for dec in ref:
-        for t in prompt[:-1]:
-            dec.step(torch.tensor([t], dtype=torch.int64))
-    rows = [(0, 0), (1, 0)]          # GPU row -> (window, row of that window's float64 decoder)
-    maskout = torch.from_numpy(sp.maskout())
-    tol = tol or STEP_LP_TOL[kv]
-    worst = 0.0
-
-    def step(parents, tokens, masked):
-        nonlocal rows, worst
-        win = [rows[p][0] for p in parents]
-        ids, lps = sess.step(win, parents, tokens, masked, bitmap, K)
-        assert sess.last_decoder() == decoder
-        if out is not None:
-            out.append((ids, lps))
-        new_rows = []
-        for w in range(2):
-            mine = [i for i in range(len(parents)) if win[i] == w]
-            ref[w].reorder([rows[parents[i]][1] for i in mine])
-            logits = ref[w].step(torch.tensor([tokens[i] for i in mine], dtype=torch.int64))
-            if masked:
-                logits = logits + maskout
-            lp = o_model.log_softmax_last(logits).numpy()
-            for j, i in enumerate(mine):
-                want = np.sort(lp[j])[::-1][:K]
-                have = lp[j][ids[i]]
-                err = float(np.abs(lps[i] - have).max())
-                worst = max(worst, err)
-                assert err < tol, f"row {i}: log-probs {lps[i]} vs float64 {have}"
-                # ids differ from float64's order only where float64's own neighbours lie within the tolerance
-                assert np.abs(have - want).max() < tol, f"row {i}: ids {ids[i]} vs float64 order {np.argsort(-lp[j])[:K]}"
-        for i in range(len(parents)):
-            w = win[i]
-            new_rows.append((w, sum(1 for q in range(i) if win[q] == w)))
-        rows = new_rows
-        return ids
-
-    ids = step([0, 1], [prompt[-1]] * 2, True)                                  # 2 rows: RC = 4
-    ids = step([0, 0, 0, 1, 1, 1], [int(ids[0, j]) for j in range(3)] + [int(ids[1, j]) for j in range(3)], True)   # fan out: 6
-    ids = step([2, 0, 1, 5, 3], [int(ids[2, 1]), int(ids[0, 0]), int(ids[1, 6]), int(ids[5, 0]), int(ids[3, 2])], False)
-    ids = step([4, 0, 2], [int(ids[4, 3]), int(ids[0, 0]), int(ids[2, 5])], False)   # back to 3 rows from other parents
-    step([1, 0, 2, 2, 1], [int(ids[1, 0]), int(ids[0, 1]), int(ids[2, 0]), int(ids[2, 4]), int(ids[1, 2])], False)
-    return worst
-
-
 # ---------------------------------------------------------------- c. full logits at the maximum text length
 @pytest.mark.parametrize("decoder,d", [(3, 384), (5, 256)])
 def test_forward_decoder_448_positions_vs_float64(decoder, d, monkeypatch):
@@ -442,17 +225,6 @@ def test_forward_decoder_448_positions_vs_float64(decoder, d, monkeypatch):
     worst = forward_decoder_448_error(dims, wh, w64)
     report(f"forward_decoder 448 positions decoder{decoder} d={d}", worst, LOGITS_REL_TOL)
     assert worst < LOGITS_REL_TOL
-
-
-def forward_decoder_448_error(dims, wh, w64):
-    """The worst relative-to-scale error of forward_decoder's logits at every one of n_text_ctx positions."""
-    d = dims.n_text_state
-    rng = np.random.default_rng(d)
-    xa = rng.standard_normal((1, 65, d)).astype(np.float32)
-    toks = rng.integers(0, dims.n_vocab, size=(1, dims.n_text_ctx)).astype(np.int64)
-    got = wh.forward_decoder(toks, xa)
-    want = o_model.forward_decoder(w64, dims, torch.from_numpy(toks), torch.from_numpy(xa).double()).numpy()
-    return max(rel_to_scale(got[0, p], want[0, p]) for p in range(dims.n_text_ctx))
 
 
 # ---------------------------------------------------------------- d. encoder at real widths, ragged windows
@@ -466,13 +238,5 @@ def test_encoder_ragged_windows_vs_float64(d, H, exact):
     Ts, waves = windows(4, seed=800 + d, order=(6, 64, 65, 750))
     sess = transcribe.Session(wh, max_windows=4, max_beams=1, max_text_len=8)
     sess.encode_waveforms(waves)
-    worst = 0.0
-    for w, T in enumerate(Ts):
-        got = sess.get_encoder_output(w)
-        assert got.shape == (T, d)
-        mel = torch.from_numpy(sess.get_mel(w)).double()[None]
-        want = o_model.forward_encoder(w64, dims, mel)[0].numpy()
-        e = rel_to_scale(got, want)
-        worst = max(worst, e)
-        assert e < ENC_REL_TOL, f"window {w} (T = {T}): {e}"
+    worst = encoder_error(sess, w64, dims, Ts, ENC_REL_TOL)
     report(f"encoder d={d} {'tensor-core' if exact else 'fp32'}", worst, ENC_REL_TOL)

@@ -8,41 +8,26 @@ the repetition cut and the context stop each end some window, which the test ass
 EOT-test gap or top-1 / top-2 logit gap falls below 1e-4 at a step, ids are compared up to that step (the decoders' logits
 differ from the oracle's in the last bits)."""
 import dataclasses
-import json
-from pathlib import Path
 
-import numpy as np
 import pytest
 import torch
 
 import oracle_greedy_loop as loop
 import wb200  # noqa: F401
+from harness import LOOP_CASES, LOOP_EOT_ID, golden, loop_model, loop_session as session, loop_window as window, \
+    same_up_to_ties
 from oracle import audio as o_audio, synth
-from whisper_burn_b200 import ffi, model, transcribe
+from whisper_burn_b200 import ffi, transcribe
 
 pytestmark = pytest.mark.gpu
-G = Path(__file__).resolve().parent / "golden"
-GAP_TOL = 1e-4
-EOT_ID = 500   # declared EOT of the synthetic models: an ordinary id whose logit is sometimes within ln 2 of the arg-max
 
-_MODELS, _ORACLE = {}, {}
-
-
-def weights(name):
-    if name not in _MODELS:
-        dims, w_np, w_t = synth.make_weights(name, seed=0)
-        _MODELS[name] = (dims, w_t, model.Whisper(dims, w_np))
-    return _MODELS[name]
-
-
-def window(i):
-    return synth.waveform(16000 * (3 + 4 * (i % 4)) + 1600 * (i // 4), seed=100 + i)
+_ORACLE = {}
 
 
 def oracle(name, i, sp, max_depth, kv):
     key = (name, i, sp.eot, max_depth, kv)
     if key not in _ORACLE:
-        dims, w_t, _ = weights(name)
+        dims, _, _, _, w_t, _ = loop_model(name)
         mel = o_audio.prep_audio(torch.from_numpy(window(i))[None])
         tr = {}
         toks = loop.mels_to_tokens_greedy_loop(w_t, dims, sp, mel, max_depth, loop.model.OracleOptions(kv_dtype=kv), trace=tr)
@@ -50,34 +35,11 @@ def oracle(name, i, sp, max_depth, kv):
     return _ORACLE[key]
 
 
-def same_up_to_ties(got, want, tr):
-    """got == want, or identical up to the first step whose EOT-test or top-1/top-2 gap is below GAP_TOL."""
-    if got == want:
-        return True
-    for s, (e, t) in enumerate(zip(tr["eot_gap"], tr["top_gap"])):
-        if abs(e) < GAP_TOL or t < GAP_TOL:
-            return got[:4 + s] == want[:4 + s]
-    return False
-
-
-def session(name, n, t_max, kv, search="greedy_loop"):
-    _, _, wh = weights(name)
-    return transcribe.Session(wh, max_windows=n, max_beams=1, max_text_len=t_max,
-                              kv_dtype=ffi.WB_KV_F16 if kv == "f16" else ffi.WB_KV_F32, search=search)
-
-
-# (decoder, model, windows, max_text_len, rules that end some window): decoder6 takes t_max <= 128 and 8+ rows here;
-# decoder5 needs d % 256 == 0 (test-c, whose logits never put id 500 within ln 2 of the arg-max on these windows)
-ALL = {"eot", "repeat", "context"}
-CASES = [(4, "test-a", 4, 448, ALL), (6, "test-a", 9, 128, ALL), (5, "test-c", 4, 448, {"repeat", "context"}),
-         (3, "test-a", 4, 448, ALL)]
-
-
 @pytest.mark.parametrize("kv", ["f32", "f16"])
-@pytest.mark.parametrize("dec,name,n,t_max,rules", CASES)
+@pytest.mark.parametrize("dec,name,n,t_max,rules", LOOP_CASES)
 def test_each_decoder_matches_the_oracle_loop(monkeypatch, dec, name, n, t_max, rules, kv):
-    dims, _, _ = weights(name)
-    sp = dataclasses.replace(synth.special_tokens(dims), eot=EOT_ID)
+    dims = loop_model(name).dims
+    sp = dataclasses.replace(synth.special_tokens(dims), eot=LOOP_EOT_ID)
     monkeypatch.setenv("WB200_DECODER", str(dec))
     s = session(name, n, t_max, kv)
     monkeypatch.delenv("WB200_DECODER")
@@ -90,15 +52,15 @@ def test_each_decoder_matches_the_oracle_loop(monkeypatch, dec, name, n, t_max, 
             want, tr = oracle(name, i, sp, max_depth, kv)
             stops.add(tr["stop"])
             assert same_up_to_ties(got[i], want, tr), f"window {i} depth {max_depth}:\n got {got[i]}\nwant {want}"
-            assert got[i][-1] == EOT_ID and len(got[i]) <= 4 + max_depth + 1
+            assert got[i][-1] == LOOP_EOT_ID and len(got[i]) <= 4 + max_depth + 1
     assert stops == rules, stops
     s.close()
 
 
 @pytest.mark.parametrize("kv", ["f32", "f16"])
 def test_tiny_en_real_shape_against_fixture(kv):
-    g = json.loads((G / "tokens_greedy_loop.json").read_text())
-    dims, _, wh = weights("tiny.en")
+    g = golden("tokens_greedy_loop")
+    dims = loop_model("tiny.en").dims
     sp = synth.special_tokens(dims)
     assert g["eot"] == sp.eot
     chunk = synth.chunk_waveform(g["chunk"])
@@ -111,8 +73,8 @@ def test_tiny_en_real_shape_against_fixture(kv):
 
 
 def test_waveform_to_tokens_in_loop_mode():
-    dims, w_t, _ = weights("test-a")
-    sp = dataclasses.replace(synth.special_tokens(dims), eot=EOT_ID)
+    dims, _, _, _, w_t, _ = loop_model("test-a")
+    sp = dataclasses.replace(synth.special_tokens(dims), eot=LOOP_EOT_ID)
     wave = synth.waveform(16000 * 35, seed=77)   # 3 reference windows
     want = loop.waveform_to_tokens(w_t, dims, sp, wave, beam_size=1, max_depth=60, search="greedy_loop")
     s = session("test-a", 2, 65, "f32")
@@ -122,7 +84,7 @@ def test_waveform_to_tokens_in_loop_mode():
 
 
 def test_search_rule_contract():
-    dims, _, wh = weights("test-a")
+    dims, _, wh, *_ = loop_model("test-a")
     sp = synth.special_tokens(dims)
     s = session("test-a", 1, 20, "f32")
     with pytest.raises(ffi.WbError) as e:

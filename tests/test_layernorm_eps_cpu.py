@@ -6,29 +6,22 @@ compares by at least MARGIN times the tolerance it is compared with:
   * any one LayerNorm's eps reset to 1e-5 (a hard-coded or default eps);
   * any two LayerNorms' eps swapped within the encoder or within the decoder (a kernel reading another LayerNorm's eps).
 
-The quantities: the encoder output (relative to its scale) against ENC_REL_TOL; the teacher-forced log-probs of the oracle's own
-DEPTH-step greedy path, and the log-probs of every position of the scoring test's sequences, against the fp32 K/V
-GREEDY_LP_TOL.  The decoder quantities are computed on one fixed encoder output, as the GPU tests check the decoders on the
+The quantities: the encoder output (relative to its scale) against harness.ENC_REL_TOL; the teacher-forced log-probs of the
+oracle's own DEPTH-step greedy path, and the log-probs of every position of the scoring test's sequences, against the fp32
+K/V harness.GREEDY_LP_TOL.  The decoder quantities are computed on one fixed encoder output, as the GPU tests check the decoders on the
 GPU's own.  With the fp16 K/V tolerance (25 times larger) only the placement is claimed."""
 import itertools
 
 import numpy as np
 import pytest
-import torch
 
+import harness as h
 import layernorm_eps as lne
-import test_f64_reference_gpu as f64
-from oracle import audio as o_audio, model as o_model, synth, transcribe as o_tr
-from test_score_tokens_gpu import random_seqs
+from harness import check_moves, greedy_path, random_seqs, window_mel
+from oracle import model as o_model, synth
 
-MARGIN = 10
 V = 2051
 T = 65
-
-
-def window_mel(dims):
-    mel = o_tr.pad_mel(o_audio.prep_audio(torch.from_numpy(synth.waveform(f64.N_OF_T[T], seed=T))[None]), dims.n_audio_ctx)
-    return mel.double()
 
 
 def changes(eps, keys, mode):
@@ -40,11 +33,7 @@ def changes(eps, keys, mode):
 
 
 def check(moved, tol, what):
-    """moved: change -> how far it moves the quantity; every one at least MARGIN * tol"""
-    short = {k: v for k, v in moved.items() if v < MARGIN * tol}
-    least = min(moved, key=moved.get)
-    print(f"\n[eps] {what}: smallest move {moved[least]:.2e} ({least}), {moved[least] / tol:.0f}x the tolerance {tol:.0e}")
-    assert not short, f"{what}: moved less than {MARGIN}x {tol:.0e}: {short}"
+    check_moves(moved, tol, what, "eps")
 
 
 @pytest.mark.parametrize("mode", lne.MODES)
@@ -59,36 +48,18 @@ def test_encoder_output_moves(d, H, mode):
     for what, e, m in changes(eps, lne.eps_keys(w_np)[0], mode):
         _, w = lne.with_eps(w_np, w64, e)
         got = o_model.forward_encoder(w, dims, mel, o_model.OracleOptions(ln_eps_mode=m))[0].numpy()
-        moved[what] = f64.rel_to_scale(got, base)
-    check(moved, f64.ENC_REL_TOL, f"encoder d={d} {mode}")
-
-
-def greedy_path(w64, dims, sp, xa, opts):
-    """the oracle's greedy ids (beam-rule mask) from the prompt, DEPTH steps or to EOT"""
-    dec = o_model.CachedDecoder(w64, dims, xa, opts)
-    toks = list(sp.prompt())
-    for t in toks[:-1]:
-        dec.step(torch.tensor([t], dtype=torch.int64))
-    maskout = torch.from_numpy(sp.maskout())
-    while len(toks) < 4 + f64.DEPTH and toks[-1] != sp.eot:
-        logits = dec.step(torch.tensor([toks[-1]], dtype=torch.int64))
-        if o_tr.masks_specials(len(toks)):
-            logits = logits + maskout
-        toks.append(int(logits.argmax()))
-    return toks
+        moved[what] = h.rel_to_scale(got, base)
+    check(moved, h.ENC_REL_TOL, f"encoder d={d} {mode}")
 
 
 def path_log_probs(w64, dims, sp, xa, toks, mode):
-    rows = o_tr.greedy_path_log_probs(w64, dims, sp, xa, toks, opts=o_model.OracleOptions(ln_eps_mode=mode))
-    return np.array([float(rows[j - 4][toks[j]]) for j in range(4, len(toks))])
+    return h.along(h.path_rows(w64, dims, sp, xa, toks, ln_eps_mode=mode), toks)
 
 
 def scored_log_probs(w64, dims, xa, seqs, mode):
     out = []
     for seq in seqs:
-        logits = o_model.forward_decoder(w64, dims, torch.tensor([seq], dtype=torch.int64), xa,
-                                         opts=o_model.OracleOptions(ln_eps_mode=mode))
-        rows = o_model.log_softmax_last(logits)[0].numpy()
+        rows = h.forward_rows(w64, dims, [xa], [seq], ln_eps_mode=mode)[0]
         out.append(rows[np.arange(len(seq) - 1), seq[1:]])
     return np.concatenate(out)
 
@@ -101,7 +72,7 @@ def test_decoder_log_probs_move(d, H, mode):
     sp = synth.special_tokens(dims)
     xa = o_model.forward_encoder(w64, dims, window_mel(dims), o_model.OracleOptions(ln_eps_mode=mode))
     toks = greedy_path(w64, dims, sp, xa, o_model.OracleOptions(ln_eps_mode=mode))
-    assert len(toks) == 4 + f64.DEPTH, toks
+    assert len(toks) == 4 + h.DEPTH, toks
     base = path_log_probs(w64, dims, sp, xa, toks, mode)
     seqs = [s for s in random_seqs(V, d) if len(s) > 1] if d == 384 else []
     base_scored = scored_log_probs(w64, dims, xa, seqs, mode) if seqs else None
@@ -112,10 +83,10 @@ def test_decoder_log_probs_move(d, H, mode):
         if seqs:
             moved_scored[what] = float(np.abs(scored_log_probs(w, dims, xa, seqs, m) - base_scored).max())
     flip = "the other placement"
-    for tol in f64.GREEDY_LP_TOL.values():
+    for tol in h.GREEDY_LP_TOL.values():
         check({flip: moved[flip]}, tol, f"greedy path d={d} {mode}, placement")
-    check(moved, f64.GREEDY_LP_TOL["f32"], f"greedy path d={d} {mode}")
+    check(moved, h.GREEDY_LP_TOL["f32"], f"greedy path d={d} {mode}")
     if seqs:
-        for tol in f64.GREEDY_LP_TOL.values():
+        for tol in h.GREEDY_LP_TOL.values():
             check({flip: moved_scored[flip]}, tol, f"scored sequences d={d} {mode}, placement")
-        check(moved_scored, f64.GREEDY_LP_TOL["f32"], f"scored sequences d={d} {mode}")
+        check(moved_scored, h.GREEDY_LP_TOL["f32"], f"scored sequences d={d} {mode}")

@@ -4,7 +4,7 @@ encoder positions (the reference's windowing stops at 750).
   (a) log-mel of native windows against the oracle (the suite's mel bar);
   (b) the encoder at real widths against float64, T = 1500 and ragged T > 750 in one batch, tensor-core and fp32 paths;
   (c) every persistent decoder's cross attention over T > 750 keys against float64: greedy top-1 log-probs per step and
-      wb_session_step candidates (the helpers and bars of test_f64_reference_gpu.py);
+      wb_session_step candidates (the helpers and bars of harness.py);
   (d) token ids against tests/golden/tokens_native.json (make_golden_native.py): greedy, the device and the host beam search;
   (e) long-form waveform_to_tokens (native windowing + overlap merge) against the same fixture;
   (f) a reference and a native session of one model side by side, each with its own frame limit.
@@ -12,20 +12,18 @@ encoder positions (the reference's windowing stops at 750).
 The oracle's native mode is the oracle on dims with n_audio_ctx doubled: it reads n_audio_ctx only as the frame limit."""
 import ctypes as C
 import dataclasses
-import json
-from pathlib import Path
 
 import numpy as np
 import pytest
 import torch
 
+import harness as h
 import wb200  # noqa: F401
-import test_f64_reference_gpu as f64
+from harness import is_special_of, kv_code
 from oracle import audio as o_audio, model as o_model, synth, transcribe as o_tr
-from whisper_burn_b200 import ffi, model, transcribe
+from whisper_burn_b200 import ffi, transcribe
 
 pytestmark = pytest.mark.gpu
-G = Path(__file__).resolve().parent / "golden"
 MEL_TOL = 1e-4   # the suite's log-mel bar (test_parity_gpu.py), relative to scale
 
 
@@ -38,22 +36,9 @@ def native(dims):
     return dataclasses.replace(dims, n_audio_ctx=2 * dims.n_audio_ctx)
 
 
-def is_special_of(sp):
-    return (np.arange(sp.n_vocab) >= sp.first_special).astype(np.uint8)
-
-
-def kv_code(kv):
-    return ffi.WB_KV_F16 if kv == "f16" else ffi.WB_KV_F32
-
-
-def gold():
-    return json.loads((G / "tokens_native.json").read_text())
-
-
 # ---------------------------------------------------------------- (a) log-mel
 def test_logmel_native_windows_vs_oracle():
-    dims, w_np, _ = synth.make_weights("test-a", seed=0)
-    wh = model.Whisper(dims, w_np)
+    dims, _, wh, *_ = h.named_model("test-a")
     lens = [480000, 478560, samples_of_T(1025), 64000]
     waves = [synth.waveform(n, seed=20 + i) for i, n in enumerate(lens)]
     sess = transcribe.Session(wh, max_windows=4, max_beams=1, max_text_len=8, windows="native")
@@ -63,10 +48,10 @@ def test_logmel_native_windows_vs_oracle():
         got = sess.get_mel(i)
         want = o_tr.pad_mel(o_audio.prep_audio(torch.from_numpy(wv)[None]), 3000).numpy()[0]
         assert got.shape == want.shape == (80, min(len(wv) // 160, 2990) + 10)
-        e = f64.rel_to_scale(got, want)
+        e = h.rel_to_scale(got, want)
         worst = max(worst, e)
         assert e < MEL_TOL, f"window {i}: {e}"
-    f64.report("native log-mel (4 windows, Tm up to 3000)", worst, MEL_TOL)
+    h.report("native log-mel (4 windows, Tm up to 3000)", worst, MEL_TOL)
 
 
 # ---------------------------------------------------------------- (b) encoder at real widths
@@ -78,20 +63,12 @@ ENC_TS = (1500, 751, 1025, 205)
 def test_encoder_native_windows_vs_float64(d, H, exact):
     """Encoder output of windows with T = 1500, 751, 1025, 205 packed in one batch (conv stems over Tm up to 3000 mel rows,
     24 attention key tiles with a ragged last one), against the float64 encoder of each window's padded mel."""
-    dims, wh, w64 = f64.make_model(d, H, 2051, exact=exact, n_text_layer=1)
+    dims, wh, w64 = h.make_model(d, H, 2051, exact=exact, n_text_layer=1)
     waves = [synth.waveform(samples_of_T(T) if T != 1500 else 480000, seed=850 + d + i) for i, T in enumerate(ENC_TS)]
     sess = transcribe.Session(wh, max_windows=4, max_beams=1, max_text_len=8, windows="native")
     sess.encode_waveforms(waves)
-    worst = 0.0
-    for w, T in enumerate(ENC_TS):
-        got = sess.get_encoder_output(w)
-        assert got.shape == (T, d)
-        mel = torch.from_numpy(sess.get_mel(w)).double()[None]
-        want = o_model.forward_encoder(w64, native(dims), mel)[0].numpy()
-        e = f64.rel_to_scale(got, want)
-        worst = max(worst, e)
-        assert e < f64.ENC_REL_TOL, f"window {w} (T = {T}): {e}"
-    f64.report(f"native encoder d={d} {'tensor-core' if exact else 'fp32'}", worst, f64.ENC_REL_TOL)
+    worst = h.encoder_error(sess, w64, native(dims), ENC_TS, h.ENC_REL_TOL)
+    h.report(f"native encoder d={d} {'tensor-core' if exact else 'fp32'}", worst, h.ENC_REL_TOL)
 
 
 # ---------------------------------------------------------------- (c) decoders over T > 750 cross keys
@@ -99,46 +76,6 @@ def test_encoder_native_windows_vs_float64(d, H, exact):
 # bulk batches over 16 CTAs' warps, decoder5's and decoder3's ceil(T / S) splits), the first length past the reference's 750,
 # and 1500 (ragged last chunk everywhere).  DESIGN.md section 2 lists the edges.
 DEC_TS = (1500, 751, 1025, 1024)
-
-
-def check_greedy_native(dims, wh, kv, n_rows, decoder, seed, depth=f64.DEPTH):
-    """test_f64_reference_gpu.check_greedy on a native session: the top-1 (id, log-prob) of every row at every step 1..depth
-    against float64 on the GPU's own path."""
-    sp = synth.special_tokens(dims)
-    bitmap = sp.is_special_bitmap()
-    Ts = [DEC_TS[i % len(DEC_TS)] for i in range(n_rows)]
-    waves = [synth.waveform(480000 if T == 1500 else samples_of_T(T), seed=seed + i) for i, T in enumerate(Ts)]
-    sess = transcribe.Session(wh, max_windows=n_rows, max_beams=1, max_text_len=4 + depth + 1, kv_dtype=kv_code(kv),
-                              windows="native")
-    full = sess.transcribe_windows(waves, sp, bitmap, beam_size=1, max_depth=depth)
-    assert sess.last_decoder() == decoder
-    xa = f64.encoder_outputs64(sess, Ts)
-    key = (dims.n_text_state, dims.n_text_head, dims.n_vocab, dims.n_text_layer, wh.weights_fp16_exact)
-    steps = range(1, depth + 1)
-    refs = [f64._ref_pool().submit(f64._greedy_ref_rows, key, sp, xa[r][0].numpy(), full[r], kv,
-                                   [s for s in steps if 4 + s <= len(full[r])]) for r in range(n_rows)]
-    got = [dict() for _ in range(n_rows)]
-    for s in steps:
-        toks = sess.transcribe_windows(waves, sp, bitmap, beam_size=1, max_depth=s)
-        assert sess.last_decoder() == decoder
-        ids, lps = sess.last_topk(n_rows, 1)
-        for r in range(n_rows):
-            assert toks[r] == full[r][:len(toks[r])]
-            if len(toks[r]) == 4 + s:
-                assert int(ids[r, 0]) == toks[r][-1]
-                got[r][s] = float(lps[r, 0])
-    tol = f64.GREEDY_LP_TOL[kv]
-    worst = 0.0
-    for r in range(n_rows):
-        ref = refs[r].result()
-        assert sorted(got[r]) == sorted(ref)
-        for s, lp in got[r].items():
-            tok = full[r][4 + s - 1]
-            err = abs(lp - ref[s][tok])
-            worst = max(worst, err)
-            assert err < tol, f"row {r} (T = {Ts[r]}) step {s}: log-prob {lp} vs float64 {ref[s][tok]}"
-            assert ref[s].max() - ref[s][tok] < tol, f"row {r} step {s}: id {tok} is not the float64 argmax"
-    return worst
 
 
 # (decoder, d, rows, exact): decoder4 <= 7 rows, decoder6 8..24 rows, decoder5 d % 256 == 0, decoder3 (both weight types)
@@ -149,30 +86,33 @@ NATIVE_DEC_CASES = [(4, 384, 1, True), (4, 384, 4, True), (6, 384, 8, True), (6,
 @pytest.mark.parametrize("kv", ["f32", "f16"])
 @pytest.mark.parametrize("decoder,d,rows,exact", NATIVE_DEC_CASES)
 def test_decoder_greedy_native_T_vs_float64(decoder, d, rows, exact, kv, monkeypatch):
-    dims, wh, _ = f64.make_model(d, d // 64, 51864 if d == 384 else 2051, exact=exact)
-    f64.use_decoder(monkeypatch, decoder)
+    dims, wh, _ = h.make_model(d, d // 64, 51864 if d == 384 else 2051, exact=exact)
+    h.use_decoder(monkeypatch, decoder)
+    seed = 2000 + 10 * decoder + rows
+    Ts = [DEC_TS[i % len(DEC_TS)] for i in range(rows)]
+    waves = [synth.waveform(480000 if T == 1500 else samples_of_T(T), seed=seed + i) for i, T in enumerate(Ts)]
     try:
-        worst = check_greedy_native(dims, wh, kv, rows, decoder, seed=2000 + 10 * decoder + rows)
+        worst = h.check_greedy(dims, wh, kv, rows, decoder, seed, inputs=(Ts, waves), mode="native")
     except ffi.WbError as e:
         if decoder == 4 and rows > 1 and e.code == ffi.WB_ERR_UNSUPPORTED:
             pytest.skip(f"decoder4 does not cover {rows} rows on this GPU (co-resident 16-CTA clusters)")
         raise
-    f64.report(f"native decoder{decoder} d={d} rows={rows} kv={kv}", worst, f64.GREEDY_LP_TOL[kv])
+    h.report(f"native decoder{decoder} d={d} rows={rows} kv={kv}", worst, h.GREEDY_LP_TOL[kv])
 
 
 @pytest.mark.parametrize("kv", ["f32", "f16"])
 @pytest.mark.parametrize("decoder,d", [(3, 384), (5, 256)])
 def test_session_step_k7_native_T_vs_float64(decoder, d, kv, monkeypatch):
     """wb_session_step with k = 7 on two windows of T = 1500 and 1025: every candidate against float64 CachedDecoder rows."""
-    dims, wh, w64 = f64.make_model(d, d // 64, 51864 if d == 384 else 2051)
-    f64.use_decoder(monkeypatch, decoder)
+    dims, wh, w64 = h.make_model(d, d // 64, 51864 if d == 384 else 2051)
+    h.use_decoder(monkeypatch, decoder)
     sp = synth.special_tokens(dims)
     bitmap = sp.is_special_bitmap()
     K = 7
     waves = [synth.waveform(480000, seed=2500), synth.waveform(samples_of_T(1025), seed=2501)]
     sess = transcribe.Session(wh, max_windows=2, max_beams=5, max_text_len=12, kv_dtype=kv_code(kv), windows="native")
     sess.encode_waveforms(waves)
-    xa = f64.encoder_outputs64(sess, [1500, 1025])
+    xa = h.encoder_outputs64(sess, [1500, 1025])
     opts = o_model.OracleOptions(kv_dtype=kv)
     prompt = sp.prompt()
     sess.begin(prompt)
@@ -181,7 +121,7 @@ def test_session_step_k7_native_T_vs_float64(decoder, d, kv, monkeypatch):
         for t in prompt[:-1]:
             dec.step(torch.tensor([t], dtype=torch.int64))
     maskout = torch.from_numpy(sp.maskout())
-    tol = f64.STEP_LP_TOL[kv]
+    tol = h.STEP_LP_TOL[kv]
     worst = 0.0
     rows = [(0, 0), (1, 0)]          # GPU row -> (window, row of that window's float64 decoder)
 
@@ -210,47 +150,36 @@ def test_session_step_k7_native_T_vs_float64(decoder, d, kv, monkeypatch):
     ids = step([0, 0, 0, 1, 1, 1], [int(ids[0, j]) for j in range(3)] + [int(ids[1, j]) for j in range(3)], True)
     ids = step([2, 0, 1, 5, 3, 4], [int(ids[p, 1]) for p in (2, 0, 1, 5, 3, 4)], False)
     step([1, 2, 0, 4, 5, 3], [int(ids[p, 2]) for p in (1, 2, 0, 4, 5, 3)], False)
-    f64.report(f"native step k=7 decoder{decoder} d={d} kv={kv}", worst, tol)
+    h.report(f"native step k=7 decoder{decoder} d={d} kv={kv}", worst, tol)
 
 
 # ---------------------------------------------------------------- (d), (e) token ids against the native fixture
-def _check_ids_where_separated(got, recs, tol=1e-4):
-    """ids identical up to the first step whose oracle top-1/top-2 gap is below tol (there fp32 rounding decides)."""
-    for i, (g, r) in enumerate(zip(got, recs)):
-        want = r["tokens"]
-        n = next((4 + s for s, v in enumerate(r.get("margins", [])) if v < tol), len(want))
-        assert g[:n] == want[:n], f"window {i}: first difference at {next(j for j in range(n) if g[j] != want[j])}"
-        if n == len(want):
-            assert g == want
-
-
 def _windows(case):
     return [synth.chunk_waveform(c)[:n] for c, n in case["windows"]]
 
 
 @pytest.fixture(scope="module")
 def tiny_en():
-    dims, w_np, _ = synth.make_weights("tiny.en", seed=0)
-    return dims, synth.special_tokens(dims), model.Whisper(dims, w_np)
+    return h.named_model("tiny.en")
 
 
 @pytest.mark.parametrize("kv", ["f32", "f16"])
 def test_tiny_en_greedy_native_golden(tiny_en, kv):
     """One batch of T = 1500, 1500, 1005 and 205, greedy depth 100, on the default decoder."""
-    dims, sp, wh = tiny_en
-    g = gold()["tiny.en"]
+    dims, sp, wh, *_ = tiny_en
+    g = h.golden("tokens_native")["tiny.en"]
     sess = transcribe.Session(wh, max_windows=4, max_beams=1, max_text_len=105, kv_dtype=kv_code(kv), windows="native")
     got = sess.transcribe_windows(_windows(g), sp, is_special_of(sp), beam_size=1, max_depth=100)
     assert [sess.get_encoder_output(i).shape[0] for i in range(4)] == [r["T"] for r in g[kv]] == [1500, 1500, 1005, 205]
     print(f"\n[native] tiny.en greedy kv={kv}: decoder{sess.last_decoder()}")
-    _check_ids_where_separated(got, g[kv])
+    h.check_ids_where_separated(got, g[kv])
 
 
 @pytest.mark.parametrize("kv", ["f32", "f16"])
 def test_tiny_en_device_beam_native_golden(tiny_en, kv):
     """Beam 5, depth 30, 2 windows (T = 1500, 1005): the whole search in one decoder6 launch."""
-    dims, sp, wh = tiny_en
-    g = gold()["tiny.en-beam"]
+    dims, sp, wh, *_ = tiny_en
+    g = h.golden("tokens_native")["tiny.en-beam"]
     sess = transcribe.Session(wh, max_windows=2, max_beams=5, max_text_len=35, kv_dtype=kv_code(kv), windows="native")
     got = sess.transcribe_windows(_windows(g), sp, is_special_of(sp), beam_size=5, max_depth=30)
     assert sess.last_decoder() == 6
@@ -259,18 +188,17 @@ def test_tiny_en_device_beam_native_golden(tiny_en, kv):
 
 @pytest.fixture(scope="module")
 def small_en():
-    dims, w_np, _ = synth.make_weights("small.en", seed=0)
-    return dims, synth.special_tokens(dims), model.Whisper(dims, w_np)
+    return h.named_model("small.en")
 
 
 @pytest.mark.parametrize("kv", ["f32", "f16"])
 def test_small_en_greedy_native_golden(small_en, kv):
-    dims, sp, wh = small_en
-    g = gold()["small.en"]
+    dims, sp, wh, *_ = small_en
+    g = h.golden("tokens_native")["small.en"]
     sess = transcribe.Session(wh, max_windows=2, max_beams=1, max_text_len=105, kv_dtype=kv_code(kv), windows="native")
     got = sess.transcribe_windows(_windows(g), sp, is_special_of(sp), beam_size=1, max_depth=100)
     assert sess.last_decoder() == 5
-    _check_ids_where_separated(got, g[kv])
+    h.check_ids_where_separated(got, g[kv])
     if kv == "f32":   # the one or two tokens these models decode carry little evidence: the 5 best log-probs of every step
         recs = g[kv]
         sess.encode_waveforms(_windows(g))
@@ -283,14 +211,14 @@ def test_small_en_greedy_native_golden(small_en, kv):
                 worst = max(worst, float(np.abs(lps[r] - np.asarray(want_lp, np.float32)).max()))
                 last[r] = recs[r]["tokens"][4 + step]
                 assert int(ids[r, 0]) == last[r]
-        f64.report("native small.en 2 rows x 100 steps, top-5 log-probs vs oracle", worst, 2e-4)
+        h.report("native small.en 2 rows x 100 steps, top-5 log-probs vs oracle", worst, 2e-4)
         assert worst < 2e-4
 
 
 def test_small_en_host_beam_native_golden(small_en):
     """Beam 5, depth 20, one window of T = 1500: the host search over decoder5 steps."""
-    dims, sp, wh = small_en
-    g = gold()["small.en-beam"]
+    dims, sp, wh, *_ = small_en
+    g = h.golden("tokens_native")["small.en-beam"]
     sess = transcribe.Session(wh, max_windows=1, max_beams=5, max_text_len=25, windows="native")
     got = sess.transcribe_windows(_windows(g), sp, is_special_of(sp), beam_size=5, max_depth=20)
     assert sess.last_decoder() == 5
@@ -299,8 +227,8 @@ def test_small_en_host_beam_native_golden(small_en):
 
 def test_tiny_en_long_form_native_golden(tiny_en):
     """waveform_to_tokens over 70 s: three native windows (T = 1500, 1500, 814) and the overlap merge."""
-    dims, sp, wh = tiny_en
-    g = gold()["tiny.en-long"]
+    dims, sp, wh, *_ = tiny_en
+    g = h.golden("tokens_native")["tiny.en-long"]
     wave = np.concatenate([synth.chunk_waveform(c) for c in g["chunks"]])[:g["samples"]]
     assert transcribe.window_bounds(len(wave), 16000, transcribe.window_samples(1500, "native")) == \
         [tuple(b) for b in g["bounds"]]
@@ -310,7 +238,7 @@ def test_tiny_en_long_form_native_golden(tiny_en):
 
 # ---------------------------------------------------------------- (f) both modes side by side
 def test_reference_and_native_sessions_side_by_side(tiny_en):
-    dims, sp, wh = tiny_en
+    dims, sp, wh, *_ = tiny_en
     ref = transcribe.Session(wh, max_windows=1, max_beams=1, max_text_len=8)
     nat = transcribe.Session(wh, max_windows=1, max_beams=1, max_text_len=8, windows="native")
     wave = synth.chunk_waveform(0)

@@ -3,56 +3,43 @@ max_by_last applied repeatedly (host/beam.hpp beamfx::rank_final), from the on-d
 from the host search.  Lists are checked against the oracle's (tests/golden/nbest_beam.json, make_golden_nbest.py): ids,
 lengths, finished flags and order; log-probs against float64 teacher forcing; rank 0 against the returned row."""
 import ctypes as C
-import json
-from pathlib import Path
 
 import numpy as np
 import pytest
 import torch
 
+import harness as h
 import oracle_prev_prompt as opp
-import test_f64_reference_gpu as f64
 import wb200  # noqa: F401
-from oracle import model as o_model, synth, transcribe as o_tr
-from whisper_burn_b200 import ffi, model, transcribe
+from harness import is_special_of, pool_waves
+from oracle import synth, transcribe as o_tr
+from whisper_burn_b200 import ffi, transcribe
 
 pytestmark = pytest.mark.gpu
-G = Path(__file__).resolve().parent / "golden"
-
-
-def is_special_of(sp):
-    return (np.arange(sp.n_vocab) >= sp.first_special).astype(np.uint8)
 
 
 @pytest.fixture(scope="module")
 def gold():
-    return json.loads((G / "nbest_beam.json").read_text())
+    return h.golden("nbest_beam")
 
 
 @pytest.fixture(scope="module")
 def small():
-    dims, w_np, w_t = synth.make_weights("test-a", seed=0)
-    return dims, o_model.as_dtype(w_t), synth.special_tokens(dims), model.Whisper(dims, w_np)
+    return h.named_model("test-a", f64=True)
 
 
 @pytest.fixture(scope="module")
 def tiny():
-    dims, w_np, w_t = synth.make_weights("tiny.en", seed=0)
-    return dims, o_model.as_dtype(w_t), synth.special_tokens(dims), model.Whisper(dims, w_np)
-
-
-def pool_waves(gold, n):
-    chunk = synth.chunk_waveform(0)
-    return [chunk[off:off + m] for off, m in (gold["pool"][i % len(gold["pool"])] for i in range(n))]
+    return h.named_model("tiny.en", f64=True)
 
 
 def session(wh, n, depth, kv, monkeypatch, decoder=0, prompt_len=4, max_beams=7):
-    f64.use_decoder(monkeypatch, decoder)
+    h.use_decoder(monkeypatch, decoder)
     try:
         return transcribe.Session(wh, max_windows=n, max_beams=max_beams, max_text_len=prompt_len + depth + 1,
-                                  kv_dtype=f64.kv_code(kv))
+                                  kv_dtype=h.kv_code(kv))
     finally:
-        f64.use_decoder(monkeypatch, 0)
+        h.use_decoder(monkeypatch, 0)
 
 
 def f64_sum(lps):
@@ -78,7 +65,7 @@ def check_list(sess, index, row, nb, n_prompt, eot):
 def match_golden(nb, want, kv):
     """ids, lengths, finished flags and order equal the golden list's; two ranks may come out swapped only where their golden
     scores differ by less than the log-prob tolerance times the sequence length"""
-    tol = f64.GREEDY_LP_TOL[kv]
+    tol = h.GREEDY_LP_TOL[kv]
     got_ids = [h[0] for h in nb]
     want_ids = [h["ids"] for h in want["hyps"]]
     assert len(got_ids) == len(want_ids) and sorted(map(tuple, got_ids)) == sorted(map(tuple, want_ids)), (got_ids, want_ids)
@@ -100,10 +87,9 @@ def check_f64(sess, w64, dims, sp, window, nb, kv, n_prompt=4, seen=None):
             if (window, tuple(ids)) in seen:
                 continue
             seen.add((window, tuple(ids)))
-        rows = o_tr.greedy_path_log_probs(w64, dims, sp, xa, ids, n_prompt=n_prompt, opts=o_model.OracleOptions(kv_dtype=kv))
-        ref = np.array([float(rows[j - n_prompt][ids[j]]) for j in range(n_prompt, len(ids))])
+        ref = h.along(h.path_rows(w64, dims, sp, xa, ids, kv, n_prompt=n_prompt), ids, n_prompt)
         err = float(np.abs(lps[n_prompt:].astype(np.float64) - ref).max(initial=0.0))
-        assert err < f64.GREEDY_LP_TOL[kv], f"window {window} {ids}: {lps[n_prompt:]} vs float64 {ref}"
+        assert err < h.GREEDY_LP_TOL[kv], f"window {window} {ids}: {lps[n_prompt:]} vs float64 {ref}"
         worst = max(worst, err)
     return worst
 
@@ -122,7 +108,7 @@ def same_lists(a, b):
 @pytest.mark.parametrize("kv", ["f32", "f16"])
 @pytest.mark.parametrize("b", [2, 3, 4, 5, 6, 7])
 def test_nbest_device_test_a(small, gold, monkeypatch, b, kv):
-    dims, w64, sp, wh = small
+    dims, sp, wh, _, _, w64 = small
     depth = gold["depth_test_a"]
     want = gold["test_a"][kv][str(b)]
     n_max = 24 // b
@@ -136,7 +122,7 @@ def test_nbest_device_test_a(small, gold, monkeypatch, b, kv):
             match_golden(nb, want[i % len(gold["pool"])], kv)
     seen: set = set()
     worst = max(check_f64(sess, w64, dims, sp, i, nb, kv, seen=seen) for i, nb in enumerate(nbs))
-    f64.report(f"last_nbest device beam test-a B={b} kv={kv}", worst, f64.GREEDY_LP_TOL[kv])
+    h.report(f"last_nbest device beam test-a B={b} kv={kv}", worst, h.GREEDY_LP_TOL[kv])
     hs = session(wh, n_max, depth, kv, monkeypatch, decoder=3)
     hids, hnbs = run(hs, pool_waves(gold, n_max), sp, b, depth)
     assert hs.last_decoder() == 3 and hids == ids and same_lists(hnbs, nbs)
@@ -144,8 +130,8 @@ def test_nbest_device_test_a(small, gold, monkeypatch, b, kv):
 
 @pytest.mark.parametrize("kv", ["f32", "f16"])
 def test_nbest_tiny_en_device_and_host(tiny, gold, monkeypatch, kv):
-    dims, w64, sp, wh = tiny
-    te = json.loads((G / "tokens_tiny_en.json").read_text())
+    dims, sp, wh, _, _, w64 = tiny
+    te = h.golden("tokens_tiny_en")
     chunk = synth.chunk_waveform(0)
     waves = [chunk[s:e] for s, e in te["bounds"]]
     depth = gold["depth_tiny_en"]
@@ -161,7 +147,7 @@ def test_nbest_tiny_en_device_and_host(tiny, gold, monkeypatch, kv):
             match_golden(lists[i], gold["tiny_en"][kv]["5"][i], kv)
     seen: set = set()
     worst = max(check_f64(sess, w64, dims, sp, i, nb, kv, seen=seen) for i, nb in enumerate(nbs))
-    f64.report(f"last_nbest device beam tiny.en B=5 kv={kv}", worst, f64.GREEDY_LP_TOL[kv])
+    h.report(f"last_nbest device beam tiny.en B=5 kv={kv}", worst, h.GREEDY_LP_TOL[kv])
 
 
 # ---------------------------------------------------------------- 3. EOT, depth limit, previous-text prompts
@@ -169,7 +155,7 @@ def test_nbest_tiny_en_device_and_host(tiny, gold, monkeypatch, kv):
 def test_nbest_eot_and_depth_limit(small, gold, monkeypatch, decoder):
     """EOT declared to be a token the search emits: both windows stop early with a finished best and live hypotheses carried
     behind it, one several steps before the other; at depth 12 (test-a, default EOT) every list is live hypotheses only"""
-    dims, w64, sp, wh = small
+    dims, sp, wh, _, _, w64 = small
     sp2 = o_tr.SpecialTokens(sp.sot, sp.lang, sp.transcribe, sp.notimestamps, gold["eot"], sp.first_special, sp.n_vocab)
     chunk = synth.chunk_waveform(0)
     waves = [chunk[:238559], chunk[:98882]]
@@ -192,7 +178,7 @@ def test_nbest_eot_and_depth_limit(small, gold, monkeypatch, decoder):
 def test_nbest_prev_prompt_mixed_lengths(small, gold, monkeypatch, decoder):
     """one launch over windows whose prompts hold 4, 7, 10 and 6 ids: each hypothesis starts with its window's own prompt,
     whose ids score 0"""
-    dims, w64, sp, wh = small
+    dims, sp, wh, _, _, w64 = small
     depth = gold["depth_test_a"]
     prevs = gold["prev_ids"]
     prompts = [opp.build_prompt(sp, p) for p in prevs]
@@ -219,7 +205,7 @@ def nbest_status(sess, index, max_hyps=14, capacity=64):
 
 
 def test_nbest_greedy_depth0_loop_and_state_rules(small, gold, monkeypatch):
-    dims, _, sp, wh = small
+    dims, sp, wh, *_ = small
     waves = pool_waves(gold, 3)
     sess = session(wh, 3, 12, "f32", monkeypatch)
     assert nbest_status(sess, 0) == ffi.WB_ERR_STATE                   # before the first decode call
@@ -269,7 +255,7 @@ def test_nbest_greedy_depth0_loop_and_state_rules(small, gold, monkeypatch):
 def test_nbest_waveforms_to_tokens_per_window(tiny, monkeypatch, prev_prompt):
     """two waveforms (30 s and 7 s) at beam 5: window k in waveform-major order has the n-best transcribe_windows(_prev) gives
     for the same slice, prompt and batch"""
-    dims, _, sp, wh = tiny
+    dims, sp, wh, *_ = tiny
     depth = 20
     chunk = synth.chunk_waveform(0)
     wave_b = synth.chunk_waveform(1)[:112000]
@@ -313,12 +299,12 @@ def test_nbest_waveforms_to_tokens_per_window(tiny, monkeypatch, prev_prompt):
 @pytest.mark.parametrize("kv", ["f32", "f16"])
 def test_nbest_rescoring_round_trip(small, gold, monkeypatch, kv):
     """score_tokens on every hypothesis of a window reproduces the log-probs the search scored its generated ids with"""
-    _, _, sp, wh = small
+    _, sp, wh, *_ = small
     sess = session(wh, 2, gold["depth_test_a"], kv, monkeypatch)
     ids, nbs = run(sess, pool_waves(gold, 2), sp, 5, gold["depth_test_a"])
     for w in range(2):
         hyps = nbs[w]
         scored = sess.score_tokens([h[0] for h in hyps], [w] * len(hyps), apply_special_mask=True, is_special=is_special_of(sp))
         for (hid, hlp, _, _), (lp, _) in zip(hyps, scored):
-            assert np.abs(lp[4:].astype(np.float64) - hlp[4:]).max() < f64.GREEDY_LP_TOL[kv], hid
+            assert np.abs(lp[4:].astype(np.float64) - hlp[4:]).max() < h.GREEDY_LP_TOL[kv], hid
         assert same_lists([sess.last_nbest(i) for i in range(2)], nbs)

@@ -5,47 +5,34 @@ Bars (north_star): log-mel within 1e-4 relative -- measured as max|a-b| / max|re
 tensor's scale; element-wise relative error is reported too, with an absolute floor, because bins at
 the f32 rounding-noise floor differ between ANY two f32 DFT implementations, SURVEY section 7);
 decoded token ids identical under greedy (and under beam 5)."""
-import json
-from pathlib import Path
-
 import numpy as np
 import pytest
 import torch
 
+import harness as h
 import wb200  # noqa: F401
+from harness import G, is_special_of, kv_code, rel_to_scale
 from oracle import audio as o_audio, model as o_model, synth, transcribe as o_tr
 from whisper_burn_b200 import audio, ffi, model, transcribe
 
 pytestmark = pytest.mark.gpu
-G = Path(__file__).resolve().parent / "golden"
 MEL_TOL = 1e-4
-
-
-def rel_to_scale(a, b):
-    return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30))
-
-
-def is_special_of(sp):
-    return (np.arange(sp.n_vocab) >= sp.first_special).astype(np.uint8)
 
 
 @pytest.fixture(scope="module")
 def small():
-    dims, w_np, w_t = synth.make_weights("test-a", seed=0)
-    return dims, w_np, w_t, synth.special_tokens(dims), model.Whisper(dims, w_np)
+    return h.named_model("test-a")
 
 
 @pytest.fixture(scope="module")
 def tiny():
-    dims, w_np, w_t = synth.make_weights("tiny.en", seed=0)
-    return dims, w_np, w_t, synth.special_tokens(dims), model.Whisper(dims, w_np)
+    return h.named_model("tiny.en")
 
 
 @pytest.fixture(scope="module")
 def wide():
     """d = 256: the configuration class the batched tensor-core decoder (decoder5.cu) covers (small.en / medium / large)."""
-    dims, w_np, w_t = synth.make_weights("test-c", seed=0)
-    return dims, w_np, w_t, synth.special_tokens(dims), model.Whisper(dims, w_np)
+    return h.named_model("test-c")
 
 
 # ---------------------------------------------------------------- log-mel (audio.rs)
@@ -95,7 +82,7 @@ def test_prep_audio_scale_property_full_size():
 # ---------------------------------------------------------------- encoder / decoder (mod.rs)
 @pytest.mark.parametrize("n_ctx", [1, 2, 301, 628, 1500])
 def test_forward_encoder_vs_oracle(small, n_ctx):
-    dims, _, w_t, _, wh = small
+    dims, _, wh, _, w_t, _ = small
     mel = torch.from_numpy(np.random.default_rng(n_ctx).standard_normal((2, 80, n_ctx)).astype(np.float32) * 0.5)
     got = wh.forward_encoder(mel.numpy())
     want = o_model.forward_encoder(w_t, dims, mel).numpy()
@@ -104,7 +91,7 @@ def test_forward_encoder_vs_oracle(small, n_ctx):
 
 
 def test_forward_encoder_contract_violations(small):
-    dims, _, _, _, wh = small
+    dims, _, wh, *_ = small
     for shape in ((1, 80, 1501), (1, 81, 100)):                                      # mod.rs:231-241 asserts
         with pytest.raises(ffi.WbError) as e:
             wh.forward_encoder(np.zeros(shape, np.float32))
@@ -112,7 +99,7 @@ def test_forward_encoder_contract_violations(small):
 
 
 def test_forward_decoder_stateless_vs_oracle(small):
-    dims, _, w_t, sp, wh = small
+    dims, sp, wh, _, w_t, _ = small
     rng = np.random.default_rng(0)
     xa = rng.standard_normal((3, 50, dims.n_audio_state)).astype(np.float32)
     toks = rng.integers(0, dims.n_vocab, size=(3, 9)).astype(np.int64)
@@ -126,7 +113,7 @@ def test_forward_decoder_stateless_vs_oracle(small):
 
 
 def test_encoder_golden_tiny_en(tiny):
-    dims, _, _, _, wh = tiny
+    dims, _, wh, *_ = tiny
     z = np.load(G / "encoder_golden.npz")
     chunk = synth.chunk_waveform(0)
     sess = transcribe.Session(wh, max_windows=1, max_beams=1, max_text_len=8)
@@ -139,7 +126,7 @@ def test_encoder_golden_tiny_en(tiny):
 
 
 def test_layernorm_eps_mode_inside(small):
-    dims, w_np, w_t, _, _ = small
+    dims, _, _, w_np, w_t, _ = small
     wh = model.Whisper(dims, w_np, ln_eps_outside=False)
     mel = torch.from_numpy(np.random.default_rng(5).standard_normal((1, 80, 200)).astype(np.float32) * 0.5)
     want = o_model.forward_encoder(w_t, dims, mel, o_model.OracleOptions("inside")).numpy()
@@ -147,9 +134,7 @@ def test_layernorm_eps_mode_inside(small):
 
 
 def test_non_fp16_exact_weights_use_fp32_storage():
-    dims, w_np, _ = synth.make_weights("test-a", seed=3)
-    w_np = {k: (v * np.float32(1.0001) if v.ndim else v) for k, v in w_np.items()}    # no longer fp16-representable
-    w_t = synth.to_torch(w_np)
+    dims, w_np, w_t, _ = h.synthetic("test-a", 3, exact=False, f64=False)    # no longer fp16-representable
     wh = model.Whisper(dims, w_np)
     assert not wh.weights_fp16_exact
     sp = synth.special_tokens(dims)
@@ -163,8 +148,8 @@ def test_non_fp16_exact_weights_use_fp32_storage():
 # ---------------------------------------------------------------- decoding (transcribe.rs + beam.rs)
 @pytest.mark.parametrize("beam_size,depth", [(1, 30), (5, 12)])
 def test_tokens_small_model_vs_oracle_and_golden(small, beam_size, depth):
-    dims, _, w_t, sp, wh = small
-    ta = json.loads((G / "tokens_test_a.json").read_text())
+    dims, sp, wh, _, w_t, _ = small
+    ta = h.golden("tokens_test_a")
     chunk = synth.chunk_waveform(0)
     waves = [chunk[:238559], chunk[:98882]]
     sess = transcribe.Session(wh, max_windows=2, max_beams=5, max_text_len=4 + depth + 1)
@@ -180,8 +165,8 @@ def test_tokens_small_model_vs_oracle_and_golden(small, beam_size, depth):
 
 @pytest.mark.parametrize("key,beam_size", [("eot_case", 1), ("eot_case_beam5", 5)])
 def test_eot_stops_search(small, key, beam_size):
-    dims, _, _, sp, wh = small
-    ta = json.loads((G / "tokens_test_a.json").read_text())
+    dims, sp, wh, *_ = small
+    ta = h.golden("tokens_test_a")
     e = ta[key]
     sp2 = o_tr.SpecialTokens(sp.sot, sp.lang, sp.transcribe, sp.notimestamps, e["eot"], sp.first_special, sp.n_vocab)
     sess = transcribe.Session(wh, max_windows=2, max_beams=5, max_text_len=4 + 30 + 1)
@@ -192,7 +177,7 @@ def test_eot_stops_search(small, key, beam_size):
 
 def test_session_step_api_matches_forward_decoder(small):
     """wb_session_step (cached, top-k) against the stateless wb_forward_decoder + host log_softmax."""
-    dims, _, w_t, sp, wh = small
+    dims, sp, wh, _, w_t, _ = small
     wave = synth.waveform(60000, seed=9)
     sess = transcribe.Session(wh, max_windows=1, max_beams=3, max_text_len=16)
     sess.encode_waveforms([wave])
@@ -218,8 +203,8 @@ def test_session_step_api_matches_forward_decoder(small):
 
 def test_tiny_en_chunk_greedy_golden(tiny):
     """BASELINE config 2: tiny.en, one 30 s chunk (3 reference windows), greedy to depth 100."""
-    dims, _, _, sp, wh = tiny
-    te = json.loads((G / "tokens_tiny_en.json").read_text())
+    dims, sp, wh, *_ = tiny
+    te = h.golden("tokens_tiny_en")
     chunk = synth.chunk_waveform(0)
     sess = transcribe.Session(wh, max_windows=3, max_beams=5, max_text_len=105)
     waves = [chunk[s:e] for s, e in te["bounds"]]
@@ -235,7 +220,7 @@ def test_tiny_en_chunk_greedy_golden(tiny):
 def test_greedy_equals_beam1_host_path_full_size(tiny):
     """Property at full size: the on-device greedy loop and the host beam search driven through
     wb_session_step with k = 1 are two code paths for the same search (beam.rs with beam_size 1)."""
-    dims, _, _, sp, wh = tiny
+    dims, sp, wh, *_ = tiny
     chunk = synth.chunk_waveform(5)
     wave = chunk[:238559]
     sess = transcribe.Session(wh, max_windows=1, max_beams=2, max_text_len=105)
@@ -253,7 +238,7 @@ def test_greedy_equals_beam1_host_path_full_size(tiny):
 def test_fp16_kv_cache_matches_oracle_f16_mode(small, beam_size, depth):
     """WB_KV_F16 (the north star's persistent fp16 K/V cache): scaled keys and values are rounded to fp16 where
     they enter the cache; the oracle restates exactly that rounding (OracleOptions.kv_dtype = "f16")."""
-    dims, _, w_t, sp, wh = small
+    dims, sp, wh, _, w_t, _ = small
     chunk = synth.chunk_waveform(0)
     waves = [chunk[:238559], chunk[:98882]]
     sess = transcribe.Session(wh, max_windows=2, max_beams=5, max_text_len=4 + depth + 1, kv_dtype=ffi.WB_KV_F16)
@@ -268,7 +253,7 @@ def test_fp16_kv_cache_matches_oracle_f16_mode(small, beam_size, depth):
 def test_npy_tree_round_trip(small, tmp_path):
     """wb_model_load_npy_tree (load::load_whisper, src/model/load.rs:295-310) == tensors set one by one."""
     from whisper_burn_b200 import npytree
-    dims, w_np, _, sp, wh = small
+    dims, sp, wh, w_np, *_ = small
     npytree.save_npy_tree(tmp_path, dims, w_np)
     wh2 = model.Whisper.from_npy_tree(tmp_path)
     assert wh2.config == dims and wh2.weights_fp16_exact
@@ -282,7 +267,7 @@ def test_npy_tree_round_trip(small, tmp_path):
 
 def test_batched_waveforms_equal_one_by_one(small):
     """wb_waveforms_to_tokens (all windows in one batch) == wb_waveform_to_tokens per waveform (transcribe.rs:23-74)."""
-    dims, _, _, sp, wh = small
+    dims, sp, wh, *_ = small
     waves = [synth.waveform(60000 + 9000 * i, seed=20 + i) for i in range(3)]
     sess = transcribe.Session(wh, 4, 1, 24)
     one = [sess.waveform_to_tokens(w, sp, is_special_of(sp), 16000, 1, 12) for w in waves]
@@ -293,33 +278,31 @@ def test_batched_waveforms_equal_one_by_one(small):
 def test_batched_tensor_core_decoder_greedy_vs_oracle(wide, kv):
     """decoder5.cu (mma.sync swap-AB, hi/lo fp16 split of the activations): 10 windows decoded in one batch,
     token ids identical to the oracle's per-window greedy search (transcribe.rs:148-383)."""
-    dims, _, w_t, sp, wh = wide
+    dims, sp, wh, _, w_t, _ = wide
     waves = [synth.waveform(30000 + 7000 * i, seed=40 + i) for i in range(10)]
     sess = transcribe.Session(wh, max_windows=10, max_beams=1, max_text_len=4 + 14 + 1,
-                              kv_dtype=ffi.WB_KV_F16 if kv == "f16" else ffi.WB_KV_F32)
+                              kv_dtype=kv_code(kv))
     got = sess.transcribe_windows(waves, sp, is_special_of(sp), beam_size=1, max_depth=14)
     assert sess.last_decoder() == 5
-    assert got == json.loads((G / "tokens_wide.json").read_text())[f"test-c_greedy_depth14_{kv}"]      # committed oracle ids
+    assert got == h.golden("tokens_wide")[f"test-c_greedy_depth14_{kv}"]      # committed oracle ids
     opts = o_model.OracleOptions(kv_dtype=kv)
     for g, wv in zip(got, waves):
         want = o_tr.mels_to_tokens(w_t, dims, sp, o_audio.prep_audio(torch.from_numpy(wv)[None]), beam_size=1, max_depth=14, opts=opts)
         assert g == want
     # batching invariance across decoders: one window alone takes the same path with a single n-tile
-    solo = transcribe.Session(wh, max_windows=1, max_beams=1, max_text_len=4 + 14 + 1, kv_dtype=ffi.WB_KV_F16 if kv == "f16" else ffi.WB_KV_F32)
+    solo = transcribe.Session(wh, max_windows=1, max_beams=1, max_text_len=4 + 14 + 1, kv_dtype=kv_code(kv))
     assert solo.transcribe_windows(waves[3:4], sp, is_special_of(sp), beam_size=1, max_depth=14)[0] == got[3]
 
 
 def test_batched_tensor_core_decoder_unsplit_cross_attention():
     """20 rows x 8 heads >= one (row, head) unit per SM: decoder5.cu runs cross attention unsplit (S = 1) and writes its output
     directly as tensor-core planes -- the configuration class of the small.en / medium batches in BASELINE.json."""
-    dims, w_np, w_t = synth.make_weights("test-d", seed=0)
-    sp = synth.special_tokens(dims)
-    wh = model.Whisper(dims, w_np)
+    dims, sp, wh, _, w_t, _ = h.named_model("test-d")
     waves = [synth.waveform(24000 + 3000 * i, seed=80 + i) for i in range(20)]
     sess = transcribe.Session(wh, max_windows=20, max_beams=1, max_text_len=4 + 6 + 1)
     got = sess.transcribe_windows(waves, sp, is_special_of(sp), beam_size=1, max_depth=6)
     assert sess.last_decoder() == 5
-    gold = json.loads((G / "tokens_wide.json").read_text())["test-d_greedy_depth6_f32"]
+    gold = h.golden("tokens_wide")["test-d_greedy_depth6_f32"]
     assert all(got[int(i)] == t for i, t in gold.items())
     for i in (0, 7, 13, 19):
         want = o_tr.mels_to_tokens(w_t, dims, sp, o_audio.prep_audio(torch.from_numpy(waves[i])[None]), beam_size=1, max_depth=6)
@@ -328,14 +311,12 @@ def test_batched_tensor_core_decoder_unsplit_cross_attention():
 
 def test_batched_tensor_core_decoder_small_en_width():
     """d = 768: decoder5.cu splits MLP2 (K = 4d) into 3 slabs of 1024 columns (fewer rounds of tiles than 4 slabs)."""
-    dims, w_np, w_t = synth.make_weights("test-e", seed=0)
-    sp = synth.special_tokens(dims)
-    wh = model.Whisper(dims, w_np)
+    dims, sp, wh, _, w_t, _ = h.named_model("test-e")
     waves = [synth.waveform(20000 + 2500 * i, seed=120 + i) for i in range(9)]
     sess = transcribe.Session(wh, max_windows=9, max_beams=1, max_text_len=4 + 6 + 1)
     got = sess.transcribe_windows(waves, sp, is_special_of(sp), beam_size=1, max_depth=6)
     assert sess.last_decoder() == 5
-    gold = json.loads((G / "tokens_wide.json").read_text())["test-e_greedy_depth6_f32"]
+    gold = h.golden("tokens_wide")["test-e_greedy_depth6_f32"]
     assert all(got[int(i)] == t for i, t in gold.items())
     for i in (0, 4, 8):
         want = o_tr.mels_to_tokens(w_t, dims, sp, o_audio.prep_audio(torch.from_numpy(waves[i])[None]), beam_size=1, max_depth=6)
@@ -343,12 +324,12 @@ def test_batched_tensor_core_decoder_small_en_width():
 
 
 def test_batched_tensor_core_decoder_beams_and_logits(wide):
-    dims, _, w_t, sp, wh = wide
+    dims, sp, wh, _, w_t, _ = wide
     waves = [synth.waveform(42000 + 9000 * i, seed=60 + i) for i in range(3)]
     sess = transcribe.Session(wh, max_windows=3, max_beams=5, max_text_len=4 + 8 + 1)
     got = sess.transcribe_windows(waves, sp, is_special_of(sp), beam_size=5, max_depth=8)      # 15 rows, ancestry table
     assert sess.last_decoder() == 5
-    assert got == json.loads((G / "tokens_wide.json").read_text())["test-c_beam5_depth8_f32"]
+    assert got == h.golden("tokens_wide")["test-c_beam5_depth8_f32"]
     for g, wv in zip(got, waves):
         assert g == o_tr.mels_to_tokens(w_t, dims, sp, o_audio.prep_audio(torch.from_numpy(wv)[None]), beam_size=5, max_depth=8)
     # stateless forward_decoder (full logits) against the oracle's decoder (mod.rs:131-157)
@@ -361,7 +342,7 @@ def test_batched_tensor_core_decoder_beams_and_logits(wide):
 
 
 def test_launch_counter_counts_kernels(small):
-    dims, _, _, sp, wh = small
+    dims, sp, wh, *_ = small
     ffi.lib().wb_kernel_launch_count_reset()
     sess = transcribe.Session(wh, 1, 1, 16)
     sess.transcribe_windows([synth.waveform(16000, seed=1)], sp, is_special_of(sp), beam_size=1, max_depth=4)
@@ -373,7 +354,7 @@ def test_batched_decoder_row_groups(wide, beam_size):
     """More rows than one launch of decoder5.cu takes (the shape of BASELINE configs[4]: beams of many windows per GPU): the session
     runs row groups of 32, one launch each; greedy 40 windows = 2 groups, beam 5 x 9 windows = 45 rows = 2 groups with the ancestry
     table addressing absolute cache rows."""
-    dims, _, w_t, sp, wh = wide
+    dims, sp, wh, _, w_t, _ = wide
     n = 40 if beam_size == 1 else 9
     waves = [synth.waveform(28000 + 1500 * i, seed=200 + i) for i in range(n)]
     sess = transcribe.Session(wh, max_windows=n, max_beams=beam_size, max_text_len=4 + 8 + 1)

@@ -12,22 +12,20 @@ prompts differ in length share one decoder launch, each row committing from its 
   6. the waveform rule of waveform(s)_to_tokens against the oracle restatement (tests/oracle_prev_prompt.py), and batched
      waveforms against each waveform alone;
   7. every error case of the two entry points."""
-import json
 from ctypes import byref as C_byref, c_int64 as C_int64
-from pathlib import Path
 
 import numpy as np
 import pytest
 import torch
 
+import harness as h
 import oracle_prev_prompt as opp
-import test_f64_reference_gpu as f64
 import wb200  # noqa: F401
-from oracle import audio as o_audio, model as o_model, synth, transcribe as o_tr
+from oracle import audio as o_audio, synth, transcribe as o_tr
 from whisper_burn_b200 import ffi, model, transcribe
 
 pytestmark = pytest.mark.gpu
-DEPTH = f64.DEPTH
+DEPTH = h.DEPTH
 
 
 def prev_lists(sp, n, long_len, seed):
@@ -37,12 +35,6 @@ def prev_lists(sp, n, long_len, seed):
     return [[int(t) for t in rng.integers(0, sp.first_special, size=k)] for k in lens]
 
 
-def f64_lps(w64, dims, sp, xa, ids, lp0, kv):
-    rows = o_tr.greedy_path_log_probs(w64, dims, opp.oracle_special(sp), xa, ids, n_prompt=lp0,
-                                      opts=o_model.OracleOptions(kv_dtype=kv))
-    return np.array([float(rows[j - lp0][ids[j]]) for j in range(lp0, len(ids))])
-
-
 # (decoder, d, heads, rows, long previous list): the long list crosses decoder6's 32-key slot, and the 128-key turn elsewhere
 RAGGED_CASES = [(4, 384, 6, 4, 130), (6, 384, 6, 9, 40), (6, 128, 2, 8, 40), (5, 256, 4, 9, 130), (3, 384, 6, 4, 130)]
 
@@ -50,14 +42,14 @@ RAGGED_CASES = [(4, 384, 6, 4, 130), (6, 384, 6, 9, 40), (6, 128, 2, 8, 40), (5,
 @pytest.mark.parametrize("kv", ["f32", "f16"])
 @pytest.mark.parametrize("decoder,d,H,rows,long_len", RAGGED_CASES)
 def test_ragged_greedy_vs_float64(decoder, d, H, rows, long_len, kv, monkeypatch):
-    dims, wh, w64 = f64.make_model(d, H, 2051)
+    dims, wh, w64 = h.make_model(d, H, 2051)
     sp = synth.special_tokens(dims)
-    _, waves = f64.windows(rows, seed=7 * d + rows)
+    _, waves = h.windows(rows, seed=7 * d + rows)
     prev = prev_lists(sp, rows, long_len, seed=d + rows)
     t_max = long_len + 5 + DEPTH + 1
-    f64.use_decoder(monkeypatch, decoder)
-    sess = transcribe.Session(wh, max_windows=rows, max_beams=1, max_text_len=t_max, kv_dtype=f64.kv_code(kv))
-    f64.use_decoder(monkeypatch, 0)
+    h.use_decoder(monkeypatch, decoder)
+    sess = transcribe.Session(wh, max_windows=rows, max_beams=1, max_text_len=t_max, kv_dtype=h.kv_code(kv))
+    h.use_decoder(monkeypatch, 0)
     ids = sess.transcribe_windows_prev(waves, prev, sp, sp.is_special_bitmap(), beam_size=1, max_depth=DEPTH)
     assert sess.last_decoder() == decoder
     worst = 0.0
@@ -69,25 +61,25 @@ def test_ragged_greedy_vs_float64(decoder, d, H, rows, long_len, kv, monkeypatch
         lps = sess.last_logprobs(r)
         assert len(lps) == len(t) and np.all(lps[:lp0] == 0.0)
         xa = torch.from_numpy(sess.get_encoder_output(r)).double()[None]
-        ref = f64_lps(w64, dims, sp, xa, t, lp0, kv)
+        ref = h.along(h.path_rows(w64, dims, opp.oracle_special(sp), xa, t, kv, n_prompt=lp0), t, lp0)
         err = float(np.abs(lps[lp0:].astype(np.float64) - ref).max(initial=0.0))
         worst = max(worst, err)
-        assert err < f64.GREEDY_LP_TOL[kv], f"row {r}: {lps[lp0:]} vs float64 {ref}"
-    f64.report(f"prev prompt ragged greedy decoder{decoder} d={d} rows={rows} kv={kv}", worst, f64.GREEDY_LP_TOL[kv])
+        assert err < h.GREEDY_LP_TOL[kv], f"row {r}: {lps[lp0:]} vs float64 {ref}"
+    h.report(f"prev prompt ragged greedy decoder{decoder} d={d} rows={rows} kv={kv}", worst, h.GREEDY_LP_TOL[kv])
 
 
 def test_deep_rows_stop_at_their_own_length(monkeypatch):
     """EOT declared as an id no row emits: every row runs to exactly Lp + max_depth ids on every greedy decoder."""
-    dims, wh, _ = f64.make_model(384, 6, 2051)
+    dims, wh, _ = h.make_model(384, 6, 2051)
     sp0 = synth.special_tokens(dims)
     sp = synth.SpecialTokens(sot=sp0.sot, lang=sp0.lang, transcribe=sp0.transcribe, notimestamps=sp0.notimestamps,
                              eot=sp0.n_vocab - 1, first_special=sp0.first_special, n_vocab=sp0.n_vocab, startofprev=sp0.startofprev)
-    _, waves = f64.windows(4, seed=5)
+    _, waves = h.windows(4, seed=5)
     prev = prev_lists(sp, 4, 40, seed=3)
     for decoder in (4, 6, 3):
-        f64.use_decoder(monkeypatch, decoder)
+        h.use_decoder(monkeypatch, decoder)
         sess = transcribe.Session(wh, max_windows=4, max_beams=1, max_text_len=45 + DEPTH + 1)
-        f64.use_decoder(monkeypatch, 0)
+        h.use_decoder(monkeypatch, 0)
         ids = sess.transcribe_windows_prev(waves, prev, sp, sp.is_special_bitmap(), beam_size=1, max_depth=DEPTH)
         assert sess.last_decoder() == decoder
         if any(sp.eot in t for t in ids):
@@ -96,14 +88,9 @@ def test_deep_rows_stop_at_their_own_length(monkeypatch):
         sess.close()
 
 
-def tiny_model(name="test-a"):
-    dims, w_np, w_t = synth.make_weights(name, seed=0)
-    return dims, model.Whisper(dims, w_np), w_t
-
-
 @pytest.mark.parametrize("beam_size", [1, 3])
 def test_empty_prev_is_bit_identical(beam_size):
-    dims, wh, _ = tiny_model()
+    dims, _, wh, *_ = h.named_model("test-a")
     sp = synth.special_tokens(dims)
     waves = [synth.waveform(48000, seed=40 + i) for i in range(4)]
     sess = transcribe.Session(wh, max_windows=4, max_beams=beam_size, max_text_len=4 + 20 + 1)
@@ -117,7 +104,7 @@ def test_empty_prev_is_bit_identical(beam_size):
 
 
 def test_ragged_batch_equals_each_window_alone_and_scoring():
-    dims, wh, _ = tiny_model()
+    dims, _, wh, *_ = h.named_model("test-a")
     sp = synth.special_tokens(dims)
     waves = [synth.waveform(48000, seed=60 + i) for i in range(6)]
     prev = prev_lists(sp, 6, 12, seed=9)
@@ -145,7 +132,7 @@ def oracle_rows(w_t, dims, sp, waves, prev, beam_size, max_depth):
 
 @pytest.mark.parametrize("name,host_decoder", [("test-a", 3), ("tiny.en", 3), ("test-d", 5)])
 def test_ragged_beam_device_host_oracle(name, host_decoder, monkeypatch):
-    dims, wh, w_t = tiny_model(name)
+    dims, _, wh, _, w_t, _ = h.named_model(name)
     sp = synth.special_tokens(dims)
     n = 4
     waves = [synth.waveform(48000, seed=80 + i) for i in range(n)]
@@ -154,9 +141,9 @@ def test_ragged_beam_device_host_oracle(name, host_decoder, monkeypatch):
     want = oracle_rows(w_t, dims, sp, waves, prev, beam_size, depth)
     runs = []
     for dec in ((6, host_decoder) if dims.n_text_state in (128, 384) else (host_decoder,)):
-        f64.use_decoder(monkeypatch, dec)
+        h.use_decoder(monkeypatch, dec)
         sess = transcribe.Session(wh, max_windows=n, max_beams=beam_size, max_text_len=14 + depth + 1)
-        f64.use_decoder(monkeypatch, 0)
+        h.use_decoder(monkeypatch, 0)
         got = sess.transcribe_windows_prev(waves, prev, sp, sp.is_special_bitmap(), beam_size=beam_size, max_depth=depth)
         assert sess.last_decoder() == dec
         for r, t in enumerate(got):
@@ -169,7 +156,7 @@ def test_ragged_beam_device_host_oracle(name, host_decoder, monkeypatch):
 
 
 def test_waveform_rule_vs_oracle_and_batched():
-    dims, wh, w_t = tiny_model()
+    dims, _, wh, _, w_t, _ = h.named_model("test-a")
     sp = synth.special_tokens(dims)
     win = o_audio.max_waveform_samples(dims.n_audio_ctx - 10)
     shift = win - 3 * 16000
@@ -197,7 +184,7 @@ def test_waveform_rule_vs_oracle_and_batched():
 
 
 def test_errors():
-    dims, wh, _ = tiny_model()
+    dims, _, wh, *_ = h.named_model("test-a")
     sp = synth.special_tokens(dims)
     waves = [synth.waveform(48000, seed=1)]
     sess = transcribe.Session(wh, max_windows=1, max_beams=1, max_text_len=12 + 8 + 1)
@@ -248,8 +235,6 @@ def test_errors():
 
 
 # ---------------------------------------------------------------- real shapes against tests/golden/tokens_prev_prompt.json
-GOLD = Path(__file__).resolve().parent / "golden" / "tokens_prev_prompt.json"
-LP_TOL = 2e-4   # test_real_shapes_gpu.py: GPU log-probs against the float32 oracle's at real shapes
 TIE_TOL = 1e-4  # ids are compared up to the first step whose oracle top-1/top-2 gap is below this
 
 
@@ -270,15 +255,15 @@ def _check_windows(sess, got, recs, beam):
         if beam == 1:
             m = min(n, len(g)) - lp0
             err = np.abs(lps[lp0:lp0 + m] - np.asarray(r["lps"][:m], dtype=np.float32)).max(initial=0.0)
-            assert err < LP_TOL, f"window {i}: log-prob error {err}"
+            assert err < h.REAL_LP_TOL, f"window {i}: log-prob error {err}"
 
 
 @pytest.mark.parametrize("case", ["tiny.en-f32", "tiny.en-f16", "tiny.en-beam", "small.en-f32", "small.en-f16", "small.en-beam",
                                   "tiny.en-native", "ragged"])
 def test_real_shapes_vs_golden(case):
     """Every window decoded from the fixture's prompt (one ragged batch per case), ids up to the first near tie and
-    log-probs within LP_TOL; for the waveform-rule cases without a near tie also the merged ids of waveform_to_tokens."""
-    g = json.loads(GOLD.read_text())[case]
+    log-probs within harness.REAL_LP_TOL; for the waveform-rule cases without a near tie also the merged ids of waveform_to_tokens."""
+    g = h.golden("tokens_prev_prompt")[case]
     dims, w_np, _ = synth.make_weights(g["model"], seed=0)
     sp = synth.special_tokens(dims)
     wh = model.Whisper(dims, w_np)
@@ -291,10 +276,9 @@ def test_real_shapes_vs_golden(case):
         wave = synth.waveform(1120000, seed=2024, kind="mix") if g["waveform"] == "long" else synth.chunk_waveform(0)
         waves = [wave[r["bounds"][0]:r["bounds"][1]] for r in recs]
     prev = [r["prompt"][1:-4] if len(r["prompt"]) > 4 else [] for r in recs]
-    kv = ffi.WB_KV_F16 if g["kv"] == "f16" else ffi.WB_KV_F32
     sess = transcribe.Session(wh, max_windows=len(recs), max_beams=max(g["beam"], 1),
                               max_text_len=max(len(r["prompt"]) for r in recs) + g["depth"] + 1,
-                              kv_dtype=kv, windows="native" if g.get("native") else "reference")
+                              kv_dtype=h.kv_code(g["kv"]), windows="native" if g.get("native") else "reference")
     got = sess.transcribe_windows_prev(waves, prev, sp, sp.is_special_bitmap(), beam_size=g["beam"], max_depth=g["depth"])
     _check_windows(sess, got, recs, g["beam"])
     if wave is not None and all(_prefix_until_tie(r) == len(r["tokens"]) for r in recs):

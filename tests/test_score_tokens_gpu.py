@@ -1,7 +1,7 @@
 """GPU tests (-m gpu) of teacher-forced token scoring (wb_session_score_tokens, Session.score_tokens): forward_decoder
 (mod.rs:131-157) + log_softmax (transcribe.rs:276) at every position of given sequences, in one sequence-parallel pass.
 
-  1. against float64 (oracle.model.forward_decoder on the real-width models of test_f64_reference_gpu.py): d = 384, 768,
+  1. against float64 (oracle.model.forward_decoder on the real-width models of harness.make_model): d = 384, 768,
      1280, fp32 and fp16 K/V, reference windows of T = 6, 64, 65, 750 and native windows of T = 1500 and 1025, random
      sequences (special ids included) of lengths around the 64-row tiles up to n_text_ctx, several on one window;
   2. the special-token mask of the beam rule (greedy_path_log_probs from the prompt on; -inf targets at j = 4, 5 only);
@@ -11,64 +11,25 @@
   5. sequence parallel and independent: a fixed launch count, bit-identical values alone, in a batch and as prefixes;
   6. the session's decode results are untouched;
   7. every error code of the header contract."""
-import json
-from pathlib import Path
-
 import numpy as np
 import pytest
 import torch
 
-import test_f64_reference_gpu as f64
+import harness as h
 import wb200  # noqa: F401
-from oracle import model as o_model, synth, transcribe as o_tr
+from harness import GAP, check_rows, is_special_of, random_seqs
+from oracle import synth
 from whisper_burn_b200 import ffi, model, transcribe
 
 pytestmark = pytest.mark.gpu
-G = Path(__file__).resolve().parent / "golden"
-LP_TOL = 2e-4      # test_real_shapes_gpu.py: GPU log-probs against the float32 oracle's at real shapes
-GAP = 1e-4         # arg-max compared where the reference's top-1 / top-2 gap is at least this
-LENGTHS = (1, 2, 63, 64, 65, 127, 128, 129, 448)
-
-
-def is_special_of(sp):
-    return (np.arange(sp.n_vocab) >= sp.first_special).astype(np.uint8)
-
-
-def random_seqs(V, seed, lengths=LENGTHS):
-    rng = np.random.default_rng(seed)
-    return [[int(t) for t in rng.integers(0, V, size=n)] for n in lengths]
-
-
-def f64_rows(w64, dims, xa, seq, kv, ln_eps_mode="outside"):
-    """float64 log-softmax rows of every position of seq: [len, V]"""
-    logits = o_model.forward_decoder(w64, dims, torch.tensor([seq], dtype=torch.int64), xa,
-                                     opts=o_model.OracleOptions(ln_eps_mode=ln_eps_mode, kv_dtype=kv))
-    return o_model.log_softmax_last(logits)[0].numpy()
-
-
-def check_rows(lp, am, ref, seq, kv, what, tol=None):
-    """lp / argmax of one sequence against its float64 rows, within tol (default GREEDY_LP_TOL[kv]; a tol given compares
-    arg-maxes only where the float64 top-1 / top-2 gap is at least 2 tol as well); returns the worst |error|"""
-    assert lp[0] == 0.0 and am[0] == -1
-    if len(seq) == 1:
-        return 0.0
-    want = np.array([ref[j - 1][seq[j]] for j in range(1, len(seq))])
-    err = float(np.abs(lp[1:].astype(np.float64) - want).max())
-    assert err < (tol or f64.GREEDY_LP_TOL[kv]), f"{what}: worst log-prob error {err}"
-    gap = GAP if tol is None else max(GAP, 2 * tol)
-    for j in range(1, len(seq)):
-        top2 = np.sort(ref[j - 1])[-2:]
-        if top2[1] - top2[0] >= gap:
-            assert am[j] == int(ref[j - 1].argmax()), f"{what} position {j}: arg-max {am[j]} vs {int(ref[j - 1].argmax())}"
-    return err
 
 
 # ---------------------------------------------------------------- 1. against float64
 def score_vs_f64(d, kv, windows, Ts, waves, seed):
-    dims, wh, w64 = f64.make_model(d, d // 64, 2051)
-    sess = transcribe.Session(wh, max_windows=len(waves), max_beams=1, max_text_len=8, kv_dtype=f64.kv_code(kv), windows=windows)
+    dims, wh, w64 = h.make_model(d, d // 64, 2051)
+    sess = transcribe.Session(wh, max_windows=len(waves), max_beams=1, max_text_len=8, kv_dtype=h.kv_code(kv), windows=windows)
     sess.encode_waveforms(waves)
-    xa = f64.encoder_outputs64(sess, Ts)
+    xa = h.encoder_outputs64(sess, Ts)
     seqs = random_seqs(dims.n_vocab, seed)
     wins = [i % len(waves) for i in range(len(seqs))]
     out = sess.score_tokens(seqs, wins)
@@ -76,15 +37,15 @@ def score_vs_f64(d, kv, windows, Ts, waves, seed):
     for i, (seq, w) in enumerate(zip(seqs, wins)):
         lp, am = out[i]
         assert lp.dtype == np.float32 and am.dtype == np.int64 and len(lp) == len(seq)
-        ref = f64_rows(w64, dims, xa[w], seq, kv) if len(seq) > 1 else None
+        ref = h.forward_rows(w64, dims, [xa[w]], [seq], kv)[0] if len(seq) > 1 else None
         worst = max(worst, check_rows(lp, am, ref, seq, kv, f"d={d} kv={kv} T={Ts[w]} len={len(seq)}"))
-    f64.report(f"score_tokens d={d} {windows} windows T={sorted(set(Ts))} kv={kv}", worst, f64.GREEDY_LP_TOL[kv])
+    h.report(f"score_tokens d={d} {windows} windows T={sorted(set(Ts))} kv={kv}", worst, h.GREEDY_LP_TOL[kv])
 
 
 @pytest.mark.parametrize("kv", ["f32", "f16"])
 @pytest.mark.parametrize("d", [384, 768, 1280])
 def test_score_vs_float64(d, kv):
-    Ts, waves = f64.windows(4, seed=7 * d)
+    Ts, waves = h.windows(4, seed=7 * d)
     score_vs_f64(d, kv, "reference", Ts, waves, seed=d)
 
 
@@ -98,33 +59,26 @@ def test_score_native_windows_vs_float64(kv):
 # ---------------------------------------------------------------- 2. the special-token mask
 @pytest.mark.parametrize("kv", ["f32", "f16"])
 def test_mask_rule_matches_greedy_path_log_probs(kv):
-    dims, wh, w64 = f64.make_model(384, 6, 2051)
+    dims, wh, w64 = h.make_model(384, 6, 2051)
     sp = synth.special_tokens(dims)
-    Ts, waves = f64.windows(2, seed=17)
-    sess = transcribe.Session(wh, max_windows=2, max_beams=1, max_text_len=8, kv_dtype=f64.kv_code(kv))
+    Ts, waves = h.windows(2, seed=17)
+    sess = transcribe.Session(wh, max_windows=2, max_beams=1, max_text_len=8, kv_dtype=h.kv_code(kv))
     sess.encode_waveforms(waves)
-    xa = f64.encoder_outputs64(sess, Ts)
-    rng = np.random.default_rng(9)
-    specials = list(range(sp.first_special, dims.n_vocab))
-    seqs = []
-    for r in range(4):
-        body = [int(t) for t in rng.integers(0, sp.first_special, size=20 + 7 * r)]
-        body[0], body[1], body[2], body[5] = specials[r], specials[r + 1], specials[r + 2], specials[r + 3]  # j = 4, 5, 6, 9
-        seqs.append(list(sp.prompt()) + body)
+    xa = h.encoder_outputs64(sess, Ts)
+    seqs = h.masked_seqs(sp, 9)   # special ids at j = 4, 5, 6, 9
     wins = [r % 2 for r in range(4)]
     out = sess.score_tokens(seqs, wins, apply_special_mask=True, is_special=is_special_of(sp))
     worst = 0.0
     for seq, w, (lp, _) in zip(seqs, wins, out):
         assert np.isneginf(lp[4]) and np.isneginf(lp[5]), lp[:8]
         assert np.all(np.isfinite(lp[6:])), lp[6:12]
-        rows = o_tr.greedy_path_log_probs(w64, dims, sp, xa[w], seq, opts=o_model.OracleOptions(kv_dtype=kv)).numpy()
-        want = np.array([rows[j - 4][seq[j]] for j in range(4, len(seq))])
+        want = h.along(h.path_rows(w64, dims, sp, xa[w], seq, kv), seq)
         assert np.array_equal(np.isneginf(want), np.isneginf(lp[4:]))
         ok = np.isfinite(want)
         err = float(np.abs(lp[4:][ok].astype(np.float64) - want[ok]).max())
         worst = max(worst, err)
-        assert err < f64.GREEDY_LP_TOL[kv]
-    f64.report(f"score_tokens masked rows d=384 kv={kv}", worst, f64.GREEDY_LP_TOL[kv])
+        assert err < h.GREEDY_LP_TOL[kv]
+    h.report(f"score_tokens masked rows d=384 kv={kv}", worst, h.GREEDY_LP_TOL[kv])
 
 
 # ---------------------------------------------------------------- 3. agreement with decoding
@@ -137,7 +91,7 @@ def close_to_decoding(sess, ids, sp, kv, masked=True, greedy=False, gaps=None):
         ok = ~np.isnan(want)   # an EOT the greedy loop's rules appended has no log-prob
         err = float(np.abs(got[ok] - want[ok]).max(initial=0.0))
         worst = max(worst, err)
-        assert err < f64.GREEDY_LP_TOL[kv], f"row {r}: scored {got} vs decoded {want}"
+        assert err < h.GREEDY_LP_TOL[kv], f"row {r}: scored {got} vs decoded {want}"
         if greedy:
             for j in range(4, len(t)):
                 if ok[j - 4] and (gaps is None or gaps[r][j] >= GAP):
@@ -151,7 +105,7 @@ def f64_gaps(w64, dims, sess, ids, kv):
     gaps = []
     for r, t in enumerate(ids):
         xa = torch.from_numpy(sess.get_encoder_output(r)).double()[None]
-        rows = o_tr.greedy_path_log_probs(w64, dims, sp, xa, t, opts=o_model.OracleOptions(kv_dtype=kv)).numpy()
+        rows = h.path_rows(w64, dims, sp, xa, t, kv)
         g = np.full(len(t), np.inf)
         for j in range(4, len(t)):
             top2 = np.sort(rows[j - 4])[-2:]
@@ -162,35 +116,30 @@ def f64_gaps(w64, dims, sess, ids, kv):
 
 @pytest.mark.parametrize("kv", ["f32", "f16"])
 def test_scores_agree_with_decoding(kv, monkeypatch):
-    beam_gold = json.loads((G / "tokens_beam.json").read_text())
-    chunk = synth.chunk_waveform(0)
     for name in ("test-a", "tiny.en"):
-        dims, w_np, w_t = synth.make_weights(name, seed=0)
-        sp = synth.special_tokens(dims)
-        wh = model.Whisper(dims, w_np)
-        w64 = o_model.as_dtype(w_t)
-        waves = [chunk[off:off + m] for off, m in beam_gold["pool"][:4]]
-        sess = transcribe.Session(wh, max_windows=4, max_beams=5, max_text_len=40, kv_dtype=f64.kv_code(kv))
+        dims, sp, wh, _, _, w64 = h.named_model(name, f64=True)
+        waves = h.pool_waves(h.golden("tokens_beam"), 4)
+        sess = transcribe.Session(wh, max_windows=4, max_beams=5, max_text_len=40, kv_dtype=h.kv_code(kv))
         ids = sess.transcribe_windows(waves, sp, is_special_of(sp), beam_size=1, max_depth=30)
         worst = close_to_decoding(sess, ids, sp, kv, greedy=True, gaps=f64_gaps(w64, dims, sess, ids, kv))
-        f64.report(f"score_tokens vs greedy last_logprobs {name} kv={kv}", worst, f64.GREEDY_LP_TOL[kv])
+        h.report(f"score_tokens vs greedy last_logprobs {name} kv={kv}", worst, h.GREEDY_LP_TOL[kv])
         ids = sess.transcribe_windows(waves, sp, is_special_of(sp), beam_size=5, max_depth=30)
         assert sess.last_decoder() == 6
         worst = close_to_decoding(sess, ids, sp, kv)
-        f64.report(f"score_tokens vs device beam last_logprobs {name} kv={kv}", worst, f64.GREEDY_LP_TOL[kv])
-        f64.use_decoder(monkeypatch, 3)
-        hs = transcribe.Session(wh, max_windows=4, max_beams=5, max_text_len=40, kv_dtype=f64.kv_code(kv))
-        f64.use_decoder(monkeypatch, 0)
+        h.report(f"score_tokens vs device beam last_logprobs {name} kv={kv}", worst, h.GREEDY_LP_TOL[kv])
+        h.use_decoder(monkeypatch, 3)
+        hs = transcribe.Session(wh, max_windows=4, max_beams=5, max_text_len=40, kv_dtype=h.kv_code(kv))
+        h.use_decoder(monkeypatch, 0)
         hids = hs.transcribe_windows(waves, sp, is_special_of(sp), beam_size=5, max_depth=30)
         assert hs.last_decoder() == 3
         worst = close_to_decoding(hs, hids, sp, kv)
-        f64.report(f"score_tokens vs host beam last_logprobs {name} kv={kv}", worst, f64.GREEDY_LP_TOL[kv])
+        h.report(f"score_tokens vs host beam last_logprobs {name} kv={kv}", worst, h.GREEDY_LP_TOL[kv])
         hs.close()
-        loop = transcribe.Session(wh, max_windows=4, max_beams=1, max_text_len=40, kv_dtype=f64.kv_code(kv), search="greedy_loop")
+        loop = transcribe.Session(wh, max_windows=4, max_beams=1, max_text_len=40, kv_dtype=h.kv_code(kv), search="greedy_loop")
         lids = loop.transcribe_windows(waves, sp, None, beam_size=1, max_depth=30)
         lids = [t[:min(len(t), 40)] for t in lids]   # a context-stop EOT past the token buffer is not scored
         worst = close_to_decoding(loop, lids, sp, kv, masked=False)
-        f64.report(f"score_tokens unmasked vs greedy loop last_logprobs {name} kv={kv}", worst, f64.GREEDY_LP_TOL[kv])
+        h.report(f"score_tokens unmasked vs greedy loop last_logprobs {name} kv={kv}", worst, h.GREEDY_LP_TOL[kv])
         loop.close()
         sess.close()
 
@@ -210,27 +159,22 @@ def check_fixture_rows(sess, sp, recs, with_lp):
                     assert am[j] == top_ids[0]
                 err = abs(float(lp[j]) - top_lp[0])
                 worst = max(worst, err)
-                assert err < LP_TOL, f"row {r} position {j}: {lp[j]} vs oracle {top_lp[0]}"
+                assert err < h.REAL_LP_TOL, f"row {r} position {j}: {lp[j]} vs oracle {top_lp[0]}"
     return worst
 
 
 def test_real_shapes_vs_golden():
-    g = json.loads((G / "tokens_real.json").read_text())
+    g = h.golden("tokens_real")
     dims, w_np, _ = synth.make_weights("small.en", seed=0)
     sp = synth.special_tokens(dims)
     wh = model.Whisper(dims, w_np)
     del w_np
     for kv in ("f32", "f16"):
-        waves, recs = [], []
-        for c, rec in enumerate(g["small.en"]["chunks"]):
-            chunk = synth.chunk_waveform(c)
-            for (s, e), r in zip(rec["bounds"], rec[kv]):
-                waves.append(chunk[s:e])
-                recs.append(r)
-        sess = transcribe.Session(wh, max_windows=24, max_beams=1, max_text_len=8, kv_dtype=f64.kv_code(kv))
+        waves, recs = h.real_windows("small.en", kv)
+        sess = transcribe.Session(wh, max_windows=24, max_beams=1, max_text_len=8, kv_dtype=h.kv_code(kv))
         sess.encode_waveforms(waves)
         worst = check_fixture_rows(sess, sp, recs, with_lp=kv == "f32")
-        f64.report(f"score_tokens small.en 24 windows kv={kv} vs golden", worst, LP_TOL)
+        h.report(f"score_tokens small.en 24 windows kv={kv} vs golden", worst, h.REAL_LP_TOL)
         sess.close()
     del sess, wh
     gm = g["medium"]
@@ -241,19 +185,19 @@ def test_real_shapes_vs_golden():
     chunk = synth.chunk_waveform(0)
     sess = transcribe.Session(wh, max_windows=3, max_beams=1, max_text_len=8)
     sess.encode_waveforms([chunk[s:e] for s, e in gm["bounds"]])
-    f64.report("score_tokens medium chunk 0 f32 vs golden", check_fixture_rows(sess, sp, gm["f32"], with_lp=True), LP_TOL)
+    h.report("score_tokens medium chunk 0 f32 vs golden", check_fixture_rows(sess, sp, gm["f32"], with_lp=True), h.REAL_LP_TOL)
 
 
 # ---------------------------------------------------------------- 5-7. shape of the pass, state, contract
 @pytest.fixture(scope="module")
 def small_model():
-    dims, wh, _ = f64.make_model(384, 6, 2051)
+    dims, wh, _ = h.make_model(384, 6, 2051)
     return dims, wh
 
 
 def test_launch_count_and_independence(small_model):
     dims, wh = small_model
-    Ts, waves = f64.windows(2, seed=23)
+    Ts, waves = h.windows(2, seed=23)
     sess = transcribe.Session(wh, max_windows=2, max_beams=1, max_text_len=8)
     sess.encode_waveforms(waves)
     lib = ffi.lib()
@@ -276,9 +220,9 @@ def test_launch_count_and_independence(small_model):
 def test_decode_state_untouched(small_model):
     dims, wh = small_model
     sp = synth.special_tokens(dims)
-    Ts, waves = f64.windows(3, seed=29)
-    sess = transcribe.Session(wh, max_windows=3, max_beams=1, max_text_len=4 + f64.DEPTH + 1)
-    ids = sess.transcribe_windows(waves, sp, is_special_of(sp), beam_size=1, max_depth=f64.DEPTH)
+    Ts, waves = h.windows(3, seed=29)
+    sess = transcribe.Session(wh, max_windows=3, max_beams=1, max_text_len=4 + h.DEPTH + 1)
+    ids = sess.transcribe_windows(waves, sp, is_special_of(sp), beam_size=1, max_depth=h.DEPTH)
     before = ([sess.last_logprobs(r) for r in range(3)], sess.last_topk(3, 1), sess.last_decoder())
     sess.score_tokens(ids + random_seqs(dims.n_vocab, 2, lengths=(448,)), [0, 1, 2, 0], apply_special_mask=True,
                       is_special=is_special_of(sp))
@@ -287,7 +231,7 @@ def test_decode_state_untouched(small_model):
         assert np.array_equal(a, b, equal_nan=True)
     assert np.array_equal(before[1][0], after[1][0]) and np.array_equal(before[1][1], after[1][1])
     assert before[2] == after[2]
-    assert sess.transcribe_windows(waves, sp, is_special_of(sp), beam_size=1, max_depth=f64.DEPTH) == ids
+    assert sess.transcribe_windows(waves, sp, is_special_of(sp), beam_size=1, max_depth=h.DEPTH) == ids
 
 
 def raw_score(sess, seqs, wins, mask=0, special=None):
@@ -303,7 +247,7 @@ def test_error_codes(small_model):
     dims, wh = small_model
     sp = synth.special_tokens(dims)
     V, n_ctx = dims.n_vocab, dims.n_text_ctx
-    Ts, waves = f64.windows(2, seed=31)
+    Ts, waves = h.windows(2, seed=31)
     sess = transcribe.Session(wh, max_windows=2, max_beams=1, max_text_len=8)
     assert raw_score(sess, [[1, 2]], [0]) == ffi.WB_ERR_STATE
     sess.encode_waveforms(waves)
@@ -318,8 +262,8 @@ def test_error_codes(small_model):
     assert raw_score(sess, [[1, 2]], [0], mask=1, special=is_special_of(sp)) == ffi.WB_OK
     sess.close()
     # the non-fp16-exact model of test_non_fp16_exact_weights_use_fp32_storage
-    dims_x, w_np, _ = synth.make_weights("test-a", seed=3)
-    wx = model.Whisper(dims_x, {k: (v * np.float32(1.0001) if v.ndim else v) for k, v in w_np.items()})
+    dims_x, w_np, _, _ = h.synthetic("test-a", 3, exact=False, f64=False)
+    wx = model.Whisper(dims_x, w_np)
     assert not wx.weights_fp16_exact
     sx = transcribe.Session(wx, max_windows=1, max_beams=1, max_text_len=8)
     sx.encode_waveforms(waves[:1])

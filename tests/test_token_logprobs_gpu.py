@@ -3,9 +3,9 @@ BeamSearchToken.log_prob of every id the reference's search returns (src/transcr
 
   1. on every path a row has one value per id, 0 for the 4 prompt ids, finite and <= 0 elsewhere except a rule's EOT;
   2. greedy on decoder3 / 4 / 5 / 6, fp32 and fp16 K/V: each value against float64 teacher forcing of the GPU's own ids
-     (greedy_path_log_probs on the reduced-depth real-width models of test_f64_reference_gpu.py, its GREEDY_LP_TOL);
+     (greedy_path_log_probs on the reduced-depth real-width models of harness.make_model, harness.GREEDY_LP_TOL);
   3. real shapes: small.en 8 chunks and medium chunk 0 against the top-1 log-probs of tests/golden/tokens_real.json, the
-     native windows against tokens_native.json (LP_TOL of test_real_shapes_gpu.py), wherever the ids match;
+     native windows against tokens_native.json (harness.REAL_LP_TOL), wherever the ids match;
   4. the greedy loop on every decoder (the cases of test_greedy_loop_gpu.py): NaN exactly at the rule-appended EOTs, the
      arg-max values against the oracle loop's unmasked log-softmax;
   5. beam: the device search (decoder6) and the host search (decoder5, decoder3) against float64 teacher forcing, and device
@@ -14,66 +14,20 @@ BeamSearchToken.log_prob of every id the reference's search returns (src/transcr
   7. the getter's contract."""
 import ctypes as C
 import dataclasses
-import json
 import math
-from pathlib import Path
 
 import numpy as np
 import pytest
 import torch
 
+import harness as h
 import oracle_logprobs as olp
-import test_f64_reference_gpu as f64
-import test_greedy_loop_gpu as gl
 import wb200  # noqa: F401
-from oracle import audio as o_audio, model as o_model, synth, transcribe as o_tr
+from harness import check_against_f64, is_special_of, pool_waves, rows_of
+from oracle import audio as o_audio, model as o_model, synth
 from whisper_burn_b200 import ffi, model, transcribe
 
 pytestmark = pytest.mark.gpu
-G = Path(__file__).resolve().parent / "golden"
-LP_TOL = 2e-4   # test_real_shapes_gpu.py: GPU log-probs against the float32 oracle's at real shapes
-
-
-def is_special_of(sp):
-    return (np.arange(sp.n_vocab) >= sp.first_special).astype(np.uint8)
-
-
-def rows_of(sess, ids, rule_eots=None):
-    """last_logprobs of every row, checked for shape, prompt and range; rule_eots[r]: the positions of row r that may be
-    NaN (an EOT a rule appended)."""
-    out = []
-    for r, t in enumerate(ids):
-        lps = sess.last_logprobs(r)
-        assert lps.dtype == np.float32 and len(lps) == len(t), f"row {r}"
-        assert np.all(lps[:4] == 0.0), f"row {r}: prompt log-probs {lps[:4]}"
-        allowed = set(rule_eots[r]) if rule_eots else set()
-        for j in range(4, len(t)):
-            if j in allowed:
-                continue
-            assert math.isfinite(lps[j]) and lps[j] <= 0.0, f"row {r} position {j}: {lps[j]}"
-        out.append(lps)
-    return out
-
-
-def teacher_forced(w, dims, sp, xa, ids, kv, unmask=False, ln_eps_mode="outside"):
-    """The log-prob of ids[j], j >= 4, given ids[:j]: one greedy_path_log_probs pass over the path (mask of the beam rule, or
-    none for the greedy loop)."""
-    rows = o_tr.greedy_path_log_probs(w, dims, olp.unmasked(sp) if unmask else sp, xa, ids,
-                                      opts=o_model.OracleOptions(ln_eps_mode=ln_eps_mode, kv_dtype=kv))
-    return np.array([float(rows[j - 4][ids[j]]) for j in range(4, len(ids))])
-
-
-def check_against_f64(sess, w64, dims, sp, ids, lps, kv, unmask=False, skip_nan=False, ln_eps_mode="outside"):
-    worst = 0.0
-    for r, t in enumerate(ids):
-        xa = torch.from_numpy(sess.get_encoder_output(r)).double()[None]
-        ref = teacher_forced(w64, dims, sp, xa, t, kv, unmask, ln_eps_mode)
-        got = lps[r][4:].astype(np.float64)
-        ok = ~np.isnan(got) if skip_nan else np.ones(len(got), bool)
-        err = np.abs(got[ok] - ref[ok]).max(initial=0.0)
-        worst = max(worst, float(err))
-        assert err < f64.GREEDY_LP_TOL[kv], f"row {r}: log-probs {got} vs float64 {ref}"
-    return worst
 
 
 # ---------------------------------------------------------------- 2. greedy, every decoder, against float64
@@ -84,21 +38,21 @@ GREEDY_CASES = [(4, 384, 6, 4), (6, 384, 6, 9), (5, 256, 4, 9), (3, 384, 6, 4)]
 @pytest.mark.parametrize("kv", ["f32", "f16"])
 @pytest.mark.parametrize("decoder,d,H,rows", GREEDY_CASES)
 def test_greedy_logprobs_every_decoder_vs_float64(decoder, d, H, rows, kv, monkeypatch):
-    dims, wh, w64 = f64.make_model(d, H, 2051)
+    dims, wh, w64 = h.make_model(d, H, 2051)
     sp = synth.special_tokens(dims)
-    Ts, waves = f64.windows(rows, seed=11 * d + rows)
-    f64.use_decoder(monkeypatch, decoder)
-    sess = transcribe.Session(wh, max_windows=rows, max_beams=1, max_text_len=4 + f64.DEPTH + 1, kv_dtype=f64.kv_code(kv))
-    f64.use_decoder(monkeypatch, 0)
-    ids = sess.transcribe_windows(waves, sp, sp.is_special_bitmap(), beam_size=1, max_depth=f64.DEPTH)
+    Ts, waves = h.windows(rows, seed=11 * d + rows)
+    h.use_decoder(monkeypatch, decoder)
+    sess = transcribe.Session(wh, max_windows=rows, max_beams=1, max_text_len=4 + h.DEPTH + 1, kv_dtype=h.kv_code(kv))
+    h.use_decoder(monkeypatch, 0)
+    ids = sess.transcribe_windows(waves, sp, sp.is_special_bitmap(), beam_size=1, max_depth=h.DEPTH)
     assert sess.last_decoder() == decoder
     lps = rows_of(sess, ids)
     for r, t in enumerate(ids):   # the greedy value of the last step is what wb_session_last_topk reports
-        if len(t) == 4 + f64.DEPTH:
+        if len(t) == 4 + h.DEPTH:
             tk, tl = sess.last_topk(rows, 1)
             assert int(tk[r, 0]) == t[-1] and float(tl[r, 0]) == float(lps[r][-1])
     worst = check_against_f64(sess, w64, dims, sp, ids, lps, kv)
-    f64.report(f"last_logprobs greedy decoder{decoder} d={d} rows={rows} kv={kv}", worst, f64.GREEDY_LP_TOL[kv])
+    h.report(f"last_logprobs greedy decoder{decoder} d={d} rows={rows} kv={kv}", worst, h.GREEDY_LP_TOL[kv])
 
 
 # ---------------------------------------------------------------- 3. real shapes against the fixtures' top-1 log-probs
@@ -112,26 +66,21 @@ def check_top1(got_ids, lps, recs):
                 break
             err = abs(float(lps[r][j]) - top_lp[0])
             worst = max(worst, err)
-            assert err < LP_TOL, f"row {r} position {j}: {lps[r][j]} vs oracle {top_lp[0]}"
+            assert err < h.REAL_LP_TOL, f"row {r} position {j}: {lps[r][j]} vs oracle {top_lp[0]}"
     return worst
 
 
 def test_small_en_8_chunks_and_medium_vs_golden_top1():
-    g = json.loads((G / "tokens_real.json").read_text())
+    g = h.golden("tokens_real")
     dims, w_np, _ = synth.make_weights("small.en", seed=0)
     sp = synth.special_tokens(dims)
     wh = model.Whisper(dims, w_np)
     del w_np
-    waves, recs = [], []
-    for c, rec in enumerate(g["small.en"]["chunks"]):
-        chunk = synth.chunk_waveform(c)
-        for (s, e), r in zip(rec["bounds"], rec["f32"]):
-            waves.append(chunk[s:e])
-            recs.append(r)
+    waves, recs = h.real_windows("small.en", "f32")
     sess = transcribe.Session(wh, max_windows=24, max_beams=1, max_text_len=105)
     ids = sess.transcribe_windows(waves, sp, is_special_of(sp), beam_size=1, max_depth=100)
     assert sess.last_decoder() == 5
-    f64.report("last_logprobs small.en 24 windows greedy f32 vs golden top-1", check_top1(ids, rows_of(sess, ids), recs), LP_TOL)
+    h.report("last_logprobs small.en 24 windows greedy f32 vs golden top-1", check_top1(ids, rows_of(sess, ids), recs), h.REAL_LP_TOL)
     sess.close()
     del sess, wh
     gm = g["medium"]
@@ -143,23 +92,23 @@ def test_small_en_8_chunks_and_medium_vs_golden_top1():
     sess = transcribe.Session(wh, max_windows=3, max_beams=1, max_text_len=35)
     ids = sess.transcribe_windows([chunk[s:e] for s, e in gm["bounds"]], sp, is_special_of(sp), beam_size=1, max_depth=30)
     assert sess.last_decoder() == 5
-    f64.report("last_logprobs medium chunk 0 greedy f32 vs golden top-1", check_top1(ids, rows_of(sess, ids), gm["f32"]), LP_TOL)
+    h.report("last_logprobs medium chunk 0 greedy f32 vs golden top-1", check_top1(ids, rows_of(sess, ids), gm["f32"]), h.REAL_LP_TOL)
 
 
 @pytest.mark.parametrize("case,max_windows", [("tiny.en", 4), ("small.en", 2)])
 def test_native_windows_vs_golden_top1(case, max_windows):
-    g = json.loads((G / "tokens_native.json").read_text())[case]
+    g = h.golden("tokens_native")[case]
     dims, w_np, _ = synth.make_weights(case, seed=0)
     sp = synth.special_tokens(dims)
     wh = model.Whisper(dims, w_np)
     del w_np
     for kv in ("f32", "f16"):
-        sess = transcribe.Session(wh, max_windows=max_windows, max_beams=1, max_text_len=105, kv_dtype=f64.kv_code(kv),
+        sess = transcribe.Session(wh, max_windows=max_windows, max_beams=1, max_text_len=105, kv_dtype=h.kv_code(kv),
                                   windows="native")
         waves = [synth.chunk_waveform(c)[:n] for c, n in g["windows"]]
         ids = sess.transcribe_windows(waves, sp, is_special_of(sp), beam_size=1, max_depth=100)
-        f64.report(f"last_logprobs native {case} greedy kv={kv} vs golden top-1", check_top1(ids, rows_of(sess, ids), g[kv]),
-                   LP_TOL)
+        h.report(f"last_logprobs native {case} greedy kv={kv} vs golden top-1", check_top1(ids, rows_of(sess, ids), g[kv]),
+                   h.REAL_LP_TOL)
         sess.close()
 
 
@@ -170,24 +119,24 @@ _LOOP = {}
 def loop_oracle(name, i, sp, max_depth, kv):
     key = (name, i, sp.eot, max_depth, kv)
     if key not in _LOOP:
-        dims, w_t, _ = gl.weights(name)
+        dims, _, _, _, w_t, _ = h.loop_model(name)
         tr = {}
-        ids, lps = olp.greedy_loop_logprobs(w_t, dims, sp, o_audio.prep_audio(torch.from_numpy(gl.window(i))[None]), max_depth,
+        ids, lps = olp.greedy_loop_logprobs(w_t, dims, sp, o_audio.prep_audio(torch.from_numpy(h.loop_window(i))[None]), max_depth,
                                             o_model.OracleOptions(kv_dtype=kv), trace=tr)
         _LOOP[key] = (ids, lps, tr)
     return _LOOP[key]
 
 
 @pytest.mark.parametrize("kv", ["f32", "f16"])
-@pytest.mark.parametrize("dec,name,n,t_max,rules", gl.CASES)
+@pytest.mark.parametrize("dec,name,n,t_max,rules", h.LOOP_CASES)
 def test_greedy_loop_logprobs(monkeypatch, dec, name, n, t_max, rules, kv):
-    dims, _, _ = gl.weights(name)
-    sp = dataclasses.replace(synth.special_tokens(dims), eot=gl.EOT_ID)
+    dims = h.loop_model(name).dims
+    sp = dataclasses.replace(synth.special_tokens(dims), eot=h.LOOP_EOT_ID)
     monkeypatch.setenv("WB200_DECODER", str(dec))
-    s = gl.session(name, n, t_max, kv)
+    s = h.loop_session(name, n, t_max, kv)
     monkeypatch.delenv("WB200_DECODER")
-    waves = [gl.window(i) for i in range(n)]
-    tol = f64.GREEDY_LP_TOL[kv]
+    waves = [h.loop_window(i) for i in range(n)]
+    tol = h.GREEDY_LP_TOL[kv]
     stops, worst = set(), 0.0
     for max_depth in (t_max - 4, 3):
         got = s.transcribe_windows(waves, sp, None, beam_size=1, max_depth=max_depth)
@@ -197,7 +146,7 @@ def test_greedy_loop_logprobs(monkeypatch, dec, name, n, t_max, rules, kv):
             want, want_lp, tr = loop_oracle(name, i, sp, max_depth, kv)
             stops.add(tr["stop"])
             if got[i] != want:   # a near tie the GPU resolved the other way (test_greedy_loop_gpu.py): compare the prefix
-                assert gl.same_up_to_ties(got[i], want, tr)
+                assert h.same_up_to_ties(got[i], want, tr)
                 n_common = min(len(got[i]), len(want))
                 m = next((j for j in range(n_common) if got[i][j] != want[j]), n_common)
                 a, b = lps[i][4:m].astype(np.float64), np.asarray(want_lp[4:m])
@@ -209,25 +158,15 @@ def test_greedy_loop_logprobs(monkeypatch, dec, name, n, t_max, rules, kv):
             worst = max(worst, float(err))
             assert err < tol, f"window {i}: {lps[i]} vs oracle {want_lp}"
     assert stops == rules, stops
-    f64.report(f"last_logprobs greedy loop decoder{dec} {name} kv={kv} vs oracle", worst, tol)
+    h.report(f"last_logprobs greedy loop decoder{dec} {name} kv={kv} vs oracle", worst, tol)
     s.close()
 
 
 # ---------------------------------------------------------------- 5. beam: device and host search
-@pytest.fixture(scope="module")
-def beam_gold():
-    return json.loads((G / "tokens_beam.json").read_text())
-
-
-def pool_waves(gold, n):
-    chunk = synth.chunk_waveform(0)
-    return [chunk[off:off + m] for off, m in (gold["pool"][i % len(gold["pool"])] for i in range(n))]
-
-
 def beam_run(wh, waves, sp, b, depth, kv, monkeypatch, decoder=0):
-    f64.use_decoder(monkeypatch, decoder)
-    sess = transcribe.Session(wh, max_windows=len(waves), max_beams=7, max_text_len=4 + depth + 1, kv_dtype=f64.kv_code(kv))
-    f64.use_decoder(monkeypatch, 0)
+    h.use_decoder(monkeypatch, decoder)
+    sess = transcribe.Session(wh, max_windows=len(waves), max_beams=7, max_text_len=4 + depth + 1, kv_dtype=h.kv_code(kv))
+    h.use_decoder(monkeypatch, 0)
     ids = sess.transcribe_windows(waves, sp, is_special_of(sp), beam_size=b, max_depth=depth)
     return sess, ids, rows_of(sess, ids)
 
@@ -242,11 +181,9 @@ def check_beam_sums(lps):
 
 
 @pytest.mark.parametrize("kv", ["f32", "f16"])
-def test_beam_test_a_device_and_host_vs_float64(beam_gold, monkeypatch, kv):
-    dims, w_np, w_t = synth.make_weights("test-a", seed=0)
-    sp = synth.special_tokens(dims)
-    wh = model.Whisper(dims, w_np)
-    w64 = o_model.as_dtype(w_t)
+def test_beam_test_a_device_and_host_vs_float64(monkeypatch, kv):
+    beam_gold = h.golden("tokens_beam")
+    dims, sp, wh, _, _, w64 = h.named_model("test-a", f64=True)
     depth = beam_gold["depth_test_a"]
     for b in range(2, 8):
         waves = pool_waves(beam_gold, 24 // b)
@@ -254,48 +191,44 @@ def test_beam_test_a_device_and_host_vs_float64(beam_gold, monkeypatch, kv):
         assert sess.last_decoder() == 6
         check_beam_sums(lps)
         worst = check_against_f64(sess, w64, dims, sp, ids, lps, kv)
-        f64.report(f"last_logprobs device beam test-a B={b} kv={kv}", worst, f64.GREEDY_LP_TOL[kv])
+        h.report(f"last_logprobs device beam test-a B={b} kv={kv}", worst, h.GREEDY_LP_TOL[kv])
         if b == 5:   # the host search (decoder3) returns the same ids; its values agree within tolerance
             hs, hids, hlps = beam_run(wh, waves, sp, b, depth, kv, monkeypatch, decoder=3)
             assert hs.last_decoder() == 3 and hids == ids
             for r in range(len(ids)):
-                assert np.abs(hlps[r].astype(np.float64) - lps[r]).max() < f64.GREEDY_LP_TOL[kv]
+                assert np.abs(hlps[r].astype(np.float64) - lps[r]).max() < h.GREEDY_LP_TOL[kv]
             check_against_f64(hs, w64, dims, sp, hids, hlps, kv)
 
 
 @pytest.mark.parametrize("kv", ["f32", "f16"])
-def test_beam_tiny_en_device_vs_float64(beam_gold, monkeypatch, kv):
-    dims, w_np, w_t = synth.make_weights("tiny.en", seed=0)
-    sp = synth.special_tokens(dims)
-    wh = model.Whisper(dims, w_np)
-    w64 = o_model.as_dtype(w_t)
-    te = json.loads((G / "tokens_tiny_en.json").read_text())
+def test_beam_tiny_en_device_vs_float64(monkeypatch, kv):
+    beam_gold = h.golden("tokens_beam")
+    dims, sp, wh, _, _, w64 = h.named_model("tiny.en", f64=True)
+    te = h.golden("tokens_tiny_en")
     chunk = synth.chunk_waveform(0)
     sess, ids, lps = beam_run(wh, [chunk[s:e] for s, e in te["bounds"]], sp, 5, beam_gold["depth_tiny_en"], kv, monkeypatch)
     assert sess.last_decoder() == 6 and ids == beam_gold["tiny_en"][kv]["5"]
     worst = check_against_f64(sess, w64, dims, sp, ids, lps, kv)
-    f64.report(f"last_logprobs device beam tiny.en B=5 kv={kv}", worst, f64.GREEDY_LP_TOL[kv])
+    h.report(f"last_logprobs device beam tiny.en B=5 kv={kv}", worst, h.GREEDY_LP_TOL[kv])
 
 
 @pytest.mark.parametrize("kv", ["f32", "f16"])
 def test_beam_host_search_decoder5_vs_float64(monkeypatch, kv):
-    dims, wh, w64 = f64.make_model(256, 4, 2051)
+    dims, wh, w64 = h.make_model(256, 4, 2051)
     sp = synth.special_tokens(dims)
-    _, waves = f64.windows(3, seed=41)
-    sess, ids, lps = beam_run(wh, waves, sp, 5, f64.DEPTH, kv, monkeypatch)
+    _, waves = h.windows(3, seed=41)
+    sess, ids, lps = beam_run(wh, waves, sp, 5, h.DEPTH, kv, monkeypatch)
     assert sess.last_decoder() == 5
     check_beam_sums(lps)
     worst = check_against_f64(sess, w64, dims, sp, ids, lps, kv)
-    f64.report(f"last_logprobs host beam decoder5 d=256 B=5 kv={kv}", worst, f64.GREEDY_LP_TOL[kv])
+    h.report(f"last_logprobs host beam decoder5 d=256 B=5 kv={kv}", worst, h.GREEDY_LP_TOL[kv])
 
 
 # ---------------------------------------------------------------- 6. the merge
 @pytest.mark.parametrize("beam_size", [1, 5])
 @pytest.mark.parametrize("windows", ["reference", "native"])
 def test_merge_carries_logprobs_with_their_ids(windows, beam_size):
-    dims, w_np, _ = synth.make_weights("test-a", seed=0)
-    sp = synth.special_tokens(dims)
-    wh = model.Whisper(dims, w_np)
+    dims, sp, wh, *_ = h.named_model("test-a")
     bitmap = is_special_of(sp)
     waves = [synth.waveform(16000 * 70, seed=78), synth.waveform(16000 * 40, seed=79)]
     wl = transcribe.window_samples(dims.n_audio_ctx, windows)
@@ -324,14 +257,12 @@ def test_merge_carries_logprobs_with_their_ids(windows, beam_size):
 
 # ---------------------------------------------------------------- 7. the getter's contract
 def test_getter_contract():
-    dims, w_np, _ = synth.make_weights("test-a", seed=0)
-    sp = synth.special_tokens(dims)
-    wh = model.Whisper(dims, w_np)
+    dims, sp, wh, *_ = h.named_model("test-a")
     sess = transcribe.Session(wh, max_windows=2, max_beams=1, max_text_len=12)
     lib, n = ffi.lib(), C.c_int64(-1)
     buf = np.zeros(64, np.float32)
     assert lib.wb_session_last_logprobs(sess._h, 0, ffi.fptr(buf), 64, C.byref(n)) == ffi.WB_ERR_STATE
-    ids = sess.transcribe_windows([gl.window(0), gl.window(1)], sp, is_special_of(sp), beam_size=1, max_depth=6)
+    ids = sess.transcribe_windows([h.loop_window(0), h.loop_window(1)], sp, is_special_of(sp), beam_size=1, max_depth=6)
     for i in (-1, 2):
         assert lib.wb_session_last_logprobs(sess._h, i, ffi.fptr(buf), 64, C.byref(n)) == ffi.WB_ERR_INVALID_ARG
     assert lib.wb_session_last_logprobs(sess._h, 1, None, 0, C.byref(n)) == ffi.WB_OK and n.value == len(ids[1])

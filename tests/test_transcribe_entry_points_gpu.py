@@ -10,9 +10,10 @@ import numpy as np
 import pytest
 import torch
 
+import harness as h
 import wb200  # noqa: F401
 from oracle import synth
-from whisper_burn_b200 import ffi, model, transcribe
+from whisper_burn_b200 import ffi, transcribe
 
 pytestmark = pytest.mark.gpu
 DEPTH = 12
@@ -22,8 +23,7 @@ SEARCHES = [("beam", 1), ("beam", 3), ("greedy_loop", 1)]
 
 @pytest.fixture(scope="module")
 def tiny():
-    dims, w_np, _ = synth.make_weights("test-a", seed=0)
-    return dims, model.Whisper(dims, w_np), synth.special_tokens(dims)
+    return h.named_model("test-a")
 
 
 def bits(a):
@@ -42,7 +42,7 @@ def on_device(waves):
 
 @pytest.mark.parametrize("search,beam_size", SEARCHES)
 def test_window_entry_points_agree(tiny, search, beam_size):
-    dims, wh, sp = tiny
+    dims, sp, wh, *_ = tiny
     waves = [synth.waveform(n, seed=70 + i) for i, n in enumerate((48000, 40000, 56000))]
     sess = transcribe.Session(wh, max_windows=3, max_beams=3, max_text_len=4 + DEPTH + 1, search=search)
     bm = None if search == "greedy_loop" else sp.is_special_bitmap()
@@ -68,7 +68,7 @@ def test_window_entry_points_agree(tiny, search, beam_size):
 
 @pytest.mark.parametrize("search,beam_size", SEARCHES)
 def test_waveform_is_the_one_waveform_batch(tiny, search, beam_size):
-    dims, wh, sp = tiny
+    dims, sp, wh, *_ = tiny
     wave = synth.waveform(400000, seed=9)   # 3 windows of the reference windowing
     sess = transcribe.Session(wh, max_windows=3, max_beams=3, max_text_len=4 + DEPTH + 1, search=search)
     bm = None if search == "greedy_loop" else sp.is_special_bitmap()
@@ -80,7 +80,7 @@ def test_waveform_is_the_one_waveform_batch(tiny, search, beam_size):
 
 
 def test_rejected_calls_leave_the_last_results(tiny):
-    dims, wh, sp = tiny
+    dims, sp, wh, *_ = tiny
     V = dims.n_vocab
     good = [synth.waveform(n, seed=80 + i) for i, n in enumerate((48000, 40000))]
     other = [synth.waveform(n, seed=90 + i) for i, n in enumerate((44000, 52000))]
