@@ -7,6 +7,7 @@
  *
  *   audio::max_waveform_samples        src/audio.rs:12-17          -> wb_max_waveform_samples
  *   audio::prep_audio                  src/audio.rs:34-56          -> wb_prep_audio
+ *   `sox audio.wav -r 16000 -c 1` step README.md:69-73 (no reference code) -> wb_resample, wb_waveforms_to_tokens_resampled
  *   WhisperConfig / Whisper            src/model/mod.rs:16-71      -> wb_model_*
  *   model::load::load_whisper          src/model/load.rs:295-310   -> wb_model_set_tensor (same npy-tree paths)
  *   Whisper::forward_encoder           src/model/mod.rs:52-54      -> wb_forward_encoder
@@ -116,6 +117,20 @@ int wb_prep_audio(int device, const float* wave, int64_t n_batch, int64_t n_samp
                   float* mel_out, int64_t* n_frames_out);
 int wb_prep_audio_dev(int device, const float* wave_dev, int64_t n_batch, int64_t n_samples,
                       float* mel_out_dev, int64_t* n_frames_out);
+/* Downmix and resampling to the 16 kHz mono every other entry point takes; the reference has none (its README converts
+ * with sox first, its binary asserts 16 kHz mono).  An input of n_frames x channels interleaved f32 samples at an integer
+ * sample_rate is downmixed, x[i] = (x[i,0] + .. + x[i,C-1]) / C (f64, channel order), and resampled as
+ * scipy.signal.resample_poly(x, up, down) with its defaults: g = gcd(sample_rate, 16000), up = 16000 / g, down =
+ * sample_rate / g, supported when sample_rate >= 1 and max(up, down) <= 1024 (8000, 11025, 22050, 44100, 48000, 96000,
+ * 192000 Hz, ...); a Kaiser (beta 5) low-pass of 2 * 10 * max(up, down) + 1 taps designed in f64, products and sums in f64,
+ * each output rounded once to f32.  16 kHz mono passes through bit-unchanged.
+ * wb_resampled_length: the output length ceil(n_frames * up / down) (host only); -1 for an unsupported rate or n_frames < 0. */
+int64_t wb_resampled_length(int64_t n_frames, int64_t sample_rate);
+/* in [n_frames][channels] (host) -> out [*n_out] (host, 16 kHz mono), *n_out = wb_resampled_length(n_frames, sample_rate).
+ * WB_ERR_UNSUPPORTED for an unsupported rate; WB_ERR_INVALID_ARG for a null pointer, n_frames < 1, channels < 1 or capacity
+ * below the output length.  Both are reported before the device is touched. */
+int wb_resample(int device, const float* in, int64_t n_frames, int64_t channels, int64_t sample_rate, float* out,
+                int64_t capacity, int64_t* n_out);
 
 /* ---- model (src/model/mod.rs, src/model/load.rs) ------------------------------------- */
 int wb_model_create(const wb_dims* dims, int device, wb_model** out);
@@ -241,7 +256,22 @@ int wb_waveform_to_tokens(wb_session* s, const float* waveform, int64_t n_sample
 int wb_waveforms_to_tokens(wb_session* s, const float* const* waveforms, const int64_t* n_samples, int64_t n_waveforms,
                            int64_t sample_rate, int beam_size, int max_depth, const wb_special_ids* ids,
                            const uint8_t* is_special, int64_t* tokens_out, int64_t capacity, int64_t* n_tokens_out);
-/* Per-token log-probs of the last wb_transcribe_windows[_dev/_prev] (index = window) or wb_waveform(s)_to_tokens (index =
+/* wb_waveforms_to_tokens for waveforms of any supported rate and channel count: waveform w is n_frames[w] x channels[w]
+ * interleaved f32 samples at sample_rates[w] (rates and channel counts may differ within a call).  All inputs are uploaded
+ * once and converted to 16 kHz mono in one launch (wb_resample's definition, same values); then the windows of the converted
+ * waveforms (wb_window_bounds at 16 kHz) are cut on the device and decoded exactly as wb_waveforms_to_tokens decodes the
+ * converted audio: search rule, previous-text prompt, max_windows batching, overlap merge.  wb_session_last_logprobs /
+ * last_nbest / last_timings / last_steps mean what they mean after wb_waveforms_to_tokens.  Every argument that does not
+ * depend on decoded ids is checked before the upload: null pointers, n_waveforms >= 1, n_frames >= 1, channels >= 1, a
+ * supported rate (WB_ERR_UNSUPPORTED), a last window of at least 400 converted samples (WB_ERR_INVALID_ARG, audio.rs:292) and
+ * the decode arguments; a call rejected there leaves the encoded windows and every wb_session_last_* result as they were.
+ * The session keeps the inputs and their conversions in device buffers grown to the largest call: 4 * (n_frames * channels +
+ * n_out) bytes summed over the call's waveforms (n_out = wb_resampled_length), plus the filters (at most 160 KB per rate). */
+int wb_waveforms_to_tokens_resampled(wb_session* s, const float* const* waveforms, const int64_t* n_frames, const int64_t* channels,
+                                     const int64_t* sample_rates, int64_t n_waveforms, int beam_size, int max_depth,
+                                     const wb_special_ids* ids, const uint8_t* is_special, int64_t* tokens_out, int64_t capacity,
+                                     int64_t* n_tokens_out);
+/* Per-token log-probs of the last wb_transcribe_windows[_dev/_prev] (index = window) or wb_waveform(s)_to_tokens[_resampled] (index =
  * waveform) call on this session, aligned with the ids that call wrote: n_out = that row's id count.  WB_ERR_STATE before the
  * first such call, WB_ERR_INVALID_ARG for an index out of range or capacity < n_out.  out == NULL only sets n_out.
  * Those calls check every argument that does not depend on decoded ids before they encode (the waveform calls: each batch's

@@ -67,6 +67,13 @@ pub mod ffi {
                                           is_special: *const u8, tokens_out: *mut i64, capacity: i64, lens_out: *mut i64) -> c_int;
         pub fn wb_session_last_nbest(s: *mut c_void, index: i64, max_hyps: i64, capacity: i64, ids_out: *mut i64, lp_out: *mut f32,
                                      lens_out: *mut i64, scores_out: *mut f64, finished_out: *mut i32, n_hyps_out: *mut i64) -> c_int;
+        pub fn wb_resampled_length(n_frames: i64, sample_rate: i64) -> i64;
+        pub fn wb_resample(device: c_int, input: *const f32, n_frames: i64, channels: i64, sample_rate: i64, out: *mut f32, capacity: i64,
+                           n_out: *mut i64) -> c_int;
+        pub fn wb_waveforms_to_tokens_resampled(s: *mut c_void, waveforms: *const *const f32, n_frames: *const i64, channels: *const i64,
+                                                sample_rates: *const i64, n_waveforms: i64, beam_size: c_int, max_depth: c_int,
+                                                ids: *const wb_special_ids, is_special: *const u8, tokens_out: *mut i64, capacity: i64,
+                                                n_tokens_out: *mut i64) -> c_int;
     }
 }
 
@@ -92,6 +99,28 @@ pub mod audio {
         let mut nf = 0i64;
         check(unsafe { ffi::wb_prep_audio(0, waveform.as_ptr(), n_batch as i64, n as i64, out.as_mut_ptr(), &mut nf) })?;
         Ok((out, nf as usize))
+    }
+    /// Downmix + resampling to the 16 kHz mono everything else takes (wb_resample; the reference's README runs
+    /// `sox audio.wav -r 16000 -c 1` instead): `waveform` is frames x `channels` interleaved samples at `sample_rate`.
+    /// Unsupported rates (gcd with 16000 leaving up or down above 1024) are an `Err`.
+    pub fn resample(waveform: &[f32], channels: usize, sample_rate: usize) -> Result<Vec<f32>, Error> {
+        let n_frames = (waveform.len() / channels.max(1)) as i64;
+        let n = unsafe { ffi::wb_resampled_length(n_frames, sample_rate as i64) };
+        if n < 0 { return Err(format!("resample: unsupported sample rate {}", sample_rate).into()); }
+        let mut out = vec![0f32; n as usize];
+        let mut n_out = 0i64;
+        check(unsafe { ffi::wb_resample(0, waveform.as_ptr(), n_frames, channels as i64, sample_rate as i64, out.as_mut_ptr(), n, &mut n_out) })?;
+        Ok(out)
+    }
+    /// load_audio_waveform (src/bin/transcribe/main.rs:31-55) over wb_load_wav: (interleaved samples, channels, sample rate).
+    /// `strict` keeps the binary's 16 kHz mono asserts (a panic here too); without it any rate and channel count loads.
+    pub fn load_audio_waveform(path: &str, strict: bool) -> Result<(Vec<f32>, usize, usize), Error> {
+        let c = CString::new(path)?;
+        let (mut n, mut sr, mut ch) = (0i64, 0i64, 0 as c_int);
+        check(unsafe { ffi::wb_load_wav(c.as_ptr(), strict as c_int, std::ptr::null_mut(), 0, &mut n, &mut sr, &mut ch) })?;
+        let mut out = vec![0f32; n as usize];
+        check(unsafe { ffi::wb_load_wav(c.as_ptr(), strict as c_int, out.as_mut_ptr(), n, &mut n, &mut sr, &mut ch) })?;
+        Ok((out, ch as usize, sr as usize))
     }
 }
 
@@ -340,6 +369,36 @@ pub mod transcribe {
         })?;
         let tokens: Vec<usize> = out[..n as usize].iter().map(|&t| t as usize).collect();
         Ok((bpe.decode(&tokens[..], true)?, tokens))
+    }
+
+    /// waveform_to_text for audio at any supported rate and channel count (`waveform`: frames x `channels` interleaved samples
+    /// at `sample_rate`): the library converts it to 16 kHz mono on the GPU (wb_waveforms_to_tokens_resampled, the conversion
+    /// of audio::resample), then windows, decodes and merges it as waveform_to_text does the converted audio.
+    pub fn waveform_to_text_resampled(whisper: &model::Whisper, bpe: &Gpt2Tokenizer, lang: Language, waveform: Vec<f32>, channels: usize,
+                                      sample_rate: usize) -> token::Result<(String, Vec<usize>)> {
+        let sp = SpecialTokens::from_tokenizer(bpe, lang);
+        let n_frames = (waveform.len() / channels.max(1)) as i64;
+        let n16 = unsafe { ffi::wb_resampled_length(n_frames, sample_rate as i64) }.max(0) as usize;   // 16 kHz samples
+        let window = audio::max_waveform_samples(whisper.encoder_ctx_size() - 10);            // transcribe.rs:32-34
+        let shift = window.saturating_sub(16000 * 3).max(1);                                   // transcribe.rs:120-123
+        let n_windows = n16.saturating_sub(1) / shift + 1;
+        let cap = n_windows * (4 + MAX_DEPTH + 1) + 16;
+        let mut out = vec![0i64; cap];
+        let mut n = 0i64;
+        let (wave, ch, sr) = (waveform.as_ptr(), channels as i64, sample_rate as i64);
+        whisper.with_session(n_windows.min(64), BEAM_SIZE, 4 + MAX_DEPTH + 1, |s| {
+            check(unsafe { ffi::wb_waveforms_to_tokens_resampled(s, &wave, &n_frames, &ch, &sr, 1, BEAM_SIZE as c_int, MAX_DEPTH as c_int,
+                                                                 &sp.ids, sp.is_special.as_ptr(), out.as_mut_ptr(), cap as i64, &mut n) })
+        })?;
+        let tokens: Vec<usize> = out[..n as usize].iter().map(|&t| t as usize).collect();
+        Ok((bpe.decode(&tokens[..], true)?, tokens))
+    }
+
+    /// What the transcribe binary does with a WAV file of any rate and channel count (src/bin/transcribe/main.rs:31-55 without
+    /// its 16 kHz mono asserts): load it as it is (wb_load_wav with strict_16k_mono = 0), then waveform_to_text_resampled.
+    pub fn wav_file_to_text(whisper: &model::Whisper, bpe: &Gpt2Tokenizer, lang: Language, path: &str) -> token::Result<(String, Vec<usize>)> {
+        let (waveform, channels, sample_rate) = audio::load_audio_waveform(path, false)?;
+        waveform_to_text_resampled(whisper, bpe, lang, waveform, channels, sample_rate)
     }
 
     /// One hypothesis of a window's n-best list: its tokens (prompt included, 0.0 log-probs there), the cumulative log-prob the

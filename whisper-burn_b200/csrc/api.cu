@@ -206,6 +206,27 @@ int wb_prep_audio_dev(int device, const float* wave_dev, int64_t n_batch, int64_
     });
 }
 
+int64_t wb_resampled_length(int64_t n_frames, int64_t sample_rate) { return wb::resampled_length(n_frames, sample_rate); }
+
+int wb_resample(int device, const float* in, int64_t n_frames, int64_t channels, int64_t sample_rate, float* out, int64_t capacity,
+                int64_t* n_out) {
+    return guarded([&] {
+        WB_REQUIRE(in && out && n_out, "resample: null pointer");
+        WB_REQUIRE(n_frames >= 1, "resample: n_frames must be >= 1");
+        WB_REQUIRE(channels >= 1 && channels <= INT32_MAX, "resample: channels must be >= 1");
+        const int64_t len = wb::resampled_length(n_frames, sample_rate);
+        if (len < 0) wb::fail(WB_ERR_UNSUPPORTED, "resample: unsupported sample rate (gcd with 16000 must leave up and down <= 1024)");
+        WB_REQUIRE(n_frames <= INT64_MAX / channels, "resample: waveform too long");
+        WB_REQUIRE(capacity >= len, "resample: capacity below wb_resampled_length");
+        require_device(device);
+        wb::ResampleBufs b;
+        std::vector<int64_t> off, n;
+        wb::resample_waveforms(b, &in, &n_frames, &channels, &sample_rate, 1, off, n, nullptr);
+        WB_CUDA(cudaMemcpy(out, b.out.p, (size_t)len * sizeof(float), cudaMemcpyDeviceToHost));
+        *n_out = len;
+    });
+}
+
 int wb_model_create(const wb_dims* dims, int device, wb_model** out) {
     return guarded([&] {
         WB_REQUIRE(dims && out, "model_create: null pointer");
@@ -493,6 +514,19 @@ int wb_waveforms_to_tokens(wb_session* s, const float* const* waveforms, const i
         WB_REQUIRE(s && waveforms && n_samples && ids && tokens_out && n_tokens_out, "waveforms_to_tokens: null pointer");
         copy_tokens_out(wb::waveforms_to_tokens(*s->impl, waveforms, n_samples, n_waveforms, sample_rate, beam_size, max_depth,
                                                 *ids, is_special, capacity),
+                        tokens_out, capacity, n_tokens_out);
+    });
+}
+
+int wb_waveforms_to_tokens_resampled(wb_session* s, const float* const* waveforms, const int64_t* n_frames, const int64_t* channels,
+                                     const int64_t* sample_rates, int64_t n_waveforms, int beam_size, int max_depth,
+                                     const wb_special_ids* ids, const uint8_t* is_special, int64_t* tokens_out, int64_t capacity,
+                                     int64_t* n_tokens_out) {
+    return guarded([&] {
+        WB_REQUIRE(s && waveforms && n_frames && channels && sample_rates && ids && tokens_out && n_tokens_out,
+                   "waveforms_to_tokens_resampled: null pointer");
+        copy_tokens_out(wb::waveforms_to_tokens_resampled(*s->impl, waveforms, n_frames, channels, sample_rates, n_waveforms, beam_size,
+                                                          max_depth, *ids, is_special, capacity),
                         tokens_out, capacity, n_tokens_out);
     });
 }

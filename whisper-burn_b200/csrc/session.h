@@ -100,6 +100,7 @@ struct Session {
     DevBuf<int> d_win_T;
     // ---- device: frontend + encoder activations
     DevBuf<float> wave;
+    ResampleBufs rs;   // waveforms_to_tokens_resampled: the interleaved inputs and their 16 kHz conversions
     DevBuf<int> max_slots;
     DevBuf<float> mel_rows, x, xa;           // token-major log-mel rows, residual stream, encoder output
     DevBuf<float> h1, xn, att, qkv, hid;     // fp32 activations of the CUDA-core encoder (weights that are not fp16-exact)
@@ -238,6 +239,13 @@ std::vector<std::vector<int64_t>> transcribe_windows(Session& s, const std::vect
 std::vector<std::vector<int64_t>> waveforms_to_tokens(Session& s, const float* const* waveforms, const int64_t* n_samples,
                                                       int64_t n_waveforms, int64_t sample_rate, int beam_size, int max_depth,
                                                       const wb_special_ids& ids, const uint8_t* is_special, int64_t capacity);
+// waveforms_to_tokens over waveforms of any supported rate and channel count: every argument checked, the interleaved inputs
+// uploaded and resampled to 16 kHz mono into s.rs in one launch, then the same window loop with windows cut on the device
+std::vector<std::vector<int64_t>> waveforms_to_tokens_resampled(Session& s, const float* const* waveforms, const int64_t* n_frames,
+                                                                const int64_t* channels, const int64_t* sample_rates,
+                                                                int64_t n_waveforms, int beam_size, int max_depth,
+                                                                const wb_special_ids& ids, const uint8_t* is_special,
+                                                                int64_t capacity);
 std::vector<std::pair<int64_t, int64_t>> window_bounds(int64_t n_samples, int64_t sample_rate, int64_t window_len);
 bool find_chunk_overlap(const int64_t* prev, int64_t n_prev, const int64_t* curr, int64_t n_curr, int64_t max_n_offsets,
                         int64_t min_n_overlaps, int64_t* prev_index, int64_t* curr_index);

@@ -195,64 +195,70 @@ std::vector<std::vector<int64_t>> transcribe_windows(Session& s, const std::vect
     return out;
 }
 
+namespace {
+
+// one window of a waveform call: samples [start, start + len) of waveform `owner`
+struct WaveWindow {
+    int owner;
+    int64_t start, len;
+};
+
+// the checks of a waveform call that come before its windows are cut
+void check_waveform_call(const Session& s, int64_t n_waveforms) {
+    WB_REQUIRE(n_waveforms >= 1, "waveforms_to_tokens: n_waveforms must be >= 1");
+    WB_REQUIRE(s.startofprev < 0 || s.search != WB_SEARCH_GREEDY_LOOP,
+               "waveform_to_tokens: the previous-text prompt (set_prev_prompt) does not combine with the greedy loop");
+}
+
+// the windows of every waveform of n_samples[w] 16 kHz samples, waveform-major (transcribe.rs:32-34, 114-138)
+std::vector<WaveWindow> waveform_windows(const Session& s, const int64_t* n_samples, int64_t n_waveforms) {
+    const int64_t window_len = window_samples(s.m->dims.n_audio_ctx, s.window_mode);
+    std::vector<WaveWindow> wins;
+    for (int64_t w = 0; w < n_waveforms; ++w)
+        for (const auto& b : window_bounds(n_samples[w], 16000, window_len)) wins.push_back(WaveWindow{(int)w, b.first, b.second - b.first});
+    return wins;
+}
+
 // windows of ALL waveforms are decoded together in batches of the session's capacity (they are independent,
 // SURVEY.md F9), then each waveform's windows are merged in order exactly like the reference's sequential
 // loop (transcribe.rs:42-71); each id's log-prob travels with it through the merge.
 // With the previous-text prompt (Session::startofprev >= 0) window i of a waveform needs the merged ids of windows
 // 0 .. i-1: round i decodes window i of every waveform that has one, in batches of the session's capacity.
-std::vector<std::vector<int64_t>> waveforms_to_tokens(Session& s, const float* const* waveforms, const int64_t* n_samples,
-                                                      int64_t n_waveforms, int64_t sample_rate, int beam_size, int max_depth,
-                                                      const wb_special_ids& ids, const uint8_t* is_special, int64_t capacity) {
-    WB_REQUIRE(n_waveforms >= 1, "waveforms_to_tokens: n_waveforms must be >= 1");
-    // the frontend tables (mel filterbank, DFT bins) are the 16 kHz ones: the reference builds them from the caller's rate
-    // (audio.rs:44, 67-143) but its binary only ever passes 16 kHz (src/bin/transcribe/main.rs:38-41 asserts it)
-    WB_REQUIRE(sample_rate == 16000, "waveform_to_tokens: only 16 kHz input is supported (frontend tables are built for 16 kHz)");
+// encode_batch encodes one batch of windows, after that batch's arguments are checked.
+std::vector<std::vector<int64_t>> window_loop(Session& s, const std::vector<WaveWindow>& wins, int64_t n_waveforms, int beam_size,
+                                              int max_depth, const wb_special_ids& ids, const uint8_t* is_special, int64_t capacity,
+                                              const std::function<void(const std::vector<WaveWindow>&)>& encode_batch) {
     const bool prev_prompt = s.startofprev >= 0;
-    WB_REQUIRE(!prev_prompt || s.search != WB_SEARCH_GREEDY_LOOP,
-               "waveform_to_tokens: the previous-text prompt (set_prev_prompt) does not combine with the greedy loop");
-    const int64_t window_len = window_samples(s.m->dims.n_audio_ctx, s.window_mode);   // transcribe.rs:32-34
-    std::vector<const float*> ptrs;
-    std::vector<int64_t> lens;
-    std::vector<int> owner;
-    for (int64_t w = 0; w < n_waveforms; ++w)
-        for (const auto& b : window_bounds(n_samples[w], sample_rate, window_len)) {
-            ptrs.push_back(waveforms[w] + b.first);
-            lens.push_back(b.second - b.first);
-            owner.push_back((int)w);
-        }
     std::vector<std::vector<int64_t>> out((size_t)n_waveforms);
     std::vector<std::vector<float>> out_lp((size_t)n_waveforms);
-    std::vector<NBest> nbest(ptrs.size());   // per window, waveform-major
+    std::vector<NBest> nbest(wins.size());   // per window, waveform-major
     // batches: window-major order (all windows at once) or, with the previous-text prompt, rounds of window index i
     std::vector<std::vector<size_t>> rounds(1);
     std::vector<size_t> idx((size_t)n_waveforms, 0);   // per waveform, the index of its next window
-    for (size_t j = 0; j < ptrs.size(); ++j) {
-        const size_t i = prev_prompt ? idx[(size_t)owner[j]]++ : 0;
+    for (size_t j = 0; j < wins.size(); ++j) {
+        const size_t i = prev_prompt ? idx[(size_t)wins[j].owner]++ : 0;
         if (rounds.size() <= i) rounds.resize(i + 1);
         rounds[i].push_back(j);
     }
     for (const std::vector<size_t>& round : rounds) {
         for (size_t b0 = 0; b0 < round.size(); b0 += (size_t)s.max_windows) {
             const size_t nb = std::min(round.size() - b0, (size_t)s.max_windows);
-            std::vector<const float*> bp(nb);
-            std::vector<int64_t> bl(nb);
+            std::vector<WaveWindow> batch(nb);
             std::vector<std::vector<int64_t>> prev(prev_prompt ? nb : 0);
             for (size_t i = 0; i < nb; ++i) {
-                const size_t j = round[b0 + i];
-                bp[i] = ptrs[j];
-                bl[i] = lens[j];
-                if (prev_prompt) prev[i] = prev_nonspecial(out[(size_t)owner[j]], is_special);
+                batch[i] = wins[round[b0 + i]];
+                if (prev_prompt) prev[i] = prev_nonspecial(out[(size_t)batch[i].owner], is_special);
             }
             const auto prompts = window_prompts(s, (int64_t)nb, beam_size, max_depth, ids, is_special, prev, s.startofprev);
             s.have_logprobs = false;
             s.have_nbest = false;
-            s.encode_waveforms_host(bp.data(), bl.data(), (int64_t)nb);
+            encode_batch(batch);
             std::vector<std::vector<int64_t>> toks;
             std::vector<std::vector<float>> lps;
             std::vector<NBest> nbs;
             decode_windows(s, prompts, beam_size, max_depth, ids.eot, is_special, toks, lps, nbs);
             for (size_t i = 0; i < nb; ++i) {
-                merge_window(out[(size_t)owner[round[b0 + i]]], out_lp[(size_t)owner[round[b0 + i]]], toks[i], lps[i]);
+                merge_window(out[(size_t)batch[i].owner], out_lp[(size_t)batch[i].owner], toks[i], lps[i]);
                 if (!nbs.empty()) nbest[round[b0 + i]] = std::move(nbs[i]);
             }
         }
@@ -264,6 +270,62 @@ std::vector<std::vector<int64_t>> waveforms_to_tokens(Session& s, const float* c
     s.last_nbest = std::move(nbest);
     s.have_nbest = s.search == WB_SEARCH_BEAM;
     return out;
+}
+
+}  // namespace
+
+std::vector<std::vector<int64_t>> waveforms_to_tokens(Session& s, const float* const* waveforms, const int64_t* n_samples,
+                                                      int64_t n_waveforms, int64_t sample_rate, int beam_size, int max_depth,
+                                                      const wb_special_ids& ids, const uint8_t* is_special, int64_t capacity) {
+    check_waveform_call(s, n_waveforms);
+    // the frontend tables (mel filterbank, DFT bins) are the 16 kHz ones: the reference builds them from the caller's rate
+    // (audio.rs:44, 67-143) but its binary only ever passes 16 kHz (src/bin/transcribe/main.rs:38-41 asserts it);
+    // waveforms_to_tokens_resampled converts other rates first
+    WB_REQUIRE(sample_rate == 16000, "waveform_to_tokens: only 16 kHz input is supported (frontend tables are built for 16 kHz)");
+    return window_loop(s, waveform_windows(s, n_samples, n_waveforms), n_waveforms, beam_size, max_depth, ids, is_special, capacity,
+                       [&](const std::vector<WaveWindow>& batch) {
+                           std::vector<const float*> bp(batch.size());
+                           std::vector<int64_t> bl(batch.size());
+                           for (size_t i = 0; i < batch.size(); ++i) {
+                               bp[i] = waveforms[batch[i].owner] + batch[i].start;
+                               bl[i] = batch[i].len;
+                           }
+                           s.encode_waveforms_host(bp.data(), bl.data(), (int64_t)batch.size());
+                       });
+}
+
+std::vector<std::vector<int64_t>> waveforms_to_tokens_resampled(Session& s, const float* const* waveforms, const int64_t* n_frames,
+                                                                const int64_t* channels, const int64_t* sample_rates,
+                                                                int64_t n_waveforms, int beam_size, int max_depth,
+                                                                const wb_special_ids& ids, const uint8_t* is_special,
+                                                                int64_t capacity) {
+    // every argument check that does not depend on decoded ids, before the upload and the resample
+    check_waveform_call(s, n_waveforms);
+    std::vector<int64_t> n16((size_t)n_waveforms);
+    for (int64_t w = 0; w < n_waveforms; ++w) {
+        WB_REQUIRE(waveforms[w] != nullptr, "waveforms_to_tokens_resampled: null waveform");
+        WB_REQUIRE(n_frames[w] >= 1, "waveforms_to_tokens_resampled: n_frames must be >= 1");
+        WB_REQUIRE(channels[w] >= 1 && channels[w] <= INT32_MAX, "waveforms_to_tokens_resampled: channels must be >= 1");
+        n16[(size_t)w] = resampled_length(n_frames[w], sample_rates[w]);
+        if (n16[(size_t)w] < 0) fail(WB_ERR_UNSUPPORTED, "waveforms_to_tokens_resampled: unsupported sample rate (gcd with 16000 "
+                                                         "must leave up and down <= 1024)");
+        WB_REQUIRE(n_frames[w] <= INT64_MAX / channels[w], "waveforms_to_tokens_resampled: waveform too long");
+    }
+    const std::vector<WaveWindow> wins = waveform_windows(s, n16.data(), n_waveforms);
+    for (const WaveWindow& win : wins) WB_REQUIRE(win.len >= N_FFT, "prep_audio: waveform shorter than n_fft (audio.rs:292)");
+    const int64_t first_batch = std::min<int64_t>(s.startofprev >= 0 ? n_waveforms : (int64_t)wins.size(), s.max_windows);
+    window_prompts(s, first_batch, beam_size, max_depth, ids, is_special);
+    std::vector<int64_t> off, n_out;
+    resample_waveforms(s.rs, waveforms, n_frames, channels, sample_rates, n_waveforms, off, n_out, s.st);
+    return window_loop(s, wins, n_waveforms, beam_size, max_depth, ids, is_special, capacity,
+                       [&](const std::vector<WaveWindow>& batch) {
+                           std::vector<int64_t> bo(batch.size()), bl(batch.size());
+                           for (size_t i = 0; i < batch.size(); ++i) {
+                               bo[i] = off[(size_t)batch[i].owner] + batch[i].start;
+                               bl[i] = batch[i].len;
+                           }
+                           s.encode_from_device_wave(s.rs.out.p, bo.data(), bl.data(), (int64_t)batch.size());
+                       });
 }
 
 }  // namespace wb

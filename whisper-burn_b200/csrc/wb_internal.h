@@ -337,6 +337,30 @@ void launch_logmel(const Model& m, const float* wave, const LogMelWindow* win_de
 void launch_rows_to_chan(const float* rows, float* chan, int n_frames, cudaStream_t st);
 void launch_chan_to_rows(const float* chan, float* rows, int n_frames, int64_t chan_stride, cudaStream_t st);
 
+// ---- resampling to 16 kHz (resample.cu) -------------------------------------------------------------
+// up / down of sample_rate -> 16 kHz after dividing by their gcd; false unless sample_rate >= 1 and max(up, down) <= 1024
+bool resample_ratio(int64_t sample_rate, int& up, int& down);
+// ceil(n_frames * up / down) (wb_resampled_length); -1 for an unsupported rate or n_frames < 0
+int64_t resampled_length(int64_t n_frames, int64_t sample_rate);
+// resample_poly's filter, scaled by up: 2 * 10 * max(up, down) + 1 f64 taps, or [1] for up = down = 1
+std::vector<double> resample_taps(int up, int down);
+struct ResampleDesc {   // one waveform of a resample launch
+    int64_t in_off, n;        // first interleaved input sample, frames
+    int64_t out_off, n_out;   // first output sample, outputs
+    int64_t taps_off, tile0;  // its filter in the taps buffer, its first output tile
+    int channels, up, down, half;
+};
+struct ResampleBufs {   // device buffers of resample_waveforms, grown to the largest call
+    DevBuf<float> in, out;
+    DevBuf<double> taps;
+    DevBuf<ResampleDesc> desc;
+};
+// Uploads n_waveforms interleaved host waveforms (frames x channels at sample_rates[w]; every rate supported) and resamples
+// all of them to 16 kHz mono in one launch: waveform w lands in b.out at out_off[w], n_out[w] samples.  Synchronises st.
+void resample_waveforms(ResampleBufs& b, const float* const* in, const int64_t* n_frames, const int64_t* channels,
+                        const int64_t* sample_rates, int64_t n_waveforms, std::vector<int64_t>& out_off,
+                        std::vector<int64_t>& n_out, cudaStream_t st);
+
 // ---- encoder pieces (encoder.cu) -----------------------------------------------------------------
 // head-major re-layout of one layer's cross K|V rows (see encoder.cu)
 void launch_ckv_relayout(const float* src, void* dst, bool dst_half, const int64_t* win_row_off, const int* win_T, int n_windows,

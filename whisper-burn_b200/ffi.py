@@ -47,6 +47,8 @@ SYMBOLS = {
     "wb_device_count": (C.c_int, [C.POINTER(C.c_int)]),
     "wb_max_waveform_samples": (C.c_int64, [C.c_int64]),
     "wb_window_samples": (C.c_int64, [C.c_int64, C.c_int]),
+    "wb_resampled_length": (C.c_int64, [C.c_int64, C.c_int64]),
+    "wb_resample": (C.c_int, [C.c_int, _F, C.c_int64, C.c_int64, C.c_int64, _F, C.c_int64, _I64]),
     "wb_prep_audio": (C.c_int, [C.c_int, _F, C.c_int64, C.c_int64, _F, _I64]),
     "wb_prep_audio_dev": (C.c_int, [C.c_int, _P, C.c_int64, C.c_int64, _P, _I64]),
     "wb_model_create": (C.c_int, [C.POINTER(Dims), C.c_int, C.POINTER(_P)]),
@@ -82,6 +84,8 @@ SYMBOLS = {
                                         C.POINTER(SpecialIds), _U8, _I64, C.c_int64, _I64]),
     "wb_waveforms_to_tokens": (C.c_int, [_P, C.POINTER(_F), _I64, C.c_int64, C.c_int64, C.c_int, C.c_int,
                                          C.POINTER(SpecialIds), _U8, _I64, C.c_int64, _I64]),
+    "wb_waveforms_to_tokens_resampled": (C.c_int, [_P, C.POINTER(_F), _I64, _I64, _I64, C.c_int64, C.c_int, C.c_int,
+                                                   C.POINTER(SpecialIds), _U8, _I64, C.c_int64, _I64]),
     "wb_session_last_logprobs": (C.c_int, [_P, C.c_int64, _F, C.c_int64, _I64]),
     "wb_session_last_nbest": (C.c_int, [_P, C.c_int64, C.c_int64, C.c_int64, _I64, _F, _I64, C.POINTER(C.c_double), _I32, _I64]),
     "wb_session_score_tokens": (C.c_int, [_P, C.c_int64, _I32, _I64, _I64, C.c_int, _U8, _F, _I64]),

@@ -194,6 +194,29 @@ class Session:
                                                   ffi.i64ptr(n)))
         return [[int(t) for t in out[i, :n[i]]] for i in range(len(ws))]
 
+    def waveforms_to_tokens_resampled(self, waveforms: Sequence[np.ndarray], sample_rates: Sequence[int], special,
+                                      is_special: np.ndarray, beam_size: int = 5, max_depth: int = 100) -> List[List[int]]:
+        """waveforms_to_tokens for waveforms of any rate and channel count (wb_waveforms_to_tokens_resampled): waveform i is
+        1-D (mono) or 2-D [n_frames, channels] at sample_rates[i]; all are converted to 16 kHz mono on the GPU as
+        audio.resample does, then decoded as waveforms_to_tokens decodes the converted audio."""
+        from .audio import _frames, resampled_length
+        ws = [_frames(w) for w in waveforms]
+        if len(sample_rates) != len(ws):
+            raise ValueError("one sample rate per waveform")
+        ptrs = (ffi._F * len(ws))(*[ffi.fptr(w) for w in ws])
+        frames = np.asarray([w.shape[0] for w in ws], dtype=np.int64)
+        channels = np.asarray([w.shape[1] for w in ws], dtype=np.int64)
+        rates = np.asarray(sample_rates, dtype=np.int64)
+        n16 = max(max(resampled_length(int(n), int(r)) for n, r in zip(frames, rates)), 0)
+        cap = (n16 // 1000 + 2) * (10 + max_depth + 1) + 16
+        out = np.zeros((len(ws), cap), dtype=np.int64)
+        n = np.zeros(len(ws), dtype=np.int64)
+        ffi.check(ffi.lib().wb_waveforms_to_tokens_resampled(self._h, ptrs, ffi.i64ptr(frames), ffi.i64ptr(channels),
+                                                            ffi.i64ptr(rates), len(ws), beam_size, max_depth,
+                                                            C.byref(_special_ids(special)), _special(is_special),
+                                                            ffi.i64ptr(out), cap, ffi.i64ptr(n)))
+        return [[int(t) for t in out[i, :n[i]]] for i in range(len(ws))]
+
     def last_logprobs(self, index: int) -> np.ndarray:
         """float32 log-prob of each id of row `index` (window or waveform) of the last transcribe_windows[_dev] /
         waveform(s)_to_tokens call: 0 for the prompt, the log-prob the search chose the id with, NaN for an EOT the greedy
