@@ -104,7 +104,7 @@ __device__ __forceinline__ void grid_sync(unsigned int* bar, unsigned int& gen) 
 }
 
 // ---- input staging ---------------------------------------------------------------------------------
-// LayerNorm (burn 0.9 form, see encoder.cu) of rows [r0, r0+RC) of src (L2) into xs[RC][d]; warp per row.
+// LayerNorm (burn 0.9 form, prims.cuh) of rows [r0, r0+RC) of src (L2) into xs[RC][d]; warp per row.
 // The row is fetched with ONE batch of independent 16-byte loads (d <= 1280 -> <= 10 per lane) and stays in
 // registers through mean / variance / normalisation: a single L2 round trip per stage.
 constexpr int LN_V4 = 10;
@@ -139,25 +139,19 @@ __device__ __forceinline__ void stage_ln(const float* src, int r0, int R, int d,
             if (c < nv) {
                 v[i].x = __fsub_rn(v[i].x, mean); v[i].y = __fsub_rn(v[i].y, mean);
                 v[i].z = __fsub_rn(v[i].z, mean); v[i].w = __fsub_rn(v[i].w, mean);
-                q = __fadd_rn(q, __fmul_rn(v[i].x, v[i].x)); q = __fadd_rn(q, __fmul_rn(v[i].y, v[i].y));
-                q = __fadd_rn(q, __fmul_rn(v[i].z, v[i].z)); q = __fadd_rn(q, __fmul_rn(v[i].w, v[i].w));
+                q = ln_sq_add4(q, v[i]);
             }
         }
         q = warp_sum(q);
         const float var = __fdiv_rn(q, (float)d);
-        const float den = eps_outside ? __fadd_rn(__fsqrt_rn(var), eps) : __fsqrt_rn(__fadd_rn(var, eps));
+        const float den = LN_DEN(var, eps, eps_outside);
 #pragma unroll
         for (int i = 0; i < LN_V4; ++i) {
             const int c = i * 32 + lane;
             if (c < nv) {
                 const float4 g4 = __ldg(reinterpret_cast<const float4*>(g) + c);
                 const float4 b4 = __ldg(reinterpret_cast<const float4*>(b) + c);
-                float4 o;
-                o.x = __fadd_rn(__fmul_rn(__fdiv_rn(v[i].x, den), g4.x), b4.x);
-                o.y = __fadd_rn(__fmul_rn(__fdiv_rn(v[i].y, den), g4.y), b4.y);
-                o.z = __fadd_rn(__fmul_rn(__fdiv_rn(v[i].z, den), g4.z), b4.z);
-                o.w = __fadd_rn(__fmul_rn(__fdiv_rn(v[i].w, den), g4.w), b4.w);
-                xr[c] = o;
+                xr[c] = ln_norm4(v[i], den, g4, b4);
             }
         }
     }
@@ -181,14 +175,13 @@ __device__ __forceinline__ void stage_ln_smem(const float* src_s, int r0, int R,
         const float mean = __fdiv_rn(sum, (float)d);
         float q = 0.0f;
         for (int c = lane; c < d; c += 32) {
-            const float dv = __fsub_rn(s[c], mean);
-            q = __fadd_rn(q, __fmul_rn(dv, dv));
+            q = ln_sq_add(q, __fsub_rn(s[c], mean));
         }
         q = warp_sum(q);
         const float var = __fdiv_rn(q, (float)d);
-        const float den = eps_outside ? __fadd_rn(__fsqrt_rn(var), eps) : __fsqrt_rn(__fadd_rn(var, eps));
+        const float den = LN_DEN(var, eps, eps_outside);
         for (int c = lane; c < d; c += 32)
-            xr[c] = __fadd_rn(__fmul_rn(__fdiv_rn(__fsub_rn(s[c], mean), den), __ldg(g + c)), __ldg(b + c));
+            xr[c] = ln_norm<true>(__fsub_rn(s[c], mean), den, g, b, c);
     }
 }
 

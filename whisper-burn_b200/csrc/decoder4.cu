@@ -269,9 +269,9 @@ __device__ __forceinline__ void ln_fetch(float* lnp, const float* __restrict__ g
         cp_async16_l2(lnp + D + 4 * (lane + 32 * k), b + 4 * (lane + 32 * k), pol);
     }
 }
-// LayerNorm (burn 0.9 form, layernorm in oracle/model.py) of the warp's register copy of x -> out_s (shared memory).  Every
-// warp stores the same values (identical arithmetic) and reads them back after its own stores.  The normalisation multiplies
-// by 1/den (<= 1.5 ulp from the divide).
+// LayerNorm (burn 0.9 eps placement; fmaf square sum and reciprocal normalisation, prims.cuh ln_sq_fma4 / ln_norm4_rcp) of the
+// warp's register copy of x -> out_s (shared memory).  Every warp stores the same values (identical arithmetic) and reads them
+// back after its own stores.
 template <int D, int PF>
 __device__ __forceinline__ void ln_warp(XRegs<PF>& x, const float* gb_s, float eps, int eps_outside, float* out_s) {
     const int lane = threadIdx.x & 31;
@@ -286,20 +286,16 @@ __device__ __forceinline__ void ln_warp(XRegs<PF>& x, const float* gb_s, float e
     for (int k = 0; k < PF; ++k) {
         x.v[k].x = __fsub_rn(x.v[k].x, mean); x.v[k].y = __fsub_rn(x.v[k].y, mean);
         x.v[k].z = __fsub_rn(x.v[k].z, mean); x.v[k].w = __fsub_rn(x.v[k].w, mean);
-        q = fmaf(x.v[k].x, x.v[k].x, q); q = fmaf(x.v[k].y, x.v[k].y, q);
-        q = fmaf(x.v[k].z, x.v[k].z, q); q = fmaf(x.v[k].w, x.v[k].w, q);
+        q = ln_sq_fma4(q, x.v[k]);
     }
     q = warp_sum(q);
     const float var = __fdiv_rn(q, (float)D);
-    const float den = eps_outside ? __fadd_rn(__fsqrt_rn(var), eps) : __fsqrt_rn(__fadd_rn(var, eps));
-    const float rinv = __fdiv_rn(1.0f, den);
+    const float rinv = __fdiv_rn(1.0f, LN_DEN(var, eps, eps_outside));
 #pragma unroll
     for (int k = 0; k < PF; ++k) {
         const float4 g = reinterpret_cast<const float4*>(gb_s)[lane + 32 * k];
         const float4 b = reinterpret_cast<const float4*>(gb_s + D)[lane + 32 * k];
-        reinterpret_cast<float4*>(out_s)[lane + 32 * k] =
-            make_float4(fmaf(__fmul_rn(x.v[k].x, rinv), g.x, b.x), fmaf(__fmul_rn(x.v[k].y, rinv), g.y, b.y),
-                        fmaf(__fmul_rn(x.v[k].z, rinv), g.z, b.z), fmaf(__fmul_rn(x.v[k].w, rinv), g.w, b.w));
+        reinterpret_cast<float4*>(out_s)[lane + 32 * k] = ln_norm4_rcp(x.v[k], rinv, g, b);
     }
     __syncwarp();
 }

@@ -155,7 +155,7 @@ dec5_kernel(const DecArgs a) {
             for (int slot = 0; slot < n_slots; ++slot) {
                 const GemmDesc& D = ds[(slot >= SL_LNF ? L : l) * 16 + slot];
                 if (D.kind == D5_KIND_LN) {
-                    // ================= LayerNorm (burn 0.9 form, dec_common.cuh stage_ln) of row blockIdx.x by ONE warp of ONE CTA,
+                    // ================= LayerNorm (burn 0.9 form, prims.cuh) of row blockIdx.x by ONE warp of ONE CTA,
                     // written as fragment-order hi/lo planes for the next linear stage (every CTA copies them after the barrier).
                     // EMB: x = tok_emb[token] + pos_emb[p] (mod.rs:141-146); FOLD: x += the four MLP2 partial sums of the
                     // previous layer (fixed order); both publish the fp32 row for the residual adds of this layer.
@@ -214,8 +214,7 @@ dec5_kernel(const DecArgs a) {
                             if (tid + i * NT < nv) {
                                 v[i].x = __fsub_rn(v[i].x, mean); v[i].y = __fsub_rn(v[i].y, mean);
                                 v[i].z = __fsub_rn(v[i].z, mean); v[i].w = __fsub_rn(v[i].w, mean);
-                                q = __fadd_rn(q, __fmul_rn(v[i].x, v[i].x)); q = __fadd_rn(q, __fmul_rn(v[i].y, v[i].y));
-                                q = __fadd_rn(q, __fmul_rn(v[i].z, v[i].z)); q = __fadd_rn(q, __fmul_rn(v[i].w, v[i].w));
+                                q = ln_sq_add4(q, v[i]);
                             }
                         }
                         q = warp_sum(q);
@@ -225,16 +224,12 @@ dec5_kernel(const DecArgs a) {
 #pragma unroll
                         for (int w = 0; w < NW; ++w) q += red[NW + w];
                         const float var = __fdiv_rn(q, (float)d);
-                        const float den = a.eps_outside ? __fadd_rn(__fsqrt_rn(var), D.eps) : __fsqrt_rn(__fadd_rn(var, D.eps));
+                        const float den = LN_DEN(var, D.eps, a.eps_outside);
 #pragma unroll
                         for (int i = 0; i < PT; ++i) {
                             const int c = tid + i * NT;
                             if (c < nv) {
-                                float4 o;
-                                o.x = __fadd_rn(__fmul_rn(__fdiv_rn(v[i].x, den), g4[i].x), b4[i].x);
-                                o.y = __fadd_rn(__fmul_rn(__fdiv_rn(v[i].y, den), g4[i].y), b4[i].y);
-                                o.z = __fadd_rn(__fmul_rn(__fdiv_rn(v[i].z, den), g4[i].z), b4[i].z);
-                                o.w = __fadd_rn(__fmul_rn(__fdiv_rn(v[i].w, den), g4[i].w), b4[i].w);
+                                const float4 o = ln_norm4(v[i], den, g4[i], b4[i]);
                                 const int oks = D.ks, osl = (c * 4) / oks;   // slab-major output planes when the consuming linear stage splits K (oks == d: one slab)
                                 store_frag(xn_hi + osl * (PL_ROWS * oks / 8), xn_lo + osl * (PL_ROWS * oks / 8), oks >> 5, r, c * 4 - osl * oks, o);
                             }

@@ -298,7 +298,7 @@ __device__ __noinline__ Counters gemv_epi6(const Pipe P, Counters c, int N, int 
     return c;
 }
 
-// LayerNorm (burn 0.9 form, dec_common.cuh stage_ln) of the row x_s[D] by the 8 consumer warps: every warp computes the
+// LayerNorm (burn 0.9 form, prims.cuh) of the row x_s[D] by the 8 consumer warps: every warp computes the
 // statistics for itself (no block reduction), thread t normalises elements t, t + 256 and writes them as the B operand.
 template <int D>
 __device__ __noinline__ void ln6(const float* x_s, const float* g, const float* b, float eps, int eps_outside, uint8_t* bx) {
@@ -311,12 +311,12 @@ __device__ __noinline__ void ln6(const float* x_s, const float* g, const float* 
     const float mean = __fdiv_rn(sum, (float)D);
     float q = 0.0f;
 #pragma unroll
-    for (int i = 0; i < D / 32; ++i) { const float dv = __fsub_rn(v[i], mean); q = __fadd_rn(q, __fmul_rn(dv, dv)); }
+    for (int i = 0; i < D / 32; ++i) q = ln_sq_add(q, __fsub_rn(v[i], mean));
     q = warp_sum(q);
     const float var = __fdiv_rn(q, (float)D);
-    const float den = eps_outside ? __fadd_rn(__fsqrt_rn(var), eps) : __fsqrt_rn(__fadd_rn(var, eps));
+    const float den = LN_DEN(var, eps, eps_outside);
 #pragma unroll 1
-    for (int c = tid; c < D; c += 256) bx_store(bx, c, __fadd_rn(__fmul_rn(__fdiv_rn(__fsub_rn(x_s[c], mean), den), g[c]), b[c]));
+    for (int c = tid; c < D; c += 256) bx_store(bx, c, ln_norm(__fsub_rn(x_s[c], mean), den, g, b, c));
 }
 
 // merges the 8 per-warp attention records (wm, wl, wo) into the head's un-normalised output, written as the B operand of the
@@ -1001,22 +1001,16 @@ dec6_kernel(const DecArgs a) {
 #pragma unroll
                         for (int i = 0; i < NV; ++i) {
                             v[i].x = __fsub_rn(v[i].x, mean); v[i].y = __fsub_rn(v[i].y, mean); v[i].z = __fsub_rn(v[i].z, mean); v[i].w = __fsub_rn(v[i].w, mean);
-                            q = __fadd_rn(q, __fmul_rn(v[i].x, v[i].x)); q = __fadd_rn(q, __fmul_rn(v[i].y, v[i].y));
-                            q = __fadd_rn(q, __fmul_rn(v[i].z, v[i].z)); q = __fadd_rn(q, __fmul_rn(v[i].w, v[i].w));
+                            q = ln_sq_add4(q, v[i]);
                         }
                         q = warp_sum(q);
                         const float var = __fdiv_rn(q, (float)D);
-                        const float den = a.eps_outside ? __fadd_rn(__fsqrt_rn(var), a.lnf_eps) : __fsqrt_rn(__fadd_rn(var, a.lnf_eps));
+                        const float den = LN_DEN(var, a.lnf_eps, a.eps_outside);
 #pragma unroll
                         for (int i = 0; i < NV; ++i) {
                             const float4 g4 = __ldg(reinterpret_cast<const float4*>(a.lnf_g) + lane + 32 * i);
                             const float4 b4 = __ldg(reinterpret_cast<const float4*>(a.lnf_b) + lane + 32 * i);
-                            float4 o;
-                            o.x = __fadd_rn(__fmul_rn(__fdiv_rn(v[i].x, den), g4.x), b4.x);
-                            o.y = __fadd_rn(__fmul_rn(__fdiv_rn(v[i].y, den), g4.y), b4.y);
-                            o.z = __fadd_rn(__fmul_rn(__fdiv_rn(v[i].z, den), g4.z), b4.z);
-                            o.w = __fadd_rn(__fmul_rn(__fdiv_rn(v[i].w, den), g4.w), b4.w);
-                            store_frag(pl_hi, pl_lo, D / 32, r, (lane + 32 * i) * 4, o);
+                            store_frag(pl_hi, pl_lo, D / 32, r, (lane + 32 * i) * 4, ln_norm4(v[i], den, g4, b4));
                         }
                     } else {
 #pragma unroll

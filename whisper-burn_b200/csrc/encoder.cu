@@ -10,53 +10,25 @@ namespace {
 
 constexpr int LN_MAX_PER_LANE = 40;   // d <= 1280
 
-// One warp per row.  burn 0.9 LayerNorm: mean, biased variance of (x-mean), then
-// (x-mean)/(sqrt(var)+eps) [eps_outside] or (x-mean)/sqrt(var+eps); * gamma + beta as separate ops.
-__global__ void __launch_bounds__(256)
-layernorm_kernel(const float* __restrict__ x, float* __restrict__ y, const float* __restrict__ g,
-                 const float* __restrict__ b, float eps, int eps_outside, int rows, int d) {
-    const int row = blockIdx.x * 8 + (threadIdx.x >> 5);
-    if (row >= rows) return;
-    const int lane = threadIdx.x & 31;
-    const float* xr = x + (int64_t)row * d;
-    float v[LN_MAX_PER_LANE];
-    float s = 0.0f;
-#pragma unroll
-    for (int i = 0; i < LN_MAX_PER_LANE; ++i) {
-        const int c = i * 32 + lane;
-        v[i] = c < d ? xr[c] : 0.0f;
-        s += v[i];
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    const float mean = __fdiv_rn(s, (float)d);
-    float q = 0.0f;
-#pragma unroll
-    for (int i = 0; i < LN_MAX_PER_LANE; ++i) {
-        const int c = i * 32 + lane;
-        const float dv = __fsub_rn(v[i], mean);
-        v[i] = dv;
-        if (c < d) q = __fadd_rn(q, __fmul_rn(dv, dv));
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
-    const float var = __fdiv_rn(q, (float)d);
-    const float den = eps_outside ? __fadd_rn(__fsqrt_rn(var), eps) : __fsqrt_rn(__fadd_rn(var, eps));
-    float* yr = y + (int64_t)row * d;
-#pragma unroll
-    for (int i = 0; i < LN_MAX_PER_LANE; ++i) {
-        const int c = i * 32 + lane;
-        if (c < d) {
-            yr[c] = __fadd_rn(__fmul_rn(__fdiv_rn(v[i], den), g[c]), b[c]);
-        }
-    }
+// Where a LayerNorm row goes: fp32 rows y, or fp16 hi / lo planes (x = hi + lo / 2048, prims.cuh) for the tensor-core GEMM
+// that consumes the row, with the fp32 rows as well when y is non-null (ln_post: the encoder output returned through the ABI).
+struct LnPlanes {
+    float* y;
+    __half* hi;
+    __half* lo;
+};
+__device__ __forceinline__ void ln_store(float* y, int64_t i, float o) { y[i] = o; }
+__device__ __forceinline__ void ln_store(const LnPlanes& p, int64_t i, float o) {
+    if (p.y) p.y[i] = o;
+    hl_split(o, p.hi[i], p.lo[i]);
 }
 
-// Same LayerNorm, output as fp16 hi / lo planes (x = hi + lo / 2048, prims.cuh) for the tensor-core GEMM that consumes the row;
-// y (fp32 rows) is written as well when non-null (ln_post: the encoder output returned through the ABI).
+// One warp per row: burn 0.9 LayerNorm (prims.cuh) of x into out (float* or LnPlanes).  The two instances replace the former
+// layernorm_kernel (fp32 rows) and layernorm_f16_kernel (planes), the names the LayerNorm-eps tests still use.
+template <typename Out>
 __global__ void __launch_bounds__(256)
-layernorm_f16_kernel(const float* __restrict__ x, float* __restrict__ y, __half* __restrict__ y_hi, __half* __restrict__ y_lo,
-                     const float* __restrict__ g, const float* __restrict__ b, float eps, int eps_outside, int rows, int d) {
+layernorm_kernel(const float* __restrict__ x, Out out, const float* __restrict__ g, const float* __restrict__ b, float eps,
+                 int eps_outside, int rows, int d) {
     const int row = blockIdx.x * 8 + (threadIdx.x >> 5);
     if (row >= rows) return;
     const int lane = threadIdx.x & 31;
@@ -78,19 +50,17 @@ layernorm_f16_kernel(const float* __restrict__ x, float* __restrict__ y, __half*
         const int c = i * 32 + lane;
         const float dv = __fsub_rn(v[i], mean);
         v[i] = dv;
-        if (c < d) q = __fadd_rn(q, __fmul_rn(dv, dv));
+        if (c < d) q = ln_sq_add(q, dv);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
     const float var = __fdiv_rn(q, (float)d);
-    const float den = eps_outside ? __fadd_rn(__fsqrt_rn(var), eps) : __fsqrt_rn(__fadd_rn(var, eps));
+    const float den = LN_DEN(var, eps, eps_outside);
 #pragma unroll
     for (int i = 0; i < LN_MAX_PER_LANE; ++i) {
         const int c = i * 32 + lane;
         if (c < d) {
-            const float o = __fadd_rn(__fmul_rn(__fdiv_rn(v[i], den), g[c]), b[c]);
-            if (y) y[(int64_t)row * d + c] = o;
-            hl_split(o, y_hi[(int64_t)row * d + c], y_lo[(int64_t)row * d + c]);
+            ln_store(out, (int64_t)row * d + c, ln_norm(v[i], den, g, b, c));
         }
     }
 }
@@ -231,18 +201,15 @@ enc_attention_kernel(const float* __restrict__ qkv, float* __restrict__ out, con
 
 }  // namespace
 
-void launch_layernorm(const float* x, float* y, const LayerNormW& ln, int rows, int d, int eps_outside, cudaStream_t st) {
+void launch_layernorm(const float* x, float* y, __half* y_hi, __half* y_lo, const LayerNormW& ln, int rows, int d, int eps_outside,
+                      cudaStream_t st) {
     WB_REQUIRE(d <= 32 * LN_MAX_PER_LANE, "layernorm: d too large");
+    WB_REQUIRE((y_hi == nullptr) == (y_lo == nullptr), "layernorm: hi and lo planes go together");
     if (rows <= 0) return;
-    layernorm_kernel<<<(rows + 7) / 8, 256, 0, st>>>(x, y, ln.g, ln.b, ln.eps, eps_outside, rows, d);
-    WB_LAUNCH_CHECK();
-}
-
-void launch_layernorm_f16(const float* x, float* y, __half* y_hi, __half* y_lo, const LayerNormW& ln, int rows, int d, int eps_outside,
-                          cudaStream_t st) {
-    WB_REQUIRE(d <= 32 * LN_MAX_PER_LANE, "layernorm: d too large");
-    if (rows <= 0) return;
-    layernorm_f16_kernel<<<(rows + 7) / 8, 256, 0, st>>>(x, y, y_hi, y_lo, ln.g, ln.b, ln.eps, eps_outside, rows, d);
+    if (y_hi)
+        layernorm_kernel<<<(rows + 7) / 8, 256, 0, st>>>(x, LnPlanes{y, y_hi, y_lo}, ln.g, ln.b, ln.eps, eps_outside, rows, d);
+    else
+        layernorm_kernel<<<(rows + 7) / 8, 256, 0, st>>>(x, y, ln.g, ln.b, ln.eps, eps_outside, rows, d);
     WB_LAUNCH_CHECK();
 }
 

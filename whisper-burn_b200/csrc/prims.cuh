@@ -1,5 +1,5 @@
 // PTX primitives of the tensor-core and async-copy kernels, each defined once: shared-memory addresses, mbarriers,
-// asynchronous copies, the m16n8k16 MMA, the erf GELU and the fp16 hi/lo split of fp32 activations.
+// asynchronous copies, the m16n8k16 MMA, the erf GELU, the LayerNorm arithmetic and the fp16 hi/lo split of fp32 activations.
 // Internal; everything lives in an anonymous namespace of the including TU.
 #pragma once
 #include <cstdint>
@@ -79,6 +79,47 @@ __device__ __forceinline__ void mma16816(float (&c)[4], uint32_t a0, uint32_t a1
 __device__ __forceinline__ float gelu_erf(float x) {
     const float t = __fadd_rn(erff(__fdiv_rn(x, 1.41421356237309504880f)), 1.0f);
     return __fdiv_rn(__fmul_rn(x, t), 2.0f);
+}
+
+// ---- LayerNorm arithmetic ------------------------------------------------------------------------------
+// burn 0.9 nn::LayerNorm (layer_norm in oracle/model.py): mean, biased variance of dv = x - mean, then dv / den * gamma + beta,
+// every op rounded on its own as the reference issues them as separate tensor ops (no FMA contraction).  Each kernel keeps its
+// own loads, reduction order and row mapping; only the arithmetic below is shared.
+// LN_DEN: burn 0.9 divides by sqrt(var) + eps (eps_outside, the default); later burn by sqrt(var + eps).  A macro, so that
+// eps is read after the eps_outside test, inside the branch, as the kernels always have: an inline function reads it ahead,
+// which reschedules decoder5's LayerNorm stage.
+#define LN_DEN(var, eps, eps_outside) ((eps_outside) ? __fadd_rn(__fsqrt_rn(var), (eps)) : __fsqrt_rn(__fadd_rn((var), (eps))))
+// the centred square sum: q += dv * dv; the float4 form adds x, y, z, w in that order
+__device__ __forceinline__ float ln_sq_add(float q, float dv) { return __fadd_rn(q, __fmul_rn(dv, dv)); }
+__device__ __forceinline__ float ln_sq_add4(float q, const float4 dv) {
+    q = ln_sq_add(q, dv.x); q = ln_sq_add(q, dv.y);
+    q = ln_sq_add(q, dv.z); return ln_sq_add(q, dv.w);
+}
+// the normalisation dv / den * gamma + beta.  The scalar form reads g[c] and b[c] itself, after the divide, where the kernels
+// have always read them (gamma and beta passed in by value are loaded, and scheduled, ahead of it); LDG reads them through the
+// read-only data cache (__ldg: global memory only).  The float4 form takes the vectors every caller loads ahead of it.
+template <bool LDG = false>
+__device__ __forceinline__ float ln_norm(float dv, float den, const float* g, const float* b, int c) {
+    return __fadd_rn(__fmul_rn(__fdiv_rn(dv, den), LDG ? __ldg(g + c) : g[c]), LDG ? __ldg(b + c) : b[c]);
+}
+__device__ __forceinline__ float4 ln_norm4(const float4 dv, float den, const float4 g, const float4 b) {
+    float4 o;
+    o.x = __fadd_rn(__fmul_rn(__fdiv_rn(dv.x, den), g.x), b.x);
+    o.y = __fadd_rn(__fmul_rn(__fdiv_rn(dv.y, den), g.y), b.y);
+    o.z = __fadd_rn(__fmul_rn(__fdiv_rn(dv.z, den), g.z), b.z);
+    o.w = __fadd_rn(__fmul_rn(__fdiv_rn(dv.w, den), g.w), b.w);
+    return o;
+}
+// decoder4's LayerNorm (ln_warp) is the one exception to the separate roundings above, for the headline decoder's speed: the
+// square sum contracts into fmaf, and the normalisation multiplies by rinv = 1 / den (<= 1.5 ulp from the divide) and
+// contracts the beta add, fmaf(dv * rinv, g, b).  The eps placement (LN_DEN) is the same.
+__device__ __forceinline__ float ln_sq_fma4(float q, const float4 dv) {
+    q = fmaf(dv.x, dv.x, q); q = fmaf(dv.y, dv.y, q);
+    q = fmaf(dv.z, dv.z, q); return fmaf(dv.w, dv.w, q);
+}
+__device__ __forceinline__ float4 ln_norm4_rcp(const float4 dv, float rinv, const float4 g, const float4 b) {
+    return make_float4(fmaf(__fmul_rn(dv.x, rinv), g.x, b.x), fmaf(__fmul_rn(dv.y, rinv), g.y, b.y),
+                       fmaf(__fmul_rn(dv.z, rinv), g.z, b.z), fmaf(__fmul_rn(dv.w, rinv), g.w, b.w));
 }
 
 // ---- fp16 hi/lo split of fp32 activations -------------------------------------------------------------

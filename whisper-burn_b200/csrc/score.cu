@@ -153,7 +153,7 @@ void Session::score_tokens(int64_t n_seqs, const int32_t* window_of_seq, const i
             const size_t site = (size_t)6 * l;
             GemmF16Params p;
             // x = x + attn(attn_ln(x), causal mask)   (mod.rs:345, 428-436)
-            launch_layernorm_f16(w.x.p, nullptr, w.xn_h.p, w.xn_l.p, B.attn_ln, M, d, m->ln_eps_outside, st);
+            launch_layernorm(w.x.p, nullptr, w.xn_h.p, w.xn_l.p, B.attn_ln, M, d, m->ln_eps_outside, st);
             p.A_hi = w.xn_h.p; p.A_lo = w.xn_l.p; p.lda = d; p.B = B.qkv.w16; p.P_hi = w.qkv_h.p; p.P_lo = w.qkv_l.p; p.ldc = 3 * d;
             p.N = 3 * d; p.K = d; p.bias = B.qkv.b; p.scale = qk_scale; p.scale_cols = 2 * d; p.max_rows = M;
             gemm(site, p);
@@ -163,7 +163,7 @@ void Session::score_tokens(int64_t n_seqs, const int32_t* window_of_seq, const i
             p.bias = B.out.b; p.residual = w.x.p; p.max_rows = M;
             gemm(site + 1, p);
             // x = x + cross_attn(cross_attn_ln(x), xa)   (mod.rs:347, 482-490); K/V: the window's cached head-major block
-            launch_layernorm_f16(w.x.p, nullptr, w.xn_h.p, w.xn_l.p, B.cross_ln, M, d, m->ln_eps_outside, st);
+            launch_layernorm(w.x.p, nullptr, w.xn_h.p, w.xn_l.p, B.cross_ln, M, d, m->ln_eps_outside, st);
             p = GemmF16Params{};
             p.A_hi = w.xn_h.p; p.A_lo = w.xn_l.p; p.lda = d; p.B = B.cq.w16; p.P_hi = w.qkv_h.p; p.P_lo = w.qkv_l.p; p.ldc = d;
             p.N = d; p.K = d; p.bias = B.cq.b; p.scale = qk_scale; p.scale_cols = d; p.max_rows = M;
@@ -176,7 +176,7 @@ void Session::score_tokens(int64_t n_seqs, const int32_t* window_of_seq, const i
             p.bias = B.cout.b; p.residual = w.x.p; p.max_rows = M;
             gemm(site + 3, p);
             // x = x + mlp(mlp_ln(x))   (mod.rs:348, 376-382)
-            launch_layernorm_f16(w.x.p, nullptr, w.xn_h.p, w.xn_l.p, B.mlp_ln, M, d, m->ln_eps_outside, st);
+            launch_layernorm(w.x.p, nullptr, w.xn_h.p, w.xn_l.p, B.mlp_ln, M, d, m->ln_eps_outside, st);
             p = GemmF16Params{};
             p.A_hi = w.xn_h.p; p.A_lo = w.xn_l.p; p.lda = d; p.B = B.mlp1.w16; p.P_hi = w.hid_h.p; p.P_lo = w.hid_l.p; p.ldc = 4 * d;
             p.N = 4 * d; p.K = d; p.bias = B.mlp1.b; p.act = ACT_GELU; p.max_rows = M;
@@ -187,7 +187,7 @@ void Session::score_tokens(int64_t n_seqs, const int32_t* window_of_seq, const i
             gemm(site + 5, p);
         }
         // logits = ln(x) tok_emb^T (mod.rs:153-156), reduced to per-tile statistics, then combined per row
-        launch_layernorm_f16(w.x.p, nullptr, w.xn_h.p, w.xn_l.p, m->dec_ln, M, d, m->ln_eps_outside, st);
+        launch_layernorm(w.x.p, nullptr, w.xn_h.p, w.xn_l.p, m->dec_ln, M, d, m->ln_eps_outside, st);
         LogitStatsParams lsp;
         lsp.A_hi = w.xn_h.p; lsp.A_lo = w.xn_l.p; lsp.E = m->tok_emb16; lsp.rows = M; lsp.K = d; lsp.V = V;
         lsp.target = w.target.p; lsp.row_mask = apply_mask ? w.row_mask.p : nullptr; lsp.is_special = w.special.p;

@@ -287,7 +287,7 @@ void Session::run_encoder_f16() {
         const EncBlockW& B = m->enc[(size_t)l];
         const size_t site = (size_t)2 + 4 * l;
         // x = x + attn(attn_ln(x))   (mod.rs:300)
-        launch_layernorm_f16(x.p, nullptr, xn_h.p, xn_l.p, B.attn_ln, M, d, m->ln_eps_outside, st);
+        launch_layernorm(x.p, nullptr, xn_h.p, xn_l.p, B.attn_ln, M, d, m->ln_eps_outside, st);
         p = GemmF16Params{};
         p.A_hi = xn_h.p; p.A_lo = xn_l.p; p.lda = d; p.B = B.qkv.w16; p.P_hi = qkv_h.p; p.P_lo = qkv_l.p; p.ldc = 3 * d; p.N = 3 * d; p.K = d;
         p.bias = B.qkv.b; p.scale = qk_scale; p.scale_cols = 2 * d; p.max_rows = M;
@@ -298,7 +298,7 @@ void Session::run_encoder_f16() {
         p.bias = B.out.b; p.residual = x.p; p.max_rows = M;
         run(site + 1, p, 0, M);
         // x = x + mlp(mlp_ln(x))     (mod.rs:301); the MLP1 epilogue (bias + GELU) emits the hidden layer as planes
-        launch_layernorm_f16(x.p, nullptr, xn_h.p, xn_l.p, B.mlp_ln, M, d, m->ln_eps_outside, st);
+        launch_layernorm(x.p, nullptr, xn_h.p, xn_l.p, B.mlp_ln, M, d, m->ln_eps_outside, st);
         p = GemmF16Params{};
         p.A_hi = xn_h.p; p.A_lo = xn_l.p; p.lda = d; p.B = B.mlp1.w16; p.P_hi = hid_h.p; p.P_lo = hid_l.p; p.ldc = 4 * d; p.N = 4 * d; p.K = d;
         p.bias = B.mlp1.b; p.act = ACT_GELU; p.max_rows = M;
@@ -308,7 +308,7 @@ void Session::run_encoder_f16() {
         p.bias = B.mlp2.b; p.residual = x.p; p.max_rows = M;
         run(site + 3, p, 0, M);
     }
-    launch_layernorm_f16(x.p, xa.p, xa_h.p, xa_l.p, m->ln_post, M, d, m->ln_eps_outside, st);   // mod.rs:259
+    launch_layernorm(x.p, xa.p, xa_h.p, xa_l.p, m->ln_post, M, d, m->ln_eps_outside, st);   // mod.rs:259
 }
 
 // fp32 CUDA-core encoder: weights that are not exactly representable in fp16
@@ -329,7 +329,7 @@ void Session::run_encoder_f32() {
     launch_gemm(p, st);
     for (int l = 0; l < D.n_audio_layer; ++l) {
         const EncBlockW& B = m->enc[(size_t)l];
-        launch_layernorm(x.p, xn.p, B.attn_ln, M, d, m->ln_eps_outside, st);
+        launch_layernorm(x.p, xn.p, nullptr, nullptr, B.attn_ln, M, d, m->ln_eps_outside, st);
         p = GemmParams{};
         p.A = xn.p; p.lda = d; p.B = B.qkv.w32; p.C = qkv.p; p.ldc = 3 * d; p.N = 3 * d; p.K = d;
         p.bias = B.qkv.b; p.scale = qk_scale; p.scale_cols = 2 * d; p.max_rows = M;
@@ -339,7 +339,7 @@ void Session::run_encoder_f32() {
         p.A = att.p; p.lda = d; p.B = B.out.w32; p.C = x.p; p.ldc = d; p.N = d; p.K = d;
         p.bias = B.out.b; p.residual = x.p; p.max_rows = M;
         launch_gemm(p, st);
-        launch_layernorm(x.p, xn.p, B.mlp_ln, M, d, m->ln_eps_outside, st);
+        launch_layernorm(x.p, xn.p, nullptr, nullptr, B.mlp_ln, M, d, m->ln_eps_outside, st);
         p = GemmParams{};
         p.A = xn.p; p.lda = d; p.B = B.mlp1.w32; p.C = hid.p; p.ldc = 4 * d; p.N = 4 * d; p.K = d;
         p.bias = B.mlp1.b; p.act = ACT_GELU; p.max_rows = M;
@@ -349,7 +349,7 @@ void Session::run_encoder_f32() {
         p.bias = B.mlp2.b; p.residual = x.p; p.max_rows = M;
         launch_gemm(p, st);
     }
-    launch_layernorm(x.p, xa.p, m->ln_post, M, d, m->ln_eps_outside, st);   // mod.rs:259
+    launch_layernorm(x.p, xa.p, nullptr, nullptr, m->ln_post, M, d, m->ln_eps_outside, st);   // mod.rs:259
 }
 
 // cross keys (pre-scaled) | values of every decoder layer, projected once per window (mod.rs:484-485 hoisted out of the step loop)

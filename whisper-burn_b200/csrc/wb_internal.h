@@ -365,7 +365,10 @@ void resample_waveforms(ResampleBufs& b, const float* const* in, const int64_t* 
 // head-major re-layout of one layer's cross K|V rows (see encoder.cu)
 void launch_ckv_relayout(const float* src, void* dst, bool dst_half, const int64_t* win_row_off, const int* win_T, int n_windows,
                          int64_t M, int d, cudaStream_t st);
-void launch_layernorm(const float* x, float* y, const LayerNormW& ln, int rows, int d, int eps_outside, cudaStream_t st);
+// LayerNorm of rows [rows][d] into fp32 rows y, or, with planes y_hi / y_lo, into fp16 hi/lo planes (and into y as well when
+// it is non-null)
+void launch_layernorm(const float* x, float* y, __half* y_hi, __half* y_lo, const LayerNormW& ln, int rows, int d, int eps_outside,
+                      cudaStream_t st);
 struct AttnWindow {
     int64_t row_off;   // first packed row of the window
     int T;
@@ -384,8 +387,5 @@ void launch_causal_attention_tc(const __half* qkv_hi, const __half* qkv_lo, __ha
 void launch_cross_attention_tc(const __half* q_hi, const __half* q_lo, const void* ckv_layer, bool kv_f16, __half* out_hi, __half* out_lo,
                                const AttnWindow* seq_dev, const int* seq_win_dev, const int64_t* win_row_off_dev, const int* win_T_dev,
                                int n_seqs, int max_T, int d, int n_head, cudaStream_t st);
-// LayerNorm whose output leaves as fp16 hi/lo planes (and optionally as fp32 rows too: y may be null)
-void launch_layernorm_f16(const float* x, float* y, __half* y_hi, __half* y_lo, const LayerNormW& ln, int rows, int d, int eps_outside,
-                          cudaStream_t st);
 
 }  // namespace wb
