@@ -321,6 +321,43 @@ int wb_session_last_nbest(wb_session* s, int64_t index, int64_t max_hyps, int64_
 int wb_session_score_tokens(wb_session* s, int64_t n_seqs, const int32_t* window_of_seq, const int64_t* tokens,
                             const int64_t* lens, int apply_special_mask, const uint8_t* is_special,
                             float* lp_out, int64_t* argmax_out);
+/* Token alignment: when in the audio each token was spoken, by openai-whisper's find_alignment (whisper/timing.py), not by
+ * timestamp tokens: a teacher-forced pass over given ids on windows this session has encoded, the cross-attention weights of
+ * chosen heads, and dynamic time warping, all on the GPU.  The ids decoded are not touched.
+ * Sequences are packed as in wb_session_score_tokens: sequence i is tokens[off_i .. off_i + lens[i]) on window
+ * window_of_seq[i].  first[i] is the index of its first aligned id (4 for a default transcribe row, the prompt length for a
+ * previous-text row).  heads holds n_heads (layer, head) int32 pairs in any order; n_heads = 0 selects openai's fallback,
+ * every head of decoder layers n_text_layer / 2 .. n_text_layer - 1 (heads may then be NULL).
+ * For sequence ids[0 .. L) on window w, with first in [1, L - 1]:
+ *   1. columns C = max(1, F_w / 2), F_w the window's mel frames that hold audio (the kept frames of a waveform window without
+ *      the 10 zero frames; n_ctx for wb_session_encode_mels);
+ *   2. for every position p in 0 .. L - 1 and selected head: the scaled cross query of p against the window's scaled keys
+ *      0 .. C - 1 (the decoders' q and k; fp16-rounded keys under WB_KV_F16), then softmax over those C columns;
+ *   3. per head and column: minus the mean over the L positions, divided by the biased std (0 where the std is 0);
+ *   4. median filter of width 7 along the columns with reflect padding (torch's; scipy's "mirror"), skipped when C <= 3;
+ *   5. sum over the heads in ascending (layer, head) order divided by their count; rows first - 1 .. L - 2 are the matrix,
+ *      N = L - first rows (row k is the query that predicts ids[first + k]);
+ *   6. DTW on -matrix with openai's dtw_cpu rules: f32 cost; diagonal if c0 < c1 && c0 < c2, else up if c1 < c0 && c1 < c2,
+ *      else left; backtrace with row 0 read as left and column 0 as up;
+ *   7. start[k] = the column where the path first enters row k, end[k] = start[k + 1], end[N - 1] = C.
+ * start_out / end_out: per aligned id (sequence i's N_i ids after those of sequences 0 .. i-1) its int32 encoder positions;
+ * one position is 20 ms from the window's start in both window modes.  matrix_out (may be NULL): each sequence's matrix, f32
+ * [N_i][C_i], packed in sequence order, matrix_capacity floats.  Word grouping is text work and stays with the caller.
+ * Sequences run in groups of at most 4096 positions; the workspace holds one layer's selected heads of one group:
+ * heads x positions x C x 4 bytes.
+ * WB_ERR_STATE before an encode call; WB_ERR_INVALID_ARG for lens[i] outside [2, n_text_ctx], first[i] outside [1, lens[i] - 1],
+ * a token outside [0, n_vocab), a window outside the encoded ones, a head outside the model or listed twice, or matrix_capacity
+ * below sum N_i C_i; WB_ERR_UNSUPPORTED when the weights are not fp16-exact, or when a sequence's DTW does not fit one CTA
+ * (N_i > 448, or its 2-bit trace N_i x ceil(C_i / 16) x 4 bytes beyond ~221 KB of shared memory: only a model with
+ * n_audio_ctx above 2016 gets there; 447 x 1500 fits).  Leaves the session's decode state and every
+ * wb_session_last_* result as they were. */
+int wb_session_align_tokens(wb_session* s, int64_t n_seqs, const int32_t* window_of_seq, const int64_t* tokens,
+                            const int64_t* lens, const int64_t* first, int64_t n_heads, const int32_t* heads,
+                            int32_t* start_out, int32_t* end_out, float* matrix_out, int64_t matrix_capacity);
+/* Step 6 and 7 of wb_session_align_tokens alone, on a caller's f32 matrix [n_rows][n_cols] (host), on the GPU: start_out /
+ * end_out [n_rows].  n_rows in [1, 448], n_cols >= 1 with the 2-bit trace, n_rows x ceil(n_cols / 16) x 4 bytes, within one
+ * CTA's shared memory (~221 KB; 447 x 1500 fits).  WB_ERR_INVALID_ARG otherwise, WB_ERR_CUDA without a device. */
+int wb_align_dtw(int device, const float* matrix, int64_t n_rows, int64_t n_cols, int32_t* start_out, int32_t* end_out);
 /* transcribe.rs:114-138: number of windows and their [start, end) bounds */
 int64_t wb_window_count(int64_t n_samples, int64_t sample_rate, int64_t window_len);
 int wb_window_bounds(int64_t n_samples, int64_t sample_rate, int64_t window_len, int64_t* starts, int64_t* ends);

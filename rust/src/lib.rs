@@ -74,6 +74,9 @@ pub mod ffi {
                                                 sample_rates: *const i64, n_waveforms: i64, beam_size: c_int, max_depth: c_int,
                                                 ids: *const wb_special_ids, is_special: *const u8, tokens_out: *mut i64, capacity: i64,
                                                 n_tokens_out: *mut i64) -> c_int;
+        pub fn wb_session_align_tokens(s: *mut c_void, n_seqs: i64, window_of_seq: *const i32, tokens: *const i64, lens: *const i64,
+                                       first: *const i64, n_heads: i64, heads: *const i32, start_out: *mut i32, end_out: *mut i32,
+                                       matrix_out: *mut f32, matrix_capacity: i64) -> c_int;
     }
 }
 
@@ -392,6 +395,37 @@ pub mod transcribe {
         })?;
         let tokens: Vec<usize> = out[..n as usize].iter().map(|&t| t as usize).collect();
         Ok((bpe.decode(&tokens[..], true)?, tokens))
+    }
+
+    /// When each token of given sequences was spoken in one audio window: openai-whisper's find_alignment (cross-attention of
+    /// the decoder layers n_text_layer / 2 .., normalised, median-filtered, averaged, then dynamic time warping), all on the GPU
+    /// (wb_session_align_tokens).  The window is encoded in the cached session; sequence i's tokens from first[i] on are
+    /// aligned (4 for a transcribed row: after sot, language, transcribe, notimestamps).  Per aligned token its (start, end)
+    /// in seconds from the window's start.
+    pub fn align_tokens(whisper: &model::Whisper, waveform_window: &[f32], sequences: &[Vec<usize>], first: &[usize])
+            -> Result<Vec<Vec<(f64, f64)>>, Error> {
+        let lens: Vec<i64> = sequences.iter().map(|q| q.len() as i64).collect();
+        let tokens: Vec<i64> = sequences.iter().flatten().map(|&t| t as i64).collect();
+        let firsts: Vec<i64> = first.iter().map(|&f| f as i64).collect();
+        if firsts.len() != sequences.len() || sequences.iter().zip(first).any(|(q, &f)| f < 1 || f >= q.len()) {
+            return Err("align_tokens: one first index per sequence, in [1, len - 1]".into());
+        }
+        let windows = vec![0i32; sequences.len()];
+        let n_ids: usize = sequences.iter().zip(first).map(|(q, &f)| q.len() - f).sum();
+        let (mut start, mut end) = (vec![0i32; n_ids.max(1)], vec![0i32; n_ids.max(1)]);
+        whisper.with_session(1, 1, 2, |s| {
+            let (wave, n) = (waveform_window.as_ptr(), waveform_window.len() as i64);
+            check(unsafe { ffi::wb_session_encode_waveforms(s, &wave, &n, 1) })?;
+            check(unsafe { ffi::wb_session_align_tokens(s, sequences.len() as i64, windows.as_ptr(), tokens.as_ptr(), lens.as_ptr(),
+                                                        firsts.as_ptr(), 0, std::ptr::null(), start.as_mut_ptr(), end.as_mut_ptr(),
+                                                        std::ptr::null_mut(), 0) })
+        })?;
+        let mut off = 0;
+        Ok(sequences.iter().zip(first).map(|(q, &f)| {
+            let r = (off..off + q.len() - f).map(|k| (start[k] as f64 * 0.02, end[k] as f64 * 0.02)).collect();
+            off += q.len() - f;
+            r
+        }).collect())
     }
 
     /// What the transcribe binary does with a WAV file of any rate and channel count (src/bin/transcribe/main.rs:31-55 without

@@ -582,6 +582,24 @@ int wb_session_score_tokens(wb_session* s, int64_t n_seqs, const int32_t* window
     });
 }
 
+int wb_session_align_tokens(wb_session* s, int64_t n_seqs, const int32_t* window_of_seq, const int64_t* tokens, const int64_t* lens,
+                            const int64_t* first, int64_t n_heads, const int32_t* heads, int32_t* start_out, int32_t* end_out,
+                            float* matrix_out, int64_t matrix_capacity) {
+    return guarded([&] {
+        WB_REQUIRE(s && window_of_seq && tokens && lens && first && start_out && end_out, "align_tokens: null pointer");
+        s->impl->align_tokens(n_seqs, window_of_seq, tokens, lens, first, n_heads, heads, start_out, end_out, matrix_out, matrix_capacity);
+    });
+}
+
+int wb_align_dtw(int device, const float* matrix, int64_t n_rows, int64_t n_cols, int32_t* start_out, int32_t* end_out) {
+    return guarded([&] {
+        WB_REQUIRE(matrix && start_out && end_out, "align_dtw: null pointer");
+        WB_REQUIRE(wb::dtw_fits(n_rows, n_cols), "align_dtw: n_rows must be in [1, 448] and n_cols >= 1, with the 2-bit trace in one CTA's shared memory");
+        require_device(device);
+        wb::align_dtw(matrix, n_rows, n_cols, start_out, end_out);
+    });
+}
+
 int wb_find_chunk_overlap(const int64_t* prev, int64_t n_prev, const int64_t* curr, int64_t n_curr, int64_t max_n_offsets,
                           int64_t min_n_overlaps, int64_t* prev_index, int64_t* curr_index) {
     int64_t pi = 0, ci = 0;

@@ -20,38 +20,15 @@
 //     fp32 K/V are split hi/lo as they are staged.
 #include <cuda_fp16.h>
 
-#include "prims.cuh"
+#include "attn_tile.cuh"
 #include "wb_internal.h"
 
 namespace wb {
 
 namespace {
 
-constexpr int TQ = 64, TK = 64, HD = 64;
 constexpr int AT_THREADS = 128;
-constexpr int TILE_B = 64 * 128;                       // one [64][64] fp16 tile = 8 KB (rows of 128 bytes)
 constexpr size_t AT_SMEM = 2 * TILE_B + 2 * 4 * TILE_B;   // Q hi/lo + 2 stages x (K hi, K lo, V hi, V lo) = 80 KB
-
-__device__ __forceinline__ void cp16(uint32_t dst, const void* src, bool ok) {
-    const int sz = ok ? 16 : 0;   // zero-fill out-of-range rows
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(sz) : "memory");
-}
-// tile [64 rows][64 halves]: 16-byte chunk c of row r sits at r * 128 + ((c ^ (r & 7)) << 4)  (conflict-free ldmatrix)
-__device__ __forceinline__ uint32_t tile_off(int r, int c) { return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4)); }
-__device__ __forceinline__ void ldsm4(uint32_t addr, uint32_t& a, uint32_t& b, uint32_t& c, uint32_t& d) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm4t(uint32_t addr, uint32_t& a, uint32_t& b, uint32_t& c, uint32_t& d) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d) : "r"(addr));
-}
-__device__ __forceinline__ void mma(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) { mma16816(c, a[0], a[1], a[2], a[3], b0, b1); }
-// two fp32 values -> fp16 hi pair and fp16 lo pair, as the A / B fragment registers of an MMA
-__device__ __forceinline__ void split2(float x, float y, uint32_t& hi, uint32_t& lo) {
-    __half2 h, l;
-    hl_split_pair(x, y, h, l);
-    hi = h2_bits(h);
-    lo = h2_bits(l);
-}
 
 // One CTA: the 64 queries [q0, q0 + 64) of one head.  load_q(sQ) stages the Q tile (hi, lo); load_kv(stage_base, k0) stages
 // K hi, K lo, V hi, V lo of keys [k0, k0 + 64) (zero rows past Tk; the lo tiles are not read with KV16); o_hi / o_lo: the

@@ -9,6 +9,8 @@
 //   cross_attn_ln -> cross-query GEMM -> cross attention over the window's cached cross K/V -> cross-out GEMM + residual ->
 //   mlp_ln -> mlp1 (GELU) -> mlp2 + residual -> final LayerNorm -> logits GEMM with the statistics epilogue ->
 //   score_combine_kernel: log-prob of each row's target and its arg-max.
+// decoder_pass (embed and the layer loop) is shared with token alignment (align.cu), which builds a row for every position and
+// stops after the cross-query GEMM of the last layer it reads.
 // Numerics as the encoder's (DESIGN.md section 3): fp32 activations travel as fp16 hi/lo planes into fp16-exact weights, fp32
 // accumulation; the self and cross K/V of WB_KV_F16 sessions enter as their fp16 rounding, as in the persistent decoders.
 #include <climits>
@@ -19,10 +21,6 @@
 namespace wb {
 
 namespace {
-
-// rows per pass: sequences are scored in groups of whole sequences holding at most this many rows, so the workspace stays
-// bounded (~56 KB per row at d = 1280)
-constexpr int SCORE_GROUP_ROWS = 4096;
 
 // x[r] = tok_emb[token] + pos_emb[position]  (mod.rs:141-146), f32 add
 __global__ void score_embed_kernel(const int* __restrict__ tok, const int* __restrict__ pos, const float* __restrict__ tok_emb,
@@ -68,11 +66,77 @@ __global__ void score_combine_kernel(const float* __restrict__ tile_m, const flo
 
 }  // namespace
 
+void Session::decoder_pass(int M, int n, int max_T, int n_layers, bool full, const std::function<void(int)>& after_cross_query) {
+    const wb_dims& D = m->dims;
+    const int d = D.n_text_state, H = D.n_text_head, L = D.n_text_layer;
+    const bool kv16 = kv_dtype == WB_KV_F16;
+    ScoreWs& w = score_ws;
+    if (w.plans.empty()) {
+        w.plans.resize((size_t)6 * L);
+        for (auto& pl : w.plans) pl.reset(new GemmF16Plan());
+    }
+    auto gemm = [&](size_t site, const GemmF16Params& p) {
+        GemmF16Plan& pl = *w.plans[site];
+        pl.build(p, 0, p.max_rows);   // the workspace may have moved since the last call
+        pl.launch(st);
+    };
+    const size_t Pd = (size_t)M * d;
+    w.x.ensure(Pd); w.xn_h.ensure(Pd); w.xn_l.ensure(Pd); w.att_h.ensure(Pd); w.att_l.ensure(Pd);
+    w.qkv_h.ensure(3 * Pd); w.qkv_l.ensure(3 * Pd); w.hid_h.ensure(4 * Pd); w.hid_l.ensure(4 * Pd);
+
+    const float qk_scale = (float)std::pow((double)d / (double)H, -0.25);   // mod.rs:503
+    {
+        const int64_t n4 = (int64_t)M * d / 4;
+        score_embed_kernel<<<(int)std::min<int64_t>((n4 + 255) / 256, 132 * 8), 256, 0, st>>>(w.tok.p, w.pos.p, m->tok_emb32, m->dec_pos, w.x.p, M, d);
+        WB_LAUNCH_CHECK();
+    }
+    for (int l = 0; l < n_layers; ++l) {
+        const DecBlockW& B = m->dec[(size_t)l];
+        const size_t site = (size_t)6 * l;
+        GemmF16Params p;
+        // x = x + attn(attn_ln(x), causal mask)   (mod.rs:345, 428-436)
+        launch_layernorm(w.x.p, nullptr, w.xn_h.p, w.xn_l.p, B.attn_ln, M, d, m->ln_eps_outside, st);
+        p.A_hi = w.xn_h.p; p.A_lo = w.xn_l.p; p.lda = d; p.B = B.qkv.w16; p.P_hi = w.qkv_h.p; p.P_lo = w.qkv_l.p; p.ldc = 3 * d;
+        p.N = 3 * d; p.K = d; p.bias = B.qkv.b; p.scale = qk_scale; p.scale_cols = 2 * d; p.max_rows = M;
+        gemm(site, p);
+        launch_causal_attention_tc(w.qkv_h.p, w.qkv_l.p, w.att_h.p, w.att_l.p, w.seqs.p, n, max_T, d, H, kv16, st);
+        p = GemmF16Params{};
+        p.A_hi = w.att_h.p; p.A_lo = w.att_l.p; p.lda = d; p.B = B.out.w16; p.C = w.x.p; p.ldc = d; p.N = d; p.K = d;
+        p.bias = B.out.b; p.residual = w.x.p; p.max_rows = M;
+        gemm(site + 1, p);
+        // x = x + cross_attn(cross_attn_ln(x), xa)   (mod.rs:347, 482-490); K/V: the window's cached head-major block
+        launch_layernorm(w.x.p, nullptr, w.xn_h.p, w.xn_l.p, B.cross_ln, M, d, m->ln_eps_outside, st);
+        p = GemmF16Params{};
+        p.A_hi = w.xn_h.p; p.A_lo = w.xn_l.p; p.lda = d; p.B = B.cq.w16; p.P_hi = w.qkv_h.p; p.P_lo = w.qkv_l.p; p.ldc = d;
+        p.N = d; p.K = d; p.bias = B.cq.b; p.scale = qk_scale; p.scale_cols = d; p.max_rows = M;
+        gemm(site + 2, p);
+        if (after_cross_query) after_cross_query(l);
+        if (!full && l == n_layers - 1) break;
+        const void* ckv_l = kv16 ? (const void*)(ckv16.p + (size_t)l * Mcap * 2 * d) : (const void*)(ckv.p + (size_t)l * Mcap * 2 * d);
+        launch_cross_attention_tc(w.qkv_h.p, w.qkv_l.p, ckv_l, kv16, w.att_h.p, w.att_l.p, w.seqs.p, w.seq_win.p, d_win_row_off.p,
+                                  d_win_T.p, n, max_T, d, H, st);
+        p = GemmF16Params{};
+        p.A_hi = w.att_h.p; p.A_lo = w.att_l.p; p.lda = d; p.B = B.cout.w16; p.C = w.x.p; p.ldc = d; p.N = d; p.K = d;
+        p.bias = B.cout.b; p.residual = w.x.p; p.max_rows = M;
+        gemm(site + 3, p);
+        // x = x + mlp(mlp_ln(x))   (mod.rs:348, 376-382)
+        launch_layernorm(w.x.p, nullptr, w.xn_h.p, w.xn_l.p, B.mlp_ln, M, d, m->ln_eps_outside, st);
+        p = GemmF16Params{};
+        p.A_hi = w.xn_h.p; p.A_lo = w.xn_l.p; p.lda = d; p.B = B.mlp1.w16; p.P_hi = w.hid_h.p; p.P_lo = w.hid_l.p; p.ldc = 4 * d;
+        p.N = 4 * d; p.K = d; p.bias = B.mlp1.b; p.act = ACT_GELU; p.max_rows = M;
+        gemm(site + 4, p);
+        p = GemmF16Params{};
+        p.A_hi = w.hid_h.p; p.A_lo = w.hid_l.p; p.lda = 4 * d; p.B = B.mlp2.w16; p.C = w.x.p; p.ldc = d; p.N = d; p.K = 4 * d;
+        p.bias = B.mlp2.b; p.residual = w.x.p; p.max_rows = M;
+        gemm(site + 5, p);
+    }
+}
+
 void Session::score_tokens(int64_t n_seqs, const int32_t* window_of_seq, const int64_t* toks, const int64_t* lens, bool apply_mask,
                            const uint8_t* is_special_host, float* lp_out, int64_t* argmax_out) {
     if (!encoded) fail(WB_ERR_STATE, "score_tokens: no window encoded yet");
     const wb_dims& D = m->dims;
-    const int d = D.n_text_state, H = D.n_text_head, L = D.n_text_layer, V = D.n_vocab;
+    const int d = D.n_text_state, L = D.n_text_layer, V = D.n_vocab;
     WB_REQUIRE(n_seqs >= 1, "score_tokens: n_seqs must be >= 1");
     WB_REQUIRE(!apply_mask || is_special_host, "score_tokens: apply_special_mask needs is_special");
     std::vector<int64_t> off((size_t)n_seqs + 1, 0);
@@ -84,22 +148,12 @@ void Session::score_tokens(int64_t n_seqs, const int32_t* window_of_seq, const i
     for (int64_t p = 0; p < off[(size_t)n_seqs]; ++p) WB_REQUIRE(toks[p] >= 0 && toks[p] < V, "score_tokens: token outside [0, n_vocab)");
     if (!m->fp16_exact) fail(WB_ERR_UNSUPPORTED, "score_tokens: the weights are not fp16-exact (the scoring pass runs on the tensor cores only)");
 
-    const bool kv16 = kv_dtype == WB_KV_F16;
     const int n_tiles = logit_stats_tiles(V);
     ScoreWs& w = score_ws;
     if (apply_mask) {
         w.special.ensure((size_t)V);
         WB_CUDA(cudaMemcpyAsync(w.special.p, is_special_host, (size_t)V, cudaMemcpyHostToDevice, st));
     }
-    if (w.plans.empty()) {
-        w.plans.resize((size_t)6 * L);
-        for (auto& pl : w.plans) pl.reset(new GemmF16Plan());
-    }
-    auto gemm = [&](size_t site, const GemmF16Params& p) {
-        GemmF16Plan& pl = *w.plans[site];
-        pl.build(p, 0, p.max_rows);   // the workspace may have moved since the last call
-        pl.launch(st);
-    };
 
     for (int64_t s0 = 0; s0 < n_seqs;) {
         // ---- one group of whole sequences: host descriptors of its rows
@@ -126,13 +180,10 @@ void Session::score_tokens(int64_t n_seqs, const int32_t* window_of_seq, const i
         if (P == 0) { s0 = s1; continue; }
 
         // ---- workspace
-        const size_t Pd = (size_t)P * d;
         w.tok.ensure((size_t)P); w.pos.ensure((size_t)P); w.target.ensure((size_t)P); w.am.ensure((size_t)P);
         w.row_mask.ensure((size_t)P); w.seq_win.ensure((size_t)n); w.seqs.ensure((size_t)n);
-        w.x.ensure(Pd); w.tgt_logit.ensure((size_t)P); w.lp.ensure((size_t)P);
+        w.tgt_logit.ensure((size_t)P); w.lp.ensure((size_t)P);
         w.tile_m.ensure((size_t)P * n_tiles); w.tile_s.ensure((size_t)P * n_tiles); w.tile_i.ensure((size_t)P * n_tiles);
-        w.xn_h.ensure(Pd); w.xn_l.ensure(Pd); w.att_h.ensure(Pd); w.att_l.ensure(Pd);
-        w.qkv_h.ensure(3 * Pd); w.qkv_l.ensure(3 * Pd); w.hid_h.ensure(4 * Pd); w.hid_l.ensure(4 * Pd);
         WB_CUDA(cudaMemcpyAsync(w.tok.p, tok.data(), tok.size() * sizeof(int), cudaMemcpyHostToDevice, st));
         WB_CUDA(cudaMemcpyAsync(w.pos.p, pos.data(), pos.size() * sizeof(int), cudaMemcpyHostToDevice, st));
         WB_CUDA(cudaMemcpyAsync(w.target.p, tgt.data(), tgt.size() * sizeof(int), cudaMemcpyHostToDevice, st));
@@ -142,50 +193,7 @@ void Session::score_tokens(int64_t n_seqs, const int32_t* window_of_seq, const i
 
         // ---- the pass
         const int M = (int)P;
-        const float qk_scale = (float)std::pow((double)d / (double)H, -0.25);   // mod.rs:503
-        {
-            const int64_t n4 = (int64_t)M * d / 4;
-            score_embed_kernel<<<(int)std::min<int64_t>((n4 + 255) / 256, 132 * 8), 256, 0, st>>>(w.tok.p, w.pos.p, m->tok_emb32, m->dec_pos, w.x.p, M, d);
-            WB_LAUNCH_CHECK();
-        }
-        for (int l = 0; l < L; ++l) {
-            const DecBlockW& B = m->dec[(size_t)l];
-            const size_t site = (size_t)6 * l;
-            GemmF16Params p;
-            // x = x + attn(attn_ln(x), causal mask)   (mod.rs:345, 428-436)
-            launch_layernorm(w.x.p, nullptr, w.xn_h.p, w.xn_l.p, B.attn_ln, M, d, m->ln_eps_outside, st);
-            p.A_hi = w.xn_h.p; p.A_lo = w.xn_l.p; p.lda = d; p.B = B.qkv.w16; p.P_hi = w.qkv_h.p; p.P_lo = w.qkv_l.p; p.ldc = 3 * d;
-            p.N = 3 * d; p.K = d; p.bias = B.qkv.b; p.scale = qk_scale; p.scale_cols = 2 * d; p.max_rows = M;
-            gemm(site, p);
-            launch_causal_attention_tc(w.qkv_h.p, w.qkv_l.p, w.att_h.p, w.att_l.p, w.seqs.p, n, max_T, d, H, kv16, st);
-            p = GemmF16Params{};
-            p.A_hi = w.att_h.p; p.A_lo = w.att_l.p; p.lda = d; p.B = B.out.w16; p.C = w.x.p; p.ldc = d; p.N = d; p.K = d;
-            p.bias = B.out.b; p.residual = w.x.p; p.max_rows = M;
-            gemm(site + 1, p);
-            // x = x + cross_attn(cross_attn_ln(x), xa)   (mod.rs:347, 482-490); K/V: the window's cached head-major block
-            launch_layernorm(w.x.p, nullptr, w.xn_h.p, w.xn_l.p, B.cross_ln, M, d, m->ln_eps_outside, st);
-            p = GemmF16Params{};
-            p.A_hi = w.xn_h.p; p.A_lo = w.xn_l.p; p.lda = d; p.B = B.cq.w16; p.P_hi = w.qkv_h.p; p.P_lo = w.qkv_l.p; p.ldc = d;
-            p.N = d; p.K = d; p.bias = B.cq.b; p.scale = qk_scale; p.scale_cols = d; p.max_rows = M;
-            gemm(site + 2, p);
-            const void* ckv_l = kv16 ? (const void*)(ckv16.p + (size_t)l * Mcap * 2 * d) : (const void*)(ckv.p + (size_t)l * Mcap * 2 * d);
-            launch_cross_attention_tc(w.qkv_h.p, w.qkv_l.p, ckv_l, kv16, w.att_h.p, w.att_l.p, w.seqs.p, w.seq_win.p, d_win_row_off.p,
-                                      d_win_T.p, n, max_T, d, H, st);
-            p = GemmF16Params{};
-            p.A_hi = w.att_h.p; p.A_lo = w.att_l.p; p.lda = d; p.B = B.cout.w16; p.C = w.x.p; p.ldc = d; p.N = d; p.K = d;
-            p.bias = B.cout.b; p.residual = w.x.p; p.max_rows = M;
-            gemm(site + 3, p);
-            // x = x + mlp(mlp_ln(x))   (mod.rs:348, 376-382)
-            launch_layernorm(w.x.p, nullptr, w.xn_h.p, w.xn_l.p, B.mlp_ln, M, d, m->ln_eps_outside, st);
-            p = GemmF16Params{};
-            p.A_hi = w.xn_h.p; p.A_lo = w.xn_l.p; p.lda = d; p.B = B.mlp1.w16; p.P_hi = w.hid_h.p; p.P_lo = w.hid_l.p; p.ldc = 4 * d;
-            p.N = 4 * d; p.K = d; p.bias = B.mlp1.b; p.act = ACT_GELU; p.max_rows = M;
-            gemm(site + 4, p);
-            p = GemmF16Params{};
-            p.A_hi = w.hid_h.p; p.A_lo = w.hid_l.p; p.lda = 4 * d; p.B = B.mlp2.w16; p.C = w.x.p; p.ldc = d; p.N = d; p.K = 4 * d;
-            p.bias = B.mlp2.b; p.residual = w.x.p; p.max_rows = M;
-            gemm(site + 5, p);
-        }
+        decoder_pass(M, n, max_T, L, true, nullptr);
         // logits = ln(x) tok_emb^T (mod.rs:153-156), reduced to per-tile statistics, then combined per row
         launch_layernorm(w.x.p, nullptr, w.xn_h.p, w.xn_l.p, m->dec_ln, M, d, m->ln_eps_outside, st);
         LogitStatsParams lsp;

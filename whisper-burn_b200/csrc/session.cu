@@ -145,9 +145,10 @@ Session::~Session() {
 }
 
 // ---- geometry helpers -------------------------------------------------------------------------
-static void set_geometry(Session& s, const std::vector<int>& Tm) {
+static void set_geometry(Session& s, const std::vector<int>& Tm, const std::vector<int>& F) {
     s.n_windows = (int)Tm.size();
     s.win_Tm = Tm;
+    s.win_F = F;
     s.win_T.resize(Tm.size());
     s.win_row_off.resize(Tm.size());
     s.M_tot = 0;
@@ -182,7 +183,7 @@ static void set_geometry(Session& s, const std::vector<int>& Tm) {
 void Session::encode_from_device_wave(const float* wave_dev, const int64_t* offsets, const int64_t* lens, int64_t n) {
     WB_REQUIRE(n >= 1 && n <= max_windows, "encode: n_windows out of range for this session");
     std::vector<LogMelWindow> lw((size_t)n);
-    std::vector<int> Tm((size_t)n);
+    std::vector<int> Tm((size_t)n), kept((size_t)n);
     int max_frames = 0;
     for (int64_t w = 0; w < n; ++w) {
         WB_REQUIRE(lens[w] >= N_FFT, "prep_audio: waveform shorter than n_fft (audio.rs:292)");
@@ -190,11 +191,12 @@ void Session::encode_from_device_wave(const float* wave_dev, const int64_t* offs
         const int F = (int)(lens[w] / HOP);                        // frames after dropping the last one
         const int keep = std::min(F, mel_limit - MEL_PADDING);      // transcribe.rs:173
         Tm[(size_t)w] = keep + MEL_PADDING;
+        kept[(size_t)w] = keep;
         lw[(size_t)w] = LogMelWindow{offsets[w], (int)lens[w], F, keep, (int)w, ((int64_t)w * TmS + 1) * N_MELS};
         max_frames = std::max(max_frames, F);
     }
     WB_CUDA(cudaMemcpyAsync(d_lmwin.p, lw.data(), lw.size() * sizeof(LogMelWindow), cudaMemcpyHostToDevice, st));
-    set_geometry(*this, Tm);   // syncs, so `lw` may go out of scope
+    set_geometry(*this, Tm, kept);   // syncs, so `lw` may go out of scope
     WB_CUDA(cudaEventRecord(ev[0], st));
     WB_CUDA(cudaMemsetAsync(mel_rows.p, 0, (size_t)n * TmS * N_MELS * sizeof(float), st));   // halo + 10 zero frames
     launch_logmel(*m, wave_dev, d_lmwin.p, (int)n, max_frames, mel_rows.p, max_slots.p, (int)n, st);
@@ -226,7 +228,7 @@ void Session::encode_mels_host(const float* mel, int64_t n, int64_t n_mels, int6
                                                  "2 * n_audio_ctx in native windowing (mod.rs:236-241)");
     WB_REQUIRE(n >= 1 && n <= max_windows, "encode: n_windows out of range for this session");
     std::vector<int> Tm((size_t)n, (int)n_ctx);
-    set_geometry(*this, Tm);
+    set_geometry(*this, Tm, Tm);
     DevBuf<float> tmp;
     tmp.alloc((size_t)n * n_mels * n_ctx);
     WB_CUDA(cudaMemcpyAsync(tmp.p, mel, tmp.n * sizeof(float), cudaMemcpyHostToDevice, st));
@@ -240,7 +242,7 @@ void Session::encode_mels_host(const float* mel, int64_t n, int64_t n_mels, int6
 void Session::load_encoder_output_host(const float* xa_host, int64_t n, int64_t T) {
     WB_REQUIRE(n >= 1 && n <= max_windows && T >= 1 && T <= Tcap, "forward_decoder: encoder output shape out of range");
     std::vector<int> Tm((size_t)n, (int)(2 * T - 1));   // any Tm with (Tm-1)/2+1 == T
-    set_geometry(*this, Tm);
+    set_geometry(*this, Tm, std::vector<int>((size_t)n, (int)(2 * T)));   // every encoder position holds audio
     const int d = m->dims.n_audio_state;
     WB_CUDA(cudaMemcpyAsync(xa.p, xa_host, (size_t)n * T * d * sizeof(float), cudaMemcpyHostToDevice, st));
     if (use_tc) launch_split_f16(xa.p, xa_h.p, xa_l.p, (int64_t)n * T * d, st);

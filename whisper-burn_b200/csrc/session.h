@@ -56,7 +56,11 @@ struct DecodeLaunch {
     }
 };
 
-// workspace of token scoring (score.cu), grown on demand
+// rows per pass of the teacher-forced decoder (token scoring, token alignment): sequences run in groups of whole sequences holding
+// at most this many rows, so the workspace stays bounded (~56 KB per row at d = 1280)
+constexpr int SCORE_GROUP_ROWS = 4096;
+
+// workspace of token scoring (score.cu) and of the decoder pass token alignment shares with it, grown on demand
 struct ScoreWs {
     DevBuf<int> tok, pos, target, seq_win, tile_i, am;   // per row: input token, position, target id; per sequence: window
     DevBuf<uint8_t> row_mask, special;
@@ -64,6 +68,20 @@ struct ScoreWs {
     DevBuf<float> x, tile_m, tile_s, tgt_logit, lp;
     DevBuf<__half> xn_h, xn_l, qkv_h, qkv_l, att_h, att_l, hid_h, hid_l;
     std::vector<std::unique_ptr<GemmF16Plan>> plans;      // per decoder layer: qkv, out, cross query, cross out, mlp1, mlp2
+};
+
+// workspace of token alignment (align.cu), grown on demand
+struct AlignSeq {        // one sequence of a group
+    int64_t row_off;     // its first row in the group's packed rows
+    int64_t mat_off;     // its first element in the group's packed matrices [N][C]
+    int L, first, C, win;
+};
+struct AlignWs {
+    DevBuf<AlignSeq> seqs;
+    DevBuf<int64_t> out_off;         // per sequence its first aligned id in start / end
+    DevBuf<int> heads, start, end;   // heads: the selected heads by layer, ascending; start / end: per aligned id
+    DevBuf<float> w, mat;            // w: [heads of a layer][rows][Cmax] weights; mat: the group's packed matrices
+    DevBuf<double> stats;            // [heads of a layer][sequences][Cmax]: column mean, biased std
 };
 
 // pinned host array
@@ -87,6 +105,7 @@ struct Session {
     // ---- geometry of the windows currently encoded (host mirrors)
     int n_windows = 0;
     std::vector<int> win_Tm, win_T;
+    std::vector<int> win_F;   // mel frames of each window that hold audio (kept frames; n_ctx of encode_mels): the alignment's columns
     std::vector<int64_t> win_row_off;
     int64_t M_tot = 0;
     int max_T = 0, max_Tm = 0;
@@ -223,6 +242,17 @@ struct Session {
     void score_tokens(int64_t n_seqs, const int32_t* window_of_seq, const int64_t* tokens, const int64_t* lens, bool apply_mask,
                       const uint8_t* is_special_host, float* lp_out, int64_t* argmax_out);
     ScoreWs score_ws;
+    // the teacher-forced decoder over the M packed rows whose token ids and positions are in score_ws.tok / score_ws.pos (n
+    // sequences, rows and windows in score_ws.seqs / score_ws.seq_win, at most max_T rows each): the embedding, then layers
+    // 0 .. n_layers - 1.  after_cross_query(l), when set, runs once layer l's scaled cross queries are in score_ws.qkv_h /
+    // score_ws.qkv_l; with full = false the last layer stops there
+    void decoder_pass(int M, int n, int max_T, int n_layers, bool full, const std::function<void(int)>& after_cross_query);
+    // token alignment (align.cu, wb_session_align_tokens): per aligned id its start and end encoder position on the DTW path
+    // through the cross-attention matrix of the selected heads; writes no decode state
+    void align_tokens(int64_t n_seqs, const int32_t* window_of_seq, const int64_t* tokens, const int64_t* lens, const int64_t* first,
+                      int64_t n_heads, const int32_t* heads, int32_t* start_out, int32_t* end_out, float* matrix_out,
+                      int64_t matrix_capacity);
+    AlignWs align_ws;
 };
 
 // host pipeline (transcribe.cu).  window_prompts checks every argument of a decode call and builds each window's prompt
@@ -249,6 +279,11 @@ std::vector<std::vector<int64_t>> waveforms_to_tokens_resampled(Session& s, cons
 std::vector<std::pair<int64_t, int64_t>> window_bounds(int64_t n_samples, int64_t sample_rate, int64_t window_len);
 bool find_chunk_overlap(const int64_t* prev, int64_t n_prev, const int64_t* curr, int64_t n_curr, int64_t max_n_offsets,
                         int64_t min_n_overlaps, int64_t* prev_index, int64_t* curr_index);
+
+// align.cu: whether the DTW kernel takes an [N][C] matrix (N <= 448 and its 2-bit trace fits one CTA's shared memory); the DTW
+// of one host matrix on the current device (wb_align_dtw) -> start / end per row
+bool dtw_fits(int64_t N, int64_t C);
+void align_dtw(const float* matrix, int64_t N, int64_t C, int32_t* start_out, int32_t* end_out);
 
 // wav.cu: load_audio_waveform (src/bin/transcribe/main.rs:31-55)
 void load_wav(const std::string& path, bool strict, std::vector<float>& out, int64_t& sample_rate, int& channels);

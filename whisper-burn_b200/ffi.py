@@ -89,6 +89,8 @@ SYMBOLS = {
     "wb_session_last_logprobs": (C.c_int, [_P, C.c_int64, _F, C.c_int64, _I64]),
     "wb_session_last_nbest": (C.c_int, [_P, C.c_int64, C.c_int64, C.c_int64, _I64, _F, _I64, C.POINTER(C.c_double), _I32, _I64]),
     "wb_session_score_tokens": (C.c_int, [_P, C.c_int64, _I32, _I64, _I64, C.c_int, _U8, _F, _I64]),
+    "wb_session_align_tokens": (C.c_int, [_P, C.c_int64, _I32, _I64, _I64, _I64, C.c_int64, _I32, _I32, _I32, _F, C.c_int64]),
+    "wb_align_dtw": (C.c_int, [C.c_int, _F, C.c_int64, C.c_int64, _I32, _I32]),
     "wb_session_last_decoder": (C.c_int, [_P]),
     "wb_session_last_topk": (C.c_int, [_P, C.c_int64, C.c_int64, _I64, _F]),
     "wb_beam_search_table": (C.c_int64, [C.POINTER(C.c_double), C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _I64, C.c_int64]),

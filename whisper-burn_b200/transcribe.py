@@ -2,8 +2,10 @@
 Detokenisation (src/token.rs) stays with the caller: the library needs 5 ids and a bitmap."""
 from __future__ import annotations
 
+import base64
 import ctypes as C
-from typing import List, Optional, Sequence
+import gzip
+from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -267,6 +269,44 @@ class Session:
         offs = np.concatenate([[0], np.cumsum(lens)])
         return [(lp[offs[i]:offs[i + 1]].copy(), am[offs[i]:offs[i + 1]].copy()) for i in range(len(lens))]
 
+    def align_tokens(self, seqs: Sequence[Sequence[int]], windows: Sequence[int], first: Sequence[int],
+                     heads: Optional[Sequence[Tuple[int, int]]] = None, return_matrix: bool = False):
+        """When each token was spoken (wb_session_align_tokens): openai-whisper's find_alignment over the encoded windows,
+        sequence i on window windows[i] with its aligned ids seqs[i][first[i]:] (first = 4 for a default transcribe row, the
+        prompt length for a previous-text row).  heads: (layer, head) pairs, None for every head of the second half of the
+        decoder layers (alignment_heads_from_openai gives a checkpoint's tuned heads).  Returns per sequence (start, end),
+        int32 encoder positions of each aligned id (20 ms each from the window's start), with return_matrix also its
+        float32 alignment matrix [len - first, C]."""
+        lens = np.asarray([len(s) for s in seqs], dtype=np.int64)
+        toks = np.ascontiguousarray(np.concatenate([np.asarray(s, dtype=np.int64) for s in seqs]) if len(seqs)
+                                    else np.zeros(0, dtype=np.int64), dtype=np.int64)
+        win = np.ascontiguousarray(windows, dtype=np.int32)
+        fst = np.ascontiguousarray(first, dtype=np.int64)
+        if len(win) != len(lens) or len(fst) != len(lens):
+            raise ValueError(f"align_tokens: {len(lens)} sequences, {len(win)} windows and {len(fst)} first indices")
+        hs = np.ascontiguousarray(np.asarray(heads if heads is not None else [], dtype=np.int32).reshape(-1, 2))
+        n_ids = int(np.clip(lens - fst, 1, None).sum()) if len(lens) else 1
+        start = np.empty(max(n_ids, 1), dtype=np.int32)
+        end = np.empty(max(n_ids, 1), dtype=np.int32)
+        cap = n_ids * self.whisper.config.n_audio_ctx if return_matrix else 0   # C <= n_audio_ctx
+        mat = np.empty(max(cap, 1), dtype=np.float32)
+        ffi.check(ffi.lib().wb_session_align_tokens(self._h, len(lens), ffi.i32ptr(win), ffi.i64ptr(toks), ffi.i64ptr(lens),
+                                                   ffi.i64ptr(fst), len(hs), ffi.i32ptr(hs) if len(hs) else None,
+                                                   ffi.i32ptr(start), ffi.i32ptr(end), ffi.fptr(mat) if return_matrix else None,
+                                                   cap))
+        out, a, m = [], 0, 0
+        for L, f in zip(lens, fst):
+            n = int(L - f)
+            st, en = start[a:a + n].copy(), end[a:a + n].copy()
+            if return_matrix:
+                c = int(en[-1])   # end of the last aligned id = the column count
+                out.append((st, en, mat[m:m + n * c].reshape(n, c).copy()))
+                m += n * c
+            else:
+                out.append((st, en))
+            a += n
+        return out
+
     def last_decoder(self) -> int:
         return int(ffi.lib().wb_session_last_decoder(self._h))
 
@@ -303,6 +343,29 @@ def waveform_to_text(whisper: Whisper, special, is_special: np.ndarray, waveform
         return s.waveform_to_tokens(waveform, special, is_special, sample_rate, beam_size, max_depth)
     finally:
         s.close()
+
+
+def align_dtw(matrix: np.ndarray, device: int = 0):
+    """(start, end) int32 per row of the DTW on -matrix that wb_session_align_tokens runs, alone, on the GPU (wb_align_dtw):
+    matrix float32 [N, C], N in [1, 448]."""
+    m = np.ascontiguousarray(matrix, dtype=np.float32)
+    if m.ndim != 2:
+        raise ValueError("align_dtw: matrix must be 2-D")
+    start = np.empty(max(m.shape[0], 1), dtype=np.int32)
+    end = np.empty(max(m.shape[0], 1), dtype=np.int32)
+    ffi.check(ffi.lib().wb_align_dtw(device, ffi.fptr(m), m.shape[0], m.shape[1], ffi.i32ptr(start), ffi.i32ptr(end)))
+    return start[:m.shape[0]], end[:m.shape[0]]
+
+
+def alignment_heads_from_openai(b85: str | bytes, dims) -> List[Tuple[int, int]]:
+    """The (layer, head) pairs of an openai-whisper alignment-head mask (whisper/__init__.py _ALIGNMENT_HEADS): base85 of a
+    gzip'ed bool array [n_text_layer][n_text_head], ascending."""
+    raw = gzip.decompress(base64.b85decode(b85))
+    if len(raw) != dims.n_text_layer * dims.n_text_head:
+        raise ValueError(f"alignment heads: {len(raw)} mask entries, not n_text_layer x n_text_head = "
+                         f"{dims.n_text_layer * dims.n_text_head}")
+    mask = np.frombuffer(raw, dtype=bool).reshape(dims.n_text_layer, dims.n_text_head)
+    return [(int(l), int(h)) for l, h in zip(*np.nonzero(mask))]
 
 
 def window_bounds(n_samples: int, sample_rate: int, window_len: int):
